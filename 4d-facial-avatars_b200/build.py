@@ -1,7 +1,6 @@
-"""Build lib/libnfb.so (the C-ABI shared library of include/nfb.h) in-tree with nvcc for sm_100a.
+"""Build lib/libnfb.so (the C-ABI shared library of include/nfb.h) in-tree with nvcc for sm_90a (H100).
 
-The .so is git-ignored but travels to the GPU box with the repo snapshot.  Rebuilds only when a
-source is newer than the library.  Usage: python 4d-facial-avatars_b200/build.py [--force] [--verbose] [--timers] | --variant NAME -D... (experiment build lib/libnfb_NAME.so)
+The .so is git-ignored; rebuilds only when a source is newer than the library.  Usage: python 4d-facial-avatars_b200/build.py [--force] [--verbose] [--timers] | --variant NAME -D... (experiment build lib/libnfb_NAME.so)
 
 --timers additionally builds lib/libnfb_timers.so with the phase timers compiled in (-DNFB_TIMERS=1; they cost registers in
 the kernels' hot loops, so the product library does not carry them); tools/phase_profile.py loads it through NFB_LIB.
@@ -14,8 +13,8 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIB_DIR, "libnfb.so")
-SOURCES = ["nfb_api.cu", "nfb_pack.cu", "nfb_optim.cu", "nfb_post.cu", "nfb_render.cu", "nfb_render2.cu", "nfb_render3.cu", "nfb_train.cu"]
-HEADERS = ["nfb_internal.h", "nfb_layout.h", "nfb_ptx.cuh", "nfb_save.cuh", "nfb_render_common.cuh", "nfb_tile2.cuh", "nfb_sampler.h", os.path.join("..", "..", "include", "nfb.h")]
+SOURCES = ["nfb_api.cu", "nfb_pack.cu", "nfb_optim.cu", "nfb_post.cu", "nfb_render.cu", "nfb_train.cu"]
+HEADERS = ["nfb_internal.h", "nfb_layout.h", "nfb_ptx.cuh", "nfb_save.cuh", "nfb_render_common.cuh", "nfb_sampler.h", os.path.join("..", "..", "include", "nfb.h")]
 
 
 def _nvcc():
@@ -42,7 +41,7 @@ def build(force=False, verbose=False, timers=False, variant=None, defines=()):
         return LIB
     os.makedirs(LIB_DIR, exist_ok=True)
     srcs = [os.path.join(CSRC, f) for f in SOURCES if os.path.exists(os.path.join(CSRC, f))]
-    cmd = [_nvcc(), "-gencode", "arch=compute_100a,code=sm_100a", "-O3", "-lineinfo", "-std=c++17",
+    cmd = [_nvcc(), "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
            "-Xcompiler", "-fPIC", "-shared", "-DNFB_BUILD"] + (["-DNFB_TIMERS=1"] if timers else []) + list(defines) + ["-o", out] + srcs
     if verbose:
         cmd.insert(1, "-Xptxas=-v")

@@ -35,10 +35,6 @@ struct NfbHandle {
   int num_sms = 0;
   nfb::NetBuffers net[2];
   bool frame_set = false;
-  bool use_render2 = true;
-  bool use_render3 = true;
-  bool train_render2 = false;   // training forward on the two-tile kernel (NFB_TRAIN_KERNEL=v6)
-  bool train_render3 = false;   // training forward on the pipelined kernel (NFB_TRAIN_KERNEL=v7); default: the one-tile kernel
   long long launches = 0;
   // cached torch.linspace(0,1,n) tables on the device
   float* lin_c = nullptr; int lin_c_n = 0;
@@ -92,10 +88,10 @@ const char* nfb_strerror(int status) {
   switch (status) {
     case NFB_OK: return "ok";
     case NFB_ERR_INVALID: return "invalid argument";
-    case NFB_ERR_UNSUPPORTED: return "configuration not supported by the sm_100a render kernel";
+    case NFB_ERR_UNSUPPORTED: return "configuration not supported by the sm_90a render kernel";
     case NFB_ERR_CUDA: return "CUDA runtime error (see nfb_last_cuda_error)";
     case NFB_ERR_STATE: return "weights or per-frame conditioning not set";
-    case NFB_ERR_ARCH: return "device is not compute capability 10.x (sm_100a code only)";
+    case NFB_ERR_ARCH: return "device is not compute capability 9.0 (sm_90a code only)";
     default: return "unknown status";
   }
 }
@@ -136,21 +132,6 @@ static int create_impl(NfbHandle* h, const cudaDeviceProp& prop) {
   NFB_CUDA(dev_alloc(&h->d_expr, nfb::kDimExpr));
   NFB_CUDA(dev_alloc(&h->d_latent, nfb::kDimLatent));
   NFB_CUDA(nfb::render_kernel_setup());
-  NFB_CUDA(nfb::render2_kernel_setup());
-  NFB_CUDA(nfb::render3_kernel_setup());
-  {  // NFB_KERNEL=v4 forces the one-tile-in-flight kernel everywhere (default: the two-tile kernel where it applies)
-    const char* k = std::getenv("NFB_KERNEL");
-    h->use_render2 = !(k && std::strcmp(k, "v4") == 0);
-    h->use_render3 = h->use_render2 && !(k && std::strcmp(k, "v6") == 0);  // NFB_KERNEL=v6: two tiles in flight, passes not pipelined
-    // The training forward defaults to the one-tile kernel: with the record stores the two-tile kernel's row warps spill
-    // (216 B) and it is slower there (measured 1.46 ms vs 1.01 ms per 2048-ray forward); NFB_TRAIN_KERNEL=v6 selects it.
-    const char* tk = std::getenv("NFB_TRAIN_KERNEL");
-    h->train_render2 = tk && std::strcmp(tk, "v6") == 0;
-    // Both two-stream kernels have SAVE variants whose records are bit-identical to the one-tile kernel's, and both are SLOWER
-    // there (2048 rays, 64c+64f: v4 0.77 ms, v6 1.46 ms, v7 1.26 ms): the record is written as 16-bit transposed stores, 2304 per
-    // row thread and tile, and with two streams the same eight row warps issue twice as many per unit of time.
-    h->train_render3 = h->use_render3 && tk && std::strcmp(tk, "v7") == 0;
-  }
   return NFB_OK;
 }
 
@@ -163,7 +144,7 @@ int nfb_create(const NfbModelDims* dims, int device, NfbHandle** out) {
   NFB_CUDA(cudaSetDevice(device));
   cudaDeviceProp prop;
   NFB_CUDA(cudaGetDeviceProperties(&prop, device));
-  if (prop.major != 10) return NFB_ERR_ARCH;
+  if (prop.major != 9 || prop.minor != 0) return NFB_ERR_ARCH;
   NfbHandle* h = new (std::nothrow) NfbHandle();
   if (!h) return NFB_ERR_INVALID;
   h->device = device;
@@ -387,8 +368,7 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
       // the outputs with the evaluation kernel now, and let the backward re-run the training forward in chunks that fit.
       if (!rays->o) { g_last_cuda_error = "training forward over budget needs explicit rays (o, d)"; return NFB_ERR_UNSUPPORTED; }
       size_t units = train_budget(h) / nfb::kRecBytes / tiles_per_unit;
-      units &= ~(size_t)1;  // whole two-tile units of work
-      if (units < 2) units = 2;
+      if (units < 1) units = 1;
       tr.chunk_rays = (int)(units * p.rays_per_unit);
       tr.full = p;
       tr.precision = exact ? 1 : 0;
@@ -402,14 +382,7 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
     tr.n_rays = rays->n_rays; tr.nc = nc; tr.nf = nf; tr.rays_per_unit = p.rays_per_unit; tr.tiles_c = p.tiles_c;
     tr.tiles_f = p.tiles_f; tr.n_units = p.n_units; tr.has_bg = rays->background != nullptr; tr.white_bkgd = p.white_bkgd;
   }
-  // fast-mode evaluation runs the two-tiles-in-flight kernel (the training forward only on request, see nfb_create); exact
-  // mode (hi+lo operands need twice the TMEM columns) and the layer probe run the one-tile kernel
-  const bool saving = train && !h->tr.chunked;
-  const bool two_tile = h->use_render2 && !exact && !p.dbg_act && (!saving || h->train_render2);
-  const bool pipelined = h->use_render3 && !exact && !p.dbg_act && (!saving || h->train_render3) && nfb::render3_supports(p);
-  if (pipelined) NFB_CUDA(nfb::launch_render3(p, h->num_sms, st, &h->launches));
-  else if (two_tile) NFB_CUDA(nfb::launch_render2(p, h->num_sms, st, &h->launches));
-  else NFB_CUDA(nfb::launch_render(p, exact ? 1 : 0, h->num_sms, st, &h->launches));
+  NFB_CUDA(nfb::launch_render(p, exact ? 1 : 0, h->num_sms, st, &h->launches));
   if (train) h->tr.valid = true;
   return NFB_OK;
 }
@@ -511,9 +484,7 @@ int nfb_render_backward(NfbHandle* h, const NfbOutGrads* og, const float* const 
       p.w_last = so + 10 * cn;
       p.save_rec = tr.rec; p.save_dnorm = tr.dnorm; p.save_raw_c = tr.raw_c; p.save_raw_f = tr.raw_f;
       p.dbg_z_c = tr.z_c; p.dbg_z_f = tr.z_f;
-      if (h->train_render3 && tr.precision == 0 && nfb::render3_supports(p)) NFB_CUDA(nfb::launch_render3(p, h->num_sms, st, &h->launches));
-      else if (h->train_render2 && tr.precision == 0) NFB_CUDA(nfb::launch_render2(p, h->num_sms, st, &h->launches));
-      else NFB_CUDA(nfb::launch_render(p, tr.precision, h->num_sms, st, &h->launches));
+      NFB_CUDA(nfb::launch_render(p, tr.precision, h->num_sms, st, &h->launches));
       rc = backward_rays(begin, n, n_units);
       if (rc) return rc;
     }
@@ -654,16 +625,10 @@ int nfb_debug_schedule(int which, int index, uint32_t* out, int out_words) {
   if (index >= 0 && (!out || out_words < 10)) return -1;
   switch (which) {
     case 0: return nfb::debug_prog_v4(index, out);
-    case 1: return nfb::debug_prog_v6(index, out);
     case 2: return nfb::debug_prog_chain(index, out);
     case 3: return nfb::debug_jobs_dw(index, out);
     case 4: return index < 0 ? 1 : nfb::debug_dw_split(out);  // in/out: {num_sms, tiles 0, tiles 1} -> {parts0, parts1, groups}
-    default:
-      if (which >= 1000) {  // 1000 + n_iter * 100 + Tc * 10 + Tf: the pipelined kernel's job sequence
-        const int w = which - 1000;
-        return nfb::debug_jobs_v7(w / 100, (w / 10) % 10, w % 10, index, out);
-      }
-      return -1;
+    default: return -1;
   }
 }
 

@@ -89,8 +89,6 @@ struct DwParams {  // ONE launch covers both networks: the first parts[0] * grou
 };
 // host copies of the compile-time schedules (nfb_debug_schedule); index < 0: number of entries; else words written or -1
 int debug_prog_v4(int index, uint32_t* out);
-int debug_prog_v6(int index, uint32_t* out);
-int debug_jobs_v7(int n_iter, int tc, int tf, int index, uint32_t* out);
 int debug_prog_chain(int index, uint32_t* out);
 int debug_jobs_dw(int index, uint32_t* out);
 int debug_dw_split(uint32_t* io);  // io: {num_sms, tiles net 0, tiles net 1} -> {parts0, parts1, groups}
@@ -117,14 +115,6 @@ cudaError_t launch_adam(float* p, float* g, float* m, float* v, long long n, flo
 // precision: 0 = fast (x1), 1 = exact (x3).  num_sms = CTAs to launch at most.
 cudaError_t launch_render(const RenderParams& p, int precision, int num_sms, cudaStream_t st, long long* launches);
 cudaError_t render_kernel_setup();  // opt-in to the large dynamic shared memory size
-// Two-tiles-in-flight kernel (nfb_render2.cu): fast mode, evaluation (no training records, no layer probe / phase timers).
-cudaError_t render2_kernel_setup();
-cudaError_t launch_render2(const RenderParams& p, int num_sms, cudaStream_t st, long long* launches);
-// Two tiles in flight + software-pipelined passes (nfb_render3.cu): fast-mode evaluation of the configurations its fixed
-// shared-memory budget covers (render3_supports), bit-identical to nfb_render2.cu.
-cudaError_t render3_kernel_setup();
-bool render3_supports(const RenderParams& p);
-cudaError_t launch_render3(const RenderParams& p, int num_sms, cudaStream_t st, long long* launches);
 
 // ---- either side of the path (nfb_post.cu)
 cudaError_t launch_frame_products(const float* rgb, const float* disp, const float* w_last, const double intr[4], int H, int W,

@@ -1,5 +1,5 @@
 // nfb_layout.h — the MLP as the kernel executes it: 10 tensor-core "steps", each a GEMM
-//   D[128 rows, N] = A[128 rows, K] * W[N, K]^T   (FP16 operands, FP32 accumulate in TMEM)
+//   D[128 rows, N] = A[128 rows, K] * W[N, K]^T   (FP16 operands, FP32 accumulate in registers)
 // and the byte layout of the packed weight stream the kernel bulk-copies into shared memory.
 // Shared by host (packing, tests) and device code.
 //
@@ -12,18 +12,16 @@
 //
 //   step  reference layer            N (half 0 + half 1)  K (atoms of 64)            A operand
 //   0     layers_xyz.0               128 + 128            64  = PE(63)+pad           SMEM (PE buffer)
-//   1,2   layers_xyz.1,2             128 + 128            256                        TMEM
-//   3     layers_xyz.3               128 + 128            320 = PE(63)+pad | h(256)  SMEM atom + TMEM
-//   4,5   layers_xyz.4,5             128 + 128            256                        TMEM
-//   6     layers_dir.0∘fc_feat | σ   128 + 16 (σ)         256                        TMEM
-//   7,8   layers_dir.1,2             128                  128                        TMEM
-//   9     fc_rgb                     16 (3 used)          128                        TMEM
+//   1,2   layers_xyz.1,2             128 + 128            256                        SMEM (activations)
+//   3     layers_xyz.3               128 + 128            320 = PE(63)+pad | h(256)  SMEM atom + activations
+//   4,5   layers_xyz.4,5             128 + 128            256                        SMEM (activations)
+//   6     layers_dir.0∘fc_feat | σ   128 + 16 (σ)         256                        SMEM (activations)
+//   7,8   layers_dir.1,2             128                  128                        SMEM (activations)
+//   9     fc_rgb                     16 (3 used)          128                        SMEM (activations)
 //
-// A weight "unit" = all N rows of the step x one 64-wide K atom (<= 32 KB), consumed by 4 tcgen05.mma (M=128, N, K=16).
-// The epilogue converts the accumulator in two column halves ("half 0" = output columns [0,128) = K atoms 0,1 of the
-// next step, "half 1" = [128,256) = atoms 2,3) and signals each; the units of the next step are grouped by what they
-// need:   [PE atom] [hidden atoms 0,1] = group 1 (needs half 0 only)   |   [hidden atoms 2,3] = group 2 (needs half 1 too)
-// so the next step starts on atoms 0,1 while the second half of the previous step is still being converted.
+// A weight "unit" = all N rows of the step x one 64-wide K atom (<= 32 KB), consumed by 4 wgmma (M=64 per warpgroup, N, K=16).
+// The accumulator is kept in two column halves ("half 0" = output columns [0,128) = K atoms 0,1 of the next step,
+// "half 1" = [128,256) = atoms 2,3), one m64n128 (or n16) wgmma accumulator each.
 #pragma once
 #include <stdint.h>
 
@@ -35,7 +33,7 @@
 
 namespace nfb {
 
-constexpr int kTileM = 128;      // rows (samples) per tensor-core tile == TMEM lanes
+constexpr int kTileM = 128;      // rows (samples) per tensor-core tile (two warpgroups of 64)
 constexpr int kAtomK = 64;       // fp16 elements per 128-byte swizzle row
 constexpr int kNumSteps = 10;
 constexpr int kMaxUnitBytes = 256 * 128;  // one weight unit: <=256 output rows x 64 K x 2 B
@@ -128,10 +126,10 @@ NFB_HD constexpr int img_offset(int rows, int k, int r) { return (r >> 6) * rows
 // Backward chain (dX): 9 tensor-core steps per 128-row tile, same machinery as the forward pass with transposed weights.
 //   step  computes                         N (half0+half1)  K atoms                A operand
 //   0     d g2 = d rgb . Wrgb              128              1 (smem, k<3 used)     SMEM (d raw operand)
-//   1     d g1 = dY8 . Wd2                 128              2                      TMEM
-//   2     d g0 = dY7 . Wd1                 128              2                      TMEM
-//   3     d h5 = dY6 . M1 + d sigma . m2   128 + 128        1 (smem, k=3) + 2      SMEM atom + TMEM
-//   4..8  d h4..h0 = dY . W5, W4, W3[:,171:], W2, W1   128 + 128   4               TMEM
+//   1     d g1 = dY8 . Wd2                 128              2                      SMEM (activations)
+//   2     d g0 = dY7 . Wd1                 128              2                      SMEM (activations)
+//   3     d h5 = dY6 . M1 + d sigma . m2   128 + 128        1 (smem, k=3) + 2      SMEM atom + activations
+//   4..8  d h4..h0 = dY . W5, W4, W3[:,171:], W2, W1   128 + 128   4               SMEM (activations)
 // The epilogue of step s multiplies by the ReLU mask of forward layer (8 - s) and yields dY(8 - s).
 constexpr int kBwdSteps = 9;
 NFB_HD constexpr StepInfo bwd_step_info(int s) {

@@ -125,12 +125,12 @@ __device__ __forceinline__ void pack_bwd_chunk(const NetParams& a, int s, int u,
   if (idx >= rows * 8) return;
   const int c16 = idx & 7, n = idx >> 3;
   const bool op_atom = si.pe_first && u == 0;
-  const int hid = u - si.pe_first;  // TMEM atom index
+  const int hid = u - si.pe_first;  // K atom of the activation buffer
   __align__(16) __half h[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
     const int kl = c16 * 8 + e;        // k inside the atom
-    const int kk = hid * 64 + kl;      // output-feature index of the forward layer (TMEM atoms)
+    const int kk = hid * 64 + kl;      // output-feature index of the forward layer (activation atoms)
     float w = 0.f;
     switch (s) {
       case 0: if (kl < 3) w = a.p[24][kl * 128 + n]; break;                       // fc_rgb.weight[kl][n]

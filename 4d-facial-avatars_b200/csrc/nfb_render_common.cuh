@@ -1,6 +1,5 @@
-// nfb_render_common.cuh — device code shared by the render kernels (nfb_render.cu: one tile in flight, both precision
-// modes and the training variant; nfb_render2.cu: two tiles in flight, fast mode): per-ray constants, the positional
-// encoding's sin/cos, the epilogue arithmetic of one accumulator chunk, and the per-ray compositing.
+// nfb_render_common.cuh — device code of the render kernel (nfb_render.cu): per-ray constants, the positional encoding's
+// sin/cos, and the per-ray compositing.
 #pragma once
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
@@ -41,67 +40,6 @@ __device__ __forceinline__ void pe_sincos(float y, float& s, float& c) {
     c = __cosf(r);
   }
 }
-
-// (a0, a1) += (b0, b1) as one packed FP32 add (sm_100 FADD2; round-to-nearest per element, like two scalar adds).
-__device__ __forceinline__ void add_f32x2(float& a0, float& a1, float b0, float b1) {
-  asm("{\n\t.reg .b64 ra, rb, rc;\n\tmov.b64 ra, {%0, %1};\n\tmov.b64 rb, {%2, %3};\n\tadd.rn.f32x2 rc, ra, rb;\n\t"
-      "mov.b64 {%0, %1}, rc;\n\t}"
-      : "+f"(a0), "+f"(a1)
-      : "f"(b0), "f"(b1));
-}
-
-// ------------------------------------------------------------------------------------------------
-// Epilogue math of one 32-column accumulator chunk: x = acc + bias (+ extra); ReLU; FP16 hi (and lo).
-template <bool EXACT>
-__device__ __forceinline__ void epi_math(const uint32_t (&v)[32], uint32_t bias, uint32_t extra,
-                                         float* __restrict__ dump, uint32_t (&hi)[16], uint32_t (&lo)[16]) {
-  float x[32];  // bias / extra are shared-memory byte addresses (extra == 0: none)
-#pragma unroll
-  for (int j = 0; j < 32; j += 4) {  // packed FP32 adds (FADD2): same rounding as scalar adds, half the issue slots
-    const float4 b = lds128(bias + j * 4);
-    x[j] = __uint_as_float(v[j]); x[j + 1] = __uint_as_float(v[j + 1]);
-    x[j + 2] = __uint_as_float(v[j + 2]); x[j + 3] = __uint_as_float(v[j + 3]);
-    add_f32x2(x[j], x[j + 1], b.x, b.y);
-    add_f32x2(x[j + 2], x[j + 3], b.z, b.w);
-  }
-  if (extra) {
-#pragma unroll
-    for (int j = 0; j < 32; j += 4) {
-      const float4 e = lds128(extra + j * 4);
-      add_f32x2(x[j], x[j + 1], e.x, e.y);
-      add_f32x2(x[j + 2], x[j + 3], e.z, e.w);
-    }
-  }
-  if (dump) {
-#pragma unroll
-    for (int j = 0; j < 32; ++j) dump[j] = fmaxf(x[j], 0.f);
-  }
-#pragma unroll
-  for (int j = 0; j < 32; j += 2) {
-    if constexpr (EXACT) {
-      const float a = fmaxf(x[j], 0.f), b = fmaxf(x[j + 1], 0.f);
-      hi[j / 2] = pack_f16x2(a, b);
-      const float2 h = unpack_f16x2(hi[j / 2]);
-      lo[j / 2] = pack_f16x2(a - h.x, b - h.y);
-    } else {
-      hi[j / 2] = pack_relu_f16x2(x[j], x[j + 1]);  // ReLU fused into the conversion
-    }
-  }
-}
-
-// ReLU mask of 32 post-activation FP16 values (bit j = feature j is non-zero).  An activation that is positive in FP32
-// but rounds to FP16 zero counts as inactive: its value is what the next layer saw.
-__device__ __forceinline__ uint32_t relu_mask32(const uint32_t (&h)[16]) {
-  uint32_t m = 0u;
-#pragma unroll
-  for (int j = 0; j < 16; ++j) {
-    m |= ((h[j] & 0xFFFFu) ? 1u : 0u) << (2 * j);
-    m |= ((h[j] >> 16) ? 1u : 0u) << (2 * j + 1);
-  }
-  return m;
-}
-
-__device__ __forceinline__ uint32_t cta_rank_early() { return cluster_ctarank(); }
 
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
@@ -170,7 +108,7 @@ __device__ __forceinline__ float composite_ray(const float4* __restrict__ pre, c
 
 // Optional phase timers (NfbDebug.prof): cycles of one observer thread per role, summed over CTAs.  Compiled in only with
 // -DNFB_TIMERS=1 (tools/phase_profile.py builds such a library): even disabled at run time they cost registers in the
-// hot loops (measured: -15 % on the two-tile kernel).
+// hot loops.
 #ifndef NFB_TIMERS
 #define NFB_TIMERS 0
 #endif

@@ -1,4 +1,4 @@
-// nfb_train.cu — backward of the render path as hand-written sm_100a kernels.
+// nfb_train.cu — backward of the render path as hand-written sm_90a kernels.
 //
 // The reference has no hand-written backward: `loss.backward()` (train_transformed_rays.py:389) runs torch.autograd over
 // the unfused graph of train_utils.py:36-162 / volume_rendering_utils.py:7-75 / models.py:236-261.  SURVEY.md §8 (a''')
@@ -8,16 +8,15 @@
 //                             Re-evaluates the compositing of both passes from what the training forward saved (depths,
 //                             colours, ReLU input of sigma) with a division-free reverse recurrence for the transmittance
 //                             term.  Also yields d fc_rgb.bias / d sigma-bias sums and the max |gradient| for the scale.
-//   2. chain_kernel           dX chain of the MLP per 128-row tile on tcgen05: 9 steps with transposed weight streams,
-//                             same machinery as the forward kernel (TMEM-resident activations converted in place, bulk-copy
-//                             weight ring with cluster multicast, two-gate epilogue).  The epilogue applies the saved ReLU
-//                             masks; four record-saver warps read every dY back from TMEM and write it as a transposed FP16
-//                             image into the tile record.
+//   2. chain_kernel           dX chain of the MLP per 128-row tile on wgmma: 9 steps with transposed weight streams,
+//                             same machinery as the forward kernel (register accumulators, shared-memory activations
+//                             overwritten in place, bulk-copy weight ring).  The epilogue applies the saved ReLU masks and
+//                             writes every dY as a transposed FP16 image into the tile record.
 //   3. dw_kernel              dW[n,k] = sum_rows dY[row,n] X[row,k] for every layer: both operands are bulk-copied from
-//                             the tile records (K-major images whose K axis is the sample row) and multiplied on tcgen05
-//                             (M=128 output features x N input features per job, FP32 accumulation in TMEM over all tiles
-//                             of the CTA), then reduced into FP32 accumulators with red.global.add.  One launch for both
-//                             networks; HBM-bound, so the job groups are laid out for L2 sharing of the input images.
+//                             the tile records (K-major images whose K axis is the sample row) and multiplied on wgmma
+//                             (M=128 output features x N input features per job, FP32 accumulation in registers over all
+//                             tiles of the CTA), then reduced into FP32 accumulators with red.global.add.  One launch for
+//                             both networks; the job groups are laid out for L2 sharing of the input images.
 //   4. finalize_kernel        un-folds the kernel's parametrisation (fc_feat pre-multiplied into fc_alpha / layers_dir.0,
 //                             conditioning columns folded into biases) by the chain rule and writes the 24 used parameter
 //                             gradients of each network in the reference's state_dict layout, plus d latent_code.
@@ -225,25 +224,28 @@ __host__ __device__ constexpr int bwd_unit_offset(int s, int u) { return bwd_ste
 // ================================================================================================
 namespace chain {
 
-constexpr int kNumSlots = 5;
-// 512 threads: warp 0 weight producer, 1 MMA issuer, 2..3 idle (setmaxnreg works on whole warpgroups), 4..11 row warps,
-// 12..15 record savers — as in the training forward (nfb_render.cu), they read each step's FP16 output back from TMEM and write
-// the transposed dY image, so the ~1,900 two-byte stores per tile and warp are off the row warps' critical path.
-constexpr int kThreads = 512;
-constexpr int kRegsLight = 80, kRegsRow = 176, kRegsSaver = 80;
-static_assert((4 * kRegsLight + 8 * kRegsRow + 4 * kRegsSaver) * 32 <= 65536, "register file");
+// 384 threads: warp 0 weight producer (warps 1..3 idle: the register file is re-partitioned per warpgroup), warpgroups 1 and 2
+// compute rows [64w, 64w+64) of the tile on wgmma with register accumulators; their epilogue applies the saved ReLU mask, writes
+// the FP16 result in place into the shared-memory activation buffer (A operand of the next step) and as the transposed dY image
+// into the tile record.
+constexpr int kNumSlots = 4;
+constexpr int kThreads = 384;
+constexpr int kRegsLight = 40, kRegsRow = 232;
+static_assert((4 * kRegsLight + 8 * kRegsRow) * 32 <= 65536, "register file");
 template <int N> __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N> __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
-constexpr int kCluster = 2;
 constexpr int kRowThreads = 256;
+constexpr uint32_t kRowBarrier = 1;  // both warpgroups; 2 + w: warpgroup w alone
 constexpr int kOffRing = 0;
-constexpr int kOffOp = kOffRing + kNumSlots * kMaxUnitBytes;  // d raw operand: [128 rows x 64 k] FP16, swizzled (k < 4 used)
+constexpr int kOffAct = kOffRing + kNumSlots * kMaxUnitBytes;  // 4 K atoms x [128 rows x 128 B]
+constexpr int kOffOp = kOffAct + 4 * kTileM * 128;             // d raw operand: [128 rows x 64 k] FP16, swizzled (k < 4 used)
 constexpr int kOffBars = kOffOp + kTileM * 128;
-constexpr int kNumBars = 2 * kNumSlots + 4 + 6;  // + bar_sv[2 halves][2 step parities], bar_saved[2 regions]
-constexpr int kOffTmemPtr = kOffBars + kNumBars * 8;
-constexpr int kSmemBytes = kOffTmemPtr + 16;
+constexpr int kSmemBytes = kOffBars + 2 * kNumSlots * 8;
+static_assert(kSmemBytes <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
 
-enum : uint32_t { kFromOp = 1u, kWait0 = 2u, kWait1 = 4u, kFirst = 8u, kCommit0 = 16u, kPostWait1 = 64u, kOddRegion = 256u };
+// Program entry per unit: x = MMA N (rows of the unit), y = K atom of the activation buffer the A operand comes from,
+// z = flags, w = (byte offset in the backward stream) / 16 | rows << 20.
+enum : uint32_t { kFromOp = 1u, kFirst = 8u, kLast = 16u };
 constexpr int total_units() {
   int n = 0;
   for (int s = 0; s < kBwdSteps; ++s) n += bwd_step_info(s).k_atoms;
@@ -253,34 +255,20 @@ constexpr int kTileUnits = total_units();  // 28
 struct ProgEntry { uint32_t x, y, z, w; };
 struct ProgTable { ProgEntry e[32]; };
 static_assert(kTileUnits <= 32, "program table too small");
-constexpr uint32_t region_col_c(int s) { return (s & 1) ? 256u : 0u; }
 constexpr ProgTable make_prog() {
   ProgTable t{};
   int i = 0;
   for (int s = 0; s < kBwdSteps; ++s) {
     const StepInfo si = bwd_step_info(s);
     const int nu = si.k_atoms;
-    bool any_g2 = false;
-    for (int j = 0; j < nu; ++j) any_g2 = any_g2 || bwd_unit_info(s, j).group == 2;
     for (int u = 0; u < nu; ++u, ++i) {
       const BwdUnit ui = bwd_unit_info(s, u);
-      bool first_g1 = true, first_g2 = true;
-      for (int j = 0; j < u; ++j) {
-        if (bwd_unit_info(s, j).group == 1) first_g1 = false;
-        if (bwd_unit_info(s, j).group == 2) first_g2 = false;
-      }
       uint32_t flags = 0;
       if (ui.from_op) flags |= kFromOp;
-      if (ui.group == 1 && first_g1) flags |= kWait0;
-      if (ui.group == 2 && first_g2) flags |= kWait1;
-      if (u == 0) flags |= kFirst;  // also: the step overwrites its region -> the savers must have read what lived there
-      if (s & 1) flags |= kOddRegion;
-      if (ui.last) flags |= kCommit0;
-      if (u == nu - 1 && !any_g2) flags |= kPostWait1;
-      const uint32_t d_col = region_col_c(s);
-      const uint32_t a_col = (region_col_c(s) ^ 256u) + (uint32_t)(u - si.pe_first) * 64u;
-      t.e[i].x = umma_idesc_f16(kTileM, ui.rows);
-      t.e[i].y = d_col | (a_col << 16);
+      if (u == 0) flags |= kFirst;
+      if (ui.last) flags |= kLast;
+      t.e[i].x = (uint32_t)ui.rows;
+      t.e[i].y = ui.from_op ? 0u : (uint32_t)(u - si.pe_first);
       t.e[i].z = flags;
       t.e[i].w = ((uint32_t)bwd_unit_offset(s, u) >> 4) | ((uint32_t)ui.rows << 20);
     }
@@ -289,22 +277,33 @@ constexpr ProgTable make_prog() {
 }
 __constant__ ProgTable c_prog = make_prog();
 
-__device__ __forceinline__ uint32_t region_col(int s) { return (s & 1) ? 256u : 0u; }
-
-// One 64-column slice of the accumulator: masked gradient -> FP16 (h a: columns [0,32), h b: [32,64)).
-__device__ __forceinline__ void bwd_epi_slice(uint32_t t_slice, uint2 m, uint32_t (&ha)[16], uint32_t (&hb)[16]) {
-  uint32_t va[32], vb[32];
-  tmem_ld32(t_slice, va);
-  tmem_ld32(t_slice + 32, vb);
-  tmem_wait_ld();
+// Epilogue of one 128-column accumulator half: masked gradient -> FP16, in place into the activation buffer and into the
+// record image of dY(L).
+__device__ __forceinline__ void bwd_epi_half(const float (&acc)[64], int L, int c_base, const uint32_t* masks, uint8_t* act,
+                                             uint8_t* rec, int r0) {
+  const int lane = threadIdx.x & 31, c = lane & 3;
+  const int W = rec_width(L);
 #pragma unroll
-  for (int j = 0; j < 32; j += 2) {
-    const float a0 = ((m.x >> j) & 1u) ? __uint_as_float(va[j]) : 0.f;
-    const float a1 = ((m.x >> (j + 1)) & 1u) ? __uint_as_float(va[j + 1]) : 0.f;
-    const float b0 = ((m.y >> j) & 1u) ? __uint_as_float(vb[j]) : 0.f;
-    const float b1 = ((m.y >> (j + 1)) & 1u) ? __uint_as_float(vb[j + 1]) : 0.f;
-    ha[j / 2] = pack_f16x2(a0, a1);
-    hb[j / 2] = pack_f16x2(b0, b1);
+  for (int hh = 0; hh < 2; ++hh) {
+    const int R = r0 + 8 * hh;
+    uint4 m = make_uint4(0u, 0u, 0u, 0u);
+    if (masks) m = *reinterpret_cast<const uint4*>(masks + (L * 128 + R) * 8 + (c_base >> 5));
+    const uint32_t mw[4] = {m.x, m.y, m.z, m.w};
+#pragma unroll
+    for (int j = 0; j < 16; ++j) {
+      const int cc = 8 * j + 2 * c;  // column inside the half
+      const uint32_t bits = mw[cc >> 5] >> (cc & 31);
+      const float a0 = (bits & 1u) ? acc[4 * j + 2 * hh] : 0.f;
+      const float a1 = (bits & 2u) ? acc[4 * j + 2 * hh + 1] : 0.f;
+      const uint32_t h = pack_f16x2(a0, a1);
+      const int col = c_base + cc;
+      *reinterpret_cast<uint32_t*>(act + (col >> 6) * (kTileM * 128) + sw128_offset(R, col & 63)) = h;
+      if (rec) {
+        uint8_t* img = rec + rec_dy_off(L);
+        *reinterpret_cast<uint16_t*>(img + img_offset(W, col, R)) = (uint16_t)(h & 0xFFFFu);
+        *reinterpret_cast<uint16_t*>(img + img_offset(W, col + 1, R)) = (uint16_t)(h >> 16);
+      }
+    }
   }
 }
 
@@ -316,141 +315,68 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
 
   const uint32_t bar_full = smem_base + kOffBars;
   const uint32_t bar_empty = bar_full + kNumSlots * 8;
-  const uint32_t bar_aready = bar_empty + kNumSlots * 8;  // [2]
-  const uint32_t bar_accfull = bar_aready + 16;           // [2] (only [0] used: one commit per step)
-  const uint32_t bar_sv = bar_accfull + 16;               // [half][step & 1]: the step's FP16 output is in TMEM -> savers
-  const uint32_t bar_saved = bar_sv + 32;                 // [region]: the savers have read the region -> MMA warp
-  volatile uint32_t* tmem_ptr_s = reinterpret_cast<volatile uint32_t*>(smem + kOffTmemPtr);
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kNumSlots; ++i) {
       mbar_init(bar_full + i * 8, 1);
-      mbar_init(bar_empty + i * 8, kCluster);
-    }
-    for (int h = 0; h < 2; ++h) {
-      mbar_init(bar_aready + h * 8, kRowThreads / 32);
-      mbar_init(bar_accfull + h * 8, 1);
-      mbar_init(bar_sv + h * 16, kRowThreads / 32);
-      mbar_init(bar_sv + h * 16 + 8, kRowThreads / 32);
-      mbar_init(bar_saved + h * 8, 4);
+      mbar_init(bar_empty + i * 8, kRowThreads / 32);
     }
     mbar_fence_init();
   }
-  if (warp == 1) {
-    tmem_alloc(smem_base + kOffTmemPtr, 512);
-    tmem_relinquish();
-  }
   for (int i = threadIdx.x; i < kTileM * 128 / 16; i += kThreads)  // operand chunks 1..7 of every row stay zero
     reinterpret_cast<uint4*>(smem + kOffOp)[i] = make_uint4(0u, 0u, 0u, 0u);
-  tc_fence_before_sync();
   __syncthreads();
-  cluster_sync_all();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr_s;
-  const uint32_t cta_rank = cluster_ctarank();
-  constexpr uint16_t kAllCtas = (1u << kCluster) - 1;
 
-  const int first_in_cluster = (int)blockIdx.x - (int)cta_rank;
-  const int n_iter = (p.n_units - first_in_cluster + (int)gridDim.x - 1) / (int)gridDim.x;
+  const int n_iter = (p.n_units - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
   const int tpu = p.tiles_c + p.tiles_f;
   const int n_tiles_cta = n_iter * tpu;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ============================== weight producer ==============================
     reg_dec<kRegsLight>();
-    uint32_t slot = 0, phase = 0, seq = 0;
-    for (int j = 0; j < n_tiles_cta; ++j) {
-      const int t = j % tpu;
-      const uint8_t* base = p.wstream[t < p.tiles_c ? 0 : 1];
-      for (int i = 0; i < kTileUnits; ++i) {
-        const uint32_t w = c_prog.e[i].w;
-        const uint32_t off = (w & 0xFFFFFu) << 4, bytes = (w >> 20) * 128u;
-        mbar_wait(bar_empty + slot * 8, phase ^ 1);
-        if (elect_one()) {
-          mbar_arrive_expect_tx(bar_full + slot * 8, bytes);
-          if ((seq % kCluster) == cta_rank)
-            bulk_g2s_multicast(smem_base + kOffRing + slot * kMaxUnitBytes, base + off, bytes, bar_full + slot * 8, kAllCtas);
-        }
-        __syncwarp();
-        ++seq;
-        if (++slot == kNumSlots) { slot = 0; phase ^= 1; }
-      }
-    }
-  } else if (warp == 1) {
-    // ============================== MMA issuer ==============================
-    reg_dec<kRegsLight>();
-    uint32_t slot = 0, phase = 0, ph_a0 = 0, ph_a1 = 0;
-    uint32_t sv_pending = 0, sv_phase = 0;  // per region bit: a step's output lives there / parity of bar_saved
-    const uint64_t op_desc = umma_smem_desc_sw128(smem_base + kOffOp);
-    for (int j = 0; j < n_tiles_cta; ++j) {
-      for (int i = 0; i < kTileUnits; ++i) {
-        const ProgEntry e = c_prog.e[i];
-        if (e.z & kFirst) {  // first unit of a step
-          const uint32_t rho = (e.z & kOddRegion) ? 1u : 0u;
-          if (sv_pending & (1u << rho)) {
-            mbar_wait(bar_saved + rho * 8, (sv_phase >> rho) & 1u);
-            sv_phase ^= 1u << rho;
-            tc_fence_after_sync();
+    if (warp == 0) {
+      uint32_t slot = 0, phase = 0;
+      for (int j = 0; j < n_tiles_cta; ++j) {
+        const int t = j % tpu;
+        const uint8_t* base = p.wstream[t < p.tiles_c ? 0 : 1];
+        for (int i = 0; i < kTileUnits; ++i) {
+          const uint32_t w = c_prog.e[i].w;
+          const uint32_t off = (w & 0xFFFFFu) << 4, bytes = (w >> 20) * 128u;
+          mbar_wait(bar_empty + slot * 8, phase ^ 1);
+          if (elect_one()) {
+            mbar_arrive_expect_tx(bar_full + slot * 8, bytes);
+            bulk_g2s(smem_base + kOffRing + slot * kMaxUnitBytes, base + off, bytes, bar_full + slot * 8);
           }
-          sv_pending |= 1u << rho;
-        }
-        if (e.z & kWait0) {
-          mbar_wait(bar_aready, ph_a0);
-          ph_a0 ^= 1;
-          tc_fence_after_sync();
-        }
-        if (e.z & kWait1) {
-          mbar_wait(bar_aready + 8, ph_a1);
-          ph_a1 ^= 1;
-          tc_fence_after_sync();
-        }
-        const uint32_t d_tmem = tmem_base + (e.y & 0xFFFFu);
-        const uint32_t a_tmem = tmem_base + (e.y >> 16);
-        const uint32_t first = (e.z & kFirst) ? 0u : 1u;
-        mbar_wait(bar_full + slot * 8, phase);
-        tc_fence_after_sync();
-        const uint64_t b_desc = umma_smem_desc_sw128(smem_base + kOffRing + slot * kMaxUnitBytes);
-        if (elect_one()) {
-#pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint64_t bd = b_desc + (uint64_t)(ks * 2);
-            const uint32_t acc_flag = (first | ks) ? 1u : 0u;
-            if (e.z & kFromOp) umma_ss(d_tmem, op_desc + (uint64_t)(ks * 2), bd, e.x, acc_flag);
-            else umma_ts(d_tmem, a_tmem + ks * 8, bd, e.x, acc_flag);
-          }
-          umma_commit_multicast(bar_empty + slot * 8, kAllCtas);
-          if (e.z & kCommit0) umma_commit(bar_accfull);
-        }
-        __syncwarp();
-        if (++slot == kNumSlots) { slot = 0; phase ^= 1; }
-        if (e.z & kPostWait1) {
-          mbar_wait(bar_aready + 8, ph_a1);
-          ph_a1 ^= 1;
+          __syncwarp();
+          if (++slot == kNumSlots) { slot = 0; phase ^= 1; }
         }
       }
     }
-  } else if (warp >= 4 && warp < 12) {
-    // ============================== row warps ==============================
+  } else {
+    // ============================== row warpgroups ==============================
     reg_inc<kRegsRow>();
     const int q = warp & 3;
     const int row = q * 32 + lane;
-    const int ch = (warp - 4) >> 2;
-    const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-    uint32_t ph_acc = 0;
+    const int ch = (warp - 4) >> 2;  // == warpgroup
+    const int wg = ch;
+    const int r0 = 64 * wg + 16 * q + (lane >> 2);
     const float scale = p.scal[0];
+    uint8_t* act = smem + kOffAct;
+    uint32_t slot = 0, phase = 0;
 
-    // d raw of tile j -> FP16 operand row in shared memory (+ its transposed image for the weight-gradient kernel)
-    auto write_operand = [&](int j) {
+    for (int j = 0; j < n_tiles_cta; ++j) {
       const int unit = blockIdx.x + (j / tpu) * gridDim.x;
       const bool real = unit < p.n_units;
       const size_t gt = (size_t)unit * tpu + (j % tpu);
+      uint8_t* rec = real ? p.rec + gt * kRecBytes : nullptr;
+      // d raw of tile j -> FP16 operand row in shared memory (+ its transposed image for the weight-gradient kernel)
       if (ch == 0) {
         float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
         if (real) d = reinterpret_cast<const float4*>(p.draw)[gt * 128 + row];
         const uint32_t h01 = pack_f16x2(d.x * scale, d.y * scale), h23 = pack_f16x2(d.z * scale, d.w * scale);
         *reinterpret_cast<uint4*>(smem + kOffOp + row * 128 + ((0 ^ (row & 7)) << 4)) = make_uint4(h01, h23, 0u, 0u);
         if (real) {
-          uint8_t* img = p.rec + gt * kRecBytes + kRecDRaw + img_row_base(16, row);
+          uint8_t* img = rec + kRecDRaw + img_row_base(16, row);
           const uint32_t cr = (uint32_t)((row & 63) >> 3);
           *reinterpret_cast<uint16_t*>(img + 0 * 128 + ((cr ^ 0u) << 4)) = (uint16_t)(h01 & 0xFFFFu);
           *reinterpret_cast<uint16_t*>(img + 1 * 128 + ((cr ^ 1u) << 4)) = (uint16_t)(h01 >> 16);
@@ -458,132 +384,50 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
           *reinterpret_cast<uint16_t*>(img + 3 * 128 + ((cr ^ 3u) << 4)) = (uint16_t)(h23 >> 16);
         }
       } else if (real) {  // rows 4..15 of the image are zero
-        uint8_t* img = p.rec + gt * kRecBytes + kRecDRaw + img_row_base(16, row);
+        uint8_t* img = rec + kRecDRaw + img_row_base(16, row);
         const uint32_t cr = (uint32_t)((row & 63) >> 3);
 #pragma unroll
         for (int k = 4; k < 16; ++k) *reinterpret_cast<uint16_t*>(img + k * 128 + ((cr ^ (uint32_t)(k & 7)) << 4)) = 0;
       }
       fence_proxy_async_smem();
-    };
+      named_bar_sync(kRowBarrier, kRowThreads);  // operand of tile j in place
 
-    if (n_tiles_cta > 0) write_operand(0);
-    for (int j = 0; j < n_tiles_cta; ++j) {
-      const int unit = blockIdx.x + (j / tpu) * gridDim.x;
-      const bool real = unit < p.n_units;
-      uint8_t* rec = real ? p.rec + ((size_t)unit * tpu + (j % tpu)) * kRecBytes : nullptr;
-      const uint32_t* masks = reinterpret_cast<const uint32_t*>(rec + kRecMask);
-      __syncwarp();
-      if (lane == 0) {  // operand of tile j is in place: both gates of step 0
-        mbar_arrive(bar_aready);
-        mbar_arrive(bar_aready + 8);
-      }
+      const uint32_t* masks = rec ? reinterpret_cast<const uint32_t*>(rec + kRecMask) : nullptr;
+      int prog = 0;
       for (int s = 0; s < kBwdSteps; ++s) {
-        const int L = 8 - s;  // forward layer whose pre-activation gradient this step produces
-        const bool two = s >= 3;
-        const uint32_t t_acc = t_lane + region_col(s);
-        const int W = rec_width(L);
-        uint2 m0 = make_uint2(0u, 0u), m1 = make_uint2(0u, 0u);
-        if (real) {
-          m0 = *reinterpret_cast<const uint2*>(masks + (L * 128 + row) * 8 + 2 * ch);
-          if (two) m1 = *reinterpret_cast<const uint2*>(masks + (L * 128 + row) * 8 + 4 + 2 * ch);
-        }
-        mbar_wait(bar_accfull, ph_acc);
-        ph_acc ^= 1;
-        tc_fence_after_sync();
-        const uint32_t par = (uint32_t)(s & 1);
-        {  // half 0: output columns [64 ch, 64 ch + 64).  The FP16 result goes back to TMEM in place: A operand of the next step
-           // and (every step, also the last) what the saver warps write to the record.
-          const int c0 = 64 * ch;
-          uint32_t ha[16], hb[16];
-          bwd_epi_slice(t_acc + c0, m0, ha, hb);
-          tmem_st16(t_acc + c0, ha);
-          tmem_st16(t_acc + c0 + 16, hb);
-          tmem_wait_st();
-          tc_fence_before_sync();
-          __syncwarp();
-          if (lane == 0) {
-            if (s < kBwdSteps - 1) mbar_arrive(bar_aready);
-            mbar_arrive(bar_sv + par * 8);
-          }
-        }
-        if (two) {  // half 1: columns [128 + 64 ch, ...)
-          const int c0 = 128 + 64 * ch;
-          uint32_t ha[16], hb[16];
-          bwd_epi_slice(t_acc + c0, m1, ha, hb);
-          tmem_st16(t_acc + c0, ha);
-          tmem_st16(t_acc + c0 + 16, hb);
-          tmem_wait_st();
-          tc_fence_before_sync();
-          __syncwarp();
-          if (lane == 0) {
-            if (s < kBwdSteps - 1) mbar_arrive(bar_aready + 8);
-            mbar_arrive(bar_sv + 16 + par * 8);
-          }
-        } else if (s < kBwdSteps - 1) {
-          tc_fence_before_sync();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_aready + 8);
-        }
-        if (s == 3 && j + 1 < n_tiles_cta) write_operand(j + 1);  // steps 0 and 3 of tile j no longer read the operand
-      }
-    }
-    tc_fence_before_sync();
-  } else if (warp >= 12) {
-    // ============================== record savers ==============================
-    // bar_sv[half][s & 1] cannot run more than one phase ahead of this warp: the step that next completes the same barrier is
-    // s + 2 (or a step of the next tile in the same region), whose MMAs wait for bar_saved of step s.
-    reg_dec<kRegsSaver>();
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-    uint32_t sv_ph = 0;  // bit (half * 2 + parity): phase of bar_sv[half][parity]
-    for (int j = 0; j < n_tiles_cta; ++j) {
-      const int unit = blockIdx.x + (j / tpu) * gridDim.x;
-      uint8_t* rec = unit < p.n_units ? p.rec + ((size_t)unit * tpu + (j % tpu)) * kRecBytes : nullptr;
-#pragma unroll 1
-      for (int s = 0; s < kBwdSteps; ++s) {
-        const int L = 8 - s, W = rec_width(L);
-        const uint32_t par = (uint32_t)(s & 1);
-        const uint32_t t_reg = t_lane + region_col(s);
-        uint8_t* img = rec ? rec + rec_dy_off(L) + img_row_base(W, row) : nullptr;
-        const int n_slices = W >> 6;
-#pragma unroll 1
-        for (int i = 0; i < n_slices; ++i) {
-          if ((i & 1) == 0) {
-            const int h = i >> 1;
-            const uint32_t bit = 1u << (h * 2 + par);
-            mbar_wait(bar_sv + h * 16 + par * 8, (sv_ph & bit) ? 1u : 0u);
-            sv_ph ^= bit;
-            tc_fence_after_sync();
-          }
-          uint32_t v[32];
-          tmem_ld32(t_reg + 64 * i, v);
-          tmem_wait_ld();
-          if (i == n_slices - 1) {  // the whole region has been read
-            tc_fence_before_sync();
-            __syncwarp();
-            if (lane == 0) mbar_arrive(bar_saved + par * 8);
-          }
-          if (img) {
-            uint32_t h0[16], h1[16];
+        const StepInfo si = bwd_step_info(s);
+        const bool two = si.nh1 > 0;
+        float acc0[64], acc1[64];
+        for (int u = 0; u < si.k_atoms; ++u, ++prog) {
+          const ProgEntry e = c_prog.e[prog];
+          const uint32_t a = ((e.z & kFromOp) ? smem_base + kOffOp : smem_base + kOffAct + e.y * (kTileM * 128)) + 64 * wg * 128;
+          const uint64_t ad = wgmma_desc_sw128(a);
+          mbar_wait(bar_full + slot * 8, phase);
+          const uint32_t b = smem_base + kOffRing + slot * kMaxUnitBytes;
+          const uint64_t b0 = wgmma_desc_sw128(b), b1 = wgmma_desc_sw128(b + 128 * 128);
+          wgmma_fence();
 #pragma unroll
-            for (int k = 0; k < 16; ++k) { h0[k] = v[k]; h1[k] = v[16 + k]; }
-            store_t32(img, row, 64 * i, h0);
-            store_t32(img, row, 64 * i + 32, h1);
+          for (int ks = 0; ks < 4; ++ks) {
+            const uint32_t accf = (u | ks) ? 1u : 0u;
+            wgmma_n128(acc0, ad + (uint64_t)(ks * 2), b0 + (uint64_t)(ks * 2), accf);
+            if (two) wgmma_n128(acc1, ad + (uint64_t)(ks * 2), b1 + (uint64_t)(ks * 2), accf);
           }
+          wgmma_commit();
+          wgmma_wait<0>();
+          reg_fence(acc0);
+          reg_fence(acc1);
+          __syncwarp();
+          if (lane == 0) mbar_arrive(bar_empty + slot * 8);
+          if (++slot == kNumSlots) { slot = 0; phase ^= 1; }
         }
+        const int L = 8 - s;  // forward layer whose pre-activation gradient this step produces
+        bwd_epi_half(acc0, L, 0, masks, act, rec, r0);
+        if (two) bwd_epi_half(acc1, L, 128, masks, act, rec, r0);
+        fence_proxy_async_smem();
+        named_bar_sync(2 + wg, 128);
       }
+      named_bar_sync(kRowBarrier, kRowThreads);  // the operand buffer is free for the next tile
     }
-    tc_fence_before_sync();
-  } else {
-    reg_dec<kRegsLight>();  // warps 2, 3: idle, but setmaxnreg is a warpgroup-wide instruction
-  }
-
-  __syncthreads();
-  cluster_sync_all();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -594,14 +438,17 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
 // ================================================================================================
 namespace dw {
 
-constexpr int kThreads = 192;  // warp 0 producer, warp 1 MMA issuer, warps 2..5 epilogue (one per TMEM lane quadrant)
+// 384 threads: warp 0 producer (warps 1..3 idle), warpgroups 1 and 2 = output features [64w, 64w+64) of the job's 128 on wgmma,
+// FP32 accumulators in registers over all tiles of the CTA, then reduced into the accumulators in global memory.
+constexpr int kThreads = 384;
+constexpr int kRegsLight = 40, kRegsRow = 232;
+using chain::reg_dec;
+using chain::reg_inc;
 constexpr int kStages = 4;
 constexpr int kStageBytes = 16384 + 32768;       // one r-atom (64 sample rows): A [128 features x 128 B], B [<=256 features x 128 B]
 constexpr int kOffOnes = kStages * kStageBytes;  // [16 rows x 64 r]: row 0 = 1.0 (bias = column sums of dY)
 constexpr int kOffBars = kOffOnes + 2048;
-constexpr int kOffTmemPtr = kOffBars + (2 * kStages + 2) * 8;
-constexpr int kSmemBytes = kOffTmemPtr + 16;
-constexpr uint32_t kBiasCol = 256;
+constexpr int kSmemBytes = kOffBars + 2 * kStages * 8;
 
 struct Job {
   int a_off, a_rows, a_half;  // A image (M side): record offset, features in the image, which 128-feature half
@@ -610,10 +457,10 @@ struct Job {
   int out_off, out_ld, out_row0;
 };
 // Jobs are dealt to kGroups groups of CTAs; within a group every CTA runs the group's jobs over its own share of the tiles (fewer
-// accumulator drains and atomics than every CTA running every job).  The kernel is HBM-bound (each job streams its two images of
-// every tile once), so the groups are balanced by BYTES per tile (172..200 KB each), and groups 2q / 2q+1 are the two
-// 128-feature output halves of the SAME layers in the SAME order: they run on neighbouring CTAs over the same tiles at the same
-// time, so the B image both need (the layer's whole input, 2/3 of a job's bytes) comes from HBM once and from L2 the second time.
+// accumulator drains and atomics than every CTA running every job).  The kernel streams each job's two images of every tile
+// once, so the groups are balanced by BYTES per tile (172..200 KB each), and groups 2q / 2q+1 are the two 128-feature output
+// halves of the SAME layers in the SAME order: they run on neighbouring CTAs over the same tiles at the same time, so the B
+// image both need (the layer's whole input, 2/3 of a job's bytes) comes from HBM once and from L2 the second time.
 constexpr int kNumJobs = 21;
 constexpr int kGroups = 8;
 struct JobTable { Job j[kNumJobs]; int group_begin[kGroups + 1]; };
@@ -654,6 +501,64 @@ constexpr JobTable make_jobs() {
 static_assert(make_jobs().group_begin[kGroups] == kNumJobs, "job table");
 __constant__ JobTable c_jobs = make_jobs();
 
+template <int N> __device__ __forceinline__ void mma_n(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t accf) {
+  if constexpr (N == 16) wgmma_n16(d, a, b, accf);
+  else if constexpr (N == 32) wgmma_n32(d, a, b, accf);
+  else if constexpr (N == 64) wgmma_n64(d, a, b, accf);
+  else wgmma_n128(d, a, b, accf);
+}
+
+// One job over the CTA's tiles j0..j1 for this warpgroup's 64 output features: NB = N of the B image (<= 128 per accumulator;
+// 256 runs as two 128-column halves).
+template <int NB>
+__device__ __forceinline__ void run_job(const Job& J, int j0, int j1, uint32_t smem_base, uint32_t bar_full, uint32_t bar_empty,
+                                        uint32_t& stage, uint32_t& phase, int wg, int lane, float* acc_net, float inv) {
+  constexpr int NA = NB > 128 ? 128 : NB;
+  constexpr int NH = NB > 128 ? 2 : 1;
+  float acc[NH][NA / 2];
+  float accb[8];
+  const bool bias = J.bias_layer >= 0;
+  const uint64_t ones = wgmma_desc_sw128(smem_base + kOffOnes);
+  for (int j = j0; j < j1; ++j) {
+    for (int a = 0; a < 2; ++a) {
+      mbar_wait(bar_full + stage * 8, phase);
+      const uint32_t sa = smem_base + stage * kStageBytes, sb = sa + 16384;
+      const uint64_t ad = wgmma_desc_sw128(sa + 64 * wg * 128);
+      wgmma_fence();
+#pragma unroll
+      for (int ks = 0; ks < 4; ++ks) {
+        const uint32_t accf = ((j - j0) | a | ks) ? 1u : 0u;
+#pragma unroll
+        for (int h = 0; h < NH; ++h) mma_n<NA>(acc[h], ad + (uint64_t)(ks * 2), wgmma_desc_sw128(sb + h * 16384) + (uint64_t)(ks * 2), accf);
+        if (bias) wgmma_n16(accb, ad + (uint64_t)(ks * 2), ones + (uint64_t)(ks * 2), accf);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+#pragma unroll
+      for (int h = 0; h < NH; ++h) reg_fence(acc[h]);
+      reg_fence(accb);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(bar_empty + stage * 8);
+      if (++stage == kStages) { stage = 0; phase ^= 1; }
+    }
+  }
+  const int c = lane & 3, r0 = 64 * wg + 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2);
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int R = r0 + 8 * hh;
+    float* out = acc_net + J.out_off + (size_t)(J.out_row0 + R) * J.out_ld;
+#pragma unroll
+    for (int h = 0; h < NH; ++h)
+#pragma unroll
+      for (int jj = 0; jj < NA / 8; ++jj) {
+        const int col = h * 128 + 8 * jj + 2 * c;
+        atomicAdd(out + col, acc[h][4 * jj + 2 * hh] * inv);
+        atomicAdd(out + col + 1, acc[h][4 * jj + 2 * hh + 1] * inv);
+      }
+    if (bias && c == 0) atomicAdd(acc_net + acc_bias_off(J.bias_layer) + J.out_row0 + R, accb[2 * hh] * inv);
+  }
+}
+
 __global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__ DwParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t smem_base = smem_u32(smem);
@@ -675,134 +580,66 @@ __global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__
   const int job0 = c_jobs.group_begin[group], job1 = c_jobs.group_begin[group + 1];
 
   const uint32_t bar_full = smem_base + kOffBars;      // [kStages]
-  const uint32_t bar_empty = bar_full + kStages * 8;   // [kStages]
-  const uint32_t bar_accfull = bar_empty + kStages * 8;
-  const uint32_t bar_accempty = bar_accfull + 8;
-  volatile uint32_t* tmem_ptr_s = reinterpret_cast<volatile uint32_t*>(smem + kOffTmemPtr);
+  const uint32_t bar_empty = bar_full + kStages * 8;   // [kStages]: one arrival per consumer warp
 
   if (threadIdx.x == 0) {
     for (int i = 0; i < kStages; ++i) {
       mbar_init(bar_full + i * 8, 1);
-      mbar_init(bar_empty + i * 8, 1);
+      mbar_init(bar_empty + i * 8, 8);
     }
-    mbar_init(bar_accfull, 1);
-    mbar_init(bar_accempty, 4);
     mbar_fence_init();
-  }
-  if (warp == 1) {
-    tmem_alloc(smem_base + kOffTmemPtr, 512);
-    tmem_relinquish();
   }
   for (int i = threadIdx.x; i < 2048 / 4; i += kThreads)  // row 0 (first 128 bytes) = FP16 ones, rows 1..15 = 0
     reinterpret_cast<uint32_t*>(smem + kOffOnes)[i] = (i < 32) ? 0x3C003C00u : 0u;
   fence_proxy_async_smem();
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_ptr_s;
 
   auto tile_rec = [&](int j) -> const uint8_t* {
     const int u = j / t_cnt, t = j - u * t_cnt;
     return p.rec + ((size_t)u * p.tpu + t_base + t) * kRecBytes;
   };
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ============================== producer ==============================
+    reg_dec<kRegsLight>();
+    if (warp == 0) {
+      uint32_t stage = 0, phase = 0;
+      for (int job = job0; job < job1; ++job) {
+        const Job J = c_jobs.j[job];
+        const uint32_t b_bytes = (uint32_t)J.b_rows * 128u;
+        for (int j = j0; j < j1; ++j) {
+          const uint8_t* rec = tile_rec(j);
+          for (int a = 0; a < 2; ++a) {
+            mbar_wait(bar_empty + stage * 8, phase ^ 1);
+            if (elect_one()) {
+              const uint32_t sa = smem_base + stage * kStageBytes, sb = sa + 16384;
+              mbar_arrive_expect_tx(bar_full + stage * 8, 16384 + b_bytes);
+              bulk_g2s(sa, rec + J.a_off + a * J.a_rows * 128 + J.a_half * 16384, 16384, bar_full + stage * 8);
+              bulk_g2s(sb, rec + J.b_off + a * J.b_rows * 128, b_bytes, bar_full + stage * 8);
+            }
+            __syncwarp();
+            if (++stage == kStages) { stage = 0; phase ^= 1; }
+          }
+        }
+      }
+    }
+  } else {
+    // ============================== MMA + epilogue warpgroups ==============================
+    reg_inc<kRegsRow>();
+    const int wg = (warp - 4) >> 2;
+    const float inv = p.scal[1];
+    float* acc_net = p.acc[net];
     uint32_t stage = 0, phase = 0;
     for (int job = job0; job < job1; ++job) {
       const Job J = c_jobs.j[job];
-      const uint32_t b_bytes = (uint32_t)J.b_rows * 128u;
-      for (int j = j0; j < j1; ++j) {
-        const uint8_t* rec = tile_rec(j);
-        for (int a = 0; a < 2; ++a) {
-          mbar_wait(bar_empty + stage * 8, phase ^ 1);
-          if (elect_one()) {
-            const uint32_t sa = smem_base + stage * kStageBytes, sb = sa + 16384;
-            mbar_arrive_expect_tx(bar_full + stage * 8, 16384 + b_bytes);
-            bulk_g2s(sa, rec + J.a_off + a * J.a_rows * 128 + J.a_half * 16384, 16384, bar_full + stage * 8);
-            bulk_g2s(sb, rec + J.b_off + a * J.b_rows * 128, b_bytes, bar_full + stage * 8);
-          }
-          __syncwarp();
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
+      switch (J.b_rows) {
+        case 16: run_job<16>(J, j0, j1, smem_base, bar_full, bar_empty, stage, phase, wg, lane, acc_net, inv); break;
+        case 32: run_job<32>(J, j0, j1, smem_base, bar_full, bar_empty, stage, phase, wg, lane, acc_net, inv); break;
+        case 64: run_job<64>(J, j0, j1, smem_base, bar_full, bar_empty, stage, phase, wg, lane, acc_net, inv); break;
+        case 128: run_job<128>(J, j0, j1, smem_base, bar_full, bar_empty, stage, phase, wg, lane, acc_net, inv); break;
+        default: run_job<256>(J, j0, j1, smem_base, bar_full, bar_empty, stage, phase, wg, lane, acc_net, inv); break;
       }
     }
-  } else if (warp == 1) {
-    // ============================== MMA issuer ==============================
-    uint32_t stage = 0, phase = 0, acc_phase = 0;
-    const uint64_t ones_desc = umma_smem_desc_sw128(smem_base + kOffOnes);
-    const uint32_t idesc_bias = umma_idesc_f16(128, 16);
-    for (int job = job0; job < job1; ++job) {
-      const Job J = c_jobs.j[job];
-      const uint32_t idesc = umma_idesc_f16(128, J.b_rows);
-      mbar_wait(bar_accempty, acc_phase ^ 1);  // the epilogue has drained the previous job's accumulator
-      tc_fence_after_sync();
-      for (int j = j0; j < j1; ++j) {
-        for (int a = 0; a < 2; ++a) {
-          mbar_wait(bar_full + stage * 8, phase);
-          tc_fence_after_sync();
-          const uint32_t sa = smem_base + stage * kStageBytes, sb = sa + 16384;
-          if (elect_one()) {
-            const uint64_t ad = umma_smem_desc_sw128(sa), bd = umma_smem_desc_sw128(sb);
-#pragma unroll
-            for (int ks = 0; ks < 4; ++ks) {
-              const uint32_t accf = ((j - j0) | a | ks) ? 1u : 0u;
-              umma_ss(tmem_base, ad + (uint64_t)(ks * 2), bd + (uint64_t)(ks * 2), idesc, accf);
-              if (J.bias_layer >= 0) umma_ss(tmem_base + kBiasCol, ad + (uint64_t)(ks * 2), ones_desc + (uint64_t)(ks * 2), idesc_bias, accf);
-            }
-            umma_commit(bar_empty + stage * 8);
-            if (j == j1 - 1 && a == 1) umma_commit(bar_accfull);
-          }
-          __syncwarp();
-          if (++stage == kStages) { stage = 0; phase ^= 1; }
-        }
-      }
-      acc_phase ^= 1;
-    }
-  } else {
-    // ============================== epilogue ==============================
-    const int q = warp & 3;
-    const int row = q * 32 + lane;
-    const uint32_t t_lane = tmem_base + ((uint32_t)(q * 32) << 16);
-    const float inv = p.scal[1];
-    uint32_t acc_phase = 0;
-    for (int job = job0; job < job1; ++job) {
-      const Job J = c_jobs.j[job];
-      mbar_wait(bar_accfull, acc_phase);
-      acc_phase ^= 1;
-      tc_fence_after_sync();
-      float* out = p.acc[net] + J.out_off + (size_t)(J.out_row0 + row) * J.out_ld;
-      if (J.b_rows == 16) {
-        uint32_t v[16];
-        tmem_ld16(t_lane, v);
-        tmem_wait_ld();
-#pragma unroll
-        for (int c = 0; c < 16; ++c) atomicAdd(out + c, __uint_as_float(v[c]) * inv);
-      } else {
-        for (int c0 = 0; c0 < J.b_rows; c0 += 32) {
-          uint32_t v[32];
-          tmem_ld32(t_lane + c0, v);
-          tmem_wait_ld();
-#pragma unroll
-          for (int c = 0; c < 32; ++c) atomicAdd(out + c0 + c, __uint_as_float(v[c]) * inv);
-        }
-      }
-      if (J.bias_layer >= 0) {
-        uint32_t v[4];
-        tmem_ld4(t_lane + kBiasCol, v);
-        tmem_wait_ld();
-        atomicAdd(p.acc[net] + acc_bias_off(J.bias_layer) + J.out_row0 + row, __uint_as_float(v[0]) * inv);
-      }
-      tc_fence_before_sync();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_accempty);
-    }
-  }
-
-  __syncthreads();
-  if (warp == 1) {
-    tc_fence_after_sync();
-    tmem_dealloc(tmem_base, 512);
   }
 }
 
@@ -997,25 +834,11 @@ cudaError_t launch_composite_bwd(const CompBwdParams& q, float* scal, cudaStream
 }
 
 cudaError_t launch_chain(const ChainParams& p, int num_sms, cudaStream_t st, long long* launches) {
-  int grid = p.n_units < num_sms ? p.n_units : num_sms;
+  const int grid = p.n_units < num_sms ? p.n_units : num_sms;
   if (grid <= 0) return cudaSuccess;
-  grid = (grid + chain::kCluster - 1) / chain::kCluster * chain::kCluster;
-  if (grid > num_sms) grid = num_sms / chain::kCluster * chain::kCluster;
-  cudaLaunchConfig_t cfg = {};
-  cfg.gridDim = dim3(grid);
-  cfg.blockDim = dim3(chain::kThreads);
-  cfg.dynamicSmemBytes = chain::kSmemBytes;
-  cfg.stream = st;
-  cudaLaunchAttribute attr[1];
-  attr[0].id = cudaLaunchAttributeClusterDimension;
-  attr[0].val.clusterDim.x = chain::kCluster;
-  attr[0].val.clusterDim.y = 1;
-  attr[0].val.clusterDim.z = 1;
-  cfg.attrs = attr;
-  cfg.numAttrs = 1;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, chain::chain_kernel, p);
+  chain::chain_kernel<<<grid, chain::kThreads, chain::kSmemBytes, st>>>(p);
   ++*launches;
-  return e != cudaSuccess ? e : cudaGetLastError();
+  return cudaGetLastError();
 }
 
 // CTAs per job group for the two networks: `num_sms / kGroups` parts split in proportion to the networks' tile counts

@@ -1,9 +1,9 @@
 """Gradients for training (train_transformed_rays.py:389 `loss.backward()`).
 
-Forward: the fused sm_100a render kernel in its training variant (nfb_render_forward_train) — the same launch as
+Forward: the fused sm_90a render kernel in its training variant (nfb_render_forward_train) — the same launch as
 evaluation, which also leaves the FP16 activations of every layer, the sample depths and the per-sample colours in
 buffers owned by the renderer.  Backward: nfb_render_backward (csrc/nfb_train.cu) — compositing backward, the dX chain
-and the weight-gradient GEMMs on tcgen05, then the chain rule through the kernel's weight folding.  No torch.autograd
+and the weight-gradient GEMMs on wgmma, then the chain rule through the kernel's weight folding.  No torch.autograd
 graph and no library GEMM is involved; the resampled depths carry no gradient, as in the reference
 (`z_samples.detach()`, train_utils.py:124), and `layers_dir.3.*` receives None (unused by the forward, models.py:257)."""
 import torch

@@ -47,7 +47,7 @@ class Renderer:
 
     def __init__(self, device: torch.device):
         if device.type != "cuda":
-            raise RuntimeError("the nfb render path runs on CUDA (sm_100a) only; there is no CPU fallback")
+            raise RuntimeError("the nfb render path runs on CUDA (sm_90a) only; there is no CPU fallback")
         self.device = device
         idx = device.index if device.index is not None else torch.cuda.current_device()
         dims = capi.NfbModelDims(10, 4, 1, 0, 76, 32)
@@ -116,13 +116,8 @@ class Renderer:
         self._frame = (e, l)
 
     def kernel_info(self, precision="fast"):
-        """Which render kernel an evaluation call in this precision runs, and the ncu capture that describes it (bench.py)."""
-        k = os.environ.get("NFB_KERNEL", "")
-        if precision != "fast" or k == "v4":
-            return dict(name="nfb::render_kernel", block_size=320, ncu_json="r2_render_kernel_exact_ncu.json")
-        if k == "v6":
-            return dict(name="nfb::v6::render2_kernel", block_size=384, ncu_json="r2_render2_kernel_ncu.json")
-        return dict(name="nfb::v7::render3_kernel", block_size=512, ncu_json="r2_render3_kernel_ncu.json")
+        """Which render kernel an evaluation call runs (bench.py): one kernel, both precision modes."""
+        return dict(name="nfb::render_kernel", block_size=384)
 
     def launch_count(self) -> int:
         n = C.c_longlong()
@@ -333,7 +328,7 @@ _renderers = {}
 
 def renderer_for(device: torch.device) -> Renderer:
     if device.type != "cuda":
-        raise RuntimeError("the nfb render path runs on CUDA (sm_100a) only; there is no CPU fallback")
+        raise RuntimeError("the nfb render path runs on CUDA (sm_90a) only; there is no CPU fallback")
     key = (device.type, device.index if device.index is not None else torch.cuda.current_device())
     r = _renderers.get(key)
     if r is None:

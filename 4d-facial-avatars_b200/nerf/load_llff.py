@@ -3,4 +3,4 @@ reference's scripts import it (train_transformed_rays.py:17-21)."""
 
 
 def load_llff_data(*args, **kwargs):
-    raise NotImplementedError("LLFF datasets are out of scope of the B200 NeRFace render path")
+    raise NotImplementedError("LLFF datasets are out of scope of the H100 NeRFace render path")

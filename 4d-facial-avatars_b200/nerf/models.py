@@ -5,7 +5,7 @@ import torch
 
 
 class ConditionalBlendshapePaperNeRFModel(torch.nn.Module):
-    """Holds the FP32 master weights.  `run_one_iter_of_nerf` never calls forward(): the fused sm_100a kernel
+    """Holds the FP32 master weights.  `run_one_iter_of_nerf` never calls forward(): the fused sm_90a kernel
     reads a packed FP16 copy of these parameters (re-packed automatically when they change).  forward() is
     kept for callers that evaluate the MLP on pre-encoded rows; it is plain torch and not the hot path."""
 

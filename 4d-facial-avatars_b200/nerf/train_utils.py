@@ -1,4 +1,4 @@
-"""Render driver with the reference's call surface (nerf/train_utils.py:36-290), backed by the fused sm_100a
+"""Render driver with the reference's call surface (nerf/train_utils.py:36-290), backed by the fused sm_90a
 kernel.  What stays on the host: argument plumbing, the reference's chunk-ordered noise draws, output reshaping."""
 import torch
 

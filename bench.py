@@ -3,6 +3,7 @@
 
     python bench.py --gpus N --steps K --warmup W            (N>1: launched under torch.distributed.run)
     python bench.py --impl reference ...                       (the reference's own implementation on the host cores)
+    python bench.py ... --dump-outputs DIR                     (also write the last timed step's outputs as DIR/<name>.npy)
 
 Headline (`value`, `e2e`, `roofline`): one step = one full 512x512 frame per GPU (BASELINE config 2; with N GPUs config 5:
 N concurrent frames with different expression codes, all-gathered into one [N,512,512,3] video tensor) => weak scaling,
@@ -13,9 +14,10 @@ value = N*H*W*K / time.  Synthetic per-frame pose / expression / latent / backgr
 `e2e`    : the same frame through the C-ABI host entry nfb_render_frame_host: pinned host expression / latent /
            background in, 11 floats per ray out, copies inside the timed region (N>1: the same all-gather as `value`).
 `roofline`: dominant kernel = the render kernel; achieved = algorithmic FLOP per launch (1,100,032 FLOP per MLP evaluation x
-           (2*Nc+Nf) evaluations per ray x rays) / its CUDA-event time; peak from MEASURED_PEAKS.json.
-`cpu_baseline`: the reference's own run_one_iter_of_nerf (staged copy, oracle/stage_reference.py; kind "reference") — or
-           the oracle port when no reference tree is reachable — on the host cores for a 64x64 crop.
+           (2*Nc+Nf) evaluations per ray x rays) / its CUDA-event time; peak from MEASURED_PEAKS.json, else the H100 SXM
+           data sheet's dense FP16 figure.
+`cpu_baseline`: the reference's own run_one_iter_of_nerf (staged in oracle/_ref by build(); kind "reference") — or the
+           oracle port when nothing is staged — on the host cores for a 64x64 crop.
 `gpu_baseline`: the same unmodified reference on this GPU through torch CUDA (TF32 off): what a user of the reference gets.
 
 Sub-records in the same JSON line (SURVEY.md §8e, the split `north_star` names):
@@ -61,6 +63,9 @@ def parse():
     ap.add_argument("--extras", default="all", help="comma list out of rows,rows_1024,train,single (exact / stress / gpu_baseline); default all")
     ap.add_argument("--train-impl", default=os.environ.get("NFB_TRAIN_IMPL", "fused"), choices=["fused", "dropin"])
     ap.add_argument("--no-train-graph", action="store_true", help="fused training step launch by launch instead of one CUDA graph replay")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the 7 outputs of the last timed step (rank 0, float32) as DIR/<name>.npy, and with N>1 the "
+                         "all-gathered video_rgb_fine.npy")
     return ap.parse_args()
 
 
@@ -69,11 +74,11 @@ def peaks():
     if os.path.exists(path):
         with open(path) as f:
             return json.load(f), "measured"
-    return {"bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0, "hbm_gbs": 6650.0}, "fallback"
+    return {"bf16_tflops": 989.0, "hbm_gbs": 3350.0}, "H100 SXM data sheet (dense FP16, 700 W)"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index):
         super().__init__(daemon=True)
@@ -111,7 +116,7 @@ class ClockSampler(threading.Thread):
 # the reference on the host cores (cpu_baseline / --impl reference) and on the GPU through torch (gpu_baseline)
 def reference_frame_crop(frame_index, H, W, crop, nc, nf, threads, device="cpu"):
     """(run, rays, kind): the reference algorithm on a crop x crop centre block of the synthetic frame.  kind "reference" =
-    the unmodified reference package (staged copy / /root/reference); "port" = oracle/nerface_oracle.py."""
+    the unmodified reference package staged in oracle/_ref by build(); "port" = oracle/nerface_oracle.py when nothing is staged."""
     import nerface_oracle as O
     import ref_loader
     if device == "cpu":
@@ -121,7 +126,7 @@ def reference_frame_crop(frame_index, H, W, crop, nc, nf, threads, device="cpu")
     r0, c0 = (H - crop) // 2, (W - crop) // 2
     ref = None
     try:
-        ref = ref_loader.load_reference()
+        ref = ref_loader.load_reference(staged_only=True)
     except Exception as e:  # a broken staged copy must not take the bench line down
         sys.stderr.write(f"reference import failed ({e!r}); using the oracle port\n")
     if ref is not None:
@@ -157,7 +162,7 @@ def pick_threads(H, W, nc, nf):
     return best[0]
 
 
-CPU_SAMPLE = {"reference": "the UNMODIFIED reference run_one_iter_of_nerf (nerf/train_utils.py:165-290, staged copy baseline/_ref, torch CPU FP32)",
+CPU_SAMPLE = {"reference": "the UNMODIFIED reference run_one_iter_of_nerf (nerf/train_utils.py:165-290, staged copy oracle/_ref, torch CPU FP32)",
               "port": "oracle/nerface_oracle.py (bit-exact port of the reference, torch CPU FP32)"}
 
 
@@ -194,9 +199,9 @@ def gpu_baseline(H, W, nc, nf, dev):
     import nerface_oracle as O
     import ref_loader
     try:
-        ref = ref_loader.load_reference()
+        ref = ref_loader.load_reference(staged_only=True)
         if ref is None:
-            return {"unavailable": "no reference tree (baseline/_ref not staged)"}
+            return {"unavailable": "no reference staged in oracle/_ref"}
         torch.backends.cuda.matmul.allow_tf32 = False
         torch.backends.cudnn.allow_tf32 = False
         fr = O.synthetic_frame(0, H, W)
@@ -295,9 +300,8 @@ def bench_rows(c, H, W, nc, nf, steps, warmup, precision):
         coll = sum(e[1].elapsed_time(e[2]) for e in evs) / k if with_mid else 0.0
         return tot, coll
 
-    n1 = max(2, min(steps, 3 if n > 512 * 512 else 5))
     step_full()
-    t1, _ = run(step_full, n1)  # the whole frame on ONE GPU (every rank does it; rank 0's time is reported)
+    t1, _ = run(step_full, steps)  # the whole frame on ONE GPU (every rank does it; rank 0's time is reported)
     for _ in range(max(1, warmup)):
         step_sharded()
     tn, coll = run(step_sharded, steps, with_mid=True)
@@ -413,15 +417,15 @@ def bench_train(c, steps, warmup, impl, rays=2048, nc=64, nf=64, graph=True):
     k = 0
     for j in range(max(3, warmup)):  # single-GPU warm-up (packs, allocations)
         step(k, False); k += 1  # noqa: E702
-    t1, _, loss1 = run(max(5, min(steps, 20)), k, False)
-    k += max(5, min(steps, 20))
+    t1, _, loss1 = run(steps, k, False)
+    k += steps
     rec = {"workload": f"{rays} rays/iter of one 512x512 frame, {nc}c+{nf}f, perturb + noise 0.1, mse x2 + latent reg, Adam",
            "impl": impl + (" + CUDA graph (one replay per iteration, all-reduce inside)" if (impl == "fused" and graph) else ""),
            "scaling": "strong", "t1_ms": t1, "rays_per_s_1gpu": rays / (t1 * 1e-3)}
     if world > 1:
         for j in range(max(3, warmup)):
             step(k, True); k += 1  # noqa: E702
-        tn, coll, lossn = run(max(5, min(steps, 20)), k, True)
+        tn, coll, lossn = run(steps, k, True)
         tn_max = max_over_ranks(c, tn)
         rec.update({"ms_per_step": tn_max, "rays_per_s": rays / (tn_max * 1e-3), "efficiency_vs_1gpu": t1 / (world * tn_max),
                     "collective_ms": None if (impl == "fused" and graph) else coll, "rays_per_rank": rays // world, "loss_last": lossn})
@@ -496,7 +500,7 @@ def main():
     eng.sync_weights(mc, mf)
     c = Ctx()
     c.O, c.eng, c.dev, c.world, c.rank, c.dist, c.peak = O, eng, dev, world, rank, dist, pk["bf16_tflops"]
-    c.flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)  # > 126 MB L2
+    c.flush = torch.empty(256 * 1024 * 1024 // 4, device=dev)  # > 50 MB L2
 
     # synthetic frames: frame f on rank r uses generator seed 42 + (f*world + r)
     n_frames = a.steps + a.warmup
@@ -510,6 +514,8 @@ def main():
     video = torch.empty((world, n, 3), device=dev) if world > 1 else None
     rgb_stage = torch.empty((n, 3), device=dev) if world > 1 else None
 
+    last_out = {}
+
     def step_resident(i, ev=None):
         fr, d = frames[i % len(frames)], dev_frames[i % len(frames)]
         eng.set_frame(d["expr"], d["latent"])
@@ -521,6 +527,7 @@ def main():
             ev[1].record()
         if world > 1:
             dist.all_gather_into_tensor(video.view(-1), v["rgb_fine"].reshape(-1))
+        last_out["v"] = v
         return v
 
     def step_host(i):
@@ -562,6 +569,13 @@ def main():
     ms_total, kernel_ms, wall = timed(step_resident, a.steps, kernel_events=True)
     launches = eng.launch_count() - l0
     clocks = sampler.stop() if sampler else None
+    if a.dump_outputs and rank == 0:  # what the last timed step returned, before anything else reuses out_buf
+        import numpy as np
+        os.makedirs(a.dump_outputs, exist_ok=True)
+        for k in NAMES:
+            np.save(os.path.join(a.dump_outputs, k + ".npy"), last_out["v"][k].float().cpu().numpy())
+        if world > 1:  # the all-gathered [N, H*W, 3] rgb_fine video tensor every rank receives
+            np.save(os.path.join(a.dump_outputs, "video_rgb_fine.npy"), video.float().cpu().numpy())
     ms_e2e, _, _ = timed(lambda i: step_host(i), a.steps)
 
     # ---- in-run parity (rank 0): two image rows of the last rendered frame against the oracle
@@ -591,7 +605,7 @@ def main():
         if want("rows"):
             extras["rows"] = bench_rows(c, 512, 512, 64, 128, a.steps, a.warmup, a.precision)
         if want("rows_1024"):
-            extras["rows_1024"] = bench_rows(c, 1024, 1024, 128, 256, max(3, min(a.steps, 5)), 1, a.precision)
+            extras["rows_1024"] = bench_rows(c, 1024, 1024, 128, 256, a.steps, 1, a.precision)
         if want("train"):
             try:
                 extras["train"] = bench_train(c, a.steps, a.warmup, a.train_impl, graph=not a.no_train_graph)
@@ -641,16 +655,7 @@ def main():
         k_ms = kernel_ms / a.steps
         achieved = flop_per_launch / (k_ms * 1e-3) / 1e12
         peak = pk["bf16_tflops"]
-        # dram bytes per launch of the dominant kernel, from the committed `ncu --set full` capture of THIS kernel build
-        kinfo = eng.kernel_info(a.precision) if hasattr(eng, "kernel_info") else {}
-        kernel_name = kinfo.get("name", "nfb::v6::render2_kernel" if a.precision == "fast" else "nfb::render_kernel")
-        traffic, traffic_src = None, None
-        tpath = os.path.join(ROOT, "profiles", kinfo.get("ncu_json", "r1b_render_kernel_ncu.json"))
-        if os.path.exists(tpath) and (H, W, nc, nf) == (512, 512, 64, 128):
-            with open(tpath) as f:
-                tj = json.load(f)
-            if tj.get("block_size") in (None, kinfo.get("block_size")):
-                traffic, traffic_src = tj.get("dram_bytes_per_launch"), os.path.basename(tpath)
+        kernel_name = eng.kernel_info(a.precision)["name"]
 
         cpu = None
         if not a.no_cpu_baseline:
@@ -668,7 +673,7 @@ def main():
             "metric": "rays/sec at 512x512 (64c+128f samples)", "value": value, "unit": "rays/s", "n_gpus": world,
             "steps": a.steps, "warmup": a.warmup, "ms_per_step": ms_total / a.steps, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None,
-            "dtype": "f16 operands / f32 accumulate (tcgen05)" if a.precision == "fast" else "f16 hi+lo split x3 / f32 accumulate (tcgen05)",
+            "dtype": "f16 operands / f32 accumulate (wgmma)" if a.precision == "fast" else "f16 hi+lo split x3 / f32 accumulate (wgmma)",
             "data": "synthetic",
             "config": {"workload": f"person_1-shaped eval: {H}x{W}, {nc} coarse + {nf} fine samples/ray, 76-dim expr + 32-dim latent, "
                                    f"one frame per GPU per step", "precision": a.precision, "parallelism": f"frame-per-gpu x{world}",
@@ -679,9 +684,8 @@ def main():
                     "d2h_bytes_per_step": 11 * n * 4, "ms_per_step": ms_e2e / a.steps},
             "gpu_launches": launches,
             "roofline": {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-                         "frac_of_sustained": achieved / pk.get("bf16_tflops_sustained", peak), "peak_source": pk_src,
-                         "kernel": kernel_name, "kernel_ms": k_ms, "flop_per_launch": flop_per_launch, "traffic": traffic,
-                         "traffic_unit": "bytes of DRAM read+write per launch (ncu --set full" + (f", profiles/{traffic_src})" if traffic_src else "; no capture of this build)")},
+                         "peak_source": pk_src,
+                         "kernel": kernel_name, "kernel_ms": k_ms, "flop_per_launch": flop_per_launch},
             "cpu_baseline": cpu, "clocks": clocks,
         }
         line.update(extras)

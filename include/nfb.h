@@ -1,4 +1,4 @@
-/* nfb.h — C ABI of the B200-native NeRFace render path ("nfb" = NeRFace on Blackwell).
+/* nfb.h — C ABI of the H100-native NeRFace render path ("nfb" = NeRFace fused render path).
  *
  * This is the drop-in boundary for ONE hot path of gafniguy/4D-Facial-Avatars: the per-ray render
  * loop reached through nerface_code/nerf-pytorch/nerf/train_utils.py (run_one_iter_of_nerf :165-290,
@@ -35,16 +35,16 @@ enum {
   NFB_ERR_UNSUPPORTED = 2, /* configuration outside what the kernel implements */
   NFB_ERR_CUDA = 3,        /* a CUDA runtime call failed; see nfb_last_cuda_error() */
   NFB_ERR_STATE = 4,       /* call order violated (weights or frame not set) */
-  NFB_ERR_ARCH = 5         /* device is not sm_100 */
+  NFB_ERR_ARCH = 5         /* device is not sm_90 */
 };
 
 /* Which of the two networks (models.coarse / models.fine in the reference YAML). */
 enum { NFB_NET_COARSE = 0, NFB_NET_FINE = 1 };
 
 /* Arithmetic used by the tensor-core MLP.
- *   NFB_PREC_FAST  : FP16 operands (round-to-nearest), FP32 accumulate, one tcgen05 pass.
+ *   NFB_PREC_FAST  : FP16 operands (round-to-nearest), FP32 accumulate, one wgmma pass.
  *   NFB_PREC_EXACT : every operand split x = hi + lo in FP16; hi*hi + hi*lo + lo*hi, FP32
- *                    accumulate (3 tcgen05 passes, ~2^-21 relative operand error). */
+ *                    accumulate (3 wgmma passes, ~2^-21 relative operand error). */
 enum { NFB_PREC_FAST = 0, NFB_PREC_EXACT = 1 };
 
 /* Encoder / conditioning dimensions; mirrors the constructor arguments of
@@ -152,7 +152,7 @@ int nfb_load_weights(NfbHandle* h, int which, const float* const params[26], voi
 int nfb_set_frame(NfbHandle* h, const float* expression, const float* latent, void* stream);
 
 /* The hot path: coarse sampling -> encode -> coarse MLP -> composite -> inverse-CDF resample -> sort
- * -> encode -> fine MLP -> composite, one persistent sm_100a kernel launch. */
+ * -> encode -> fine MLP -> composite, one persistent sm_90a kernel launch. */
 int nfb_render_forward(NfbHandle* h, const NfbRays* rays, const NfbSampling* sampling,
                        const NfbNoise* noise /* nullable */, const NfbOutputs* out,
                        const NfbDebug* dbg /* nullable */, void* stream);
@@ -180,7 +180,7 @@ typedef struct {
   const float* w_last;
 } NfbOutGrads;
 
-/* Backward of the last nfb_render_forward_train: compositing backward -> tcgen05 dX chain -> tcgen05 weight-gradient GEMMs
+/* Backward of the last nfb_render_forward_train: compositing backward -> wgmma dX chain -> wgmma weight-gradient GEMMs
  * -> gradients in the reference's parameter layout.  `params_*` are the 26 FP32 parameter pointers given to
  * nfb_load_weights; `grads_*` receive dL/dparam with the same shapes (entries 22, 23 = layers_dir.3.*, unused by the
  * forward, models.py:257: may be NULL and are never written).  `grad_latent` [32] receives dL/d latent_code (NULL: skipped);
@@ -310,12 +310,10 @@ int nfb_render_frame_host(NfbHandle* h, const float pose[12], const double intri
                           const float* background_host /* [rows*width,3] or NULL */,
                           const NfbSampling* sampling, float* out_host, void* stream);
 
-/* Test hook, host only (no CUDA call): the compile-time schedules the kernels execute.  which: 0 = one-tile render program,
- * 1 = two-tile render program (word 4 = half-step group), 2 = backward chain program (each: idesc, TMEM columns, flags,
- * (stream offset / 16) | rows << 20), 3 = weight-gradient jobs (a_off, a_rows, a_half, b_off, b_rows, bias_layer, out_off,
+/* Test hook, host only (no CUDA call): the compile-time schedules the kernels execute.  which: 0 = render program,
+ * 2 = backward chain program (each: MMA N, K atom of the A operand, flags, (stream offset / 16) | rows << 20), 3 = weight-gradient jobs (a_off, a_rows, a_half, b_off, b_rows, bias_layer, out_off,
  * out_ld, out_row0, group), 4 = the CTA split of the weight-gradient launch (in/out: out[0..2] = SMs, tiles of network 0, tiles of
- * network 1 -> parts of network 0, parts of network 1, job groups per part), 1000 + 100 n_iter + 10 Tc + Tf = the pipelined render kernel's job sequence for a CTA with n_iter units of work and
- * Tc / Tf tile pairs per pass (unit iteration, pass, tile, then the kernel's shared-memory bytes and row limits).  index < 0: returns the number of entries; otherwise fills out[0..] (out_words >= 10) and returns
+ * network 1 -> parts of network 0, parts of network 1, job groups per part).  index < 0: returns the number of entries; otherwise fills out[0..] (out_words >= 10) and returns
  * the number of words written, or -1. */
 int nfb_debug_schedule(int which, int index, uint32_t* out, int out_words);
 

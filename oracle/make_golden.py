@@ -1,6 +1,6 @@
 """Generate tests/golden/*.npz by executing the UNMODIFIED reference (read-only, /root/reference).
 
-Runs only in the build container (the GPU box has no /root/reference).  For every case it
+Runs only where a reference checkout is readable.  For every case it
   1. imports the reference ``nerf`` package with empty stand-ins for the absent, hot-path-unused
      modules (pytorch3d, torchsearchsorted, imageio) — SURVEY.md §8(c);
   2. runs ``run_one_iter_of_nerf`` on seeded synthetic inputs, recording every torch.rand/randn draw

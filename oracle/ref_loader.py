@@ -1,7 +1,7 @@
 """Import the UNMODIFIED reference `nerf` package (test / baseline infrastructure only — never from the product).
 
-Looks for the reference tree at /root/reference (build container) and then at baseline/_ref (the byte-for-byte copy
-staged by oracle/stage_reference.py, which is what exists on the GPU box).  The package is loaded under the alias
+Looks for the reference tree at /root/reference (a reference checkout) and then at oracle/_ref (the byte-for-byte copy
+staged by oracle/stage_reference.py); `staged_only=True` looks at the staged copy alone.  The package is loaded under the alias
 `nerf_reference`, so it never collides with this repository's drop-in package, which is importable as `nerf`.
 
 Hot-path-unused dependencies that are absent from the image (SURVEY.md §8c: pytorch3d, torchsearchsorted, imageio) get
@@ -15,12 +15,13 @@ import types
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(HERE)
-CANDIDATES = ["/root/reference", os.path.join(ROOT, "baseline", "_ref")]
+STAGED = os.path.join(HERE, "_ref")
+CANDIDATES = ["/root/reference", STAGED]
 NP = os.path.join("nerface_code", "nerf-pytorch")
 
 
-def reference_root():
-    for c in CANDIDATES:
+def reference_root(staged_only=False):
+    for c in ([STAGED] if staged_only else CANDIDATES):
         if os.path.isfile(os.path.join(c, NP, "nerf", "train_utils.py")):
             return c
     return None
@@ -32,11 +33,11 @@ def script_path(name):
     return os.path.join(r, NP, name) if r else None
 
 
-def load_reference(relu_clone=False):
+def load_reference(relu_clone=False, staged_only=False):
     """Returns the reference package (module `nerf_reference`) or None when no reference tree is reachable."""
     if "nerf_reference" in sys.modules:
         return sys.modules["nerf_reference"]
-    root = reference_root()
+    root = reference_root(staged_only)
     if root is None:
         return None
     for name in ("pytorch3d", "pytorch3d.transforms", "torchsearchsorted", "imageio"):

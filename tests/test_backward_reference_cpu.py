@@ -5,56 +5,36 @@ reference's run_one_iter_of_nerf (mode "train", perturbation and sigma noise on,
 the depths the reference sampled; parameter gradients of both networks and the latent-code gradient must agree to FP32 rounding.
 
 So the chain for SURVEY.md §8 row a11 is: CUDA backward  <->  torch_reference (GPU tests)  <->  reference autograd (this file).
-Needs the reference tree (/root/reference or the staged copy baseline/_ref); CPU only."""
+What the reference computed (its outputs, its four random draws, the loss, the latent gradient and a fixed sample of 512
+entries plus the max |g| of every parameter gradient) was recorded by running it (oracle/make_golden_live.py ->
+tests/golden/live/backward.npz); CPU only."""
 import os
-import sys
 
-import numpy as np
 import pytest
 import torch
 
+import golden_io
+import make_golden_live as ML
 import nerface_oracle as O
 import torch_reference as TR
 
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "oracle"))
-import make_golden as MG  # noqa: E402  (only its Recorder of torch.rand / torch.randn draws)
-import ref_loader  # noqa: E402
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "live", "backward.npz")
 
-pytestmark = pytest.mark.skipif(ref_loader.reference_root() is None, reason="no reference tree (run oracle/stage_reference.py)")
+
+@pytest.fixture(scope="module")
+def gold():
+    return golden_io.load(GOLD)
 
 
 @pytest.mark.parametrize("stress,white,use_bg", [(False, False, True), (True, False, True), (True, True, False)],
                          ids=["random_init", "opaque_stress", "opaque_stress_white_nobg"])
-def test_torch_reference_gradients_equal_reference_autograd(stress, white, use_bg, monkeypatch):
-    ref = ref_loader.load_reference()
-    # `sigma_a[:, -1] += 1e-6` (volume_rendering_utils.py:53) writes into the output of F.relu in place, which torch >= 2 refuses to
-    # differentiate through; the one patch BASELINE.md §4 names for gradient baselines (ref_loader.load_reference(relu_clone=True),
-    # also what the launcher of the unmodified train script installs): F.relu returns a copy — same values, same gradients.
-    orig_relu = torch.nn.functional.relu
-    monkeypatch.setattr(torch.nn.functional, "relu", lambda x, *a, **k: orig_relu(x).clone())
-    H, W, nc, nf, near, far = 2, 5, 64, 64, 0.2, 0.8
-    s = O.Sampling(nc, nf, True, 0.1, white, 2048)
-    fr = O.synthetic_frame(31, H, W)
-    pc, pf = O.random_init_params(100, stress), O.random_init_params(101, stress)
-    ro, rd = ref.get_ray_bundle(H, W, np.array(fr["intrinsics"]), fr["pose"][:3, :4])
-    ro, rd = ro.reshape(-1, 3).clone(), rd.reshape(-1, 3).clone()
-    n = ro.shape[0]
-    bg = fr["bg"].reshape(-1, 3) if use_bg else None
-    target = torch.rand(n, 3, generator=torch.Generator().manual_seed(5))
-
-    # ---- the reference: forward in train mode with gradients, the script's loss, autograd
-    mc, mf = ref_loader.build_model(ref, pc), ref_loader.build_model(ref, pf)
-    lat_ref = fr["latent"].clone().requires_grad_(True)
-    cfg = ref_loader.make_cfg(ref, nc, nf, True, 0.1, white, 2048, "train", near, far)
-    torch.manual_seed(77)
-    with MG.Recorder() as rec:
-        out = ref.run_one_iter_of_nerf(H, W, fr["intrinsics"], mc, mf, ro.clone(), rd.clone(), cfg, mode="train",
-                                       encode_position_fn=ref.get_embedding_function(10, True, True),
-                                       encode_direction_fn=ref.get_embedding_function(4, False, True),
-                                       expressions=fr["expr"], background_prior=bg, latent_code=lat_ref)
-    loss_ref = torch.nn.functional.mse_loss(out[0][..., :3], target) + torch.nn.functional.mse_loss(out[3][..., :3], target)
-    loss_ref.backward()
-    draws = [t for _, t in rec.draws]
+def test_torch_reference_gradients_equal_reference_autograd(gold, stress, white, use_bg, request):
+    tag = request.node.callspec.id
+    g = gold[tag]
+    H, W, s, fr, pc, pf, ro, rd, bg, target = ML.backward_inputs(stress, white, use_bg)
+    near, far = ML.NEAR, ML.FAR
+    out = g["out"]
+    draws = g["draws"]
     assert len(draws) == 4  # rand[N,Nc], randn[N,Nc], rand[N,Nf], randn[N,Nc+Nf] (train_utils.py:69-76, 105-119)
     noise = O.Noise(t_rand=draws[0], n_c=draws[1], u=draws[2], n_f=draws[3])
 
@@ -64,7 +44,7 @@ def test_torch_reference_gradients_equal_reference_autograd(stress, white, use_b
     with torch.no_grad():
         o_out = O.render_chunk(rays, pc, pf, s, fr["expr"], fr["latent"], bg, noise, extras=ex)
     for a, b in zip(out, o_out):
-        assert torch.equal(a.detach(), b)
+        assert torch.equal(a, b)
 
     # ---- the backward tests' floating-point reference at those depths
     lc = {k: v.clone().requires_grad_(True) for k, v in pc.items()}
@@ -73,26 +53,28 @@ def test_torch_reference_gradients_equal_reference_autograd(stress, white, use_b
     got = TR.render_at_depths(rays, lc, lf, fr["expr"], lat, ex["z_coarse"], ex["z_fine"], near, far, 0.1,
                               {"n_c": noise.n_c, "n_f": noise.n_f}, white, bg, None)
     for i in (0, 1, 2, 3, 4, 5, 6):
-        assert float((got[i].detach() - out[i].detach()).abs().max()) <= 2e-6 * max(1.0, float(out[i].detach().abs().max())), i
+        assert float((got[i].detach() - out[i]).abs().max()) <= 2e-6 * max(1.0, float(out[i].abs().max())), i
     loss = torch.nn.functional.mse_loss(got[0], target) + torch.nn.functional.mse_loss(got[3], target)
-    assert abs(float(loss.detach()) - float(loss_ref.detach())) <= 1e-7
+    assert abs(float(loss.detach()) - g["loss"]) <= 1e-7
     loss.backward()
 
-    def close(a, b, what):
-        scale = max(float(b.abs().max()), 1e-12)
+    def close(a, b, scale, what):
+        scale = max(scale, 1e-12)
         assert float((a - b).abs().max()) <= 2e-5 * scale, (what, float((a - b).abs().max()), scale)
 
     n_checked = 0
-    for leaves, model, tag in ((lc, mc, "coarse"), (lf, mf, "fine")):
-        named = dict(model.named_parameters())
+    for leaves, tag_net in ((lc, "coarse"), (lf, "fine")):
         for k in TR.PARAM_ORDER:
-            g_ref = named[k].grad
+            ref = g["grads"][f"{tag_net}/{k}"]
             if k.startswith("layers_dir.3"):  # built by the reference model but never used by its forward (models.py:257)
-                assert g_ref is None and leaves[k].grad is None
+                assert ref is None and leaves[k].grad is None
                 continue
-            assert g_ref is not None and leaves[k].grad is not None, (tag, k)
-            close(leaves[k].grad, g_ref, (tag, k))
+            assert ref is not None and leaves[k].grad is not None, (tag_net, k)
+            ours = leaves[k].grad
+            assert list(ours.shape) == ref["shape"]
+            close(ours.reshape(-1)[torch.from_numpy(ref["index"])], ref["value"], ref["absmax"], (tag_net, k))
+            assert abs(float(ours.abs().max()) - ref["absmax"]) <= 2e-5 * max(ref["absmax"], 1e-12), (tag_net, k)
             n_checked += 1
     assert n_checked == 2 * 24
-    close(lat.grad, lat_ref.grad, "latent")
-    assert float(lat_ref.grad.abs().max()) > 0
+    close(lat.grad, g["latent_grad"], float(g["latent_grad"].abs().max()), "latent")
+    assert float(g["latent_grad"].abs().max()) > 0

@@ -2,7 +2,7 @@
 4d-facial-avatars_b200/run_reference_script.py it imports `nerf` (ours), parses the shipped paper-model YAML, loads the synthetic
 FLAME-style dataset with our loader, builds both networks, the latent codes and the optimizer, draws the first importance-sampled
 ray batch — and stops exactly at its first `run_one_iter_of_nerf` call (train_transformed_rays.py:336), where the product path
-refuses to run without CUDA (no CPU fallback).  On a B200 the same command trains (profiles/r2_cli/).  Needs the reference tree."""
+refuses to run without CUDA (no CPU fallback).  On an H100 the same command trains.  Needs the reference tree."""
 import os
 import re
 import subprocess

@@ -1,121 +1,110 @@
 """The small tensor helpers of the drop-in `nerf` package (nerf/nerf_helpers.py) that the reference's unmodified scripts call on
-the host side of the boundary, against the live reference's own functions on CPU: same values bit for bit, same shapes, same
-chunking.  Needs the reference tree (/root/reference or the staged copy baseline/_ref); CPU only."""
+the host side of the boundary, against what the reference's own functions return on CPU: same values bit for bit, same shapes,
+same chunking.  The reference's results on these inputs were recorded by running it (oracle/make_golden_live.py ->
+tests/golden/live/dropin_helpers.npz); CPU only."""
 import os
-import sys
 
 import numpy as np
 import pytest
 import torch
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, os.path.join(ROOT, "oracle"))
-import ref_loader  # noqa: E402
+import golden_io
+import make_golden_live as ML
+import nerface_oracle as O
 
-pytestmark = pytest.mark.skipif(ref_loader.reference_root() is None, reason="no reference tree (run oracle/stage_reference.py)")
+GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "live", "dropin_helpers.npz")
 
 
 @pytest.fixture(scope="module")
 def both(built_lib):
-    sys.path.insert(0, os.path.join(ROOT, "4d-facial-avatars_b200"))
     import nerf
-    return nerf, ref_loader.load_reference()
+    return nerf, golden_io.load(GOLD)
 
 
-def _pose(seed):
-    g = torch.Generator().manual_seed(seed)
-    q, _ = torch.linalg.qr(torch.randn(3, 3, generator=g))
-    p = torch.eye(4)
-    p[:3, :3] = q
-    p[:3, 3] = torch.randn(3, generator=g) * 0.3
-    return p
-
-
-@pytest.mark.parametrize("H,W,intr", [(7, 5, [1200.0, 1250.0, 0.5, 0.5]), (4, 9, [-900.0, 910.0, 0.48, 0.53]), (16, 16, [333.3, -444.4, 0.1, 0.9])])
+@pytest.mark.parametrize("H,W,intr", ML.RAY_BUNDLE_CASES)
 def test_get_ray_bundle(both, H, W, intr):
-    nerf, ref = both
-    pose = _pose(H * 100 + W)
-    want = ref.get_ray_bundle(H, W, np.array(intr), pose[:3, :4])
+    nerf, gold = both
+    pose = ML.dropin_pose(H * 100 + W)
+    want = gold["ray_bundle"][ML.RAY_BUNDLE_CASES.index((H, W, intr))]
     got = nerf.get_ray_bundle(H, W, intr, pose)
     got34 = nerf.get_ray_bundle(H, W, np.array(intr), pose[:3, :4])
     for a, b, c in zip(want, got, got34):
         assert a.shape == b.shape == (H, W, 3) and torch.equal(a, b) and torch.equal(a, c)
 
 
-@pytest.mark.parametrize("n_freq,include_input,log_sampling", [(10, True, True), (4, False, True), (6, True, False), (1, False, True), (0, True, True)])
+@pytest.mark.parametrize("n_freq,include_input,log_sampling", ML.PE_CASES)
 def test_positional_encoding_and_embedding_function(both, n_freq, include_input, log_sampling):
-    nerf, ref = both
+    nerf, gold = both
+    k = ML.PE_CASES.index((n_freq, include_input, log_sampling))
     x = torch.randn(37, 3, generator=torch.Generator().manual_seed(n_freq)) * 3.0
-    want = ref.positional_encoding(x, n_freq, include_input, log_sampling)
+    want = gold["pe"][k]
     got = nerf.positional_encoding(x, n_freq, include_input, log_sampling)
     assert want.shape == got.shape and torch.equal(want, got)
-    f_ref = ref.get_embedding_function(n_freq, include_input, log_sampling)
     f = nerf.get_embedding_function(n_freq, include_input, log_sampling)
-    assert torch.equal(f_ref(x), f(x))
+    assert torch.equal(gold["embedding"][k], f(x))
 
 
 def test_meshgrid_minibatches_and_metrics(both):
-    nerf, ref = both
+    nerf, gold = both
     a, b = torch.arange(5, dtype=torch.float32), torch.arange(3, dtype=torch.float32) * 2.0
-    for u, v in zip(ref.meshgrid_xy(a, b), nerf.meshgrid_xy(a, b)):
+    got = nerf.meshgrid_xy(a, b)
+    assert len(got) == len(gold["meshgrid"])
+    for u, v in zip(gold["meshgrid"], got):
         assert u.shape == v.shape and torch.equal(u, v)
     x = torch.randn(23, 4, generator=torch.Generator().manual_seed(3))
-    for cs in (1, 7, 23, 100):
-        w, g = ref.get_minibatches(x, chunksize=cs), nerf.get_minibatches(x, chunksize=cs)
+    for w, cs in zip(gold["minibatches"], (1, 7, 23, 100)):
+        g = nerf.get_minibatches(x, chunksize=cs)
         assert len(w) == len(g) and all(torch.equal(p, q) for p, q in zip(w, g))
     y = torch.randn(23, 4, generator=torch.Generator().manual_seed(4))
-    assert torch.equal(ref.img2mse(x, y), nerf.img2mse(x, y))
-    for m in (0.0, 1e-5, 0.0123, 1.0):
-        assert ref.mse2psnr(m) == nerf.mse2psnr(m)
+    assert torch.equal(gold["img2mse"], nerf.img2mse(x, y))
+    for want, m in zip(gold["mse2psnr"], (0.0, 1e-5, 0.0123, 1.0)):
+        got = nerf.mse2psnr(m)
+        assert type(got) is type(want) and got == want
 
 
-def test_cfgnode_on_the_shipped_yaml(both):
+def test_cfgnode_on_a_script_shaped_config(both):
     """The scripts build `CfgNode(yaml.load(...))`, read nested attributes and write `cfg.dump()` next to the checkpoints
-    (train_transformed_rays.py:46-50, 126-128): same tree, same leaves, a dump that loads back to the same dict."""
+    (train_transformed_rays.py:46-50, 126-128): same tree, same leaves and leaf types as the reference's CfgNode on the same
+    config, a dump that loads back to the same dict."""
     import yaml
-    nerf, ref = both
-    path = ref_loader.script_path(os.path.join("config", "dave", "dave_dvp_lcode_fixed_bg_512_paper_model.yml"))
-    raw = yaml.load(open(path), Loader=yaml.FullLoader)
-    a, b = ref.CfgNode(raw), nerf.CfgNode(raw)
+    nerf, gold = both
+    b = nerf.CfgNode(ML.CFG_RAW)
 
-    def walk(x, y, trail):
-        assert set(x.keys()) == set(y.keys()), trail
-        for k in x.keys():
-            u, v = getattr(x, k), getattr(y, k)
-            if isinstance(u, dict):
-                assert isinstance(v, dict) and isinstance(v, nerf.CfgNode), trail + [k]
-                walk(u, v, trail + [k])
+    def leaves(node, trail):
+        res = []
+        for k in node.keys():
+            v = getattr(node, k)
+            if isinstance(v, dict):
+                assert isinstance(v, nerf.CfgNode), trail + [k]
+                res.append([trail + [k], "dict", "CfgNode"])
+                res += leaves(v, trail + [k])
             else:
-                assert u == v and type(u) is type(v), (trail + [k], u, v)
+                res.append([trail + [k], type(v).__name__, v])
+        return res
 
-    walk(a, b, [])
+    key = lambda e: tuple(e[0])  # noqa: E731
+    assert sorted(leaves(b, []), key=key) == sorted(gold["cfg_leaves"], key=key)
     assert b.nerf.train.num_coarse == 64 and b.nerf.validation.num_fine == 64 and b.dataset.no_ndc is True
-    assert getattr(b.nerf, "train").chunksize == a.nerf.train.chunksize
-    assert yaml.safe_load(b.dump()) == yaml.safe_load(a.dump()) == raw
+    assert gold["cfg_dump_roundtrip_equal"] and yaml.safe_load(b.dump()) == ML.CFG_RAW
     with pytest.raises(AttributeError):
         b.nerf.no_such_option
 
 
 def test_model_class_against_the_reference_class(both):
     """ConditionalBlendshapePaperNeRFModel built with the keyword arguments the scripts pass (train_transformed_rays.py:150-176):
-    same state_dict keys / shapes / dtypes, a reference checkpoint loads into the drop-in and back (strict), the torch forward of
-    the drop-in (not the hot path) returns the reference module's values bit for bit, and the attributes the scripts and the
-    renderer read are the same."""
-    nerf, ref = both
-    kw = dict(num_layers=8, hidden_size=256, skip_connect_every=3, num_encoding_fn_xyz=10, num_encoding_fn_dir=4,
-              include_input_xyz=True, include_input_dir=False, use_viewdirs=True, include_expression=True, latent_code_dim=32)
-    torch.manual_seed(11)
-    m_ref = ref.models.ConditionalBlendshapePaperNeRFModel(**kw)
-    m = nerf.models.ConditionalBlendshapePaperNeRFModel(**kw)
-    sd_ref, sd = m_ref.state_dict(), m.state_dict()
-    assert [(k, tuple(v.shape), v.dtype) for k, v in sd_ref.items()] == [(k, tuple(v.shape), v.dtype) for k, v in sd.items()]
-    m.load_state_dict(sd_ref, strict=True)
-    m_ref.load_state_dict(m.state_dict(), strict=True)
-    for name in ("dim_xyz", "dim_dir", "dim_expression", "dim_latent_code", "use_viewdirs"):
-        assert getattr(m, name) == getattr(m_ref, name), name
+    same state_dict keys / shapes / dtypes and parameter count as the reference class, the same parameters load strictly, the
+    torch forward of the drop-in (not the hot path) returns the reference module's values bit for bit, and the attributes the
+    scripts and the renderer read are the same."""
+    nerf, gold = both
+    m = nerf.models.ConditionalBlendshapePaperNeRFModel(**ML.MODEL_KW)
+    sd = m.state_dict()
+    assert [[k, list(v.shape), str(v.dtype)] for k, v in sd.items()] == gold["state_dict"]
+    m.load_state_dict(O.random_init_params(100), strict=True)
+    for name, want in gold["attributes"].items():
+        assert getattr(m, name) == want, name
     g = torch.Generator().manual_seed(12)
     x = torch.randn(19, m.dim_xyz + m.dim_dir, generator=g)
     expr, lat = torch.randn(76, generator=g), torch.randn(32, generator=g)
     with torch.no_grad():
-        assert torch.equal(m(x, expr, lat), m_ref(x, expr, lat))
-    assert sum(p.numel() for p in m.parameters()) == sum(p.numel() for p in m_ref.parameters())
+        assert torch.equal(m(x, expr, lat), gold["forward"])
+    assert sum(p.numel() for p in m.parameters()) == gold["numel"]

@@ -37,7 +37,7 @@ def psnr(a, b):
 
 @pytest.mark.parametrize("H,nc,nf,n_samp", [(512, 64, 128, 4096), (1024, 128, 256, 4096)], ids=["512_64c128f", "1024_128c256f"])
 def test_full_frame_against_oracle(env, H, nc, nf, n_samp):
-    """BASELINE configs 2 and 4 at FULL size: the whole frame is rendered in one launch (all 148 CTAs, hundreds of units each),
+    """BASELINE configs 2 and 4 at FULL size: the whole frame is rendered in one launch (every SM's CTA, hundreds of units each),
     4096 rays spread evenly over the launch — every CTA, early and late iterations, all four ray slots of a unit — are compared
     with the oracle in both precision modes (north_star: 1e-4 max-abs on random-init weights)."""
     nerf, _engine, dev = env

@@ -1,4 +1,4 @@
-"""Parity of the fused sm_100a render path against the reference's outputs (tests/golden) and the CPU oracle.
+"""Parity of the fused sm_90a render path against the reference's outputs (tests/golden) and the CPU oracle.
 Tolerances (north_star): 1e-4 max-abs on all seven outputs; reported per precision mode below."""
 import glob
 import os

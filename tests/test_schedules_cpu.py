@@ -1,6 +1,6 @@
 """Host-only checks of the compile-time schedules the kernels execute (nfb_debug_schedule): every weight byte of the packed
-streams is consumed exactly once per tile by each render program and by the backward chain, units fit their ring slots, TMEM
-operand columns stay inside their regions, and the weight-gradient jobs tile the accumulator space without overlap.  These are
+streams is consumed exactly once per tile by the render program and by the backward chain, units fit their ring slots, A
+operands come from the activation buffer's four K atoms, and the weight-gradient jobs tile the accumulator space without overlap.  These are
 the invariants a change to csrc/nfb_layout.h or to one of the program builders can silently break; no GPU involved."""
 import ctypes as C
 
@@ -37,10 +37,6 @@ def spans(ents):
     return [((e[3] & 0xFFFFF) << 4, (e[3] >> 20) * 128) for e in ents]
 
 
-def idesc_n(x):
-    return ((x >> 17) & 0x3F) << 3
-
-
 def assert_exact_cover(sp, total):
     sp = sorted(sp)
     pos = 0
@@ -57,48 +53,19 @@ def test_one_tile_program_covers_the_weight_stream(lib):
     assert_exact_cover(sp, STREAM_X1)
     for e, (off, nbytes) in zip(ents, sp):
         assert nbytes <= 32768 and off % 1024 == 0          # one ring slot, swizzle-aligned
-        assert idesc_n(e[0]) * 128 == nbytes                 # MMA N == rows of the unit
-        d_col, a_col = e[1] & 0xFFFF, e[1] >> 16
-        assert d_col in (0, 256) and (e[2] & 1 or (a_col ^ d_col) & 256)   # operand and accumulator in different regions
-    assert sum(1 for e in ents if e[2] & 16) == 10           # one "accumulator complete" commit per step
-
-
-def test_two_tile_program_covers_the_weight_stream_in_half_units(lib):
-    """One entry per PIECE (a [rows x 64 K] block of the stream); pieces are grouped into LOADS, one ring slot each."""
-    ents = entries(lib, 1)
-    assert len(ents) == 58
-    sp = spans(ents)
-    assert_exact_cover(sp, STREAM_X1)                        # each half-unit once per tile pair
-    groups, loads = {}, {}
-    for e, (off, nbytes) in zip(ents, sp):
-        assert nbytes in (16384, 2048) and off % 16 == 0     # N = 128 or 16 rows of 128 bytes
-        assert idesc_n(e[0]) * 128 == nbytes
-        assert e[1] in (0, 32, 64, 96) or (e[2] & 1)         # K atom inside the 128-column operand region
-        groups.setdefault(e[4], []).append(e)
-        loads.setdefault(e[5], []).append((e, nbytes))
-    assert len(groups) == 17
-    for g in groups.values():
-        assert g[0][2] & 2 and g[-1][2] & 4                  # first / last flags
-        assert all(not (e[2] & 2) for e in g[1:]) and all(not (e[2] & 4) for e in g[:-1])
-        assert len({e[5] for e in g}) <= 5                   # a group never needs more than 5 of the 9 ring slots at once
-    # static ring: 54 loads = 6 full rounds of 9 slots, so every tile starts at slot 0 with the same mbarrier parity
-    assert sorted(loads) == list(range(54))
-    for i, pieces in loads.items():
-        assert all(e[6] == i % 9 for e, _ in pieces)
-        pos = 0
-        for e, nbytes in pieces:                             # pieces are packed back to back, 1024-byte (swizzle) aligned
-            assert e[7] == pos and pos % 1024 == 0
-            pos += nbytes
-        assert pos <= 16384
-        assert len({e[4] for e, _ in pieces}) == 1           # a load never straddles two half-step groups
+        assert e[0] * 128 == nbytes                          # MMA N == rows of the unit
+        assert (e[2] & 1 and e[1] == 0) or e[1] < 4          # A operand: the PE buffer or one K atom of the activation buffer
+    assert sum(1 for e in ents if e[2] & 16) == 10           # one "step complete" unit per step
+    assert sum(1 for e in ents if e[2] & 8) == 10            # one "first unit" per step
 
 
 def test_backward_chain_program(lib):
     ents = entries(lib, 2)
     assert len(ents) == 28
     assert_exact_cover(spans(ents), STREAM_BWD)
-    for e in ents:
-        assert idesc_n(e[0]) in (128, 256)
+    for e, (off, nbytes) in zip(ents, spans(ents)):
+        assert e[0] in (128, 256) and e[0] * 128 == nbytes
+        assert (e[2] & 1 and e[1] == 0) or e[1] < 4
     assert sum(1 for e in ents if e[2] & 16) == 9            # nine steps
 
 
@@ -130,33 +97,6 @@ def test_weight_gradient_jobs(lib):
     biased = [j[5] for j in jobs if j[5] < (1 << 31)]
     assert sorted(set(biased)) == list(range(9))                         # every layer's bias is produced ...
     assert len([b for b in biased if b <= 5]) == 12                      # ... by both halves of the 256-wide layers, once each
-
-
-@pytest.mark.parametrize("n_iter,tc,tf", [(1, 1, 3), (2, 1, 3), (5, 1, 3), (4, 1, 2), (3, 1, 1)])
-def test_pipelined_kernel_job_sequence(lib, n_iter, tc, tf):
-    """csrc/nfb_render3.cu: every role of the pipelined kernel walks C(0) | C(1) F(0,.) | C(2) F(1,.) | ...  Invariants the
-    hand-offs rely on: every (unit, pass, tile) exactly once; the coarse pass of unit u+1 is issued BEFORE the fine pass of unit u
-    (so the sampler resamples u while the tensor core runs C(u+1)) but never two coarse passes ahead (the per-unit buffers are
-    double-buffered by unit parity, three ray-constant slots); tiles of a pass in order; the shared-memory map fits 227 KB."""
-    which = 1000 + 100 * n_iter + 10 * tc + tf
-    jobs = [tuple(e[:3]) for e in entries(lib, which)]
-    extra = entries(lib, which)[0][3:7]
-    assert extra[0] <= 232448 and extra[1] == 128 and extra[2] == 384 and extra[3] >= 2 * extra[2]
-    assert len(jobs) == n_iter * (tc + tf) and len(set(jobs)) == len(jobs)
-    pos = {j: k for k, j in enumerate(jobs)}
-    for u in range(n_iter):
-        for t in range(tc):
-            assert (u, 0, t) in pos
-            if t:
-                assert pos[(u, 0, t)] == pos[(u, 0, t - 1)] + 1
-        for t in range(tf):
-            assert pos[(u, 1, t)] > pos[(u, 0, tc - 1)]                       # fine after its own coarse pass
-            if t:
-                assert pos[(u, 1, t)] == pos[(u, 1, t - 1)] + 1
-        if u + 1 < n_iter:
-            assert pos[(u + 1, 0, 0)] < pos[(u, 1, 0)]                        # C(u+1) before F(u, 0)
-        if u + 2 < n_iter:
-            assert pos[(u + 2, 0, 0)] > pos[(u, 1, tf - 1)]                   # ... but C(u+2) only after F(u) has been issued
 
 
 @pytest.mark.parametrize("sms,t0,t1", [(148, 1024, 2048), (148, 128, 256), (148, 24, 48), (148, 5, 0), (148, 1, 2), (148, 3, 1000),

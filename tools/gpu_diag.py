@@ -1,4 +1,4 @@
-"""First-light diagnostic for the fused kernel (run on the GPU box): compares every stage the kernel can dump
+"""First-light diagnostic for the fused kernel (run on an H100): compares every stage the kernel can dump
 (sample depths, positional encoding, each layer's activations, raw MLP outputs, the seven outputs) with the CPU
 oracle.  Usage: python tools/gpu_diag.py [fast|exact] [--stress]"""
 import os

@@ -1,8 +1,7 @@
 """Phase-cycle profile of the render kernels (NfbDebug.prof).  Usage: python tools/phase_profile.py [fast|exact] [H W]
 
 Needs a library with the timers compiled in: `python 4d-facial-avatars_b200/build.py --timers` (lib/libnfb_timers.so, picked
-up here unless NFB_LIB is set).  NFB_KERNEL=v4 profiles the one-tile kernel in fast mode.  In the two-tile kernel the slots
-"wait MMA step s" / "epilogue step s" sum all half-step events (both halves, both streams) of step s."""
+up here unless NFB_LIB is set)."""
 import os
 import sys
 
@@ -42,7 +41,7 @@ e1.record()
 torch.cuda.synchronize()
 ms = e0.elapsed_time(e1)
 c = prof.cpu().tolist()
-ctas = min(148, H * W // 2)
+ctas = min(132, H * W // 2)
 units = H * W / 2
 tiles = units * 4
 names = {0: "ray setup", 1: "dir term", 2: "prologue (z+PE)", 3: "end-of-pass barrier", 4: "composite", 5: "cdf", 6: "inverse-cdf", 7: "sort",

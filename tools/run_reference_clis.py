@@ -1,12 +1,12 @@
 #!/usr/bin/env python
-"""Drive the reference's two command-line programs UNMODIFIED on the B200 render path (SURVEY.md §8b, §8f rank 1):
+"""Drive the reference's two command-line programs UNMODIFIED on the H100 render path (SURVEY.md §8b, §8f rank 1):
 
     train_transformed_rays.py  (callers of the path: :336-352 train, :488-504 in-loop validation, optimizer :391-399)
     eval_transformed_rays.py   (:449-467, plus its normal-map / PNG tail)
 
 through 4d-facial-avatars_b200/run_reference_script.py, which only puts this repository's drop-in `nerf` package first on
 sys.path (and, under torchrun, shards run_one_iter_of_nerf over the ranks — nerf/parallel.py).  The script bodies come from the
-reference tree (/root/reference here, the staged byte-for-byte copy baseline/_ref on the GPU box); the dataset is synthetic
+reference tree (/root/reference, or the staged byte-for-byte copy oracle/_ref); the dataset is synthetic
 (tools/make_synthetic_dataset.py); the YAML is the shipped paper-model config with only paths and iteration counts replaced.
 
     python tools/run_reference_clis.py --out gpurun_out/cli --gpus 1 --iters 40

@@ -131,7 +131,7 @@ def main():
         step_ms = float(ms[0]) / a.steps
         evals = 2 * a.num_coarse + a.num_fine
         flop = 3 * 1100032 * evals * a.rays
-        peak = 1652.1
+        peak = 989.0  # H100 SXM data sheet, dense FP16
         pk = os.path.join(ROOT, "MEASURED_PEAKS.json")
         if os.path.exists(pk):
             peak = json.load(open(pk))["bf16_tflops"]
