@@ -14,7 +14,7 @@ CSRC = os.path.join(HERE, "csrc")
 LIB_DIR = os.path.join(HERE, "lib")
 LIB = os.path.join(LIB_DIR, "libnfb.so")
 SOURCES = ["nfb_api.cu", "nfb_pack.cu", "nfb_optim.cu", "nfb_post.cu", "nfb_render.cu", "nfb_train.cu"]
-HEADERS = ["nfb_internal.h", "nfb_layout.h", "nfb_ptx.cuh", "nfb_save.cuh", "nfb_render_common.cuh", "nfb_sampler.h", os.path.join("..", "..", "include", "nfb.h")]
+HEADERS = ["nfb_internal.h", "nfb_layout.h", "nfb_pipeline.cuh", "nfb_ptx.cuh", "nfb_save.cuh", "nfb_render_common.cuh", "nfb_sampler.h", os.path.join("..", "..", "include", "nfb.h")]
 
 
 def _nvcc():

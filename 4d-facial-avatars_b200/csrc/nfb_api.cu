@@ -621,11 +621,21 @@ int nfb_host_map_cdf(const NfbRayMap* map, const long long* zeroed_sorted, int n
   return NFB_OK;
 }
 
+// Host copy of the per-tile unit program a kernel follows through a weight stream (nfb_layout.h: make_prog).
+static int debug_prog(int stream, int index, uint32_t* out) {
+  const int n = nfb::prog_units(stream);
+  if (index < 0) return n;
+  if (index >= n) return -1;
+  const nfb::ProgEntry e = nfb::make_prog(stream).e[index];
+  out[0] = e.x; out[1] = e.y; out[2] = e.z; out[3] = e.w;
+  return 4;
+}
+
 int nfb_debug_schedule(int which, int index, uint32_t* out, int out_words) {
   if (index >= 0 && (!out || out_words < 10)) return -1;
   switch (which) {
-    case 0: return nfb::debug_prog_v4(index, out);
-    case 2: return nfb::debug_prog_chain(index, out);
+    case 0: return debug_prog(nfb::kFwdStream, index, out);
+    case 2: return debug_prog(nfb::kBwdStream, index, out);
     case 3: return nfb::debug_jobs_dw(index, out);
     case 4: return index < 0 ? 1 : nfb::debug_dw_split(out);  // in/out: {num_sms, tiles 0, tiles 1} -> {parts0, parts1, groups}
     default: return -1;

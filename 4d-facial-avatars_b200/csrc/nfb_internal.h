@@ -88,8 +88,6 @@ struct DwParams {  // ONE launch covers both networks: the first parts[0] * grou
   const float* scal;
 };
 // host copies of the compile-time schedules (nfb_debug_schedule); index < 0: number of entries; else words written or -1
-int debug_prog_v4(int index, uint32_t* out);
-int debug_prog_chain(int index, uint32_t* out);
 int debug_jobs_dw(int index, uint32_t* out);
 int debug_dw_split(uint32_t* io);  // io: {num_sms, tiles net 0, tiles net 1} -> {parts0, parts1, groups}
 cudaError_t train_kernels_setup();

@@ -1,7 +1,7 @@
 // nfb_layout.h — the MLP as the kernel executes it: 10 tensor-core "steps", each a GEMM
 //   D[128 rows, N] = A[128 rows, K] * W[N, K]^T   (FP16 operands, FP32 accumulate in registers)
-// and the byte layout of the packed weight stream the kernel bulk-copies into shared memory.
-// Shared by host (packing, tests) and device code.
+// and the byte layout of the packed weight streams (forward and backward chain) the kernels bulk-copy into shared memory,
+// with the per-tile unit program they follow through them.  Shared by host (packing, tests) and device code.
 //
 // Reference model: ConditionalBlendshapePaperNeRFModel.forward (nerf/models.py:236-261).  Exact
 // algebra applied at load / per frame (SURVEY.md §8 a''):
@@ -61,43 +61,8 @@ NFB_HD constexpr StepInfo step_info(int s) {
 }
 constexpr int kBiasFloats = 1952;  // 6*256 + 144 + 128 + 128 + 16
 
-// Bytes of the FP16 "hi" weights of one step (x1 stream); the x3 stream stores hi then lo per unit.
-NFB_HD constexpr int step_bytes_x1(int s) {
-  return (step_info(s).nh0 + step_info(s).nh1) * step_info(s).k_atoms * 128;
-}
-NFB_HD constexpr int step_offset_x1(int s) {
-  int off = 0;
-  for (int i = 0; i < s; ++i) off += step_bytes_x1(i);
-  return off;
-}
-constexpr int kStreamBytesX1 = step_offset_x1(kNumSteps);  // 864256
-constexpr int kStreamBytesX3 = 2 * kStreamBytesX1;
-
-// The u-th weight unit of step s in consumption order.
-struct UnitInfo {
-  int16_t h;        // N-half (0/1): accumulator half and row block [h ? nh0 : 0, ...) of the layer's weight matrix
-  int16_t ka;       // K atom of the step's logical K axis (0 = the PE atom when the step has one)
-  int16_t from_pe;  // A operand comes from the shared-memory PE buffer
-  int16_t group;    // 1: needs the previous step's half-0 epilogue only; 2: also its half-1 epilogue
-  int16_t rows;     // output rows (MMA N) of the unit
-  int16_t last;     // last unit of its half in this step (-> commit "accumulator half complete")
-};
-NFB_HD constexpr int num_units(int s) { return step_info(s).k_atoms; }
-NFB_HD constexpr UnitInfo unit_info(int s, int u) {
-  const StepInfo si = step_info(s);
-  const int hid = u - si.pe_first;  // hidden atom index (< 0: the PE atom)
-  const int group = (hid >= 2) ? 2 : 1;
-  return UnitInfo{0, (int16_t)u, (int16_t)(si.pe_first && u == 0), (int16_t)group, (int16_t)(si.nh0 + si.nh1),
-                  (int16_t)(u == si.k_atoms - 1)};
-}
-// Byte offset of unit u inside its step, x1 stream.
-NFB_HD constexpr int unit_offset_in_step(int s, int u) {
-  int off = 0;
-  for (int i = 0; i < u; ++i) off += unit_info(s, i).rows * 128;
-  return off;
-}
 // Byte offset of element (row n, k in [0,64)) inside one swizzled unit: 128-byte rows, 16-byte chunks
-// XORed with (row & 7) — the SWIZZLE_128B pattern the UMMA shared-memory descriptor expects.
+// XORed with (row & 7) — the SWIZZLE_128B pattern the wgmma shared-memory descriptor expects.
 NFB_HD constexpr int sw128_offset(int n, int k) { return n * 128 + ((((k >> 3) ^ (n & 7)) & 7) << 4) + ((k & 7) << 1); }
 
 
@@ -138,13 +103,56 @@ NFB_HD constexpr StepInfo bwd_step_info(int s) {
          : s == 3 ? StepInfo{128, 128, 3, 1, 0, 0}
                   : StepInfo{128, 128, 4, 0, 0, 0};
 }
-NFB_HD constexpr int bwd_step_bytes(int s) { return (bwd_step_info(s).nh0 + bwd_step_info(s).nh1) * bwd_step_info(s).k_atoms * 128; }
-NFB_HD constexpr int bwd_step_offset(int s) {
+
+// ------------------------------------------------------------------------------------------------
+// The two weight streams: the forward MLP (step_info) and the backward chain (bwd_step_info, transposed weights).  Both are
+// laid out by one rule: a unit = all N rows of a step x one 64-wide K atom, units in consumption order (step by step, K atom
+// by K atom), so unit u of step s starts at (offset of step s) + u * rows * 128.  The x1 stream holds FP16 weights; the x3
+// stream of exact mode holds the hi unit then the lo unit at twice the x1 offset.  Written by repack_kernel (nfb_pack.cu),
+// read by the kernels through the unit program below.
+enum : int { kFwdStream = 0, kBwdStream = 1 };
+NFB_HD constexpr int stream_steps(int stream) { return stream == kFwdStream ? kNumSteps : kBwdSteps; }
+NFB_HD constexpr StepInfo stream_step(int stream, int s) { return stream == kFwdStream ? step_info(s) : bwd_step_info(s); }
+NFB_HD constexpr int unit_rows(int stream, int s) { return stream_step(stream, s).nh0 + stream_step(stream, s).nh1; }
+NFB_HD constexpr int unit_offset(int stream, int s, int u) {
   int off = 0;
-  for (int i = 0; i < s; ++i) off += bwd_step_bytes(i);
-  return off;
+  for (int i = 0; i < s; ++i) off += stream_step(stream, i).k_atoms * unit_rows(stream, i) * 128;
+  return off + u * unit_rows(stream, s) * 128;
 }
-constexpr int kBwdStreamBytes = bwd_step_offset(kBwdSteps);  // 835584
+constexpr int kStreamBytesX1 = unit_offset(kFwdStream, kNumSteps, 0);  // 864256
+constexpr int kStreamBytesX3 = 2 * kStreamBytesX1;
+constexpr int kBwdStreamBytes = unit_offset(kBwdStream, kBwdSteps, 0);  // 835584
+
+// Per-tile unit program of a stream, built at compile time: one entry per unit in consumption order.  x = MMA N (rows of the
+// unit), y = K atom of the activation buffer the A operand comes from, z = flags, w = (byte offset in the stream, x1 layout)
+// / 16 | rows << 20.  kUnitFromOperand: the A operand is the step's own shared-memory operand (the PE buffer forward, the d raw
+// operand backward), not the activation buffer.
+enum : uint32_t { kUnitFromOperand = 1u, kUnitFirst = 8u, kUnitLast = 16u };
+struct ProgEntry { uint32_t x, y, z, w; };
+constexpr int kMaxProgUnits = 32;
+struct ProgTable { ProgEntry e[kMaxProgUnits]; };
+NFB_HD constexpr int prog_units(int stream) {
+  int n = 0;
+  for (int s = 0; s < stream_steps(stream); ++s) n += stream_step(stream, s).k_atoms;
+  return n;
+}
+static_assert(prog_units(kFwdStream) <= kMaxProgUnits && prog_units(kBwdStream) <= kMaxProgUnits, "program table too small");
+constexpr ProgTable make_prog(int stream) {
+  ProgTable t{};
+  int i = 0;
+  for (int s = 0; s < stream_steps(stream); ++s) {
+    const StepInfo si = stream_step(stream, s);
+    const uint32_t rows = (uint32_t)unit_rows(stream, s);  // <= 256
+    for (int u = 0; u < si.k_atoms; ++u, ++i) {
+      const bool from_op = si.pe_first && u == 0;
+      t.e[i].x = rows;
+      t.e[i].y = from_op ? 0u : (uint32_t)(u - si.pe_first);
+      t.e[i].z = (from_op ? kUnitFromOperand : 0u) | (u == 0 ? kUnitFirst : 0u) | (u == si.k_atoms - 1 ? kUnitLast : 0u);
+      t.e[i].w = ((uint32_t)unit_offset(stream, s, u) >> 4) | (rows << 20);
+    }
+  }
+  return t;
+}
 
 // Weight-gradient accumulators of one network (FP32, float offsets), in the kernel's folded parametrisation.
 constexpr int kAcc0 = 0;                       // [256][64]   d W0[:, PE lanes]

@@ -2,7 +2,8 @@
 //   * fold_feat_kernel : fc_feat pre-multiplied into fc_alpha and layers_dir.0[:, :256] (FP64 accumulate), both networks
 //   * repack_kernel    : ONE launch per weight update, both networks: FP32 weights -> FP16 hi/lo as the swizzled shared-memory images the
 //                        render kernels bulk-copy (forward streams) and the transposed stream of the backward chain, static
-//                        biases, conditioning columns, transposed direction columns
+//                        biases, conditioning columns, transposed direction columns.  Units land at nfb_layout.h unit_offset,
+//                        the function the kernels' unit programs are built from.
 //   * frame_fold_kernel: per-frame expression/latent fold into the layer-0 / layer-3 biases
 // Reference semantics: nerf/models.py:236-261 (forward), :218-233 (parameter shapes).
 #include <cuda_fp16.h>
@@ -60,19 +61,18 @@ __device__ __forceinline__ int step_rows(int s) { return s <= 5 ? 256 : (s == 6 
 __device__ __forceinline__ void pack_fwd_chunk(const NetParams& a, int s, int u, int idx, uint8_t* __restrict__ dst_x1,
                                                uint8_t* __restrict__ dst_x3) {
   const StepInfo si = step_info(s);
-  if (u >= num_units(s)) return;
-  const UnitInfo ui = unit_info(s, u);
-  if (idx >= ui.rows * 8) return;
+  if (u >= si.k_atoms) return;
+  const int rows = unit_rows(kFwdStream, s);
+  if (idx >= rows * 8) return;
   const float* __restrict__ src = a.p[step_src(s)];
   const int ld = step_ld(s), n_valid = step_rows(s);
   const int c16 = idx & 7;
-  const int n_local = idx >> 3;
-  const int n = (ui.h ? si.nh0 : 0) + n_local;  // row of the step's logical weight matrix
+  const int n = idx >> 3;  // row of the step's weight matrix
   __align__(16) __half hi[8];
   __align__(16) __half lo[8];
 #pragma unroll
   for (int e = 0; e < 8; ++e) {
-    const int k = ui.ka * 64 + c16 * 8 + e;  // logical K index of this step
+    const int k = u * 64 + c16 * 8 + e;  // logical K index of this step
     float w = 0.f;
     if (n < n_valid) {
       if (s == 6) w = a.w6[n * 256 + k];
@@ -86,12 +86,12 @@ __device__ __forceinline__ void pack_fwd_chunk(const NetParams& a, int s, int u,
     hi[e] = __float2half_rn(w);
     lo[e] = __float2half_rn(w - __half2float(hi[e]));
   }
-  const size_t unit_x1 = (size_t)step_offset_x1(s) + unit_offset_in_step(s, u);
-  const int inner = n_local * 128 + ((c16 ^ (n_local & 7)) << 4);
+  const size_t unit_x1 = (size_t)unit_offset(kFwdStream, s, u);
+  const int inner = n * 128 + ((c16 ^ (n & 7)) << 4);
   *reinterpret_cast<uint4*>(dst_x1 + unit_x1 + inner) = *reinterpret_cast<const uint4*>(hi);
   const size_t unit_x3 = 2 * unit_x1;
   *reinterpret_cast<uint4*>(dst_x3 + unit_x3 + inner) = *reinterpret_cast<const uint4*>(hi);
-  *reinterpret_cast<uint4*>(dst_x3 + unit_x3 + (size_t)ui.rows * 128 + inner) = *reinterpret_cast<const uint4*>(lo);
+  *reinterpret_cast<uint4*>(dst_x3 + unit_x3 + (size_t)rows * 128 + inner) = *reinterpret_cast<const uint4*>(lo);
 }
 
 // Static bias block, the 108 conditioning columns of layers_xyz.0/.3 and the transposed direction columns of layers_dir.0.
@@ -121,7 +121,7 @@ __device__ __forceinline__ void gather_elem(const NetParams& g, int t, float* __
 __device__ __forceinline__ void pack_bwd_chunk(const NetParams& a, int s, int u, int idx, uint8_t* __restrict__ dst) {
   const StepInfo si = bwd_step_info(s);
   if (u >= si.k_atoms) return;
-  const int rows = si.nh0 + si.nh1;
+  const int rows = unit_rows(kBwdStream, s);
   if (idx >= rows * 8) return;
   const int c16 = idx & 7, n = idx >> 3;
   const bool op_atom = si.pe_first && u == 0;
@@ -146,7 +146,7 @@ __device__ __forceinline__ void pack_bwd_chunk(const NetParams& a, int s, int u,
     }
     h[e] = __float2half_rn(w);
   }
-  const int off = bwd_step_offset(s) + u * rows * 128;
+  const int off = unit_offset(kBwdStream, s, u);
   *reinterpret_cast<uint4*>(dst + off + n * 128 + ((c16 ^ (n & 7)) << 4)) = *reinterpret_cast<const uint4*>(h);
 }
 

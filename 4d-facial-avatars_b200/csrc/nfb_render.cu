@@ -18,16 +18,16 @@
 // ([N rows x 64 K], the layout a wgmma shared-memory descriptor reads): 3 slots in fast mode, 1 in exact mode, whose hi+lo
 // activation buffers take the space.
 //
-// Warp roles (384 threads): warp 0 = weight producer (warps 1..3 idle: the register file is re-partitioned per warpgroup),
-// warpgroups 1 and 2 = "row" warps.  For the per-row work (sampling, positional encoding, compositing, inverse-CDF
-// resampling, the per-ray sort) thread <-> sample row, the two warpgroups splitting the columns; for the MLP each warpgroup
-// issues the wgmma of its 64 rows and runs their epilogues.
+// Warp roles (nfb_pipeline.cuh): warp 0 = weight producer, warpgroups 1 and 2 = "row" warps.  For the per-row work
+// (sampling, positional encoding, compositing, inverse-CDF resampling, the per-ray sort) thread <-> sample row, the two
+// warpgroups splitting the columns; for the MLP each warpgroup issues the wgmma of its 64 rows and runs their epilogues.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <math_constants.h>
 
 #include "nfb_internal.h"
 #include "nfb_layout.h"
+#include "nfb_pipeline.cuh"
 #include "nfb_ptx.cuh"
 #include "nfb_save.cuh"
 #include "nfb_render_common.cuh"
@@ -35,18 +35,12 @@
 namespace nfb {
 
 constexpr int kRowsMax = 512;   // sample rows of one pass of one unit of work
-constexpr int kThreads = 384;   // producer warpgroup + 2 row warpgroups
-constexpr int kRegsLight = 40, kRegsRow = 232;
-static_assert((4 * kRegsLight + 8 * kRegsRow) * 32 <= 65536, "register file");
-template <int N> __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
-template <int N> __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
-constexpr int kRowThreads = 256;
-constexpr uint32_t kRowBarrier = 1;  // named barrier id of the eight row warps; 2 + w: warpgroup w alone
 
 // shared memory map (bytes from the 1024-aligned base).  Activation buffers: 4 K atoms x [128 rows x 128 B], swizzled.
 template <bool EXACT>
 struct SmemMap {
   static constexpr int kSlots = EXACT ? 1 : 3;
+  using WeightRing = Ring<kSlots, kMaxUnitBytes>;
   static constexpr int kRing = 0;
   static constexpr int kActHi = kRing + kSlots * kMaxUnitBytes;
   static constexpr int kActLo = kActHi + 4 * kTileM * 128;
@@ -67,61 +61,27 @@ struct SmemMap {
   static_assert(kRaw % 16 == 0 && kBars % 8 == 0, "alignment");
 };
 
-// Per-unit program entry, precomputed at compile time: x = MMA N (rows of the unit), y = K atom of the activation buffer
-// the A operand comes from, z = flags, w = (byte offset in the x1 weight stream) / 16 | rows << 20.
-enum : uint32_t { kUnitFromPe = 1u, kUnitFirst = 8u, kUnitLast = 16u };
-constexpr int kMaxProg = 40;
-constexpr int total_units() {
-  int n = 0;
-  for (int s = 0; s < kNumSteps; ++s) n += num_units(s);
-  return n;
-}
-constexpr int kTileUnits = total_units();
-static_assert(kTileUnits <= kMaxProg, "program area too small");
-
-struct ProgEntry { uint32_t x, y, z, w; };
-struct ProgTable { ProgEntry e[kMaxProg]; };
-constexpr ProgTable make_prog() {
-  ProgTable t{};
-  int i = 0;
-  for (int s = 0; s < kNumSteps; ++s) {
-    const StepInfo si = step_info(s);
-    const int nu = num_units(s);
-    for (int u = 0; u < nu; ++u, ++i) {
-      const UnitInfo ui = unit_info(s, u);
-      uint32_t flags = 0;
-      if (ui.from_pe) flags |= kUnitFromPe;
-      if (u == 0) flags |= kUnitFirst;
-      if (ui.last) flags |= kUnitLast;
-      t.e[i].x = (uint32_t)ui.rows;
-      t.e[i].y = ui.from_pe ? 0u : (uint32_t)(ui.ka - si.pe_first);
-      t.e[i].z = flags;
-      t.e[i].w = ((uint32_t)(step_offset_x1(s) + unit_offset_in_step(s, u)) >> 4) | ((uint32_t)ui.rows << 20);  // rows <= 256
-    }
-  }
-  return t;
-}
-__constant__ ProgTable c_prog = make_prog();
+constexpr int kTileUnits = prog_units(kFwdStream);
+__constant__ ProgTable c_prog = make_prog(kFwdStream);
 
 // The MMAs of one step for this warpgroup's 64 rows: acc0 = output columns [0, 128) (or [0, 16) in acc_s when the step has
-// nh0 == 16), acc1 = [128, 256), acc_s = the 16-column second half of step 6.  Consumes the step's units from the ring.
+// nh0 == 16), acc1 = [128, 256), acc_s = the 16-column second half of step 6.  Consumes the step's units from the ring
+// (exact mode: two slots per unit, hi then lo weights).
 template <bool EXACT>
-__device__ __forceinline__ void mlp_step_mma(int s, int& prog, uint32_t& slot, uint32_t& phase, uint32_t ring, uint32_t bar_full,
-                                             uint32_t bar_empty, uint32_t act_hi, uint32_t act_lo, uint32_t pe_hi, uint32_t pe_lo,
-                                             uint32_t row_off, int lane, float (&acc0)[64], float (&acc1)[64], float (&acc_s)[8]) {
+__device__ __forceinline__ void mlp_step_mma(int s, int& prog, typename SmemMap<EXACT>::WeightRing& ring, uint32_t act_hi,
+                                             uint32_t act_lo, uint32_t pe_hi, uint32_t pe_lo, uint32_t row_off,
+                                             float (&acc0)[64], float (&acc1)[64], float (&acc_s)[8]) {
   constexpr int NPART = EXACT ? 2 : 1;
-  constexpr uint32_t NSLOT = SmemMap<EXACT>::kSlots;
   const StepInfo si = step_info(s);
   for (int u = 0; u < si.k_atoms; ++u, ++prog) {
     const ProgEntry e = c_prog.e[prog];
-    const bool from_pe = (e.z & kUnitFromPe) != 0;
+    const bool from_pe = (e.z & kUnitFromOperand) != 0;
     const uint32_t a_hi = (from_pe ? pe_hi : act_hi + e.y * (kTileM * 128)) + row_off;
     const uint32_t a_lo = (from_pe ? pe_lo : act_lo + e.y * (kTileM * 128)) + row_off;
     const uint64_t dh = wgmma_desc_sw128(a_hi), dl = wgmma_desc_sw128(a_lo);
 #pragma unroll
     for (int part = 0; part < NPART; ++part) {
-      mbar_wait(bar_full + slot * 8, phase);
-      const uint32_t b = ring + slot * kMaxUnitBytes;
+      const uint32_t b = ring.wait_full();
       const uint64_t b0 = wgmma_desc_sw128(b), b1 = wgmma_desc_sw128(b + si.nh0 * 128);
       wgmma_fence();
 #pragma unroll
@@ -149,9 +109,7 @@ __device__ __forceinline__ void mlp_step_mma(int s, int& prog, uint32_t& slot, u
       reg_fence(acc0);
       reg_fence(acc1);
       reg_fence(acc_s);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_empty + slot * 8);  // this warp's reads of the slot are complete
-      if (++slot == NSLOT) { slot = 0; phase ^= 1; }
+      ring.release();
     }
   }
 }
@@ -229,22 +187,12 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
   // Use the dynamic shared array directly (no integer round trip) so the compiler keeps the shared address
   // space and emits LDS/STS instead of generic loads; the swizzled operands need 1024-byte alignment.
   extern __shared__ __align__(1024) uint8_t smem[];
-  const uint32_t smem_base = smem_u32(smem);
-  if ((smem_base & 1023u) != 0u) __trap();
+  const uint32_t smem_base = smem_base_aligned(smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   constexpr int NPART = EXACT ? 2 : 1;
-  constexpr uint32_t NSLOT = M::kSlots;
 
-  const uint32_t bar_full = smem_base + M::kBars;   // [NSLOT]
-  const uint32_t bar_empty = bar_full + NSLOT * 8;  // [NSLOT]: one arrival per row warp
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < (int)NSLOT; ++i) {
-      mbar_init(bar_full + i * 8, 1);
-      mbar_init(bar_empty + i * 8, kRowThreads / 32);
-    }
-    mbar_fence_init();
-  }
+  typename M::WeightRing ring(smem_base + M::kRing, smem_base + M::kBars);
+  if (threadIdx.x == 0) ring.init();
   __syncthreads();
 
   const int n_iter = (p.n_units - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
@@ -255,7 +203,6 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
     // The whole warp runs the (warp-uniform) loop; one elected lane issues the copies.
     reg_dec<kRegsLight>();
     if (warp == 0) {
-      uint32_t slot = 0, phase = 0;
       for (int it = 0; it < n_iter; ++it) {
         for (int t = 0; t < tiles_per_unit; ++t) {
           const uint8_t* base = p.wstream[t < p.tiles_c ? 0 : 1];
@@ -263,16 +210,8 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
             const uint32_t w = c_prog.e[i].w;
             const uint32_t off = (w & 0xFFFFFu) << 4, bytes = (w >> 20) * 128u;
 #pragma unroll
-            for (int part = 0; part < NPART; ++part) {
-              const uint8_t* src = EXACT ? base + 2 * (size_t)off + part * bytes : base + off;
-              mbar_wait(bar_empty + slot * 8, phase ^ 1);
-              if (elect_one()) {
-                mbar_arrive_expect_tx(bar_full + slot * 8, bytes);
-                bulk_g2s(smem_base + M::kRing + slot * kMaxUnitBytes, src, bytes, bar_full + slot * 8);
-              }
-              __syncwarp();
-              if (++slot == NSLOT) { slot = 0; phase ^= 1; }
-            }
+            for (int part = 0; part < NPART; ++part)  // exact mode: the hi unit, then the lo unit
+              ring.produce(EXACT ? base + 2 * (size_t)off + part * bytes : base + off, bytes);
           }
         }
       }
@@ -303,7 +242,6 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
     float4* tile_raw = reinterpret_cast<float4*>(smem + M::kTileRaw);
     const int R = p.rays_per_unit;
     const bool has_bg = p.bg != nullptr;
-    uint32_t slot = 0, phase = 0;
     PhaseTimer tm(p.prof, p.prof != nullptr && etid == 0);
 
     for (int it = 0; it < n_iter; ++it) {
@@ -509,9 +447,8 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
             const int ray0 = prow0 < rows ? prow0 / S : 0, ray1 = prow1 < rows ? prow1 / S : 0;
             for (int s = 0; s < kNumSteps; ++s) {
               const StepInfo si = step_info(s);
-              mlp_step_mma<EXACT>(s, prog, slot, phase, smem_base + M::kRing, bar_full, bar_empty, smem_base + M::kActHi,
-                                  smem_base + M::kActLo, smem_base + M::kPeHi, smem_base + M::kPeLo, (uint32_t)(64 * wg * 128),
-                                  lane, acc0, acc1, acc_s);
+              mlp_step_mma<EXACT>(s, prog, ring, smem_base + M::kActHi, smem_base + M::kActLo, smem_base + M::kPeHi,
+                                  smem_base + M::kPeLo, (uint32_t)(64 * wg * 128), acc0, acc1, acc_s);
               float* dump = (probe && p.dbg_act_step == s) ? p.dbg_act : nullptr;
               const float* bias = bias_n + si.bias_off;
               if (s <= 8) {
@@ -708,14 +645,6 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
       }  // pass
     }    // units
   }
-}
-
-int debug_prog_v4(int index, uint32_t* out) {  // host copy of the per-tile unit program (tests)
-  constexpr ProgTable t = make_prog();
-  if (index < 0) return kTileUnits;
-  if (index >= kTileUnits) return -1;
-  out[0] = t.e[index].x; out[1] = t.e[index].y; out[2] = t.e[index].z; out[3] = t.e[index].w;
-  return 4;
 }
 
 cudaError_t render_kernel_setup() {

@@ -10,7 +10,7 @@
 //                             term.  Also yields d fc_rgb.bias / d sigma-bias sums and the max |gradient| for the scale.
 //   2. chain_kernel           dX chain of the MLP per 128-row tile on wgmma: 9 steps with transposed weight streams,
 //                             same machinery as the forward kernel (register accumulators, shared-memory activations
-//                             overwritten in place, bulk-copy weight ring).  The epilogue applies the saved ReLU masks and
+//                             overwritten in place, the bulk-copy ring of nfb_pipeline.cuh).  The epilogue applies the saved ReLU masks and
 //                             writes every dY as a transposed FP16 image into the tile record.
 //   3. dw_kernel              dW[n,k] = sum_rows dY[row,n] X[row,k] for every layer: both operands are bulk-copied from
 //                             the tile records (K-major images whose K axis is the sample row) and multiplied on wgmma
@@ -27,6 +27,7 @@
 
 #include "nfb_internal.h"
 #include "nfb_layout.h"
+#include "nfb_pipeline.cuh"
 #include "nfb_ptx.cuh"
 #include "nfb_save.cuh"
 
@@ -206,36 +207,16 @@ __global__ void scale_kernel(const unsigned int* __restrict__ absmax, float* __r
 }
 
 // ================================================================================================
-// backward weight stream: unit (step s, K atom) = [N rows x 64 K] FP16, 128-byte swizzled, element (n, k) = W^T
-// ================================================================================================
-struct BwdUnit { int16_t from_op, group, rows, last, ka; };
-__host__ __device__ constexpr BwdUnit bwd_unit_info(int s, int u) {
-  const StepInfo si = bwd_step_info(s);
-  const int hid = u - si.pe_first;
-  return BwdUnit{(int16_t)(si.pe_first && u == 0), (int16_t)((hid >= 2) ? 2 : 1), (int16_t)(si.nh0 + si.nh1),
-                 (int16_t)(u == si.k_atoms - 1), (int16_t)u};
-}
-__host__ __device__ constexpr int bwd_unit_offset(int s, int u) { return bwd_step_offset(s) + u * (bwd_step_info(s).nh0 + bwd_step_info(s).nh1) * 128; }
-
-// (the transposed stream is written by repack_kernel, nfb_pack.cu)
-
-// ================================================================================================
 // 2. dX chain kernel
 // ================================================================================================
 namespace chain {
 
-// 384 threads: warp 0 weight producer (warps 1..3 idle: the register file is re-partitioned per warpgroup), warpgroups 1 and 2
-// compute rows [64w, 64w+64) of the tile on wgmma with register accumulators; their epilogue applies the saved ReLU mask, writes
-// the FP16 result in place into the shared-memory activation buffer (A operand of the next step) and as the transposed dY image
-// into the tile record.
+// Roles as in the forward kernel (nfb_pipeline.cuh): warp 0 streams the transposed weights (kBwdStream, written by
+// repack_kernel in nfb_pack.cu), warpgroups 1 and 2 compute rows [64w, 64w+64) of the tile on wgmma with register
+// accumulators; their epilogue applies the saved ReLU mask, writes the FP16 result in place into the shared-memory activation
+// buffer (A operand of the next step) and as the transposed dY image into the tile record.
 constexpr int kNumSlots = 4;
-constexpr int kThreads = 384;
-constexpr int kRegsLight = 40, kRegsRow = 232;
-static_assert((4 * kRegsLight + 8 * kRegsRow) * 32 <= 65536, "register file");
-template <int N> __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
-template <int N> __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
-constexpr int kRowThreads = 256;
-constexpr uint32_t kRowBarrier = 1;  // both warpgroups; 2 + w: warpgroup w alone
+using WeightRing = Ring<kNumSlots, kMaxUnitBytes>;
 constexpr int kOffRing = 0;
 constexpr int kOffAct = kOffRing + kNumSlots * kMaxUnitBytes;  // 4 K atoms x [128 rows x 128 B]
 constexpr int kOffOp = kOffAct + 4 * kTileM * 128;             // d raw operand: [128 rows x 64 k] FP16, swizzled (k < 4 used)
@@ -243,39 +224,8 @@ constexpr int kOffBars = kOffOp + kTileM * 128;
 constexpr int kSmemBytes = kOffBars + 2 * kNumSlots * 8;
 static_assert(kSmemBytes <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
 
-// Program entry per unit: x = MMA N (rows of the unit), y = K atom of the activation buffer the A operand comes from,
-// z = flags, w = (byte offset in the backward stream) / 16 | rows << 20.
-enum : uint32_t { kFromOp = 1u, kFirst = 8u, kLast = 16u };
-constexpr int total_units() {
-  int n = 0;
-  for (int s = 0; s < kBwdSteps; ++s) n += bwd_step_info(s).k_atoms;
-  return n;
-}
-constexpr int kTileUnits = total_units();  // 28
-struct ProgEntry { uint32_t x, y, z, w; };
-struct ProgTable { ProgEntry e[32]; };
-static_assert(kTileUnits <= 32, "program table too small");
-constexpr ProgTable make_prog() {
-  ProgTable t{};
-  int i = 0;
-  for (int s = 0; s < kBwdSteps; ++s) {
-    const StepInfo si = bwd_step_info(s);
-    const int nu = si.k_atoms;
-    for (int u = 0; u < nu; ++u, ++i) {
-      const BwdUnit ui = bwd_unit_info(s, u);
-      uint32_t flags = 0;
-      if (ui.from_op) flags |= kFromOp;
-      if (u == 0) flags |= kFirst;
-      if (ui.last) flags |= kLast;
-      t.e[i].x = (uint32_t)ui.rows;
-      t.e[i].y = ui.from_op ? 0u : (uint32_t)(u - si.pe_first);
-      t.e[i].z = flags;
-      t.e[i].w = ((uint32_t)bwd_unit_offset(s, u) >> 4) | ((uint32_t)ui.rows << 20);
-    }
-  }
-  return t;
-}
-__constant__ ProgTable c_prog = make_prog();
+constexpr int kTileUnits = prog_units(kBwdStream);  // 28
+__constant__ ProgTable c_prog = make_prog(kBwdStream);
 
 // Epilogue of one 128-column accumulator half: masked gradient -> FP16, in place into the activation buffer and into the
 // record image of dY(L).
@@ -309,20 +259,11 @@ __device__ __forceinline__ void bwd_epi_half(const float (&acc)[64], int L, int 
 
 __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constant__ ChainParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  const uint32_t smem_base = smem_u32(smem);
-  if ((smem_base & 1023u) != 0u) __trap();
+  const uint32_t smem_base = smem_base_aligned(smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  const uint32_t bar_full = smem_base + kOffBars;
-  const uint32_t bar_empty = bar_full + kNumSlots * 8;
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < kNumSlots; ++i) {
-      mbar_init(bar_full + i * 8, 1);
-      mbar_init(bar_empty + i * 8, kRowThreads / 32);
-    }
-    mbar_fence_init();
-  }
+  WeightRing ring(smem_base + kOffRing, smem_base + kOffBars);
+  if (threadIdx.x == 0) ring.init();
   for (int i = threadIdx.x; i < kTileM * 128 / 16; i += kThreads)  // operand chunks 1..7 of every row stay zero
     reinterpret_cast<uint4*>(smem + kOffOp)[i] = make_uint4(0u, 0u, 0u, 0u);
   __syncthreads();
@@ -335,20 +276,12 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
     // ============================== weight producer ==============================
     reg_dec<kRegsLight>();
     if (warp == 0) {
-      uint32_t slot = 0, phase = 0;
       for (int j = 0; j < n_tiles_cta; ++j) {
         const int t = j % tpu;
         const uint8_t* base = p.wstream[t < p.tiles_c ? 0 : 1];
         for (int i = 0; i < kTileUnits; ++i) {
           const uint32_t w = c_prog.e[i].w;
-          const uint32_t off = (w & 0xFFFFFu) << 4, bytes = (w >> 20) * 128u;
-          mbar_wait(bar_empty + slot * 8, phase ^ 1);
-          if (elect_one()) {
-            mbar_arrive_expect_tx(bar_full + slot * 8, bytes);
-            bulk_g2s(smem_base + kOffRing + slot * kMaxUnitBytes, base + off, bytes, bar_full + slot * 8);
-          }
-          __syncwarp();
-          if (++slot == kNumSlots) { slot = 0; phase ^= 1; }
+          ring.produce(base + ((w & 0xFFFFFu) << 4), (w >> 20) * 128u);
         }
       }
     }
@@ -362,7 +295,6 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
     const int r0 = 64 * wg + 16 * q + (lane >> 2);
     const float scale = p.scal[0];
     uint8_t* act = smem + kOffAct;
-    uint32_t slot = 0, phase = 0;
 
     for (int j = 0; j < n_tiles_cta; ++j) {
       const int unit = blockIdx.x + (j / tpu) * gridDim.x;
@@ -400,10 +332,9 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
         float acc0[64], acc1[64];
         for (int u = 0; u < si.k_atoms; ++u, ++prog) {
           const ProgEntry e = c_prog.e[prog];
-          const uint32_t a = ((e.z & kFromOp) ? smem_base + kOffOp : smem_base + kOffAct + e.y * (kTileM * 128)) + 64 * wg * 128;
+          const uint32_t a = ((e.z & kUnitFromOperand) ? smem_base + kOffOp : smem_base + kOffAct + e.y * (kTileM * 128)) + 64 * wg * 128;
           const uint64_t ad = wgmma_desc_sw128(a);
-          mbar_wait(bar_full + slot * 8, phase);
-          const uint32_t b = smem_base + kOffRing + slot * kMaxUnitBytes;
+          const uint32_t b = ring.wait_full();
           const uint64_t b0 = wgmma_desc_sw128(b), b1 = wgmma_desc_sw128(b + 128 * 128);
           wgmma_fence();
 #pragma unroll
@@ -416,9 +347,7 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
           wgmma_wait<0>();
           reg_fence(acc0);
           reg_fence(acc1);
-          __syncwarp();
-          if (lane == 0) mbar_arrive(bar_empty + slot * 8);
-          if (++slot == kNumSlots) { slot = 0; phase ^= 1; }
+          ring.release();
         }
         const int L = 8 - s;  // forward layer whose pre-activation gradient this step produces
         bwd_epi_half(acc0, L, 0, masks, act, rec, r0);
@@ -438,14 +367,11 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
 // ================================================================================================
 namespace dw {
 
-// 384 threads: warp 0 producer (warps 1..3 idle), warpgroups 1 and 2 = output features [64w, 64w+64) of the job's 128 on wgmma,
+// Roles (nfb_pipeline.cuh): warp 0 producer, warpgroups 1 and 2 = output features [64w, 64w+64) of the job's 128 on wgmma,
 // FP32 accumulators in registers over all tiles of the CTA, then reduced into the accumulators in global memory.
-constexpr int kThreads = 384;
-constexpr int kRegsLight = 40, kRegsRow = 232;
-using chain::reg_dec;
-using chain::reg_inc;
 constexpr int kStages = 4;
 constexpr int kStageBytes = 16384 + 32768;       // one r-atom (64 sample rows): A [128 features x 128 B], B [<=256 features x 128 B]
+using StageRing = Ring<kStages, kStageBytes>;
 constexpr int kOffOnes = kStages * kStageBytes;  // [16 rows x 64 r]: row 0 = 1.0 (bias = column sums of dY)
 constexpr int kOffBars = kOffOnes + 2048;
 constexpr int kSmemBytes = kOffBars + 2 * kStages * 8;
@@ -511,8 +437,8 @@ template <int N> __device__ __forceinline__ void mma_n(float (&d)[N / 2], uint64
 // One job over the CTA's tiles j0..j1 for this warpgroup's 64 output features: NB = N of the B image (<= 128 per accumulator;
 // 256 runs as two 128-column halves).
 template <int NB>
-__device__ __forceinline__ void run_job(const Job& J, int j0, int j1, uint32_t smem_base, uint32_t bar_full, uint32_t bar_empty,
-                                        uint32_t& stage, uint32_t& phase, int wg, int lane, float* acc_net, float inv) {
+__device__ __forceinline__ void run_job(const Job& J, int j0, int j1, uint32_t smem_base, StageRing& ring, int wg, int lane,
+                                        float* acc_net, float inv) {
   constexpr int NA = NB > 128 ? 128 : NB;
   constexpr int NH = NB > 128 ? 2 : 1;
   float acc[NH][NA / 2];
@@ -521,8 +447,7 @@ __device__ __forceinline__ void run_job(const Job& J, int j0, int j1, uint32_t s
   const uint64_t ones = wgmma_desc_sw128(smem_base + kOffOnes);
   for (int j = j0; j < j1; ++j) {
     for (int a = 0; a < 2; ++a) {
-      mbar_wait(bar_full + stage * 8, phase);
-      const uint32_t sa = smem_base + stage * kStageBytes, sb = sa + 16384;
+      const uint32_t sa = ring.wait_full(), sb = sa + 16384;
       const uint64_t ad = wgmma_desc_sw128(sa + 64 * wg * 128);
       wgmma_fence();
 #pragma unroll
@@ -537,9 +462,7 @@ __device__ __forceinline__ void run_job(const Job& J, int j0, int j1, uint32_t s
 #pragma unroll
       for (int h = 0; h < NH; ++h) reg_fence(acc[h]);
       reg_fence(accb);
-      __syncwarp();
-      if (lane == 0) mbar_arrive(bar_empty + stage * 8);
-      if (++stage == kStages) { stage = 0; phase ^= 1; }
+      ring.release();
     }
   }
   const int c = lane & 3, r0 = 64 * wg + 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2);
@@ -561,8 +484,7 @@ __device__ __forceinline__ void run_job(const Job& J, int j0, int j1, uint32_t s
 
 __global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__ DwParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
-  const uint32_t smem_base = smem_u32(smem);
-  if ((smem_base & 1023u) != 0u) __trap();
+  const uint32_t smem_base = smem_base_aligned(smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // this CTA: network x job group (blockIdx.x % kGroups) x a contiguous share of the network's tiles
@@ -579,16 +501,8 @@ __global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__
   if (part >= parts || j0 >= j1) return;  // uniform for the whole CTA
   const int job0 = c_jobs.group_begin[group], job1 = c_jobs.group_begin[group + 1];
 
-  const uint32_t bar_full = smem_base + kOffBars;      // [kStages]
-  const uint32_t bar_empty = bar_full + kStages * 8;   // [kStages]: one arrival per consumer warp
-
-  if (threadIdx.x == 0) {
-    for (int i = 0; i < kStages; ++i) {
-      mbar_init(bar_full + i * 8, 1);
-      mbar_init(bar_empty + i * 8, 8);
-    }
-    mbar_fence_init();
-  }
+  StageRing ring(smem_base, smem_base + kOffBars);
+  if (threadIdx.x == 0) ring.init();
   for (int i = threadIdx.x; i < 2048 / 4; i += kThreads)  // row 0 (first 128 bytes) = FP16 ones, rows 1..15 = 0
     reinterpret_cast<uint32_t*>(smem + kOffOnes)[i] = (i < 32) ? 0x3C003C00u : 0u;
   fence_proxy_async_smem();
@@ -603,23 +517,14 @@ __global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__
     // ============================== producer ==============================
     reg_dec<kRegsLight>();
     if (warp == 0) {
-      uint32_t stage = 0, phase = 0;
       for (int job = job0; job < job1; ++job) {
         const Job J = c_jobs.j[job];
         const uint32_t b_bytes = (uint32_t)J.b_rows * 128u;
         for (int j = j0; j < j1; ++j) {
           const uint8_t* rec = tile_rec(j);
-          for (int a = 0; a < 2; ++a) {
-            mbar_wait(bar_empty + stage * 8, phase ^ 1);
-            if (elect_one()) {
-              const uint32_t sa = smem_base + stage * kStageBytes, sb = sa + 16384;
-              mbar_arrive_expect_tx(bar_full + stage * 8, 16384 + b_bytes);
-              bulk_g2s(sa, rec + J.a_off + a * J.a_rows * 128 + J.a_half * 16384, 16384, bar_full + stage * 8);
-              bulk_g2s(sb, rec + J.b_off + a * J.b_rows * 128, b_bytes, bar_full + stage * 8);
-            }
-            __syncwarp();
-            if (++stage == kStages) { stage = 0; phase ^= 1; }
-          }
+          for (int a = 0; a < 2; ++a)  // one stage = the A and the B image of one r-atom
+            ring.produce(rec + J.a_off + a * J.a_rows * 128 + J.a_half * 16384, 16384, 16384, rec + J.b_off + a * J.b_rows * 128,
+                         b_bytes);
         }
       }
     }
@@ -629,15 +534,14 @@ __global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__
     const int wg = (warp - 4) >> 2;
     const float inv = p.scal[1];
     float* acc_net = p.acc[net];
-    uint32_t stage = 0, phase = 0;
     for (int job = job0; job < job1; ++job) {
       const Job J = c_jobs.j[job];
       switch (J.b_rows) {
-        case 16: run_job<16>(J, j0, j1, smem_base, bar_full, bar_empty, stage, phase, wg, lane, acc_net, inv); break;
-        case 32: run_job<32>(J, j0, j1, smem_base, bar_full, bar_empty, stage, phase, wg, lane, acc_net, inv); break;
-        case 64: run_job<64>(J, j0, j1, smem_base, bar_full, bar_empty, stage, phase, wg, lane, acc_net, inv); break;
-        case 128: run_job<128>(J, j0, j1, smem_base, bar_full, bar_empty, stage, phase, wg, lane, acc_net, inv); break;
-        default: run_job<256>(J, j0, j1, smem_base, bar_full, bar_empty, stage, phase, wg, lane, acc_net, inv); break;
+        case 16: run_job<16>(J, j0, j1, smem_base, ring, wg, lane, acc_net, inv); break;
+        case 32: run_job<32>(J, j0, j1, smem_base, ring, wg, lane, acc_net, inv); break;
+        case 64: run_job<64>(J, j0, j1, smem_base, ring, wg, lane, acc_net, inv); break;
+        case 128: run_job<128>(J, j0, j1, smem_base, ring, wg, lane, acc_net, inv); break;
+        default: run_job<256>(J, j0, j1, smem_base, ring, wg, lane, acc_net, inv); break;
       }
     }
   }
@@ -654,7 +558,7 @@ struct FinArgs {
   const float* acc;    // this network's accumulators
   const float* cond;   // [108] = [expression / 3 ; latent]
 };
-__device__ __forceinline__ int fin_numel(int t) {
+__host__ __device__ __forceinline__ int fin_numel(int t) {
   switch (t) {
     case 0: return 256 * 171;
     case 6: return 256 * 427;
@@ -798,13 +702,6 @@ __device__ void latent_grad_block(const FinAll& f) {  // one block of 256 thread
 // ================================================================================================
 // host-side launchers
 // ================================================================================================
-int debug_prog_chain(int index, uint32_t* out) {
-  constexpr chain::ProgTable t = chain::make_prog();
-  if (index < 0) return chain::kTileUnits;
-  if (index >= chain::kTileUnits) return -1;
-  out[0] = t.e[index].x; out[1] = t.e[index].y; out[2] = t.e[index].z; out[3] = t.e[index].w;
-  return 4;
-}
 int debug_jobs_dw(int index, uint32_t* out) {
   constexpr dw::JobTable t = dw::make_jobs();
   if (index < 0) return dw::kNumJobs;
@@ -836,7 +733,7 @@ cudaError_t launch_composite_bwd(const CompBwdParams& q, float* scal, cudaStream
 cudaError_t launch_chain(const ChainParams& p, int num_sms, cudaStream_t st, long long* launches) {
   const int grid = p.n_units < num_sms ? p.n_units : num_sms;
   if (grid <= 0) return cudaSuccess;
-  chain::chain_kernel<<<grid, chain::kThreads, chain::kSmemBytes, st>>>(p);
+  chain::chain_kernel<<<grid, kThreads, chain::kSmemBytes, st>>>(p);
   ++*launches;
   return cudaGetLastError();
 }
@@ -870,25 +767,9 @@ cudaError_t launch_dw(const DwParams& p_in, int num_sms, cudaStream_t st, long l
   if (tot0 + tot1 <= 0) return cudaSuccess;
   dw_split(num_sms, tot0, tot1, &p.parts[0], &p.parts[1]);
   if (p.parts[0] + p.parts[1] < 1) return cudaSuccess;
-  dw::dw_kernel<<<(p.parts[0] + p.parts[1]) * dw::kGroups, dw::kThreads, dw::kSmemBytes, st>>>(p);
+  dw::dw_kernel<<<(p.parts[0] + p.parts[1]) * dw::kGroups, kThreads, dw::kSmemBytes, st>>>(p);
   ++*launches;
   return cudaGetLastError();
-}
-
-static int fin_numel_host(int t) {
-  switch (t) {
-    case 0: return 256 * 171;
-    case 6: return 256 * 427;
-    case 2: case 4: case 8: case 10: case 12: return 65536;
-    case 1: case 3: case 5: case 7: case 9: case 11: case 13: case 14: return 256;
-    case 15: return 1;
-    case 16: return 128 * 280;
-    case 18: case 20: return 128 * 128;
-    case 17: case 19: case 21: return 128;
-    case 24: return 3 * 128;
-    case 25: return 3;
-    default: return 0;
-  }
 }
 
 // Chain rule through the folds for one or both networks + d latent, two launches in all.
@@ -905,7 +786,7 @@ cudaError_t launch_finalize_all(const float* const params_c[26], float* const gr
   f.net[0].acc = acc_c; f.net[1].acc = acc_f;
   f.net[0].cond = f.net[1].cond = cond;
   int blocks = 1;  // + the latent block
-  for (int t = 0; t < 26; ++t) blocks += (fin_numel_host(t) + 255) / 256;
+  for (int t = 0; t < 26; ++t) blocks += (fin_numel(t) + 255) / 256;
   finalize_kernel<<<dim3(blocks, f.nets), 256, 0, st>>>(f);
   ++*launches;
   fin_dir0_kernel<<<dim3((128 * 256 + 256) * 32 / 256, f.nets), 256, 0, st>>>(f);
