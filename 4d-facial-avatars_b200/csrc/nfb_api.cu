@@ -57,6 +57,10 @@ struct NfbHandle {
     // backward re-runs the training forward chunk by chunk from the saved launch parameters (the caller keeps the inputs alive)
     bool chunked = false;
     nfb::RenderParams full;      // the forward call's parameters (pointers into caller memory)
+    // handle-owned state `full` points at, copied at the forward: the folded per-frame biases (nfb_set_frame overwrites
+    // bias_frame in place) and the linspace tables when they came from the handle's cache (a later sample count replaces it)
+    float* bias[2] = {nullptr, nullptr};
+    float *lin_c = nullptr, *lin_f = nullptr; size_t cap_lin_c = 0, cap_lin_f = 0;
     int chunk_rays = 0, precision = 0;
     float* scratch_out = nullptr; size_t scratch_cap = 0;   // [11 * chunk_rays] outputs of the re-run forwards (discarded)
   } tr;
@@ -164,8 +168,9 @@ int nfb_destroy(NfbHandle* h) {
     nfb::NetBuffers& nb = h->net[n];
     cudaFree(nb.stream_x1); cudaFree(nb.stream_x3); cudaFree(nb.w6); cudaFree(nb.b6); cudaFree(nb.bias_static);
     cudaFree(nb.bias_frame); cudaFree(nb.w0c); cudaFree(nb.w3c); cudaFree(nb.wd0b_t); cudaFree(nb.stream_bwd);
-    cudaFree(h->tr.acc[n]);
+    cudaFree(h->tr.acc[n]); cudaFree(h->tr.bias[n]);
   }
+  cudaFree(h->tr.lin_c); cudaFree(h->tr.lin_f);
   cudaFree(h->tr.rec); cudaFree(h->tr.draw); cudaFree(h->tr.z_c); cudaFree(h->tr.raw_c); cudaFree(h->tr.z_f); cudaFree(h->tr.raw_f);
   cudaFree(h->tr.dnorm); cudaFree(h->tr.scal); cudaFree(h->tr.cond); cudaFree(h->tr.scratch_out); cudaFree(h->cond);
   cudaFree(h->minmax); cudaFree(h->smp_runs); cudaFree(h->smp_segs); cudaFree(h->smp_first);
@@ -372,6 +377,23 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
       tr.chunk_rays = (int)(units * p.rays_per_unit);
       tr.full = p;
       tr.precision = exact ? 1 : 0;
+      // the re-run forwards must read THIS call's frame and depth tables, whatever is rendered before the backward
+      for (int n = 0; n < (nf > 0 ? 2 : 1); ++n) {
+        if (!tr.bias[n]) NFB_CUDA(dev_alloc(&tr.bias[n], nfb::kBiasFloats));
+        NFB_CUDA(cudaMemcpyAsync(tr.bias[n], h->net[n].bias_frame, nfb::kBiasFloats * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        tr.full.bias[n] = tr.bias[n];
+      }
+      if (nf == 0) tr.full.bias[1] = tr.full.bias[0];
+      if (p.t_coarse == h->lin_c) {
+        if ((rc = ensure_cap(&tr.lin_c, &tr.cap_lin_c, (size_t)nc))) return rc;
+        NFB_CUDA(cudaMemcpyAsync(tr.lin_c, h->lin_c, nc * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        tr.full.t_coarse = tr.lin_c;
+      }
+      if (nf > 0 && p.u_fine == h->lin_f) {
+        if ((rc = ensure_cap(&tr.lin_f, &tr.cap_lin_f, (size_t)nf))) return rc;
+        NFB_CUDA(cudaMemcpyAsync(tr.lin_f, h->lin_f, nf * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        tr.full.u_fine = tr.lin_f;
+      }
     } else if ((rc = ensure_train_buffers(tr, n, tiles, nc, nf))) return rc;
     // a later nfb_set_frame (e.g. a validation render before the backward) must not change what the backward differentiates
     NFB_CUDA(cudaMemcpyAsync(tr.cond, h->cond, nfb::kDimCond * sizeof(float), cudaMemcpyDeviceToDevice, st));

@@ -143,7 +143,14 @@ __device__ __forceinline__ uint32_t pack_f16x2(float lo_elem, float hi_elem) {
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));
   return r;
 }
-// Same with ReLU fused into the conversion (negative inputs and NaN become +0).
+// Same without saturation: a value beyond the FP16 range becomes +-inf.  The backward chain uses it for its loss-scaled
+// gradients, where a clamp to 65504 would turn an overflow into finite, wrong parameter gradients.
+__device__ __forceinline__ uint32_t pack_f16x2_inf(float lo_elem, float hi_elem) {
+  uint32_t r;
+  asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));
+  return r;
+}
+// Same as pack_f16x2 with ReLU fused into the conversion (negative inputs and NaN become +0).
 __device__ __forceinline__ uint32_t pack_relu_f16x2(float lo_elem, float hi_elem) {
   uint32_t r;
   asm("cvt.rn.relu.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));

@@ -245,7 +245,7 @@ __device__ __forceinline__ void bwd_epi_half(const float (&acc)[64], int L, int 
       const uint32_t bits = mw[cc >> 5] >> (cc & 31);
       const float a0 = (bits & 1u) ? acc[4 * j + 2 * hh] : 0.f;
       const float a1 = (bits & 2u) ? acc[4 * j + 2 * hh + 1] : 0.f;
-      const uint32_t h = pack_f16x2(a0, a1);
+      const uint32_t h = pack_f16x2_inf(a0, a1);  // an overflow stays visible (non-finite gradients)
       const int col = c_base + cc;
       *reinterpret_cast<uint32_t*>(act + (col >> 6) * (kTileM * 128) + sw128_offset(R, col & 63)) = h;
       if (rec) {
@@ -305,7 +305,7 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
       if (ch == 0) {
         float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
         if (real) d = reinterpret_cast<const float4*>(p.draw)[gt * 128 + row];
-        const uint32_t h01 = pack_f16x2(d.x * scale, d.y * scale), h23 = pack_f16x2(d.z * scale, d.w * scale);
+        const uint32_t h01 = pack_f16x2_inf(d.x * scale, d.y * scale), h23 = pack_f16x2_inf(d.z * scale, d.w * scale);
         *reinterpret_cast<uint4*>(smem + kOffOp + row * 128 + ((0 ^ (row & 7)) << 4)) = make_uint4(h01, h23, 0u, 0u);
         if (real) {
           uint8_t* img = rec + kRecDRaw + img_row_base(16, row);

@@ -160,8 +160,10 @@ int nfb_render_forward(NfbHandle* h, const NfbRays* rays, const NfbSampling* sam
 /* ---- Training (replaces torch.autograd over the unfused graph, train_transformed_rays.py:389) ----
  * nfb_render_forward_train is nfb_render_forward that additionally keeps, in buffers owned by the handle, what the
  * backward needs: per-sample depths, colours and ReLU inputs of both passes, and per 128-row tile the FP16 activations
- * of every layer (about 1 MiB per tile; 2048 rays at 64+64 samples = 3 GiB).  The next nfb_render_backward on the same
- * handle consumes that state; weights must not be re-loaded in between.
+ * of every layer (about 1 MiB per tile; 2048 rays at 64+64 samples = 3 GiB).  nfb_render_backward on the same handle
+ * consumes that state.  Between the two, nfb_set_frame and nfb_render_forward calls (e.g. a validation render of another
+ * frame, with other sample counts) are allowed and do not change what is differentiated; re-loading weights
+ * (nfb_load_weights, nfb_repack) is not.
  * Memory: when the records of the whole call would exceed the budget (environment NFB_TRAIN_MEM_MB, default 60 % of the free
  * device memory) — e.g. a full frame rendered with gradients enabled — the forward only renders (evaluation kernel) and the
  * backward re-runs the training forward chunk by chunk inside the budget: same gradients, one extra forward; the caller must
@@ -185,6 +187,9 @@ typedef struct {
  * nfb_load_weights; `grads_*` receive dL/dparam with the same shapes (entries 22, 23 = layers_dir.3.*, unused by the
  * forward, models.py:257: may be NULL and are never written).  `grad_latent` [32] receives dL/d latent_code (NULL: skipped);
  * the sample depths carry no gradient (z_samples.detach(), train_utils.py:124).  Gradients are OVERWRITTEN, not accumulated.
+ * The call may be repeated on one saved forward with other output gradients (each call starts from zeroed accumulators).
+ * A non-finite output gradient gives non-finite parameter gradients, as autograd does; so does a loss-scaled FP16 gradient
+ * that overflows inside the dX chain (it is not clamped).
  * params_fine / grads_fine may be NULL when the forward had num_fine == 0. */
 int nfb_render_backward(NfbHandle* h, const NfbOutGrads* out_grads, const float* const params_coarse[26],
                         const float* const params_fine[26], float* const grads_coarse[26], float* const grads_fine[26],
