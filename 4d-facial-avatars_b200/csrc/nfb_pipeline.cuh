@@ -28,11 +28,15 @@ __device__ __forceinline__ uint32_t smem_base_aligned(const uint8_t* smem) {
 
 // A ring of SLOTS shared-memory slots, STRIDE bytes apart from `base`, with a full and an empty mbarrier per slot at `bars`
 // (2 * SLOTS * 8 bytes).  Every thread keeps its own copy of the position (slot, phase); the producer warp and every consumer
-// warp walk the slots in the same order.
+// warp walk the slots in the same order.  A consumer has two cursors: `slot` (the next slot to wait on) and `rel` (the oldest
+// slot it has read but not yet released), so it may hold up to kLag + 1 slots: it issues the MMAs of unit u + 1 before it
+// waits for those of unit u and releases u's slot.  With one slot there is nothing to read ahead into, so kLag = 0.
 template <int SLOTS, int STRIDE>
 struct Ring {
+  static constexpr int kLag = SLOTS >= 2 ? 1 : 0;
   uint32_t base, bars;
   uint32_t slot = 0, phase = 0;
+  uint32_t rel = 0;
 
   __device__ __forceinline__ Ring(uint32_t base_, uint32_t bars_) : base(base_), bars(bars_) {}
 
@@ -59,17 +63,19 @@ struct Ring {
     });
   }
 
-  // Consumer, the whole warp: wait until the current slot is full; returns its shared address.
-  __device__ __forceinline__ uint32_t wait_full() const {
+  // Consumer, the whole warp: wait until the next slot is full; returns its shared address.
+  __device__ __forceinline__ uint32_t wait_full() {
     mbar_wait(full_bar(slot), phase);
-    return base + slot * STRIDE;
+    const uint32_t addr = base + slot * STRIDE;
+    advance();
+    return addr;
   }
-  // Consumer, the whole warp, once this warp's reads of the slot are complete (its wgmma waited on): one lane releases the
-  // slot to the producer.
+  // Consumer, the whole warp, once this warp's reads of the oldest unreleased slot are complete (its wgmma waited on): one
+  // lane releases that slot to the producer.
   __device__ __forceinline__ void release() {
     __syncwarp();
-    if ((threadIdx.x & 31) == 0) mbar_arrive(empty_bar(slot));
-    advance();
+    if ((threadIdx.x & 31) == 0) mbar_arrive(empty_bar(rel));
+    if (++rel == SLOTS) rel = 0;
   }
 
  private:

@@ -12,10 +12,13 @@
 // Work decomposition.  A "unit of work" is R (1 or 2) rays.  One CTA per SM loops over them; per unit it runs the coarse
 // pass (R*Nc sample rows) and the fine pass (R*(Nc+Nf) rows) as 128-row tiles.  Per tile the MLP is 10 GEMM steps
 // (nfb_layout.h), each on wgmma: warpgroup w computes rows [64w, 64w+64) of the tile with its FP32 accumulators in
-// registers; its epilogue (bias, ReLU, FP16 hi[/lo] split) writes the rows back IN PLACE into the shared-memory activation
-// buffer the step has just finished reading — the A operand of the next step — so hidden activations never leave the SM.
+// registers.  Its epilogue (bias, ReLU, FP16 conversion) produces the A operand of the next step: in fast mode as packed
+// register fragments (an m64nN accumulator fragment is, packed to f16x2, the A fragment of the next register-A wgmma), in
+// exact mode as hi and lo halves written back in place into the shared-memory activation buffer the step has just finished
+// reading.  Either way hidden activations never leave the SM.  In fast mode the steps are unrolled at compile time, so each
+// weight unit's wgmmas are issued as one batch, and one unit stays in flight while the next is issued.
 // Weights stream L2 -> shared memory through the bulk-copy (TMA) engine into a ring of pre-swizzled 32 KB units
-// ([N rows x 64 K], the layout a wgmma shared-memory descriptor reads): 3 slots in fast mode, 1 in exact mode, whose hi+lo
+// ([N rows x 64 K], the layout a wgmma shared-memory descriptor reads): 5 slots in fast mode, 1 in exact mode, whose hi+lo
 // activation buffers take the space.
 //
 // Warp roles (nfb_pipeline.cuh): warp 0 = weight producer, warpgroups 1 and 2 = "row" warps.  For the per-row work
@@ -36,15 +39,17 @@ namespace nfb {
 
 constexpr int kRowsMax = 512;   // sample rows of one pass of one unit of work
 
-// shared memory map (bytes from the 1024-aligned base).  Activation buffers: 4 K atoms x [128 rows x 128 B], swizzled.
+// shared memory map (bytes from the 1024-aligned base).  Activation buffers (exact mode only; fast mode keeps the hidden
+// activations in registers): 4 K atoms x [128 rows x 128 B], swizzled.
 template <bool EXACT>
 struct SmemMap {
-  static constexpr int kSlots = EXACT ? 1 : 3;
+  static constexpr int kSlots = EXACT ? 1 : 5;
   using WeightRing = Ring<kSlots, kMaxUnitBytes>;
+  static constexpr int kActBytes = EXACT ? 4 * kTileM * 128 : 0;
   static constexpr int kRing = 0;
   static constexpr int kActHi = kRing + kSlots * kMaxUnitBytes;
-  static constexpr int kActLo = kActHi + 4 * kTileM * 128;
-  static constexpr int kPeHi = kActLo + (EXACT ? 4 * kTileM * 128 : 0);
+  static constexpr int kActLo = kActHi + kActBytes;
+  static constexpr int kPeHi = kActLo + kActBytes;
   static constexpr int kPeLo = kPeHi + kTileM * 128;
   static constexpr int kRaw = kPeLo + (EXACT ? kTileM * 128 : 0);
   static constexpr int kZ = kRaw + kRowsMax * 16;
@@ -64,65 +69,132 @@ struct SmemMap {
 constexpr int kTileUnits = prog_units(kFwdStream);
 __constant__ ProgTable c_prog = make_prog(kFwdStream);
 
-// The MMAs of one step for this warpgroup's 64 rows: acc0 = output columns [0, 128) (or [0, 16) in acc_s when the step has
+// A compile-time MLP step: converts to its index, and keeps it usable as a constant expression (Step::value).
+template <int V>
+struct StepC {
+  static constexpr int value = V;
+  __device__ constexpr operator int() const { return V; }
+};
+// Calls f(StepC<I>{}) for I = B, ..., E - 1: the MLP steps as compile-time constants, so that each step's MMA issue and
+// epilogue are straight-line code.
+template <int B, int E, class F>
+__device__ __forceinline__ void static_for(F&& f) {
+  if constexpr (B < E) {
+    f(StepC<B>{});
+    static_for<B + 1, E>(f);
+  }
+}
+
+// m64nNk16 wgmma into a 128- or 16-column accumulator, A from a shared-memory descriptor or from four register fragments.
+__device__ __forceinline__ void mma_ss(float (&d)[64], uint64_t a, uint64_t b, uint32_t accf) { wgmma_n128(d, a, b, accf); }
+__device__ __forceinline__ void mma_ss(float (&d)[8], uint64_t a, uint64_t b, uint32_t accf) { wgmma_n16(d, a, b, accf); }
+__device__ __forceinline__ void mma_rs(float (&d)[64], const uint32_t* a, uint64_t b, uint32_t accf) {
+  wgmma_rs_n128(d, a[0], a[1], a[2], a[3], b, accf);
+}
+__device__ __forceinline__ void mma_rs(float (&d)[8], const uint32_t* a, uint64_t b, uint32_t accf) {
+  wgmma_rs_n16(d, a[0], a[1], a[2], a[3], b, accf);
+}
+
+// The MMAs of step `step` for this warpgroup's 64 rows: acc0 = output columns [0, 128) (or [0, 16) in acc_s when the step has
 // nh0 == 16), acc1 = [128, 256), acc_s = the 16-column second half of step 6.  Consumes the step's units from the ring
-// (exact mode: two slots per unit, hi then lo weights).
-template <bool EXACT>
-__device__ __forceinline__ void mlp_step_mma(int s, int& prog, typename SmemMap<EXACT>::WeightRing& ring, uint32_t act_hi,
-                                             uint32_t act_lo, uint32_t pe_hi, uint32_t pe_lo, uint32_t row_off,
-                                             float (&acc0)[64], float (&acc1)[64], float (&acc_s)[8]) {
+// (exact mode: two slots per unit, hi then lo weights), each slot's wgmmas issued as one batch.  The ring's kLag batches
+// stay in flight: a slot is released once the batch after it has been issued and its own batch waited on.  On return every
+// MMA of the step is complete.
+// A operand: the PE buffer for the step's PE atom; otherwise the activation buffer (exact mode) or the packed fragments the
+// previous step's epilogue left in registers (fast mode: act[16 a + 4 ks + i] = fragment register i of K atom a, K slice ks).
+// `step` is a StepC in fast mode (the steps unrolled, each unit's wgmmas one straight-line batch) and a
+// runtime int in exact mode, whose steps stay a loop: exact mode gains nothing from the unrolling but code size.
+template <bool EXACT, class Step, class WeightRing>
+__device__ __forceinline__ void mlp_step_mma(Step step, WeightRing& ring, uint32_t act_hi, uint32_t act_lo, uint32_t pe_hi, uint32_t pe_lo,
+                                             uint32_t row_off, uint32_t (&act)[64], float (&acc0)[64], float (&acc1)[64],
+                                             float (&acc_s)[8], PhaseTimer& tm) {
   constexpr int NPART = EXACT ? 2 : 1;
-  const StepInfo si = step_info(s);
-  for (int u = 0; u < si.k_atoms; ++u, ++prog) {
-    const ProgEntry e = c_prog.e[prog];
-    const bool from_pe = (e.z & kUnitFromOperand) != 0;
-    const uint32_t a_hi = (from_pe ? pe_hi : act_hi + e.y * (kTileM * 128)) + row_off;
-    const uint32_t a_lo = (from_pe ? pe_lo : act_lo + e.y * (kTileM * 128)) + row_off;
+  constexpr int kLag = WeightRing::kLag;
+  const StepInfo si = step_info(step);
+  asm volatile("" : "+r"(row_off));  // as in epi_half: the operand descriptors are formed per step, not hoisted and held
+#pragma unroll
+  for (int u = 0; u < si.k_atoms; ++u) {
+    const bool from_pe = si.pe_first && u == 0;
+    const bool rs = !EXACT && !from_pe;
+    const int atom = u - si.pe_first;
+    const uint32_t a_hi = (from_pe ? pe_hi : act_hi + atom * (kTileM * 128)) + row_off;
+    const uint32_t a_lo = (from_pe ? pe_lo : act_lo + atom * (kTileM * 128)) + row_off;
     const uint64_t dh = wgmma_desc_sw128(a_hi), dl = wgmma_desc_sw128(a_lo);
 #pragma unroll
     for (int part = 0; part < NPART; ++part) {
       const uint32_t b = ring.wait_full();
+      tm.lap(10);
       const uint64_t b0 = wgmma_desc_sw128(b), b1 = wgmma_desc_sw128(b + si.nh0 * 128);
       wgmma_fence();
 #pragma unroll
       for (int ks = 0; ks < 4; ++ks) {
         const uint32_t accf = (u | part | ks) ? 1u : 0u;
         const uint64_t ah = dh + (uint64_t)(ks * 2), al = dl + (uint64_t)(ks * 2);
+        const uint32_t* af = act + (rs ? 16 * atom + 4 * ks : 0);
+        auto mma = [&](auto& d, uint64_t bd) {
+          if (rs) {
+            mma_rs(d, af, bd, accf);
+          } else {
+            mma_ss(d, ah, bd, accf);
+            if (EXACT && part == 0) mma_ss(d, al, bd, 1u);
+          }
+        };
         const uint64_t bh0 = b0 + (uint64_t)(ks * 2), bh1 = b1 + (uint64_t)(ks * 2);
         if (si.nh0 == 16) {
-          wgmma_n16(acc_s, ah, bh0, accf);
-          if (EXACT && part == 0) wgmma_n16(acc_s, al, bh0, 1u);
+          mma(acc_s, bh0);
         } else {
-          wgmma_n128(acc0, ah, bh0, accf);
-          if (EXACT && part == 0) wgmma_n128(acc0, al, bh0, 1u);
-          if (si.nh1 == 128) {
-            wgmma_n128(acc1, ah, bh1, accf);
-            if (EXACT && part == 0) wgmma_n128(acc1, al, bh1, 1u);
-          } else if (si.nh1 == 16) {
-            wgmma_n16(acc_s, ah, bh1, accf);
-            if (EXACT && part == 0) wgmma_n16(acc_s, al, bh1, 1u);
-          }
+          mma(acc0, bh0);
+          if (si.nh1 == 128) mma(acc1, bh1);
+          else if (si.nh1 == 16) mma(acc_s, bh1);
         }
       }
       wgmma_commit();
-      wgmma_wait<0>();
-      reg_fence(acc0);
-      reg_fence(acc1);
-      reg_fence(acc_s);
-      ring.release();
+      if (u * NPART + part >= kLag) {
+        wgmma_wait<kLag>();
+        reg_fence(acc0);
+        reg_fence(acc1);
+        reg_fence(acc_s);
+        ring.release();
+      }
+      tm.lap(11);
     }
   }
+  if constexpr (kLag > 0) {
+    wgmma_wait<0>();
+    reg_fence(acc0);
+    reg_fence(acc1);
+    reg_fence(acc_s);
+    ring.release();
+    tm.lap(11);
+  }
+  // The fragments were read asynchronously: the epilogue overwrites them only from here.
+  if constexpr (!EXACT) reg_fence<16 * (step_info(Step::value).k_atoms - step_info(Step::value).pe_first)>(act);
 }
 
 // Epilogue of one 128-column accumulator half (columns [c_base, c_base + 128)) of a ReLU layer: + bias (+ the per-ray
-// direction term of step 6), ReLU, FP16 hi (and lo) written in place into the activation buffer; the training record image
-// and ReLU mask of the layer (SAVE), and the layer probe dump.
+// direction term of step 6), ReLU, FP16 hi (and lo) written in place into the activation buffer (exact mode) or packed
+// into the A fragments of the next step (fast mode: act[c_base / 4 + 2 j + hh] holds columns c_base + 8 j + 2 c, +1 of
+// row r0 + 8 hh); the training record image and ReLU mask of the layer (SAVE), and the layer probe dump.
 template <bool EXACT, bool SAVE>
 __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_base, const float* __restrict__ bias,
                                          const float* dirb0, const float* dirb1, uint8_t* act_hi, uint8_t* act_lo,
-                                         int r0, uint8_t* rec, float* dump) {
-  const int lane = threadIdx.x & 31, c = lane & 3;
+                                         uint32_t (&act)[64], int r0, uint8_t* rec, float* dump) {
+  int c = threadIdx.x & 3;
+  // Fast mode unrolls the steps: without this the compiler hoists the per-thread addresses of all ten epilogues out of the
+  // tile loop and keeps them in registers (spilling) across the MMAs.
+  asm volatile("" : "+r"(r0), "+r"(c));
   uint32_t mask[2][4] = {{0u, 0u, 0u, 0u}, {0u, 0u, 0u, 0u}};
+  // SAVE: byte offset of element (feature col, sample R) of the layer's transposed record image is
+  // img_offset(W, col, R) = (c_base + 8 j) * 128 + img_base[hh][e] for col = c_base + 8 j + 2 c + e, R = r0 + 8 hh, since
+  // col & 7 == 2 c + e for every j: one base per (hh, e) and compile-time offsets, instead of the full swizzle per element.
+  int img_base[2][2] = {{0, 0}, {0, 0}};
+  if constexpr (SAVE) {
+    const int W = rec_width(s);
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh)
+#pragma unroll
+      for (int e = 0; e < 2; ++e) img_base[hh][e] = img_offset(W, 2 * c + e, r0 + 8 * hh);
+  }
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     const int col = c_base + 8 * j + 2 * c;
@@ -143,15 +215,19 @@ __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_ba
       } else {
         hi = pack_relu_f16x2(x0, x1);
       }
-      const int off = (col >> 6) * (kTileM * 128) + sw128_offset(R, col & 63);
-      *reinterpret_cast<uint32_t*>(act_hi + off) = hi;
-      if constexpr (EXACT) *reinterpret_cast<uint32_t*>(act_lo + off) = lo;
+      if constexpr (EXACT) {
+        const int off = (col >> 6) * (kTileM * 128) + sw128_offset(R, col & 63);
+        *reinterpret_cast<uint32_t*>(act_hi + off) = hi;
+        *reinterpret_cast<uint32_t*>(act_lo + off) = lo;
+      } else {
+        act[c_base / 4 + 2 * j + hh] = hi;
+      }
       if constexpr (SAVE) {
         if (rec) {
           uint8_t* img = rec + rec_x_off(s);
-          const int W = rec_width(s);
-          *reinterpret_cast<uint16_t*>(img + img_offset(W, col, R)) = (uint16_t)(hi & 0xFFFFu);
-          *reinterpret_cast<uint16_t*>(img + img_offset(W, col + 1, R)) = (uint16_t)(hi >> 16);
+          uint8_t* img_j = img + (c_base + 8 * j) * 128;
+          *reinterpret_cast<uint16_t*>(img_j + img_base[hh][0]) = (uint16_t)(hi & 0xFFFFu);
+          *reinterpret_cast<uint16_t*>(img_j + img_base[hh][1]) = (uint16_t)(hi >> 16);
           const uint32_t bits = ((hi & 0xFFFFu) ? 1u : 0u) | ((hi >> 16) ? 2u : 0u);
           mask[hh][j >> 2] |= bits << ((col & 31));
         }
@@ -441,28 +517,32 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
           // ---- the MLP: this warpgroup's 64 rows
           {
             const bool probe = p.dbg_act && unit == 0 && pass == 0 && t == 0;
-            int prog = 0;
             float acc0[64], acc1[64], acc_s[8];
+            uint32_t act[64];  // fast mode: this thread's part of the hidden activations, as the next step's A fragments
             const int prow0 = t * 128 + r0, prow1 = prow0 + 8;
             const int ray0 = prow0 < rows ? prow0 / S : 0, ray1 = prow1 < rows ? prow1 / S : 0;
-            for (int s = 0; s < kNumSteps; ++s) {
+            auto mlp_step = [&](auto step) {
+              const int s = step;
               const StepInfo si = step_info(s);
-              mlp_step_mma<EXACT>(s, prog, ring, smem_base + M::kActHi, smem_base + M::kActLo, smem_base + M::kPeHi,
-                                  smem_base + M::kPeLo, (uint32_t)(64 * wg * 128), acc0, acc1, acc_s);
+              mlp_step_mma<EXACT>(step, ring, smem_base + M::kActHi, smem_base + M::kActLo, smem_base + M::kPeHi,
+                                     smem_base + M::kPeLo, (uint32_t)(64 * wg * 128), act, acc0, acc1, acc_s, tm);
               float* dump = (probe && p.dbg_act_step == s) ? p.dbg_act : nullptr;
               const float* bias = bias_n + si.bias_off;
               if (s <= 8) {
                 const float* db0 = (s == 6) ? dirbias + ray0 * 128 : nullptr;
                 const float* db1 = (s == 6) ? dirbias + ray1 * 128 : nullptr;
-                epi_half<EXACT, SAVE>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, r0, rec, dump);
-                if (si.nh1 == 128) epi_half<EXACT, SAVE>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, r0, rec, dump);
+                epi_half<EXACT, SAVE>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, act, r0, rec, dump);
+                if (si.nh1 == 128)
+                  epi_half<EXACT, SAVE>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, act, r0, rec, dump);
                 if (s == 6 && (lane & 3) == 0) {  // sigma = first column of the 16-column half
                   const float b = bias[128];
                   tile_raw[r0].w = acc_s[0] + b;
                   tile_raw[r0 + 8].w = acc_s[2] + b;
                 }
-                fence_proxy_async_smem();  // generic-proxy activation stores -> the next step's wgmma
-                named_bar_sync(2 + wg, 128);
+                if constexpr (EXACT) {
+                  fence_proxy_async_smem();  // generic-proxy activation stores -> the next step's wgmma
+                  named_bar_sync(2 + wg, 128);
+                }
               } else {  // fc_rgb: raw colour of columns 0..2
                 const int c = lane & 3;
                 if (c == 0) {
@@ -473,9 +553,17 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
                   tile_raw[r0 + 8].z = acc_s[2] + bias[2];
                 }
               }
+              tm.lap(12);
+            };
+            if constexpr (EXACT) {
+#pragma unroll 1
+              for (int s = 0; s < kNumSteps; ++s) mlp_step(s);
+            } else {
+              static_for<0, kNumSteps>(mlp_step);
             }
           }
           named_bar_sync(kRowBarrier, kRowThreads);  // tile_raw complete; PE and activation buffers free
+          tm.lap(14);
           // fc_rgb output.  Prepare what compositing needs per sample: colour and sigma (volume_rendering_utils.py:29-33,
           // 41-53); the exp(-sigma*delta) needs the neighbour depth and stays in composite_ray.
           if (ch == 0) {
@@ -513,7 +601,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
               }
             }
           }
-          tm.lap(20);
+          tm.lap(13);
         }  // tiles
         named_bar_sync(kRowBarrier, kRowThreads);
         tm.lap(3);

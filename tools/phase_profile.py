@@ -1,7 +1,9 @@
-"""Phase-cycle profile of the render kernels (NfbDebug.prof).  Usage: python tools/phase_profile.py [fast|exact] [H W]
+"""Phase-cycle profile of the render kernels (NfbDebug.prof).  Usage: python tools/phase_profile.py [fast|exact] [H W [NC NF]]
 
 Needs a library with the timers compiled in: `python 4d-facial-avatars_b200/build.py --timers` (lib/libnfb_timers.so, picked
-up here unless NFB_LIB is set)."""
+up here unless NFB_LIB is set).  The observer is one row-warp thread per CTA (warpgroup 0); its cycles are summed over CTAs
+and reported per tile (MLP phases) and per unit of work (per-ray phases).  "wait MMAs" includes issuing them and releasing
+the weight slots."""
 import os
 import sys
 
@@ -20,7 +22,7 @@ from nerf import _engine  # noqa: E402
 
 prec = "exact" if "exact" in sys.argv else "fast"
 nums = [int(a) for a in sys.argv[1:] if a.isdigit()]
-H, W = (nums + [256, 256])[:2]
+H, W, NC, NF = (nums + [256, 256, 64, 128][len(nums):])[:4]
 dev = torch.device("cuda", 0)
 fr = O.synthetic_frame(0, H, W)
 mk = lambda: nerf.models.ConditionalBlendshapePaperNeRFModel(num_encoding_fn_xyz=10, num_encoding_fn_dir=4, include_input_xyz=True, include_input_dir=False)  # noqa: E731
@@ -32,31 +34,31 @@ eng.sync_weights(mc, mf)
 eng.set_frame(fr["expr"].to(dev), fr["latent"].to(dev))
 bg = fr["bg"].reshape(-1, 3).to(dev)
 for _ in range(2):
-    eng.render_camera(fr["pose"], fr["intrinsics"], H, W, 0, H, 0.2, 0.8, 64, 128, background=bg, precision=prec)
+    eng.render_camera(fr["pose"], fr["intrinsics"], H, W, 0, H, 0.2, 0.8, NC, NF, background=bg, precision=prec)
 prof = torch.zeros(64, dtype=torch.int64, device=dev)
 e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
 e0.record()
-eng.render_camera(fr["pose"], fr["intrinsics"], H, W, 0, H, 0.2, 0.8, 64, 128, background=bg, precision=prec, prof=prof)
+eng.render_camera(fr["pose"], fr["intrinsics"], H, W, 0, H, 0.2, 0.8, NC, NF, background=bg, precision=prec, prof=prof)
 e1.record()
 torch.cuda.synchronize()
 ms = e0.elapsed_time(e1)
 c = prof.cpu().tolist()
-ctas = min(132, H * W // 2)
-units = H * W / 2
-tiles = units * 4
-names = {0: "ray setup", 1: "dir term", 2: "prologue (z+PE)", 3: "end-of-pass barrier", 4: "composite", 5: "cdf", 6: "inverse-cdf", 7: "sort",
-         39: "loop", 41: "producer: wait free slot", 40: "producer: issue", 44: "mma: issue", 45: "mma: wait A operand", 46: "mma: wait weights"}
-names[47] = "mma: wait A operand (half 1)"
-for s in range(10):
-    names[10 + s] = f"wait MMA step {s} half 0"
-    names[20 + s] = f"epilogue step {s} half 0"
-    names[48 + s] = f"epilogue step {s} half 1"
-for s in range(8):
-    names[30 + s] = f"wait MMA step {s}{'+' if s == 7 else ''} half 1"
-row_total = sum(c[i] for i in list(range(0, 8)) + list(range(10, 40)) + list(range(48, 58)))
-print(f"{prec} {H}x{W}: {ms:.2f} ms, {H*W/ms*1e3:.3e} rays/s; row-warp observer total {row_total/ctas/1e6:.2f} Mcycles per CTA")
+
+# the kernel's work decomposition (nfb_api.cu): R rays per unit, tiles_c + tiles_f 128-row tiles per unit
+R = 2 if 2 * (NC + NF) <= 512 else 1
+tiles_per_unit = -(-R * NC // 128) + (-(-R * (NC + NF) // 128) if NF > 0 else 0)
+units = -(-H * W // R)
+ctas = min(torch.cuda.get_device_properties(dev).multi_processor_count, units)
+tiles = units * tiles_per_unit
+per_tile = {2: "prologue (z + PE)", 10: "wait weights (wait_full)", 11: "wait MMAs", 12: "epilogue", 14: "end-of-MLP barrier",
+            13: "post-processing"}
+per_unit = {39: "unit loop", 0: "ray setup", 3: "end-of-pass barrier", 4: "composite", 5: "cdf", 6: "inverse-cdf", 7: "sort"}
+total = sum(c[i] for i in list(per_tile) + list(per_unit))
+print(f"{prec} {H}x{W} {NC}c+{NF}f: {ms:.2f} ms, {H*W/ms*1e3:.3e} rays/s; {R} rays/unit, {tiles_per_unit} tiles/unit, "
+      f"{tiles/ctas:.0f} tiles per CTA; row-warp observer {total/ctas/1e6:.2f} Mcycles per CTA")
 print(f"{'phase':28s} {'cycles/tile':>12s} {'share':>7s}")
-for i in sorted(names):
-    if c[i]:
-        share = c[i] / row_total if (i < 40 or i >= 48) else c[i] / sum(c[40:48])
-        print(f"{names[i]:28s} {c[i]/tiles:12.0f} {100*share:6.1f}%")
+for i, name in per_tile.items():
+    print(f"{name:28s} {c[i]/tiles:12.0f} {100*c[i]/total:6.1f}%")
+print(f"{'phase':28s} {'cycles/unit':>12s} {'share':>7s}")
+for i, name in per_unit.items():
+    print(f"{name:28s} {c[i]/units:12.0f} {100*c[i]/total:6.1f}%")
