@@ -53,6 +53,11 @@ struct NfbHandle {
     float* cond = nullptr;                              // [108] conditioning vector of the frame the forward rendered
     int n_rays = 0, nc = 0, nf = 0, rays_per_unit = 0, tiles_c = 0, tiles_f = 0, n_units = 0, has_bg = 0, white_bkgd = 0;
     bool valid = false;
+    // for input gradients (nfb_render_backward_ex): the forward's rays (copied unless chunked), per-row / per-ray scratch
+    bool has_rays = false, has_dir_z = false;
+    float* ray = nullptr; size_t cap_ray = 0;          // [n][7] = (o, d, v0), written by the SAVE forward
+    float* rows = nullptr; size_t cap_rows = 0;        // [tiles][128][4]
+    float *ray_dn = nullptr, *ray_bg = nullptr; size_t cap_rdn = 0, cap_rbg = 0;
     // chunked mode (the records of the whole call would exceed the memory budget): the forward only produced the outputs; the
     // backward re-runs the training forward chunk by chunk from the saved launch parameters (the caller keeps the inputs alive)
     bool chunked = false;
@@ -172,6 +177,7 @@ int nfb_destroy(NfbHandle* h) {
   }
   cudaFree(h->tr.lin_c); cudaFree(h->tr.lin_f);
   cudaFree(h->tr.rec); cudaFree(h->tr.draw); cudaFree(h->tr.z_c); cudaFree(h->tr.raw_c); cudaFree(h->tr.z_f); cudaFree(h->tr.raw_f);
+  cudaFree(h->tr.ray); cudaFree(h->tr.rows); cudaFree(h->tr.ray_dn); cudaFree(h->tr.ray_bg);
   cudaFree(h->tr.dnorm); cudaFree(h->tr.scal); cudaFree(h->tr.cond); cudaFree(h->tr.scratch_out); cudaFree(h->cond);
   cudaFree(h->minmax); cudaFree(h->smp_runs); cudaFree(h->smp_segs); cudaFree(h->smp_first);
   cudaFree(h->lin_c); cudaFree(h->lin_f); cudaFree(h->d_expr); cudaFree(h->d_latent); cudaFree(h->d_bg); cudaFree(h->d_out);
@@ -287,6 +293,7 @@ static int ensure_train_buffers(NfbHandle::Train& tr, size_t n, size_t tiles, in
   if ((rc = ensure_cap(&tr.z_c, &tr.cap_zc, n * nc))) return rc;
   if ((rc = ensure_cap(&tr.raw_c, &tr.cap_rawc, n * nc * 4))) return rc;
   if ((rc = ensure_cap(&tr.dnorm, &tr.cap_dn, n))) return rc;
+  if ((rc = ensure_cap(&tr.ray, &tr.cap_ray, 7 * n))) return rc;
   if (nf > 0) {
     if ((rc = ensure_cap(&tr.z_f, &tr.cap_zf, n * (nc + nf)))) return rc;
     if ((rc = ensure_cap(&tr.raw_f, &tr.cap_rawf, n * (nc + nf) * 4))) return rc;
@@ -400,7 +407,9 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
     if (!tr.chunked) {
       p.save_rec = tr.rec; p.save_dnorm = tr.dnorm; p.save_raw_c = tr.raw_c; p.save_raw_f = tr.raw_f;
       p.dbg_z_c = tr.z_c; p.dbg_z_f = tr.z_f;
+      p.save_ray = tr.ray;  // the rays, for input gradients (the backward does not read the caller's buffers)
     }
+    tr.has_rays = rays->o != nullptr; tr.has_dir_z = rays->dir_z != nullptr;
     tr.n_rays = rays->n_rays; tr.nc = nc; tr.nf = nf; tr.rays_per_unit = p.rays_per_unit; tr.tiles_c = p.tiles_c;
     tr.tiles_f = p.tiles_f; tr.n_units = p.n_units; tr.has_bg = rays->background != nullptr; tr.white_bkgd = p.white_bkgd;
   }
@@ -422,15 +431,32 @@ int nfb_render_forward_train(NfbHandle* h, const NfbRays* rays, const NfbSamplin
 int nfb_render_backward(NfbHandle* h, const NfbOutGrads* og, const float* const params_coarse[26],
                         const float* const params_fine[26], float* const grads_coarse[26], float* const grads_fine[26],
                         float* grad_latent, void* stream) {
-  if (!h || !og || !params_coarse || !grads_coarse) return NFB_ERR_INVALID;
+  if (!grads_coarse) return NFB_ERR_INVALID;  // input-only mode is nfb_render_backward_ex's
+  return nfb_render_backward_ex(h, og, params_coarse, params_fine, grads_coarse, grads_fine, grad_latent, nullptr, stream);
+}
+
+int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* const params_coarse[26],
+                           const float* const params_fine[26], float* const grads_coarse[26], float* const grads_fine[26],
+                           float* grad_latent, const NfbInputGrads* in_grads, void* stream) {
+  if (!h || !og || !params_coarse) return NFB_ERR_INVALID;
   NfbHandle::Train& tr = h->tr;
   if (!tr.valid) return NFB_ERR_STATE;
   const bool fine = tr.nf > 0;
-  if (fine && (!params_fine || !grads_fine)) return NFB_ERR_INVALID;
+  const bool input_only = !grads_coarse && !grads_fine;
+  if (input_only && !in_grads) return NFB_ERR_INVALID;
+  if (!input_only && !grads_coarse) return NFB_ERR_INVALID;
+  if (fine && (!params_fine || (!input_only && !grads_fine))) return NFB_ERR_INVALID;
   for (int i = 0; i < 26; ++i) {
     if (!params_coarse[i] || (fine && !params_fine[i])) return NFB_ERR_INVALID;
-    if (i != 22 && i != 23 && (!grads_coarse[i] || (fine && !grads_fine[i]))) return NFB_ERR_INVALID;
+    if (!input_only && i != 22 && i != 23 && (!grads_coarse[i] || (fine && !grads_fine[i]))) return NFB_ERR_INVALID;
   }
+  NfbInputGrads ig;
+  std::memset(&ig, 0, sizeof(ig));
+  if (in_grads) ig = *in_grads;
+  if ((ig.dir_z && !tr.has_dir_z) || (ig.background && !tr.has_bg)) return NFB_ERR_INVALID;
+  const bool ray_grads = ig.ray_origins || ig.ray_directions || ig.dir_z;
+  if (ray_grads && !tr.has_rays) return NFB_ERR_UNSUPPORTED;
+  const bool per_ray = ray_grads || ig.background;
   NFB_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   NFB_CUDA(cudaMemsetAsync(tr.acc[0], 0, nfb::kAccFloats * sizeof(float), st));
@@ -454,6 +480,12 @@ int nfb_render_backward(NfbHandle* h, const NfbOutGrads* og, const float* const 
     q.g_rgb[1] = off3(og->rgb_fine); q.g_disp[1] = off1(og->disp_fine); q.g_acc[1] = off1(og->acc_fine); q.g_wlast = off1(og->w_last);
     q.draw = tr.draw; q.acc[0] = tr.acc[0]; q.acc[1] = tr.acc[1];
     q.absmax = reinterpret_cast<unsigned int*>(tr.scal + 2);
+    if (per_ray) {
+      int rc;
+      if ((rc = ensure_cap(&tr.ray_dn, &tr.cap_rdn, 2 * (size_t)n)) || (rc = ensure_cap(&tr.ray_bg, &tr.cap_rbg, 6 * (size_t)n))) return rc;
+      if (ray_grads && (rc = ensure_cap(&tr.rows, &tr.cap_rows, tiles * 512))) return rc;
+      q.ray_dn = tr.ray_dn; q.ray_bg = tr.ray_bg;
+    }
     NFB_CUDA(nfb::launch_composite_bwd(q, tr.scal, st, &h->launches));
 
     nfb::ChainParams c;
@@ -462,13 +494,30 @@ int nfb_render_backward(NfbHandle* h, const NfbOutGrads* og, const float* const 
     c.wstream[0] = h->net[0].stream_bwd;
     c.wstream[1] = fine ? h->net[1].stream_bwd : h->net[0].stream_bwd;
     NFB_CUDA(nfb::launch_chain(c, h->num_sms, st, &h->launches));
-    {
+    if (!input_only || grad_latent || ig.expression) {  // input-only: the PE jobs only serve d latent / d expression
       nfb::DwParams d = {};
       d.rec = tr.rec; d.n_units = n_units; d.tpu = tr.tiles_c + tr.tiles_f;
       d.t_base[0] = 0; d.t_cnt[0] = tr.tiles_c;
       d.t_base[1] = tr.tiles_c; d.t_cnt[1] = fine ? tr.tiles_f : 0;
       d.acc[0] = tr.acc[0]; d.acc[1] = tr.acc[1]; d.scal = tr.scal;
-      NFB_CUDA(nfb::launch_dw(d, h->num_sms, st, &h->launches));  // both networks in one launch
+      NFB_CUDA(nfb::launch_dw(d, h->num_sms, st, &h->launches, input_only));  // both networks in one launch
+    }
+    if (per_ray) {
+      nfb::InGradRowParams r = {};
+      r.rec = tr.rec; r.n_units = n_units; r.tiles_c = tr.tiles_c; r.tiles_f = tr.tiles_f; r.rays_per_unit = tr.rays_per_unit;
+      r.nc = tr.nc; r.s_fine = tr.nc + tr.nf; r.n_rays = n;
+      r.z_c = tr.z_c; r.z_f = tr.z_f; r.ray = tr.ray; r.scal = tr.scal;
+      const float* const* pf = fine ? params_fine : params_coarse;
+      r.w0[0] = params_coarse[0]; r.w3[0] = params_coarse[6]; r.wd0[0] = params_coarse[16];
+      r.w0[1] = pf[0]; r.w3[1] = pf[6]; r.wd0[1] = pf[16];
+      r.out = tr.rows;
+      nfb::InGradRayParams a = {};
+      a.n_rays = n; a.nc = tr.nc; a.nf = tr.nf; a.s_fine = tr.nc + tr.nf; a.rays_per_unit = tr.rays_per_unit;
+      a.tiles_c = tr.tiles_c; a.tiles_f = tr.tiles_f; a.has_dir_z = tr.has_dir_z;
+      a.z_c = tr.z_c; a.z_f = tr.z_f; a.ray = tr.ray; a.dnorm = tr.dnorm; a.ray_dn = tr.ray_dn; a.ray_bg = tr.ray_bg;
+      auto at = [&](float* p, int w) { return p ? p + (size_t)w * begin : nullptr; };
+      a.g_o = at(ig.ray_origins, 3); a.g_d = at(ig.ray_directions, 3); a.g_dir_z = at(ig.dir_z, 1); a.g_bg = at(ig.background, 3);
+      NFB_CUDA(nfb::launch_input_grads(r, a, h->num_sms, st, &h->launches));
     }
     return NFB_OK;
   };
@@ -504,15 +553,16 @@ int nfb_render_backward(NfbHandle* h, const NfbOutGrads* og, const float* const 
       const size_t cn = (size_t)tr.chunk_rays;
       p.rgb_c = so; p.disp_c = so + 3 * cn; p.acc_c = so + 4 * cn; p.rgb_f = so + 5 * cn; p.disp_f = so + 8 * cn; p.acc_f = so + 9 * cn;
       p.w_last = so + 10 * cn;
-      p.save_rec = tr.rec; p.save_dnorm = tr.dnorm; p.save_raw_c = tr.raw_c; p.save_raw_f = tr.raw_f;
+      p.save_rec = tr.rec; p.save_dnorm = tr.dnorm; p.save_raw_c = tr.raw_c; p.save_raw_f = tr.raw_f; p.save_ray = tr.ray;
       p.dbg_z_c = tr.z_c; p.dbg_z_f = tr.z_f;
       NFB_CUDA(nfb::launch_render(p, tr.precision, h->num_sms, st, &h->launches));
       rc = backward_rays(begin, n, n_units);
       if (rc) return rc;
     }
   }
-  NFB_CUDA(nfb::launch_finalize_all(params_coarse, grads_coarse, tr.acc[0], fine ? params_fine : nullptr, fine ? grads_fine : nullptr,
-                                    tr.acc[1], tr.cond, grad_latent, st, &h->launches));
+  NFB_CUDA(nfb::launch_finalize_all(params_coarse, input_only ? nullptr : grads_coarse, tr.acc[0], fine ? params_fine : nullptr,
+                                    (fine && !input_only) ? grads_fine : nullptr, tr.acc[1], tr.cond, grad_latent, st, &h->launches,
+                                    ig.expression));
   return NFB_OK;
 }
 

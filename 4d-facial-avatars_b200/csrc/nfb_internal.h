@@ -56,6 +56,7 @@ struct RenderParams {
   // sample (colour or bg, ReLU input of sigma) of both passes
   uint8_t* save_rec;
   float* save_dnorm;
+  float* save_ray;  // optional [n][7] = (o, d, direction-encoder input d_z or dir_z)
   float *save_raw_c, *save_raw_f;
   // debug
   float *dbg_z_c, *dbg_raw_c, *dbg_z_f, *dbg_raw_f, *dbg_act;
@@ -71,6 +72,22 @@ struct CompBwdParams {
   float* draw;                                                          // [tiles][128][4] dL/d(rgb_raw, sigma_raw), zero-initialised
   float* acc[2];                                                        // per-network accumulators (kAccBRaw sums land here)
   unsigned int* absmax;                                                 // max |d raw| as float bits
+  float *ray_dn, *ray_bg;  // non-null: input-gradient terms per (pass, ray): dL/d|d| [2][n], w_last G_rgb [2][n][3] (with a background)
+};
+// Input gradients (nfb_render_backward_ex): per-row (dp, d v0) of every tile, then per-ray sums.
+struct InGradRowParams {
+  const uint8_t* rec;
+  int n_units, tiles_c, tiles_f, rays_per_unit, nc, s_fine, n_rays;
+  int parts[2];                       // CTAs working on network 0 / network 1
+  const float *z_c, *z_f, *ray;        // ray: the training forward's [n][7] = (o, d, v0)
+  const float* scal;
+  const float *w0[2], *w3[2], *wd0[2];  // FP32 layers_xyz.0 / .3 / layers_dir.0 weights of the two networks
+  float* out;                         // [tiles][128] float4
+};
+struct InGradRayParams {
+  int n_rays, nc, nf, s_fine, rays_per_unit, tiles_c, tiles_f, has_dir_z;
+  const float *rows, *z_c, *z_f, *ray, *dnorm, *ray_dn, *ray_bg;
+  float *g_o, *g_d, *g_dir_z, *g_bg;  // any may be null
 };
 struct ChainParams {
   int n_units, tiles_c, tiles_f;
@@ -93,10 +110,12 @@ int debug_dw_split(uint32_t* io);  // io: {num_sms, tiles net 0, tiles net 1} ->
 cudaError_t train_kernels_setup();
 cudaError_t launch_composite_bwd(const CompBwdParams& q, float* scal, cudaStream_t st, long long* launches);
 cudaError_t launch_chain(const ChainParams& p, int num_sms, cudaStream_t st, long long* launches);
-cudaError_t launch_dw(const DwParams& p, int num_sms, cudaStream_t st, long long* launches);
+cudaError_t launch_dw(const DwParams& p, int num_sms, cudaStream_t st, long long* launches, bool pe_only = false);
+// grads_c == nullptr: input-gradient-only backward (d latent and d expression alone, one small launch).
 cudaError_t launch_finalize_all(const float* const params_c[26], float* const grads_c[26], const float* acc_c,
                                 const float* const params_f[26], float* const grads_f[26], const float* acc_f, const float* cond,
-                                float* latent_out, cudaStream_t st, long long* launches);
+                                float* latent_out, cudaStream_t st, long long* launches, float* expr_out = nullptr);
+cudaError_t launch_input_grads(const InGradRowParams& r, const InGradRayParams& q, int num_sms, cudaStream_t st, long long* launches);
 
 // Two launches (fold, pack): FP32 parameters of n_nets (1 or 2) networks -> forward / backward weight streams, bias block, conditioning and
 // direction columns (nfb_pack.cu: repack_kernel).

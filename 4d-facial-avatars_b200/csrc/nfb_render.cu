@@ -348,7 +348,13 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
           rp.dnorm = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(d0, d0), __fmul_rn(d1, d1)), __fmul_rn(d2, d2)));
           if (has_bg) { rp.bg[0] = p.bg[3 * g]; rp.bg[1] = p.bg[3 * g + 1]; rp.bg[2] = p.bg[3 * g + 2]; }
           rp.dz = p.dir_z ? p.dir_z[g] : d2;
-          if constexpr (SAVE) p.save_dnorm[g] = rp.dnorm;
+          if constexpr (SAVE) {
+            p.save_dnorm[g] = rp.dnorm;
+            if (p.save_ray) {  // the ray as the input gradients need it: o, d, direction-encoder input
+              float* sr = p.save_ray + 7 * (size_t)g;
+              sr[0] = o0; sr[1] = o1; sr[2] = o2; sr[3] = d0; sr[4] = d1; sr[5] = d2; sr[6] = rp.dz;
+            }
+          }
         } else {
           for (int k = 0; k < 3; ++k) { rp.o[k] = 0.f; rp.d[k] = 0.f; rp.bg[k] = 0.f; }
           rp.dnorm = 0.f;

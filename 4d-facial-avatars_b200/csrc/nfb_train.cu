@@ -39,6 +39,10 @@ namespace nfb {
 // One WARP per (ray, pass); samples are lane-blocked (lane l owns samples [l*per, (l+1)*per)).  The forward product of
 // (1 - alpha + 1e-10) and the reverse affine recurrence  C_{i-1} = dLdw_i alpha_i + omega_i C_i  are both scans: in-lane
 // sequential, across lanes a shuffle scan (of products / of composed affine maps).
+// kInputs: also the per-ray terms of the input gradients, from values the sweep already has:
+//   ray_dn[pass][g]     = dL/d|d| through the sample spacings  = sum_i dsig_i sigma_i / |d|   (delta_i = dz_i |d|)
+//   ray_bg[pass][g][3]  = w_{S-1} G_rgb (the background replaces the colour of the last sample)
+template <bool kInputs>
 __global__ void __launch_bounds__(256) composite_bwd_kernel(const CompBwdParams q) {
   const int lane = threadIdx.x & 31;
   const int idx = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
@@ -141,6 +145,7 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const CompBwdParams 
   const int unit = g / q.rays_per_unit, rr = g - unit * q.rays_per_unit;
   const int tile0 = unit * (q.tiles_c + q.tiles_f) + (pass ? q.tiles_c : 0);
   float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f, amax = 0.f;
+  float gdn = 0.f;  // kInputs: sum of dsig_i sigma_i over this lane's samples
   // transmittance in front of each sample of this block, walking down from the block's end
   float Tj[kPer];
   {
@@ -166,8 +171,13 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const CompBwdParams 
       const float dsig = dalpha * (delta * e);  // d alpha / d sigma = delta exp(-sigma delta); (1e10 * 0) stays 0
       float4 d;
       d.w = (r4.w > 0.f) ? dsig : 0.f;          // ReLU (the +1e-6 on the last sample is an additive constant)
+      if constexpr (kInputs) gdn = fmaf(dsig, fmaxf(r4.w, 0.f) + (i == S - 1 ? 1e-6f : 0.f), gdn);
       if (q.has_bg && i == S - 1) {
         d.x = d.y = d.z = 0.f;                  // background colour is data (train_background=False)
+        if constexpr (kInputs) {
+          float* bgo = q.ray_bg + ((size_t)pass * q.n_rays + g) * 3;
+          bgo[0] = w * G0; bgo[1] = w * G1; bgo[2] = w * G2;
+        }
       } else {
         d.x = w * G0 * r4.x * (1.f - r4.x);     // sigmoid
         d.y = w * G1 * r4.y * (1.f - r4.y);
@@ -186,6 +196,10 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const CompBwdParams 
     s2 += __shfl_xor_sync(0xffffffffu, s2, o); s3 += __shfl_xor_sync(0xffffffffu, s3, o);
     const float t = __shfl_xor_sync(0xffffffffu, amax, o);
     amax = (t != t || amax != amax) ? __int_as_float(0x7fc00000) : fmaxf(amax, t);
+    if constexpr (kInputs) gdn += __shfl_xor_sync(0xffffffffu, gdn, o);
+  }
+  if constexpr (kInputs) {
+    if (lane == 0) q.ray_dn[(size_t)pass * q.n_rays + g] = gdn / dn;
   }
   if (lane == 0) {
     float* braw = q.acc[pass] + kAccBRaw;
@@ -425,6 +439,9 @@ constexpr JobTable make_jobs() {
   return t;
 }
 static_assert(make_jobs().group_begin[kGroups] == kNumJobs, "job table");
+static_assert(make_jobs().group_begin[5] - make_jobs().group_begin[4] == 3 && make_jobs().j[make_jobs().group_begin[4] + 1].b_off == kRecPE &&
+                  make_jobs().j[make_jobs().group_begin[5] + 2].b_off == kRecPE && make_jobs().group_begin[6] - make_jobs().group_begin[5] == 3,
+              "the PE-only weight-gradient launch runs jobs 1 and 2 of groups 4 and 5");
 __constant__ JobTable c_jobs = make_jobs();
 
 template <int N> __device__ __forceinline__ void mma_n(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t accf) {
@@ -482,14 +499,19 @@ __device__ __forceinline__ void run_job(const Job& J, int j0, int j1, uint32_t s
   }
 }
 
+// kPeOnly (input-gradient-only backward): only the four jobs that read the PE image — dW0, dW3a and with them the column sums
+// db0, db3 that d latent and d expression need — i.e. groups 4 and 5 without their first (hidden-part) job.
+constexpr int kPeGroup = 4, kPeGroups = 2;
+template <bool kPeOnly>
 __global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__ DwParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t smem_base = smem_base_aligned(smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
   // this CTA: network x job group (blockIdx.x % kGroups) x a contiguous share of the network's tiles
-  const int group = (int)blockIdx.x % kGroups;
-  int part = (int)blockIdx.x / kGroups;
+  constexpr int kG = kPeOnly ? kPeGroups : kGroups;
+  const int group = (kPeOnly ? kPeGroup : 0) + (int)blockIdx.x % kG;
+  int part = (int)blockIdx.x / kG;
   const int net = (part >= p.parts[0]) ? 1 : 0;
   if (net) part -= p.parts[0];
   const int parts = p.parts[net];
@@ -499,7 +521,7 @@ __global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__
   const int j0 = part * per;
   const int j1 = min(total, j0 + per);
   if (part >= parts || j0 >= j1) return;  // uniform for the whole CTA
-  const int job0 = c_jobs.group_begin[group], job1 = c_jobs.group_begin[group + 1];
+  const int job0 = c_jobs.group_begin[group] + (kPeOnly ? 1 : 0), job1 = c_jobs.group_begin[group + 1];
 
   StageRing ring(smem_base, smem_base + kOffBars);
   if (threadIdx.x == 0) ring.init();
@@ -575,15 +597,18 @@ __host__ __device__ __forceinline__ int fin_numel(int t) {
 }
 // ONE launch finishes both networks: blockIdx.y = network; blockIdx.x walks the 26 tensors back to back in 256-element blocks
 // (2.2 k blocks per network instead of a 427 x 26 grid that is mostly empty); the last block of network 0 computes d latent.
-struct FinAll { FinArgs net[2]; int nets; float* latent_out; };
+// The two blocks after the last tensor of network 0 compute d latent and d expression.
+struct FinAll { FinArgs net[2]; int nets; float* latent_out; float* expr_out; };
 __device__ __forceinline__ int fin_blocks(int t) { return (fin_numel(t) + 255) >> 8; }
 __device__ void latent_grad_block(const FinAll& f);
+__device__ void expr_grad_block(const FinAll& f);
 __global__ void __launch_bounds__(256) finalize_kernel(const FinAll f) {
   const FinArgs& a = f.net[blockIdx.y];
   int b = blockIdx.x, t = 0;
   while (t < 26 && b >= fin_blocks(t)) { b -= fin_blocks(t); ++t; }
-  if (t == 26) {  // the block after the last tensor
+  if (t == 26) {  // the blocks after the last tensor
     if (blockIdx.y == 0 && b == 0 && f.latent_out) latent_grad_block(f);
+    if (blockIdx.y == 0 && b == 1 && f.expr_out) expr_grad_block(f);
     return;
   }
   const int e = b * 256 + threadIdx.x;
@@ -699,6 +724,205 @@ __device__ void latent_grad_block(const FinAll& f) {  // one block of 256 thread
   }
 }
 
+// d expression[j] = (1/3) sum over networks, n of W0[n][63 + j] db0[n] + W3[n][63 + j] db3[n]  (cond = [expression / 3 ; latent]).
+// One block of 256 threads: thread = (n-chunk of 64 rows, j); 76 of every 128 threads work.
+__device__ void expr_grad_block(const FinAll& f) {
+  __shared__ float part[2][kDimExpr];
+  const int j = threadIdx.x & 127, c = threadIdx.x >> 7;  // c in {0, 1}: rows [128c, 128c + 128)
+  float s = 0.f;
+  if (j < kDimExpr) {
+    for (int net = 0; net < f.nets; ++net) {
+      const float* b0 = f.net[net].acc + acc_bias_off(0);
+      const float* b3 = f.net[net].acc + acc_bias_off(3);
+      const float* w0 = f.net[net].p[0];
+      const float* w3 = f.net[net].p[6];
+      for (int n = c * 128; n < c * 128 + 128; ++n) {
+        s = fmaf(w0[n * 171 + kDimXyz + j], b0[n], s);
+        s = fmaf(w3[(size_t)n * 427 + kDimXyz + j], b3[n], s);
+      }
+    }
+    part[c][j] = s;
+  }
+  __syncthreads();
+  if (c == 0 && j < kDimExpr) f.expr_out[j] = (part[0][j] + part[1][j]) * (1.f / 3.f);
+}
+
+// Input-gradient-only backward: the latent and expression blocks of finalize_kernel alone.
+__global__ void __launch_bounds__(256) cond_grad_kernel(const FinAll f) {
+  if (blockIdx.x == 0 && f.latent_out) latent_grad_block(f);
+  if (blockIdx.x == 1 && f.expr_out) expr_grad_block(f);
+}
+
+// ================================================================================================
+// 5. input gradients (rays, direction, background; nfb_render_backward_ex)
+// ================================================================================================
+// Per sample row of every tile (after the dX chain, which left dY0, dY3 and dY6 in the tile record):
+//   dPE  = W0[:, :63]^T dY0 + W3[:, :63]^T dY3,   dPEd[6j], dPEd[6j+3] = Wd0[:, 256+6j]^T dY6, Wd0[:, 259+6j]^T dY6
+//   dp   = dPE[0:3] + sum_j 2^j (cos(2^j p) dPE[3+6j:6+6j] - sin(2^j p) dPE[6+6j:9+6j])        p = o + d z
+//   dv0  = sum_j 2^j (cos(2^j v0) dPEd[6j] - sin(2^j v0) dPEd[6j+3])                          v0 = dir_z or d.z
+// written as one float4 (dp, dv0) per row.  SIMT with the FP32 master columns in shared memory: thread = (row, quarter of the
+// 64 PE columns); a warp is 32 rows of one quarter, so every weight load is a broadcast.  The chain and weight-gradient kernels
+// are untouched by this (their parameter-only code stays as it is); the cost is one extra pass over 160 KB of each record.
+namespace ing {
+constexpr int kThreadsRow = 512;
+constexpr int kOffW3 = 256 * 64 * 4;
+constexpr int kOffWd = 2 * kOffW3;              // [128][8]: the v0 columns sin/cos of the 4 frequencies
+constexpr int kOffRed = kOffWd + 128 * 8 * 4;   // [4][128] float4
+constexpr int kSmemBytes = kOffRed + 4 * 128 * 16;
+
+__global__ void __launch_bounds__(kThreadsRow, 1) row_kernel(const InGradRowParams p) {
+  extern __shared__ __align__(16) uint8_t smem[];
+  float* w0s = reinterpret_cast<float*>(smem);
+  float* w3s = reinterpret_cast<float*>(smem + kOffW3);
+  float* wds = reinterpret_cast<float*>(smem + kOffWd);
+  float4* red = reinterpret_cast<float4*>(smem + kOffRed);
+  const int net = (int)blockIdx.x >= p.parts[0] ? 1 : 0;
+  const int part = (int)blockIdx.x - (net ? p.parts[0] : 0);
+  const int parts = p.parts[net];
+  for (int i = threadIdx.x; i < 256 * 64; i += kThreadsRow) {
+    const int n = i >> 6, k = i & 63;
+    w0s[i] = k < kDimXyz ? p.w0[net][n * 171 + k] : 0.f;
+    w3s[i] = k < kDimXyz ? p.w3[net][(size_t)n * 427 + k] : 0.f;
+  }
+  for (int i = threadIdx.x; i < 128 * 8; i += kThreadsRow) {
+    const int n = i >> 3, c = i & 7;
+    wds[i] = p.wd0[net][n * 280 + 256 + 6 * (c >> 1) + 3 * (c & 1)];
+  }
+  __syncthreads();
+  const int row = threadIdx.x & 127, kq = threadIdx.x >> 7;
+  const float inv = p.scal[1];
+  const int t_cnt = net ? p.tiles_f : p.tiles_c, t_base = net ? p.tiles_c : 0;
+  const int S = net ? p.s_fine : p.nc;
+  const float* zp = net ? p.z_f : p.z_c;
+  const int total = p.n_units * t_cnt;
+  for (int j = part; j < total; j += parts) {
+    const int unit = j / t_cnt, tl = j - unit * t_cnt;
+    const size_t gt = (size_t)unit * (p.tiles_c + p.tiles_f) + t_base + tl;
+    const uint8_t* rec = p.rec + gt * kRecBytes;
+    float acc[16];
+#pragma unroll
+    for (int k = 0; k < 16; ++k) acc[k] = 0.f;
+#pragma unroll 1
+    for (int L = 0; L < 2; ++L) {
+      const uint8_t* img = rec + rec_dy_off(3 * L);
+      const float* ws = (L ? w3s : w0s) + 16 * kq;
+#pragma unroll 4
+      for (int n = 0; n < 256; ++n) {
+        const float dy = __half2float(*reinterpret_cast<const __half*>(img + img_offset(256, n, row)));
+        const float4* w4 = reinterpret_cast<const float4*>(ws + n * 64);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float4 w = w4[q];
+          acc[4 * q] = fmaf(w.x, dy, acc[4 * q]); acc[4 * q + 1] = fmaf(w.y, dy, acc[4 * q + 1]);
+          acc[4 * q + 2] = fmaf(w.z, dy, acc[4 * q + 2]); acc[4 * q + 3] = fmaf(w.w, dy, acc[4 * q + 3]);
+        }
+      }
+    }
+    float ds = 0.f, dc = 0.f;  // dPEd of sin / cos of frequency kq
+    {
+      const uint8_t* img = rec + rec_dy_off(6);
+#pragma unroll 4
+      for (int n = 0; n < 128; ++n) {
+        const float dy = __half2float(*reinterpret_cast<const __half*>(img + img_offset(128, n, row)));
+        ds = fmaf(wds[n * 8 + 2 * kq], dy, ds);
+        dc = fmaf(wds[n * 8 + 2 * kq + 1], dy, dc);
+      }
+    }
+    float4 r = make_float4(0.f, 0.f, 0.f, 0.f);
+    const int prow = tl * 128 + row, rr = prow / S, i = prow - rr * S, g = unit * p.rays_per_unit + rr;
+    if (rr < p.rays_per_unit && g < p.n_rays) {
+      const float z = zp[(size_t)g * S + i];
+      const float* ray = p.ray + 7 * (size_t)g;
+      const float px = fmaf(ray[3], z, ray[0]), py = fmaf(ray[4], z, ray[1]), pz = fmaf(ray[5], z, ray[2]);
+#pragma unroll
+      for (int kk = 0; kk < 16; ++kk) {
+        const int k = 16 * kq + kk;
+        if (k >= kDimXyz) continue;
+        const float a = acc[kk];
+        if (k < 3) {
+          if (k == 0) r.x += a; else if (k == 1) r.y += a; else r.z += a;
+          continue;
+        }
+        const int kp = k - 3, fj = kp / 6, wi = kp - 6 * fj, comp = wi % 3;
+        const float f = (float)(1 << fj);
+        const float x = f * (comp == 0 ? px : comp == 1 ? py : pz);
+        const float v = f * a * (wi < 3 ? cosf(x) : -sinf(x));
+        if (comp == 0) r.x += v; else if (comp == 1) r.y += v; else r.z += v;
+      }
+      const float f = (float)(1 << kq), x = f * ray[6];
+      r.w = f * (cosf(x) * ds - sinf(x) * dc);
+    }
+    red[kq * 128 + row] = r;
+    __syncthreads();
+    if (kq == 0) {
+      float4 s = red[row];
+#pragma unroll
+      for (int q = 1; q < 4; ++q) {
+        const float4 t = red[q * 128 + row];
+        s.x += t.x; s.y += t.y; s.z += t.z; s.w += t.w;
+      }
+      s.x *= inv; s.y *= inv; s.z *= inv; s.w *= inv;
+      reinterpret_cast<float4*>(p.out)[gt * 128 + row] = s;
+    }
+    __syncthreads();
+  }
+}
+
+// One warp per ray: sums the row float4s of both passes (lane-strided over the samples, then a butterfly: deterministic, no
+// atomics), d o += dp, d d += z dp, and adds the |d| term of the compositing and the background term.
+__global__ void __launch_bounds__(256) ray_kernel(const InGradRayParams p) {
+  const int lane = threadIdx.x & 31;
+  const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  if (g >= p.n_rays) return;  // whole warps
+  const int npass = p.nf > 0 ? 2 : 1;
+  float so0 = 0.f, so1 = 0.f, so2 = 0.f, sd0 = 0.f, sd1 = 0.f, sd2 = 0.f, sv = 0.f;
+  if (p.rows) {
+    const int unit = g / p.rays_per_unit, rr = g - unit * p.rays_per_unit;
+    for (int pass = 0; pass < npass; ++pass) {
+      const int S = pass ? p.s_fine : p.nc;
+      const float* z = (pass ? p.z_f : p.z_c) + (size_t)g * S;
+      const size_t tile0 = (size_t)unit * (p.tiles_c + p.tiles_f) + (pass ? p.tiles_c : 0);
+      for (int i = lane; i < S; i += 32) {
+        const int prow = rr * S + i;
+        const float4 v = reinterpret_cast<const float4*>(p.rows)[(tile0 + (prow >> 7)) * 128 + (prow & 127)];
+        const float zi = z[i];
+        so0 += v.x; so1 += v.y; so2 += v.z;
+        sd0 = fmaf(zi, v.x, sd0); sd1 = fmaf(zi, v.y, sd1); sd2 = fmaf(zi, v.z, sd2);
+        sv += v.w;
+      }
+    }
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) {
+      so0 += __shfl_xor_sync(0xffffffffu, so0, o); so1 += __shfl_xor_sync(0xffffffffu, so1, o);
+      so2 += __shfl_xor_sync(0xffffffffu, so2, o); sd0 += __shfl_xor_sync(0xffffffffu, sd0, o);
+      sd1 += __shfl_xor_sync(0xffffffffu, sd1, o); sd2 += __shfl_xor_sync(0xffffffffu, sd2, o);
+      sv += __shfl_xor_sync(0xffffffffu, sv, o);
+    }
+  }
+  if (lane != 0) return;
+  if (p.g_o) { p.g_o[3 * g] = so0; p.g_o[3 * g + 1] = so1; p.g_o[3 * g + 2] = so2; }
+  if (p.g_d) {
+    float gdn = p.ray_dn[g];
+    if (npass == 2) gdn += p.ray_dn[p.n_rays + g];
+    const float* ray = p.ray + 7 * (size_t)g;
+    const float dx = ray[3], dy = ray[4], dz = ray[5];
+    const float s = gdn / p.dnorm[g];
+    p.g_d[3 * g] = fmaf(s, dx, sd0);
+    p.g_d[3 * g + 1] = fmaf(s, dy, sd1);
+    p.g_d[3 * g + 2] = fmaf(s, dz, sd2) + (p.has_dir_z ? 0.f : sv);
+  }
+  if (p.g_dir_z) p.g_dir_z[g] = sv;
+  if (p.g_bg) {
+#pragma unroll
+    for (int c = 0; c < 3; ++c) {
+      float b = p.ray_bg[3 * g + c];
+      if (npass == 2) b += p.ray_bg[3 * ((size_t)p.n_rays + g) + c];
+      p.g_bg[3 * g + c] = b;
+    }
+  }
+}
+}  // namespace ing
+
 // ================================================================================================
 // host-side launchers
 // ================================================================================================
@@ -718,12 +942,17 @@ int debug_jobs_dw(int index, uint32_t* out) {
 cudaError_t train_kernels_setup() {
   cudaError_t e = cudaFuncSetAttribute(chain::chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, chain::kSmemBytes);
   if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(dw::dw_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, dw::kSmemBytes);
+  e = cudaFuncSetAttribute(dw::dw_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dw::kSmemBytes);
+  if (e != cudaSuccess) return e;
+  e = cudaFuncSetAttribute(dw::dw_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, dw::kSmemBytes);
+  if (e != cudaSuccess) return e;
+  return cudaFuncSetAttribute(ing::row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ing::kSmemBytes);
 }
 
 cudaError_t launch_composite_bwd(const CompBwdParams& q, float* scal, cudaStream_t st, long long* launches) {
   const int n = (q.nf > 0 ? 2 : 1) * q.n_rays;
-  composite_bwd_kernel<<<(n + 7) / 8, 256, 0, st>>>(q);  // one warp per (ray, pass)
+  if (q.ray_dn) composite_bwd_kernel<true><<<(n + 7) / 8, 256, 0, st>>>(q);  // one warp per (ray, pass)
+  else composite_bwd_kernel<false><<<(n + 7) / 8, 256, 0, st>>>(q);
   ++*launches;
   scale_kernel<<<1, 1, 0, st>>>(q.absmax, scal);
   ++*launches;
@@ -761,13 +990,15 @@ int debug_dw_split(uint32_t* io) {  // in: num_sms, tiles of network 0, tiles of
   return 3;
 }
 
-cudaError_t launch_dw(const DwParams& p_in, int num_sms, cudaStream_t st, long long* launches) {
+cudaError_t launch_dw(const DwParams& p_in, int num_sms, cudaStream_t st, long long* launches, bool pe_only) {
   DwParams p = p_in;
   const long long tot0 = (long long)p.n_units * p.t_cnt[0], tot1 = (long long)p.n_units * p.t_cnt[1];
   if (tot0 + tot1 <= 0) return cudaSuccess;
-  dw_split(num_sms, tot0, tot1, &p.parts[0], &p.parts[1]);
+  // PE-only: two job groups, so num_sms / 2 CTAs per group
+  dw_split(pe_only ? num_sms * dw::kGroups / dw::kPeGroups : num_sms, tot0, tot1, &p.parts[0], &p.parts[1]);
   if (p.parts[0] + p.parts[1] < 1) return cudaSuccess;
-  dw::dw_kernel<<<(p.parts[0] + p.parts[1]) * dw::kGroups, kThreads, dw::kSmemBytes, st>>>(p);
+  if (pe_only) dw::dw_kernel<true><<<(p.parts[0] + p.parts[1]) * dw::kPeGroups, kThreads, dw::kSmemBytes, st>>>(p);
+  else dw::dw_kernel<false><<<(p.parts[0] + p.parts[1]) * dw::kGroups, kThreads, dw::kSmemBytes, st>>>(p);
   ++*launches;
   return cudaGetLastError();
 }
@@ -775,21 +1006,45 @@ cudaError_t launch_dw(const DwParams& p_in, int num_sms, cudaStream_t st, long l
 // Chain rule through the folds for one or both networks + d latent, two launches in all.
 cudaError_t launch_finalize_all(const float* const params_c[26], float* const grads_c[26], const float* acc_c,
                                 const float* const params_f[26], float* const grads_f[26], const float* acc_f, const float* cond,
-                                float* latent_out, cudaStream_t st, long long* launches) {
+                                float* latent_out, cudaStream_t st, long long* launches, float* expr_out) {
   FinAll f;
   f.nets = params_f ? 2 : 1;
   f.latent_out = latent_out;
+  f.expr_out = expr_out;
   for (int i = 0; i < 26; ++i) {
-    f.net[0].p[i] = params_c[i]; f.net[0].g[i] = grads_c[i];
-    f.net[1].p[i] = params_f ? params_f[i] : nullptr; f.net[1].g[i] = params_f ? grads_f[i] : nullptr;
+    f.net[0].p[i] = params_c[i]; f.net[0].g[i] = grads_c ? grads_c[i] : nullptr;
+    f.net[1].p[i] = params_f ? params_f[i] : nullptr; f.net[1].g[i] = (params_f && grads_f) ? grads_f[i] : nullptr;
   }
   f.net[0].acc = acc_c; f.net[1].acc = acc_f;
   f.net[0].cond = f.net[1].cond = cond;
-  int blocks = 1;  // + the latent block
+  if (!grads_c) {  // input gradients only: no parameter gradient, only the latent / expression blocks
+    if (!latent_out && !expr_out) return cudaSuccess;
+    cond_grad_kernel<<<2, 256, 0, st>>>(f);
+    ++*launches;
+    return cudaGetLastError();
+  }
+  int blocks = expr_out ? 2 : 1;  // + the latent (and expression) blocks
   for (int t = 0; t < 26; ++t) blocks += (fin_numel(t) + 255) / 256;
   finalize_kernel<<<dim3(blocks, f.nets), 256, 0, st>>>(f);
   ++*launches;
   fin_dir0_kernel<<<dim3((128 * 256 + 256) * 32 / 256, f.nets), 256, 0, st>>>(f);
+  ++*launches;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_input_grads(const InGradRowParams& r_in, const InGradRayParams& q_in, int num_sms, cudaStream_t st, long long* launches) {
+  InGradRayParams q = q_in;
+  if (q.g_o || q.g_d || q.g_dir_z) {
+    InGradRowParams r = r_in;
+    const long long tot0 = (long long)r.n_units * r.tiles_c, tot1 = q.nf > 0 ? (long long)r.n_units * r.tiles_f : 0;
+    dw_split(num_sms * dw::kGroups, tot0, tot1, &r.parts[0], &r.parts[1]);  // num_sms CTAs, split by tile counts
+    ing::row_kernel<<<r.parts[0] + r.parts[1], ing::kThreadsRow, ing::kSmemBytes, st>>>(r);
+    ++*launches;
+    q.rows = r.out;
+  } else {
+    q.rows = nullptr;
+  }
+  ing::ray_kernel<<<(q.n_rays + 7) / 8, 256, 0, st>>>(q);  // one warp per ray
   ++*launches;
   return cudaGetLastError();
 }

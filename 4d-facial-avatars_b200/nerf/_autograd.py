@@ -1,25 +1,34 @@
-"""Gradients for training (train_transformed_rays.py:389 `loss.backward()`).
+"""Gradients for training (train_transformed_rays.py:389 `loss.backward()`) and for fitting a frozen avatar to images.
 
 Forward: the fused sm_90a render kernel in its training variant (nfb_render_forward_train) — the same launch as
 evaluation, which also leaves the FP16 activations of every layer, the sample depths and the per-sample colours in
-buffers owned by the renderer.  Backward: nfb_render_backward (csrc/nfb_train.cu) — compositing backward, the dX chain
+buffers owned by the renderer.  Backward: nfb_render_backward_ex (csrc/nfb_train.cu) — compositing backward, the dX chain
 and the weight-gradient GEMMs on wgmma, then the chain rule through the kernel's weight folding.  No torch.autograd
 graph and no library GEMM is involved; the resampled depths carry no gradient, as in the reference
-(`z_samples.detach()`, train_utils.py:124), and `layers_dir.3.*` receives None (unused by the forward, models.py:257)."""
+(`z_samples.detach()`, train_utils.py:124), and `layers_dir.3.*` receives None (unused by the forward, models.py:257).
+
+Like the reference's autograd, every floating-point input that requires grad gets a gradient: the rays (origins and
+directions; the near/far columns get zero), the expression, the latent code, the background and the ablation directions
+(dir_z).  When no parameter requires grad (a frozen avatar), the backward runs in input-only mode and forms no parameter
+gradient, which is most of its cost."""
 import torch
 
 from ._engine import PARAM_ORDER
 
+_N_IN = 8  # inputs before the parameters: eng, args, has_fine, rays, expr, latent, background, dir_z
+
 
 class _RenderFn(torch.autograd.Function):
     @staticmethod
-    def forward(ctx, eng, rays, args, has_fine, expr, latent, *params):
-        out = eng.render(rays[:, :3], rays[:, 3:6], train=True, **args)
+    def forward(ctx, eng, args, has_fine, rays, expr, latent, background, dir_z, *params):
+        out = eng.render(rays[:, :3], rays[:, 3:6], train=True, background=background, dir_z=dir_z, **args)
         ctx.eng = eng
         ctx.keep = out.get("_keep")  # the chunked backward (include/nfb.h) re-reads the forward's inputs
         ctx.token = eng.train_token
         ctx.has_fine = has_fine
-        ctx.latent_shape = latent.shape
+        ctx.shapes = dict(rays=rays.shape, expr=expr.shape, latent=latent.shape,
+                          background=background.shape if background is not None else None,
+                          dir_z=dir_z.shape if dir_z is not None else None)
         ctx.save_for_backward(*params)
         ctx.set_materialize_grads(False)
         res = (out["rgb_coarse"], out["disp_coarse"], out["acc_coarse"],
@@ -34,20 +43,47 @@ class _RenderFn(torch.autograd.Function):
                                "next training-mode render on the same device")
         params = ctx.saved_tensors
         npar = len(PARAM_ORDER)
+        n_in = _N_IN
         if all(g is None for g in gouts):
-            return (None,) * (6 + len(params))
+            return (None,) * (n_in + len(params))
         gouts = [g if (g is not None and g.numel() > 0) else None for g in gouts]
-        grads_c, grads_f, glat = eng.backward(gouts, params[:npar], params[npar:2 * npar] if ctx.has_fine else None)
-        gpar = list(grads_c) + (list(grads_f) if ctx.has_fine else [])
-        return (None, None, None, None, None, glat.reshape(ctx.latent_shape)) + tuple(gpar)
+        need = ctx.needs_input_grad
+        want_params = any(need[n_in:])
+        inputs = []
+        if need[3]:
+            inputs += ["ray_origins", "ray_directions"]
+        if need[4]:
+            inputs.append("expression")
+        if need[6]:
+            inputs.append("background")
+        if need[7]:
+            inputs.append("dir_z")
+        grads_c, grads_f, glat, ing = eng.backward(gouts, params[:npar], params[npar:2 * npar] if ctx.has_fine else None,
+                                                   want_params=want_params, inputs=inputs)
+        if want_params:
+            gpar = tuple(grads_c) + (tuple(grads_f) if ctx.has_fine else ())
+        else:
+            gpar = (None,) * len(params)
+        g_rays = None
+        if need[3]:
+            g_rays = torch.zeros(ctx.shapes["rays"], device=glat.device, dtype=torch.float32)
+            g_rays[:, 0:3] = ing["ray_origins"]
+            g_rays[:, 3:6] = ing["ray_directions"]
+        g_expr = ing["expression"].reshape(ctx.shapes["expr"]) if need[4] else None
+        g_bg = ing["background"].reshape(ctx.shapes["background"]) if need[6] else None
+        g_dz = ing["dir_z"].reshape(ctx.shapes["dir_z"]) if need[7] else None
+        return (None, None, None, g_rays, g_expr, glat.reshape(ctx.shapes["latent"]), g_bg, g_dz) + gpar
 
 
 def render_with_grad(eng, rays, model_coarse, model_fine, expressions, latent_code, args):
+    """args: the keyword arguments of Renderer.render; its `background` and `dir_z` tensors become inputs of the graph."""
     sd_c = dict(model_coarse.named_parameters())
     params = [sd_c[k] for k in PARAM_ORDER]
     has_fine = model_fine is not None
     if has_fine:
         sd_f = dict(model_fine.named_parameters())
         params += [sd_f[k] for k in PARAM_ORDER]
-    res = _RenderFn.apply(eng, rays, args, has_fine, expressions, latent_code, *params)
+    args = dict(args)
+    background, dir_z = args.pop("background", None), args.pop("dir_z", None)
+    res = _RenderFn.apply(eng, args, has_fine, rays, expressions, latent_code, background, dir_z, *params)
     return tuple(r if r.numel() > 0 else None for r in res)

@@ -12,7 +12,7 @@ NFB_PREC_FAST, NFB_PREC_EXACT = 0, 1
 
 EXPORTS = ["nfb_version", "nfb_strerror", "nfb_last_cuda_error", "nfb_create", "nfb_destroy", "nfb_load_weights",
            "nfb_set_frame", "nfb_render_forward", "nfb_render_frame_host", "nfb_launch_count", "nfb_host_linspace",
-           "nfb_render_forward_train", "nfb_render_backward", "nfb_train_debug", "nfb_debug_schedule", "nfb_loss_mse_grad",
+           "nfb_render_forward_train", "nfb_render_backward", "nfb_render_backward_ex", "nfb_train_debug", "nfb_debug_schedule", "nfb_loss_mse_grad",
            "nfb_adam_step", "nfb_adam_step_dev", "nfb_repack", "nfb_frame_products", "nfb_sample_rays", "nfb_host_map_cdf"]
 
 
@@ -50,6 +50,11 @@ class NfbDebug(C.Structure):
 class NfbOutGrads(C.Structure):
     _fields_ = [("rgb_coarse", C.c_void_p), ("disp_coarse", C.c_void_p), ("acc_coarse", C.c_void_p),
                 ("rgb_fine", C.c_void_p), ("disp_fine", C.c_void_p), ("acc_fine", C.c_void_p), ("w_last", C.c_void_p)]
+
+
+class NfbInputGrads(C.Structure):
+    _fields_ = [("ray_origins", C.c_void_p), ("ray_directions", C.c_void_p), ("dir_z", C.c_void_p), ("background", C.c_void_p),
+                ("expression", C.c_void_p)]
 
 
 class NfbTrainDebug(C.Structure):
@@ -103,6 +108,9 @@ def _load():
                                              C.POINTER(NfbOutputs), C.c_void_p]
     lib.nfb_render_backward.argtypes = [C.c_void_p, C.POINTER(NfbOutGrads), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                         C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p]
+    lib.nfb_render_backward_ex.argtypes = [C.c_void_p, C.POINTER(NfbOutGrads), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                           C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.POINTER(NfbInputGrads),
+                                           C.c_void_p]
     lib.nfb_train_debug.argtypes = [C.c_void_p, C.POINTER(NfbTrainDebug)]
     lib.nfb_loss_mse_grad.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p]
@@ -119,7 +127,7 @@ def _load():
     lib.nfb_host_linspace.argtypes = [C.POINTER(C.c_float), C.c_int]
     for fn in ("nfb_create", "nfb_destroy", "nfb_load_weights", "nfb_set_frame", "nfb_render_forward",
                "nfb_render_frame_host", "nfb_launch_count", "nfb_host_linspace", "nfb_render_forward_train",
-               "nfb_render_backward", "nfb_train_debug", "nfb_loss_mse_grad", "nfb_adam_step", "nfb_adam_step_dev", "nfb_repack", "nfb_frame_products",
+               "nfb_render_backward", "nfb_render_backward_ex", "nfb_train_debug", "nfb_loss_mse_grad", "nfb_adam_step", "nfb_adam_step_dev", "nfb_repack", "nfb_frame_products",
                "nfb_sample_rays", "nfb_host_map_cdf"):
         getattr(lib, fn).restype = C.c_int
     return lib

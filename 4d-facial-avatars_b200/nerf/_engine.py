@@ -14,6 +14,8 @@ PARAM_ORDER = ([f"layers_xyz.{i}.{k}" for i in range(6) for k in ("weight", "bia
                + ["fc_feat.weight", "fc_feat.bias", "fc_alpha.weight", "fc_alpha.bias"]
                + [f"layers_dir.{i}.{k}" for i in range(4) for k in ("weight", "bias")]
                + ["fc_rgb.weight", "fc_rgb.bias"])
+# Members of NfbInputGrads (include/nfb.h): the input gradients Renderer.backward can return.
+INPUT_GRADS = ("ray_origins", "ray_directions", "dir_z", "background", "expression")
 
 _precision = os.environ.get("NFB_PRECISION", "fast")
 
@@ -60,6 +62,7 @@ class Renderer:
         self._versions = [None, None]
         self._keep = [None, None]  # contiguous FP32 copies handed to the pack kernels
         self.train_token = 0       # bumped by every training forward: the handle keeps ONE saved state
+        self.train_rays = 0        # rays of that forward
         weakref.finalize(self, capi.lib.nfb_destroy, h)
 
     def _params(self, model):
@@ -182,6 +185,7 @@ class Renderer:
                 dbg.act_dump, dbg.act_step = out["act"].data_ptr(), int(act_step)
         if train:
             self.train_token += 1
+            self.train_rays = n
             capi.check(capi.lib.nfb_render_forward_train(self._h, C.byref(rays), C.byref(sm), C.byref(nz) if noise else None,
                                                          C.byref(o), _stream()), "render_forward_train")
         else:
@@ -231,10 +235,13 @@ class Renderer:
                                                 _ptr(grad_latent), _stream()), "render_backward")
         self._bwd_keep = keep
 
-    def backward(self, out_grads, params_c, params_f, want_latent=True):
-        """nfb_render_backward for the last training forward.  out_grads: 7 CUDA tensors or None (rgb_c, disp_c, acc_c,
+    def backward(self, out_grads, params_c, params_f, want_latent=True, want_params=True, inputs=None):
+        """nfb_render_backward_ex for the last training forward.  out_grads: 7 CUDA tensors or None (rgb_c, disp_c, acc_c,
         rgb_f, disp_f, acc_f, w_last); params_*: the 26 FP32 parameter tensors in PARAM_ORDER (params_f None without a
-        fine network).  Returns (grads_c, grads_f, grad_latent) — lists aligned with PARAM_ORDER, None for layers_dir.3.*."""
+        fine network).  Returns (grads_c, grads_f, grad_latent) — lists aligned with PARAM_ORDER, None for layers_dir.3.*.
+        inputs: names of the input gradients wanted, out of INPUT_GRADS ("ray_origins", "ray_directions", "dir_z", "background",
+        "expression"); then a 4th element, a dict name -> tensor, is returned.  want_params=False: input-only backward (no
+        parameter gradient is formed; grads_c / grads_f are None)."""
         dev = self.device
         keep = []
         og = capi.NfbOutGrads()
@@ -255,9 +262,22 @@ class Renderer:
 
         pc, gc, grads_c = pack(params_c)
         pf, gf, grads_f = pack(params_f)
+        if not want_params:
+            gc = gf = grads_c = grads_f = None
         glat = torch.empty(32, device=dev, dtype=torch.float32) if want_latent else None
-        capi.check(capi.lib.nfb_render_backward(self._h, C.byref(og), pc, pf, gc, gf, _ptr(glat), _stream()), "render_backward")
+        ig, ing = None, {}
+        if inputs is not None:
+            n = self.train_rays
+            shapes = dict(ray_origins=(n, 3), ray_directions=(n, 3), dir_z=(n,), background=(n, 3), expression=(76,))
+            ig = capi.NfbInputGrads()
+            for name in inputs:
+                ing[name] = torch.empty(shapes[name], device=dev, dtype=torch.float32)
+                setattr(ig, name, ing[name].data_ptr())
+        capi.check(capi.lib.nfb_render_backward_ex(self._h, C.byref(og), pc, pf, gc, gf, _ptr(glat),
+                                                   C.byref(ig) if ig is not None else None, _stream()), "render_backward")
         self._bwd_keep = keep
+        if inputs is not None:
+            return grads_c, grads_f, glat, ing
         return grads_c, grads_f, glat
 
     def train_debug(self):

@@ -111,6 +111,11 @@ def data_parallel(run_fn, group=None):
         if world == 1:
             return run_fn(height, width, focal_length, model_coarse, model_fine, ray_origins, ray_directions, options, mode,
                           encode_position_fn, encode_direction_fn, expressions, background_prior, latent_code, ray_directions_ablation)
+        if torch.is_grad_enabled() and any(torch.is_tensor(t) and t.requires_grad for t in (
+                ray_origins, ray_directions, expressions, background_prior, ray_directions_ablation)):
+            raise NotImplementedError("data_parallel differentiates the parameters and the latent code only: gradients with "
+                                      "respect to rays, expressions, background or ablation directions would need all-reduces "
+                                      "it does not do (run the fit in one process)")
         rank = dist.get_rank(group)
         if mode == "validation":
             H, W = ray_directions.shape[0], ray_directions.shape[1]

@@ -62,7 +62,7 @@ def _render(rays, near, far, model_coarse, model_fine, opts, expressions, backgr
     needs_grad = torch.is_grad_enabled() and (
         any(p.requires_grad for p in model_coarse.parameters())
         or (has_fine and any(p.requires_grad for p in model_fine.parameters()))
-        or latent_code.requires_grad)
+        or any(t is not None and t.requires_grad for t in (latent_code, rays, expressions, background_prior, dir_z)))
     args = dict(near=float(near), far=float(far), num_coarse=opts["num_coarse"], num_fine=opts["num_fine"] if has_fine else 0,
                 perturb=opts["perturb"], noise_std=opts["noise_std"], white_bkgd=opts["white_bkgd"],
                 background=background_prior, dir_z=dir_z, noise=noise)

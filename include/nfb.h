@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define NFB_VERSION 120
+#define NFB_VERSION 130
 
 typedef struct NfbHandle NfbHandle;
 
@@ -194,6 +194,34 @@ typedef struct {
 int nfb_render_backward(NfbHandle* h, const NfbOutGrads* out_grads, const float* const params_coarse[26],
                         const float* const params_fine[26], float* const grads_coarse[26], float* const grads_fine[26],
                         float* grad_latent, void* stream);
+
+/* Gradients with respect to the render's inputs (device pointers; any member may be NULL = not computed).  Shapes as in
+ * NfbRays: ray_origins, ray_directions [n,3], dir_z [n], background [n,3]; expression [76] is dL/d the expression given to
+ * nfb_set_frame before the forward (before its division by 3).  Outputs are OVERWRITTEN, never accumulated.  Both passes add
+ * into the same per-ray gradients.  The near/far bounds (NfbRays.near_/far_) and the sample depths carry no gradient: the
+ * coarse depths depend only on near/far/t_rand, the fine ones are detached as in the reference (train_utils.py:124). */
+typedef struct {
+  float* ray_origins;
+  float* ray_directions;
+  float* dir_z;
+  float* background;
+  float* expression;
+} NfbInputGrads;
+
+/* nfb_render_backward plus input gradients (in_grads NULL: exactly nfb_render_backward).
+ * Input-only mode: grads_coarse and grads_fine both NULL.  No parameter gradient is formed; of the weight-gradient GEMMs only
+ * the four that yield the layer-0 / layer-3 bias sums run (d latent and d expression need them), and the finalize step runs
+ * only its latent / expression block.  This is what fitting a frozen avatar (expression, pose, latent) to images uses.
+ * params_* are still required (the input gradients multiply by the PE, conditioning and direction columns).
+ * Errors: NFB_ERR_INVALID when a dir_z or background gradient is requested and the forward had no dir_z / background;
+ * NFB_ERR_UNSUPPORTED when a ray gradient (origins, directions, dir_z) is requested after a forward that generated its rays
+ * in the kernel (NfbRays.o == NULL).  Works through the chunked backward.  The training forward saves o, d and the direction
+ * input per ray (28 B) with its other state, so no caller buffer beyond those nfb_render_backward already needs must stay
+ * alive.  In input-only mode with neither grad_latent nor in_grads->expression, the weight-gradient launch is skipped.
+ * Launches: nfb_render_backward's, plus one (background / expression only) or two (ray gradients) per chunk. */
+int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* out_grads, const float* const params_coarse[26],
+                           const float* const params_fine[26], float* const grads_coarse[26], float* const grads_fine[26],
+                           float* grad_latent, const NfbInputGrads* in_grads, void* stream);
 
 /* ---- Training-step tail: loss, optimizer, re-pack (replaces train_transformed_rays.py:355-400 for callers that adopt it;
  * the drop-in Python surface keeps working with torch.nn.functional.mse_loss + torch.optim.Adam) ----
