@@ -166,7 +166,8 @@ __device__ __forceinline__ float4 lds128(uint32_t saddr) {
 
 // ------------------------------------------------------------------ FP16 helpers
 // Two floats -> packed f16x2 with the FIRST argument in the low half (lower K index), round-to-nearest,
-// saturating to +-65504 so an out-of-range activation cannot become inf inside the tensor core.
+// saturating to +-65504 (NaN stays NaN).  For the positional encoding and exact mode's hi half, whose remainder the
+// unsaturated lo half carries; a hidden activation must not go through it alone (see pack_relu_f16x2).
 __device__ __forceinline__ uint32_t pack_f16x2(float lo_elem, float hi_elem) {
   uint32_t r;
   asm("cvt.rn.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));
@@ -179,10 +180,23 @@ __device__ __forceinline__ uint32_t pack_f16x2_inf(float lo_elem, float hi_elem)
   asm("cvt.rn.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));
   return r;
 }
-// Same as pack_f16x2 with ReLU fused into the conversion (negative inputs and NaN become +0).
+// ReLU fused into the conversion, without saturation: negative inputs become +0, NaN stays NaN, a value beyond the FP16
+// range becomes +inf.  Fast mode's hidden activations: a clamp to 65504 would give a finite, wrong render.
 __device__ __forceinline__ uint32_t pack_relu_f16x2(float lo_elem, float hi_elem) {
   uint32_t r;
-  asm("cvt.rn.relu.satfinite.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));
+  asm("cvt.rn.relu.f16x2.f32 %0, %1, %2;" : "=r"(r) : "f"(hi_elem), "f"(lo_elem));
+  return r;
+}
+// max(x, 0) that keeps NaN (fmaxf returns the non-NaN operand, torch.relu keeps the NaN).
+__device__ __forceinline__ float relu_nan(float x) {
+  float r;
+  asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(r) : "f"(x));
+  return r;
+}
+// max(a, b) that keeps NaN, as torch.max / torch.maximum do.
+__device__ __forceinline__ float fmax_nan(float a, float b) {
+  float r;
+  asm("max.NaN.f32 %0, %1, %2;" : "=f"(r) : "f"(a), "f"(b));
   return r;
 }
 __device__ __forceinline__ float2 unpack_f16x2(uint32_t p) {

@@ -205,13 +205,15 @@ __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_ba
       float x0 = __fadd_rn(acc[4 * j + 2 * hh], b.x), x1 = __fadd_rn(acc[4 * j + 2 * hh + 1], b.y);
       const float* db = hh ? dirb1 : dirb0;
       if (db) { x0 = __fadd_rn(x0, db[col]); x1 = __fadd_rn(x1, db[col + 1]); }
-      if (dump) { dump[R * 256 + col] = fmaxf(x0, 0.f); dump[R * 256 + col + 1] = fmaxf(x1, 0.f); }
+      if (dump) { dump[R * 256 + col] = relu_nan(x0); dump[R * 256 + col + 1] = relu_nan(x1); }
       uint32_t hi, lo = 0u;
       if constexpr (EXACT) {
-        const float a = fmaxf(x0, 0.f), bb = fmaxf(x1, 0.f);
+        // NaN stays NaN; hi saturates at 65504 and lo carries the rest, so hi + lo reaches ~131008 and beyond that lo is
+        // inf: out of range gives a non-finite render, never a clamped one.
+        const float a = relu_nan(x0), bb = relu_nan(x1);
         hi = pack_f16x2(a, bb);
         const float2 h = unpack_f16x2(hi);
-        lo = pack_f16x2(a - h.x, bb - h.y);
+        lo = pack_f16x2_inf(a - h.x, bb - h.y);
       } else {
         hi = pack_relu_f16x2(x0, x1);
       }
@@ -589,7 +591,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
               if (p.noise_std > 0.f && rp.valid)
                 sig = __fadd_rn(sig, __fmul_rn((pass ? p.noise_f : p.noise_c)[(size_t)rp.gidx * S + i], p.noise_std));
               const float sig_in = sig;  // what the ReLU sees (volume_rendering_utils.py:52)
-              sig = fmaxf(sig, 0.f);
+              sig = relu_nan(sig);
               float4 pre;
               if (i == S - 1) {
                 sig = __fadd_rn(sig, 1e-6f);
@@ -709,7 +711,8 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
         // ---- torch.sort(cat(z, z_samples)) (train_utils.py:126) as a rank merge: the coarse depths are sorted, the
         //      samples need not be (stochastic u), so an element's rank = (# coarse before it, by binary search)
         //      + (# samples before it, counted).  Ties: coarse first, then samples by index — equal values make any
-        //      tie order give the same sorted array.
+        //      tie order give the same sorted array.  A NaN sample (from non-finite weights) goes after every number, by
+        //      index, as torch.sort places it; no comparison with a NaN counts, so the other ranks stay as they are.
         for (int k = etid; k < R * SF; k += kRowThreads) {
           const int rr = k / SF, i = k - rr * SF;
           const float* zc = scr_sort + rr * SF;
@@ -719,6 +722,10 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
           if (i < p.nc) {
             rank = i;
             for (int j = 0; j < p.nf; ++j) rank += (zs[j] < v) ? 1 : 0;
+          } else if (v != v) {
+            const int jm = i - p.nc;
+            rank = p.nc;
+            for (int j = 0; j < p.nf; ++j) rank += (zs[j] == zs[j] || j < jm) ? 1 : 0;
           } else {
             const int jm = i - p.nc;
             int lo = 0, hi = p.nc;  // # coarse depths <= v

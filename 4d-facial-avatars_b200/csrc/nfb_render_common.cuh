@@ -99,7 +99,7 @@ __device__ __forceinline__ float composite_ray(const float4* __restrict__ pre, c
   if (lane == 0 && out_rgb) {
     if (white_bkgd) { r += 1.f - acc; g += 1.f - acc; b += 1.f - acc; }
     out_rgb[0] = r; out_rgb[1] = g; out_rgb[2] = b;
-    *out_disp = 1.f / fmaxf(1e-10f, depth / acc);
+    *out_disp = 1.f / fmax_nan(1e-10f, depth / acc);
     *out_acc = acc;
   }
   return wl;

@@ -172,14 +172,7 @@ class Renderer:
                             out["acc_fine"].data_ptr() if has_fine else None, out["w_last"].data_ptr())
         dbg = None
         if debug or act_step is not None:
-            s = num_coarse + num_fine
-            out["z_coarse"] = torch.zeros((n, num_coarse), device=dev)
-            out["raw_coarse"] = torch.zeros((n, num_coarse, 4), device=dev)
-            dbg = capi.NfbDebug(out["z_coarse"].data_ptr(), out["raw_coarse"].data_ptr(), None, None, None, 0)
-            if has_fine:
-                out["z_fine"] = torch.zeros((n, s), device=dev)
-                out["raw_fine"] = torch.zeros((n, s, 4), device=dev)
-                dbg.z_fine, dbg.raw_fine = out["z_fine"].data_ptr(), out["raw_fine"].data_ptr()
+            dbg = self._debug_dumps(out, n, num_coarse, num_fine)
             if act_step is not None:
                 out["act"] = torch.zeros((128, 256), device=dev)
                 dbg.act_dump, dbg.act_step = out["act"].data_ptr(), int(act_step)
@@ -194,6 +187,19 @@ class Renderer:
                        "render_forward")
         out["_keep"] = keep  # inputs must outlive the asynchronous launch
         return out
+
+    def _debug_dumps(self, out, n, num_coarse, num_fine):
+        """NfbDebug with the per-sample dumps (depths and MLP outputs of both passes) allocated into `out`."""
+        dev = self.device
+        out["z_coarse"] = torch.zeros((n, num_coarse), device=dev)
+        out["raw_coarse"] = torch.zeros((n, num_coarse, 4), device=dev)
+        dbg = capi.NfbDebug(out["z_coarse"].data_ptr(), out["raw_coarse"].data_ptr(), None, None, None, 0)
+        if num_fine > 0:
+            s = num_coarse + num_fine
+            out["z_fine"] = torch.zeros((n, s), device=dev)
+            out["raw_fine"] = torch.zeros((n, s, 4), device=dev)
+            dbg.z_fine, dbg.raw_fine = out["z_fine"].data_ptr(), out["raw_fine"].data_ptr()
+        return dbg
 
     def loss_mse_grad(self, rgb_c, rgb_f, target, n_total, grad_c, grad_f, loss):
         """nfb_loss_mse_grad: d mse / d rgb into grad_c / grad_f ([n,3] CUDA buffers), loss[0:2] += this shard's share."""
@@ -286,10 +292,11 @@ class Renderer:
         return d
 
     def render_camera(self, pose, intrinsics, height, width, row_begin, rows, near, far, num_coarse, num_fine,
-                      background=None, out=None, precision=None, white_bkgd=False, prof=None):
+                      background=None, out=None, precision=None, white_bkgd=False, prof=None, debug=False):
         """Deterministic render of image rows [row_begin, row_begin+rows) with in-kernel ray generation
         (no o/d tensors in HBM).  pose: 3x4 / 4x4 CPU tensor; background: [rows*width,3] CUDA tensor or None.
-        `out`: optional preallocated [11, rows*width] CUDA buffer; returns the dict of output views."""
+        `out`: optional preallocated [11, rows*width] CUDA buffer; returns the dict of output views (+ the per-sample
+        dumps of `render` when debug)."""
         dev = self.device
         n = rows * width
         if out is None:
@@ -319,9 +326,10 @@ class Renderer:
                             views["rgb_fine"].data_ptr() if has_fine else None,
                             views["disp_fine"].data_ptr() if has_fine else None,
                             views["acc_fine"].data_ptr() if has_fine else None, views["w_last"].data_ptr())
-        dbg = None
+        dbg = self._debug_dumps(views, n, num_coarse, num_fine) if debug else None
         if prof is not None:  # int64[64] CUDA tensor of phase-cycle counters
-            dbg = capi.NfbDebug()
+            if dbg is None:
+                dbg = capi.NfbDebug()
             dbg.prof = prof.data_ptr()
         capi.check(capi.lib.nfb_render_forward(self._h, C.byref(rays), C.byref(sm), None, C.byref(o),
                                                C.byref(dbg) if dbg is not None else None, _stream()), "render_forward")

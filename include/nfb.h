@@ -152,7 +152,11 @@ int nfb_load_weights(NfbHandle* h, int which, const float* const params[26], voi
 int nfb_set_frame(NfbHandle* h, const float* expression, const float* latent, void* stream);
 
 /* The hot path: coarse sampling -> encode -> coarse MLP -> composite -> inverse-CDF resample -> sort
- * -> encode -> fine MLP -> composite, one persistent sm_90a kernel launch. */
+ * -> encode -> fine MLP -> composite, one persistent sm_90a kernel launch.
+ * Non-finite values: a NaN or inf in an input (ray, background, noise draw, parameter, expression) gives non-finite outputs
+ * wherever FP32 torch would, never finite ones: the ReLUs keep NaN, and NaN fine samples sort last.  A hidden activation
+ * beyond the FP16 range (65504 in fast mode; about 131008, hi + lo, in exact mode) becomes inf, never a clamped value.
+ * Only the rays an input belongs to are affected. */
 int nfb_render_forward(NfbHandle* h, const NfbRays* rays, const NfbSampling* sampling,
                        const NfbNoise* noise /* nullable */, const NfbOutputs* out,
                        const NfbDebug* dbg /* nullable */, void* stream);
