@@ -49,6 +49,10 @@ struct NfbHandle {
     float *z_c = nullptr, *raw_c = nullptr, *z_f = nullptr, *raw_f = nullptr, *dnorm = nullptr;
     size_t cap_zc = 0, cap_rawc = 0, cap_zf = 0, cap_rawf = 0, cap_dn = 0;
     float* acc[2] = {nullptr, nullptr};                 // kAccFloats each
+    // what the backward sums in a fixed order instead of with atomics: per-ray bias sums of the compositing backward
+    // ([pass][ray][4]) and one weight-gradient partial per (network, part) (nfb::dw_workspace_floats)
+    float* bsum = nullptr; size_t cap_bsum = 0;
+    float* dw_ws = nullptr; size_t cap_ws = 0;
     float* scal = nullptr;                              // [0] scale, [1] 1/scale, [2] max |d raw| (bits)
     float* cond = nullptr;                              // [108] conditioning vector of the frame the forward rendered
     int n_rays = 0, nc = 0, nf = 0, rays_per_unit = 0, tiles_c = 0, tiles_f = 0, n_units = 0, has_bg = 0, white_bkgd = 0;
@@ -177,7 +181,7 @@ int nfb_destroy(NfbHandle* h) {
   }
   cudaFree(h->tr.lin_c); cudaFree(h->tr.lin_f);
   cudaFree(h->tr.rec); cudaFree(h->tr.draw); cudaFree(h->tr.z_c); cudaFree(h->tr.raw_c); cudaFree(h->tr.z_f); cudaFree(h->tr.raw_f);
-  cudaFree(h->tr.ray); cudaFree(h->tr.rows); cudaFree(h->tr.ray_dn); cudaFree(h->tr.ray_bg);
+  cudaFree(h->tr.ray); cudaFree(h->tr.rows); cudaFree(h->tr.ray_dn); cudaFree(h->tr.ray_bg); cudaFree(h->tr.bsum); cudaFree(h->tr.dw_ws);
   cudaFree(h->tr.dnorm); cudaFree(h->tr.scal); cudaFree(h->tr.cond); cudaFree(h->tr.scratch_out); cudaFree(h->cond);
   cudaFree(h->minmax); cudaFree(h->smp_runs); cudaFree(h->smp_segs); cudaFree(h->smp_first);
   cudaFree(h->lin_c); cudaFree(h->lin_f); cudaFree(h->d_expr); cudaFree(h->d_latent); cudaFree(h->d_bg); cudaFree(h->d_out);
@@ -285,11 +289,13 @@ static size_t train_budget(NfbHandle* h) {
   return h->train_budget = budget;
 }
 
-// (Re)size the buffers a training launch over n rays / `tiles` tiles writes.
-static int ensure_train_buffers(NfbHandle::Train& tr, size_t n, size_t tiles, int nc, int nf) {
+// (Re)size the buffers a training launch over n rays / `tiles` tiles and its backward write.
+static int ensure_train_buffers(NfbHandle::Train& tr, size_t n, size_t tiles, int nc, int nf, int num_sms) {
   int rc;
   if ((rc = ensure_cap(&tr.rec, &tr.rec_tiles, tiles * nfb::kRecBytes))) return rc;
   if ((rc = ensure_cap(&tr.draw, &tr.draw_tiles, tiles * 512))) return rc;
+  if ((rc = ensure_cap(&tr.bsum, &tr.cap_bsum, 8 * n))) return rc;
+  if ((rc = ensure_cap(&tr.dw_ws, &tr.cap_ws, nfb::dw_workspace_floats(num_sms)))) return rc;
   if ((rc = ensure_cap(&tr.z_c, &tr.cap_zc, n * nc))) return rc;
   if ((rc = ensure_cap(&tr.raw_c, &tr.cap_rawc, n * nc * 4))) return rc;
   if ((rc = ensure_cap(&tr.dnorm, &tr.cap_dn, n))) return rc;
@@ -401,7 +407,7 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
         NFB_CUDA(cudaMemcpyAsync(tr.lin_f, h->lin_f, nf * sizeof(float), cudaMemcpyDeviceToDevice, st));
         tr.full.u_fine = tr.lin_f;
       }
-    } else if ((rc = ensure_train_buffers(tr, n, tiles, nc, nf))) return rc;
+    } else if ((rc = ensure_train_buffers(tr, n, tiles, nc, nf, h->num_sms))) return rc;
     // a later nfb_set_frame (e.g. a validation render before the backward) must not change what the backward differentiates
     NFB_CUDA(cudaMemcpyAsync(tr.cond, h->cond, nfb::kDimCond * sizeof(float), cudaMemcpyDeviceToDevice, st));
     if (!tr.chunked) {
@@ -462,9 +468,9 @@ int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* con
   NFB_CUDA(cudaMemsetAsync(tr.acc[0], 0, nfb::kAccFloats * sizeof(float), st));
   NFB_CUDA(cudaMemsetAsync(tr.acc[1], 0, nfb::kAccFloats * sizeof(float), st));
 
-  // compositing backward -> dX chain -> weight-gradient GEMMs for the rays [begin, begin + n) whose training state the buffers
-  // hold; the FP32 accumulators tr.acc add up over chunks (each chunk has its own power-of-two loss scale, divided out again
-  // before the accumulation)
+  // compositing backward -> dX chain -> weight-gradient GEMMs -> fixed-order reduction for the rays [begin, begin + n) whose
+  // training state the buffers hold; the FP32 accumulators tr.acc add up over chunks in chunk order (each chunk has its own
+  // power-of-two loss scale, divided out again before the accumulation)
   auto backward_rays = [&](int begin, int n, int n_units) -> int {
     const size_t tiles = (size_t)n_units * (tr.tiles_c + tr.tiles_f);
     NFB_CUDA(cudaMemsetAsync(tr.draw, 0, tiles * 512 * sizeof(float), st));
@@ -478,7 +484,7 @@ int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* con
     auto off1 = [&](const float* p) { return p ? p + (size_t)begin : nullptr; };
     q.g_rgb[0] = off3(og->rgb_coarse); q.g_disp[0] = off1(og->disp_coarse); q.g_acc[0] = off1(og->acc_coarse);
     q.g_rgb[1] = off3(og->rgb_fine); q.g_disp[1] = off1(og->disp_fine); q.g_acc[1] = off1(og->acc_fine); q.g_wlast = off1(og->w_last);
-    q.draw = tr.draw; q.acc[0] = tr.acc[0]; q.acc[1] = tr.acc[1];
+    q.draw = tr.draw; q.bsum = tr.bsum;
     q.absmax = reinterpret_cast<unsigned int*>(tr.scal + 2);
     if (per_ray) {
       int rc;
@@ -494,14 +500,16 @@ int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* con
     c.wstream[0] = h->net[0].stream_bwd;
     c.wstream[1] = fine ? h->net[1].stream_bwd : h->net[0].stream_bwd;
     NFB_CUDA(nfb::launch_chain(c, h->num_sms, st, &h->launches));
-    if (!input_only || grad_latent || ig.expression) {  // input-only: the PE jobs only serve d latent / d expression
-      nfb::DwParams d = {};
+    const bool dw = !input_only || grad_latent || ig.expression;  // input-only: the PE jobs only serve d latent / d expression
+    nfb::DwParams d = {};
+    if (dw) {
       d.rec = tr.rec; d.n_units = n_units; d.tpu = tr.tiles_c + tr.tiles_f;
       d.t_base[0] = 0; d.t_cnt[0] = tr.tiles_c;
       d.t_base[1] = tr.tiles_c; d.t_cnt[1] = fine ? tr.tiles_f : 0;
-      d.acc[0] = tr.acc[0]; d.acc[1] = tr.acc[1]; d.scal = tr.scal;
+      d.ws = tr.dw_ws; d.scal = tr.scal;
       NFB_CUDA(nfb::launch_dw(d, h->num_sms, st, &h->launches, input_only));  // both networks in one launch
     }
+    NFB_CUDA(nfb::launch_grad_reduce(dw ? &d : nullptr, input_only, tr.bsum, n, fine ? 2 : 1, tr.acc, h->num_sms, st, &h->launches));
     if (per_ray) {
       nfb::InGradRowParams r = {};
       r.rec = tr.rec; r.n_units = n_units; r.tiles_c = tr.tiles_c; r.tiles_f = tr.tiles_f; r.rays_per_unit = tr.rays_per_unit;
@@ -531,7 +539,7 @@ int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* con
       const int n = tr.n_rays - begin < tr.chunk_rays ? tr.n_rays - begin : tr.chunk_rays;
       const int n_units = (n + R - 1) / R;
       const size_t tiles = (size_t)n_units * (tr.tiles_c + tr.tiles_f);
-      int rc = ensure_train_buffers(tr, (size_t)n, tiles, tr.nc, tr.nf);
+      int rc = ensure_train_buffers(tr, (size_t)n, tiles, tr.nc, tr.nf, h->num_sms);
       if (rc) return rc;
       if (tr.scratch_cap < 11 * (size_t)tr.chunk_rays) {
         if (tr.scratch_out) NFB_CUDA(cudaFree(tr.scratch_out));

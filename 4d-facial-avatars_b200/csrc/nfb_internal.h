@@ -70,7 +70,7 @@ struct CompBwdParams {
   const float *z_c, *raw_c, *z_f, *raw_f, *dnorm;                       // saved by the training forward
   const float *g_rgb[2], *g_disp[2], *g_acc[2], *g_wlast;               // dL/d outputs (coarse, fine); any may be null
   float* draw;                                                          // [tiles][128][4] dL/d(rgb_raw, sigma_raw), zero-initialised
-  float* acc[2];                                                        // per-network accumulators (kAccBRaw sums land here)
+  float* bsum;                                                          // [pass][ray][4] per-ray sums of d raw (grad_reduce_kernel adds them into kAccBRaw)
   unsigned int* absmax;                                                 // max |d raw| as float bits
   float *ray_dn, *ray_bg;  // non-null: input-gradient terms per (pass, ray): dL/d|d| [2][n], w_last G_rgb [2][n][3] (with a background)
 };
@@ -101,7 +101,8 @@ struct DwParams {  // ONE launch covers both networks: the first parts[0] * grou
   int n_units, tpu;
   int t_base[2], t_cnt[2];  // tiles of network i: unit * tpu + t_base[i] + [0, t_cnt[i])
   int parts[2];             // CTAs per job group of network i (set by launch_dw, proportional to the tile counts)
-  float* acc[2];
+  float* ws;                // partial sums: slot (network 0's parts, then network 1's) of ws_stride floats per part
+  int ws_stride;            // set by launch_dw: kAccBRaw, or the compact PE-only slot (nfb_train.cu dw::kPeSlotFloats)
   const float* scal;
 };
 // host copies of the compile-time schedules (nfb_debug_schedule); index < 0: number of entries; else words written or -1
@@ -110,7 +111,13 @@ int debug_dw_split(uint32_t* io);  // io: {num_sms, tiles net 0, tiles net 1} ->
 cudaError_t train_kernels_setup();
 cudaError_t launch_composite_bwd(const CompBwdParams& q, float* scal, cudaStream_t st, long long* launches);
 cudaError_t launch_chain(const ChainParams& p, int num_sms, cudaStream_t st, long long* launches);
-cudaError_t launch_dw(const DwParams& p, int num_sms, cudaStream_t st, long long* launches, bool pe_only = false);
+// Writes one partial per (network, part) into p.ws and fills in p.parts / p.ws_stride for launch_grad_reduce.
+cudaError_t launch_dw(DwParams& p, int num_sms, cudaStream_t st, long long* launches, bool pe_only = false);
+size_t dw_workspace_floats(int num_sms);  // floats of DwParams::ws that either weight-gradient launch may write
+// One launch: acc[net] += the partials of the weight-gradient launch `d` in ascending part order (d == nullptr: there was none),
+// and acc[pass][kAccBRaw..+4] += the compositing backward's per-ray sums bsum[pass][0..n_rays) in a fixed order.
+cudaError_t launch_grad_reduce(const DwParams* d, bool pe_only, const float* bsum, int n_rays, int npass, float* const acc[2], int num_sms,
+                               cudaStream_t st, long long* launches);
 // grads_c == nullptr: input-gradient-only backward (d latent and d expression alone, one small launch).
 cudaError_t launch_finalize_all(const float* const params_c[26], float* const grads_c[26], const float* acc_c,
                                 const float* const params_f[26], float* const grads_f[26], const float* acc_f, const float* cond,

@@ -13,12 +13,15 @@ namespace nfb {
 // d/d rgb of  mean((rgb - target)^2)  taken over n_total * 3 elements (n_total = the GLOBAL batch when the rays of this call
 // are one shard of it: a SUM all-reduce of the parameter gradients then yields the single-process gradient).
 // loss[0] += sum((rgb_c - t)^2) / (3 n_total), loss[1] likewise for the fine pass (each call adds its shard's share).
-__global__ void __launch_bounds__(256) loss_grad_kernel(const float* __restrict__ rgb_c, const float* __restrict__ rgb_f,
-                                                        const float* __restrict__ target, int n_elems, float inv_count,
-                                                        float* __restrict__ g_c, float* __restrict__ g_f, float* __restrict__ loss) {
-  __shared__ float part[2][8];
+// ONE block: the partial sums meet in a fixed order (thread-strided, warp butterfly, warps in order) with no atomics, so the loss
+// repeats bit for bit.  A training batch is a few thousand rays: a handful of elements per thread.
+constexpr int kLossThreads = 1024;
+__global__ void __launch_bounds__(kLossThreads) loss_grad_kernel(const float* __restrict__ rgb_c, const float* __restrict__ rgb_f,
+                                                                 const float* __restrict__ target, int n_elems, float inv_count,
+                                                                 float* __restrict__ g_c, float* __restrict__ g_f, float* __restrict__ loss) {
+  __shared__ float part[2][kLossThreads / 32];
   float sc = 0.f, sf = 0.f;
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_elems; i += gridDim.x * blockDim.x) {
+  for (int i = threadIdx.x; i < n_elems; i += kLossThreads) {
     const float t = target[i];
     const float dc = rgb_c[i] - t;
     g_c[i] = 2.f * dc * inv_count;
@@ -39,8 +42,8 @@ __global__ void __launch_bounds__(256) loss_grad_kernel(const float* __restrict_
   __syncthreads();
   if (threadIdx.x < 2) {
     float s = 0.f;
-    for (int k = 0; k < 8; ++k) s += part[threadIdx.x][k];
-    atomicAdd(loss + threadIdx.x, s * inv_count);
+    for (int k = 0; k < kLossThreads / 32; ++k) s += part[threadIdx.x][k];
+    loss[threadIdx.x] += s * inv_count;
   }
 }
 
@@ -148,9 +151,7 @@ cudaError_t launch_loss_grad(const float* rgb_c, const float* rgb_f, const float
                              float* g_f, float* loss, cudaStream_t st, long long* launches) {
   const int n = 3 * n_rays;
   if (n <= 0) return cudaSuccess;
-  int blocks = (n + 255) / 256;
-  if (blocks > 296) blocks = 296;
-  loss_grad_kernel<<<blocks, 256, 0, st>>>(rgb_c, rgb_f, target, n, 1.f / (3.f * (float)n_total), g_c, g_f, loss);
+  loss_grad_kernel<<<1, kLossThreads, 0, st>>>(rgb_c, rgb_f, target, n, 1.f / (3.f * (float)n_total), g_c, g_f, loss);
   ++*launches;
   return cudaGetLastError();
 }

@@ -7,7 +7,7 @@
 //   1. composite_bwd_kernel   G = dL/d(rgb, disp, acc, w_last) per ray  ->  dL/d(rgb_raw, sigma_raw) per sample.
 //                             Re-evaluates the compositing of both passes from what the training forward saved (depths,
 //                             colours, ReLU input of sigma) with a division-free reverse recurrence for the transmittance
-//                             term.  Also yields d fc_rgb.bias / d sigma-bias sums and the max |gradient| for the scale.
+//                             term.  Also yields per-ray d fc_rgb.bias / d sigma-bias sums and the max |gradient| for the scale.
 //   2. chain_kernel           dX chain of the MLP per 128-row tile on wgmma: 9 steps with transposed weight streams,
 //                             same machinery as the forward kernel (register accumulators, shared-memory activations
 //                             overwritten in place, the bulk-copy ring of nfb_pipeline.cuh).  The epilogue applies the saved ReLU masks and
@@ -15,8 +15,11 @@
 //   3. dw_kernel              dW[n,k] = sum_rows dY[row,n] X[row,k] for every layer: both operands are bulk-copied from
 //                             the tile records (K-major images whose K axis is the sample row) and multiplied on wgmma
 //                             (M=128 output features x N input features per job, FP32 accumulation in registers over all
-//                             tiles of the CTA), then reduced into FP32 accumulators with red.global.add.  One launch for
-//                             both networks; the job groups are laid out for L2 sharing of the input images.
+//                             tiles of the CTA), then stored as that CTA's partial.  One launch for both networks; the job
+//                             groups are laid out for L2 sharing of the input images.
+//   3b. grad_reduce_kernel    adds the partials into the FP32 accumulators in ascending part order, and the compositing
+//                             backward's per-ray bias sums in a fixed order: no floating-point atomics, so the backward
+//                             repeats bit for bit (include/nfb.h).
 //   4. finalize_kernel        un-folds the kernel's parametrisation (fc_feat pre-multiplied into fc_alpha / layers_dir.0,
 //                             conditioning columns folded into biases) by the chain rule and writes the 24 used parameter
 //                             gradients of each network in the reference's state_dict layout, plus d latent_code.
@@ -202,9 +205,8 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const CompBwdParams 
     if (lane == 0) q.ray_dn[(size_t)pass * q.n_rays + g] = gdn / dn;
   }
   if (lane == 0) {
-    float* braw = q.acc[pass] + kAccBRaw;
-    atomicAdd(braw + 0, s0); atomicAdd(braw + 1, s1); atomicAdd(braw + 2, s2); atomicAdd(braw + 3, s3);
-    if (amax == amax && amax < 3.0e38f) atomicMax(q.absmax, __float_as_uint(amax));
+    reinterpret_cast<float4*>(q.bsum)[(size_t)pass * q.n_rays + g] = make_float4(s0, s1, s2, s3);  // summed by grad_reduce_kernel
+    if (amax == amax && amax < 3.0e38f) atomicMax(q.absmax, __float_as_uint(amax));  // a max: independent of the order
   }
 }
 
@@ -382,7 +384,8 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
 namespace dw {
 
 // Roles (nfb_pipeline.cuh): warp 0 producer, warpgroups 1 and 2 = output features [64w, 64w+64) of the job's 128 on wgmma,
-// FP32 accumulators in registers over all tiles of the CTA, then reduced into the accumulators in global memory.
+// FP32 accumulators in registers over all tiles of the CTA, then stored (plain stores, one writer per element) into the
+// CTA's partial slot, which grad_reduce_kernel adds into the accumulators in global memory.
 constexpr int kStages = 4;
 constexpr int kStageBytes = 16384 + 32768;       // one r-atom (64 sample rows): A [128 features x 128 B], B [<=256 features x 128 B]
 using StageRing = Ring<kStages, kStageBytes>;
@@ -397,7 +400,7 @@ struct Job {
   int out_off, out_ld, out_row0;
 };
 // Jobs are dealt to kGroups groups of CTAs; within a group every CTA runs the group's jobs over its own share of the tiles (fewer
-// accumulator drains and atomics than every CTA running every job).  The kernel streams each job's two images of every tile
+// accumulator drains and partials than every CTA running every job).  The kernel streams each job's two images of every tile
 // once, so the groups are balanced by BYTES per tile (172..200 KB each), and groups 2q / 2q+1 are the two 128-feature output
 // halves of the SAME layers in the SAME order: they run on neighbouring CTAs over the same tiles at the same time, so the B
 // image both need (the layer's whole input, 2/3 of a job's bytes) comes from HBM once and from L2 the second time.
@@ -442,7 +445,26 @@ static_assert(make_jobs().group_begin[kGroups] == kNumJobs, "job table");
 static_assert(make_jobs().group_begin[5] - make_jobs().group_begin[4] == 3 && make_jobs().j[make_jobs().group_begin[4] + 1].b_off == kRecPE &&
                   make_jobs().j[make_jobs().group_begin[5] + 2].b_off == kRecPE && make_jobs().group_begin[6] - make_jobs().group_begin[5] == 3,
               "the PE-only weight-gradient launch runs jobs 1 and 2 of groups 4 and 5");
+static_assert(make_jobs().j[make_jobs().group_begin[4] + 1].b_rows == 64 && make_jobs().j[make_jobs().group_begin[4] + 2].b_rows == 64 &&
+                  make_jobs().j[make_jobs().group_begin[5] + 1].b_rows == 64 && make_jobs().j[make_jobs().group_begin[5] + 2].b_rows == 64,
+              "dw_kernel<true> compiles run_job for the 64-row PE image only");
 __constant__ JobTable c_jobs = make_jobs();
+
+// Partial slots.  A part of the full launch writes every accumulator below kAccBRaw exactly once (the groups' output blocks tile
+// it), so its slot mirrors that range.  A part of the PE-only launch writes four blocks only; its slot packs them as
+// [dW0 | dW3a | db0 | db3] instead of reserving kAccFloats.
+constexpr int kPeSlotFloats = 2 * 256 * 64 + 2 * 256;
+__host__ __device__ constexpr int pe_slot_off(int a) {  // accumulator offset inside one of the four blocks -> slot offset
+  return a < kAcc1 ? a : a < kAccB ? a - kAcc3a + 16384 : a < acc_bias_off(1) ? a - kAccB + 32768 : a - acc_bias_off(3) + 33024;
+}
+__host__ __device__ constexpr int pe_slot_to_acc(int e) {
+  return e < 16384 ? e : e < 32768 ? kAcc3a + (e - 16384) : e < 33024 ? kAccB + (e - 32768) : acc_bias_off(3) + (e - 33024);
+}
+static_assert(pe_slot_off(kAcc3a) == 16384 && pe_slot_off(acc_bias_off(0)) == 32768 && pe_slot_off(acc_bias_off(3)) == 33024 &&
+                  pe_slot_to_acc(pe_slot_off(acc_bias_off(3) + 255)) == acc_bias_off(3) + 255 && pe_slot_to_acc(32767) == kAcc3a + 16383,
+              "PE-only slot layout");
+static_assert(kAccBRaw % 4 == 0 && kPeSlotFloats % 4 == 0 && kAcc3a % 4 == 0 && kAccB % 4 == 0 && acc_bias_off(3) % 4 == 0,
+              "grad_reduce_kernel adds float4s");
 
 template <int N> __device__ __forceinline__ void mma_n(float (&d)[N / 2], uint64_t a, uint64_t b, uint32_t accf) {
   if constexpr (N == 16) wgmma_n16(d, a, b, accf);
@@ -451,11 +473,16 @@ template <int N> __device__ __forceinline__ void mma_n(float (&d)[N / 2], uint64
   else wgmma_n128(d, a, b, accf);
 }
 
+// kPeOnly (input-gradient-only backward): only the four jobs that read the PE image — dW0, dW3a and with them the column sums
+// db0, db3 that d latent and d expression need — i.e. groups 4 and 5 without their first (hidden-part) job.
+constexpr int kPeGroup = 4, kPeGroups = 2;
+
 // One job over the CTA's tiles j0..j1 for this warpgroup's 64 output features: NB = N of the B image (<= 128 per accumulator;
-// 256 runs as two 128-column halves).
-template <int NB>
-__device__ __forceinline__ void run_job(const Job& J, int j0, int j1, uint32_t smem_base, StageRing& ring, int wg, int lane,
-                                        float* acc_net, float inv) {
+// 256 runs as two 128-column halves).  The result and the bias column sums go to the CTA's partial slot; where exactly is
+// worked out only after the tile loop, from the parameter block, so no address stays live in registers across it.
+template <bool kPeOnly, int NB>
+__device__ __forceinline__ void run_job(const DwParams& p, const Job& J, int j0, int j1, uint32_t smem_base, StageRing& ring,
+                                        int wg, int lane) {
   constexpr int NA = NB > 128 ? 128 : NB;
   constexpr int NH = NB > 128 ? 2 : 1;
   float acc[NH][NA / 2];
@@ -482,26 +509,27 @@ __device__ __forceinline__ void run_job(const Job& J, int j0, int j1, uint32_t s
       ring.release();
     }
   }
+  constexpr int kG = kPeOnly ? kPeGroups : kGroups;
+  float* slot = p.ws + (size_t)(blockIdx.x / kG) * p.ws_stride;  // this (network, part)'s partial
+  const int bias_acc = bias ? acc_bias_off(J.bias_layer) : 0;
+  const int out_off = kPeOnly ? pe_slot_off(J.out_off) : J.out_off, bias_off = kPeOnly ? pe_slot_off(bias_acc) : bias_acc;
+  const float inv = p.scal[1];
   const int c = lane & 3, r0 = 64 * wg + 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2);
 #pragma unroll
   for (int hh = 0; hh < 2; ++hh) {
     const int R = r0 + 8 * hh;
-    float* out = acc_net + J.out_off + (size_t)(J.out_row0 + R) * J.out_ld;
+    float* out = slot + out_off + (size_t)(J.out_row0 + R) * J.out_ld;
 #pragma unroll
     for (int h = 0; h < NH; ++h)
 #pragma unroll
       for (int jj = 0; jj < NA / 8; ++jj) {
         const int col = h * 128 + 8 * jj + 2 * c;
-        atomicAdd(out + col, acc[h][4 * jj + 2 * hh] * inv);
-        atomicAdd(out + col + 1, acc[h][4 * jj + 2 * hh + 1] * inv);
+        *reinterpret_cast<float2*>(out + col) = make_float2(acc[h][4 * jj + 2 * hh] * inv, acc[h][4 * jj + 2 * hh + 1] * inv);
       }
-    if (bias && c == 0) atomicAdd(acc_net + acc_bias_off(J.bias_layer) + J.out_row0 + R, accb[2 * hh] * inv);
+    if (bias && c == 0) slot[bias_off + J.out_row0 + R] = accb[2 * hh] * inv;
   }
 }
 
-// kPeOnly (input-gradient-only backward): only the four jobs that read the PE image — dW0, dW3a and with them the column sums
-// db0, db3 that d latent and d expression need — i.e. groups 4 and 5 without their first (hidden-part) job.
-constexpr int kPeGroup = 4, kPeGroups = 2;
 template <bool kPeOnly>
 __global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__ DwParams p) {
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -554,22 +582,84 @@ __global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__
     // ============================== MMA + epilogue warpgroups ==============================
     reg_inc<kRegsRow>();
     const int wg = (warp - 4) >> 2;
-    const float inv = p.scal[1];
-    float* acc_net = p.acc[net];
     for (int job = job0; job < job1; ++job) {
       const Job J = c_jobs.j[job];
+      if constexpr (kPeOnly) {  // both PE jobs multiply by the 64-row PE image: only that shape is compiled in
+        run_job<kPeOnly, 64>(p, J, j0, j1, smem_base, ring, wg, lane);
+        continue;
+      }
       switch (J.b_rows) {
-        case 16: run_job<16>(J, j0, j1, smem_base, ring, wg, lane, acc_net, inv); break;
-        case 32: run_job<32>(J, j0, j1, smem_base, ring, wg, lane, acc_net, inv); break;
-        case 64: run_job<64>(J, j0, j1, smem_base, ring, wg, lane, acc_net, inv); break;
-        case 128: run_job<128>(J, j0, j1, smem_base, ring, wg, lane, acc_net, inv); break;
-        default: run_job<256>(J, j0, j1, smem_base, ring, wg, lane, acc_net, inv); break;
+        case 16: run_job<kPeOnly, 16>(p, J, j0, j1, smem_base, ring, wg, lane); break;
+        case 32: run_job<kPeOnly, 32>(p, J, j0, j1, smem_base, ring, wg, lane); break;
+        case 64: run_job<kPeOnly, 64>(p, J, j0, j1, smem_base, ring, wg, lane); break;
+        case 128: run_job<kPeOnly, 128>(p, J, j0, j1, smem_base, ring, wg, lane); break;
+        default: run_job<kPeOnly, 256>(p, J, j0, j1, smem_base, ring, wg, lane); break;
       }
     }
   }
 }
 
 }  // namespace dw
+
+// ================================================================================================
+// 3b. fixed-order reduction of the partials
+// ================================================================================================
+struct ReduceParams {
+  float* acc[2];
+  const float* ws;          // the weight-gradient partials (DwParams::ws)
+  int stride;               // floats per slot
+  int first1, filled[2];    // network i's partials, in part order: slots [0, filled[0]) and [first1, first1 + filled[1])
+  int net0, nets;           // the networks that have partials: [net0, net0 + nets)
+  int pe_only;              // slots in the compact PE-only layout
+  int dw_blocks;            // blocks [0, dw_blocks) add the partials; block dw_blocks + pass sums bsum[pass]
+  const float* bsum;        // [pass][n_rays][4] (CompBwdParams::bsum)
+  int n_rays;
+};
+constexpr int kBsumThreads = 256;
+__global__ void __launch_bounds__(256) grad_reduce_kernel(const ReduceParams r) {
+  if ((int)blockIdx.x >= r.dw_blocks) {
+    // d b_rgb, d b_sigma of pass `pass`: thread t sums rays t, t + 256, ... in order, then a fixed tree over the threads
+    __shared__ float4 red[kBsumThreads];
+    const int pass = (int)blockIdx.x - r.dw_blocks;
+    const float4* b = reinterpret_cast<const float4*>(r.bsum) + (size_t)pass * r.n_rays;
+    float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+    for (int g = threadIdx.x; g < r.n_rays; g += kBsumThreads) {
+      const float4 t = b[g];
+      s.x += t.x; s.y += t.y; s.z += t.z; s.w += t.w;
+    }
+    red[threadIdx.x] = s;
+    __syncthreads();
+#pragma unroll
+    for (int h = kBsumThreads / 2; h > 0; h >>= 1) {
+      if ((int)threadIdx.x < h) {
+        const float4 t = red[threadIdx.x + h];
+        float4& u = red[threadIdx.x];
+        u.x += t.x; u.y += t.y; u.z += t.z; u.w += t.w;
+      }
+      __syncthreads();
+    }
+    if (threadIdx.x < 4) {
+      const float4 t = red[0];
+      (pass ? r.acc[1] : r.acc[0])[kAccBRaw + threadIdx.x] += threadIdx.x == 0 ? t.x : threadIdx.x == 1 ? t.y : threadIdx.x == 2 ? t.z : t.w;
+    }
+    return;
+  }
+  // acc += p_0 + p_1 + ... one float4 per thread, strictly left to right: ((acc + p_0) + p_1) + ...
+  const int nv = r.stride >> 2;
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < r.nets * nv; i += r.dw_blocks * blockDim.x) {
+    const int net = r.net0 + (i >= nv ? 1 : 0), v = i >= nv ? i - nv : i;
+    const int n = net ? r.filled[1] : r.filled[0];  // (no dynamic index into the parameter block: no local copy)
+    float4* a = reinterpret_cast<float4*>((net ? r.acc[1] : r.acc[0]) + (r.pe_only ? dw::pe_slot_to_acc(4 * v) : 4 * v));
+    const float4* p = reinterpret_cast<const float4*>(r.ws + (size_t)(net ? r.first1 : 0) * r.stride) + v;
+    float4 s = *a;
+#pragma unroll 4
+    for (int k = 0; k < n; ++k) {
+      const float4 t = p[(size_t)k * nv];
+      s.x += t.x; s.y += t.y; s.z += t.z; s.w += t.w;
+    }
+    *a = s;
+  }
+}
 
 // ================================================================================================
 // 4. finalize: accumulators (folded parametrisation) -> reference parameter gradients
@@ -990,15 +1080,57 @@ int debug_dw_split(uint32_t* io) {  // in: num_sms, tiles of network 0, tiles of
   return 3;
 }
 
-cudaError_t launch_dw(const DwParams& p_in, int num_sms, cudaStream_t st, long long* launches, bool pe_only) {
-  DwParams p = p_in;
+// CTAs dw_split gives a launch (PE-only: two job groups, so num_sms / 2 CTAs per group).
+static int dw_split_sms(int num_sms, bool pe_only) { return pe_only ? num_sms * dw::kGroups / dw::kPeGroups : num_sms; }
+
+size_t dw_workspace_floats(int num_sms) {  // the most parts dw_split deals out (both networks), times the slot size
+  auto most = [](int sms) { const int parts = sms / dw::kGroups; return (size_t)(parts < 2 ? 2 : parts); };
+  const size_t full = most(dw_split_sms(num_sms, false)) * kAccBRaw, pe = most(dw_split_sms(num_sms, true)) * dw::kPeSlotFloats;
+  return full > pe ? full : pe;
+}
+
+cudaError_t launch_dw(DwParams& p, int num_sms, cudaStream_t st, long long* launches, bool pe_only) {
+  p.parts[0] = p.parts[1] = 0;
+  p.ws_stride = pe_only ? dw::kPeSlotFloats : kAccBRaw;
   const long long tot0 = (long long)p.n_units * p.t_cnt[0], tot1 = (long long)p.n_units * p.t_cnt[1];
   if (tot0 + tot1 <= 0) return cudaSuccess;
-  // PE-only: two job groups, so num_sms / 2 CTAs per group
-  dw_split(pe_only ? num_sms * dw::kGroups / dw::kPeGroups : num_sms, tot0, tot1, &p.parts[0], &p.parts[1]);
+  dw_split(dw_split_sms(num_sms, pe_only), tot0, tot1, &p.parts[0], &p.parts[1]);
   if (p.parts[0] + p.parts[1] < 1) return cudaSuccess;
   if (pe_only) dw::dw_kernel<true><<<(p.parts[0] + p.parts[1]) * dw::kPeGroups, kThreads, dw::kSmemBytes, st>>>(p);
   else dw::dw_kernel<false><<<(p.parts[0] + p.parts[1]) * dw::kGroups, kThreads, dw::kSmemBytes, st>>>(p);
+  ++*launches;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_grad_reduce(const DwParams* d, bool pe_only, const float* bsum, int n_rays, int npass, float* const acc[2], int num_sms,
+                               cudaStream_t st, long long* launches) {
+  ReduceParams r = {};
+  r.acc[0] = acc[0]; r.acc[1] = acc[1];
+  r.bsum = bsum; r.n_rays = n_rays;
+  r.pe_only = pe_only ? 1 : 0;
+  r.stride = pe_only ? dw::kPeSlotFloats : kAccBRaw;
+  if (d) {
+    r.ws = d->ws;
+    r.stride = d->ws_stride;
+    for (int net = 0; net < 2; ++net) {  // the parts dw_kernel gave tiles: the leading ones (j0 = part * per)
+      const long long total = (long long)d->n_units * d->t_cnt[net];
+      const int parts = d->parts[net];
+      if (parts > 0 && total > 0) {
+        const long long per = (total + parts - 1) / parts;
+        r.filled[net] = (int)((total + per - 1) / per);
+      }
+    }
+    r.first1 = d->parts[0];
+    r.net0 = r.filled[0] > 0 ? 0 : 1;
+    r.nets = (r.filled[0] > 0) + (r.filled[1] > 0);
+  }
+  const int work = r.nets * (r.stride / 4);  // one thread per float4 of every network that has partials
+  int blocks = (work + 255) / 256;
+  if (blocks > 8 * num_sms) blocks = 8 * num_sms;
+  r.dw_blocks = blocks;
+  const int grid = blocks + (n_rays > 0 ? npass : 0);
+  if (grid == 0) return cudaSuccess;
+  grad_reduce_kernel<<<grid, 256, 0, st>>>(r);
   ++*launches;
   return cudaGetLastError();
 }
