@@ -175,10 +175,13 @@ __device__ __forceinline__ void mlp_step_mma(Step step, WeightRing& ring, uint32
 // direction term of step 6), ReLU, FP16 hi (and lo) written in place into the activation buffer (exact mode) or packed
 // into the A fragments of the next step (fast mode: act[c_base / 4 + 2 j + hh] holds columns c_base + 8 j + 2 c, +1 of
 // row r0 + 8 hh); the training record image and ReLU mask of the layer (SAVE), and the layer probe dump.
+// SAVE: bit hh of `live` is set when row r0 + 8 hh holds a sample of a valid ray.  The other rows (the tile's rows beyond
+// R*S, the rows of an invalid ray) still go through the MLP, at points no reference evaluates; their records and masks are
+// stored as zero, so that an out-of-range activation there cannot reach a weight gradient as 0 * inf.
 template <bool EXACT, bool SAVE>
 __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_base, const float* __restrict__ bias,
                                          const float* dirb0, const float* dirb1, uint8_t* act_hi, uint8_t* act_lo,
-                                         uint32_t (&act)[64], int r0, uint8_t* rec, float* dump) {
+                                         uint32_t (&act)[64], int r0, uint8_t* rec, uint32_t live, float* dump) {
   int c = threadIdx.x & 3;
   // Fast mode unrolls the steps: without this the compiler hoists the per-thread addresses of all ten epilogues out of the
   // tile loop and keeps them in registers (spilling) across the MMAs.
@@ -206,7 +209,7 @@ __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_ba
       const float* db = hh ? dirb1 : dirb0;
       if (db) { x0 = __fadd_rn(x0, db[col]); x1 = __fadd_rn(x1, db[col + 1]); }
       if (dump) { dump[R * 256 + col] = relu_nan(x0); dump[R * 256 + col + 1] = relu_nan(x1); }
-      uint32_t hi, lo = 0u;
+      uint32_t hi, lo = 0u, saved;
       if constexpr (EXACT) {
         // NaN stays NaN; hi saturates at 65504 and lo carries the rest, so hi + lo reaches ~131008 and beyond that lo is
         // inf: out of range gives a non-finite render, never a clamped one.
@@ -214,8 +217,12 @@ __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_ba
         hi = pack_f16x2(a, bb);
         const float2 h = unpack_f16x2(hi);
         lo = pack_f16x2_inf(a - h.x, bb - h.y);
+        // the record is one FP16 value: converted without saturation, so an activation beyond its range is inf there (a
+        // non-finite weight gradient), not 65504 (a finite, wrong one); equal to hi for every activation up to 65504
+        saved = SAVE ? pack_f16x2_inf(a, bb) : hi;
       } else {
         hi = pack_relu_f16x2(x0, x1);
+        saved = hi;
       }
       if constexpr (EXACT) {
         const int off = (col >> 6) * (kTileM * 128) + sw128_offset(R, col & 63);
@@ -228,9 +235,10 @@ __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_ba
         if (rec) {
           uint8_t* img = rec + rec_x_off(s);
           uint8_t* img_j = img + (c_base + 8 * j) * 128;
-          *reinterpret_cast<uint16_t*>(img_j + img_base[hh][0]) = (uint16_t)(hi & 0xFFFFu);
-          *reinterpret_cast<uint16_t*>(img_j + img_base[hh][1]) = (uint16_t)(hi >> 16);
-          const uint32_t bits = ((hi & 0xFFFFu) ? 1u : 0u) | ((hi >> 16) ? 2u : 0u);
+          const uint32_t v = ((live >> hh) & 1u) ? saved : 0u;
+          *reinterpret_cast<uint16_t*>(img_j + img_base[hh][0]) = (uint16_t)(v & 0xFFFFu);
+          *reinterpret_cast<uint16_t*>(img_j + img_base[hh][1]) = (uint16_t)(v >> 16);
+          const uint32_t bits = ((v & 0xFFFFu) ? 1u : 0u) | ((v >> 16) ? 2u : 0u);
           mask[hh][j >> 2] |= bits << ((col & 31));
         }
       }
@@ -529,6 +537,9 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
             uint32_t act[64];  // fast mode: this thread's part of the hidden activations, as the next step's A fragments
             const int prow0 = t * 128 + r0, prow1 = prow0 + 8;
             const int ray0 = prow0 < rows ? prow0 / S : 0, ray1 = prow1 < rows ? prow1 / S : 0;
+            uint32_t live = 0u;  // SAVE: which of this thread's two rows hold a sample (see epi_half)
+            if constexpr (SAVE)
+              live = ((prow0 < rows && rayp[ray0].valid) ? 1u : 0u) | ((prow1 < rows && rayp[ray1].valid) ? 2u : 0u);
             auto mlp_step = [&](auto step) {
               const int s = step;
               const StepInfo si = step_info(s);
@@ -539,9 +550,9 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
               if (s <= 8) {
                 const float* db0 = (s == 6) ? dirbias + ray0 * 128 : nullptr;
                 const float* db1 = (s == 6) ? dirbias + ray1 * 128 : nullptr;
-                epi_half<EXACT, SAVE>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, act, r0, rec, dump);
+                epi_half<EXACT, SAVE>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, act, r0, rec, live, dump);
                 if (si.nh1 == 128)
-                  epi_half<EXACT, SAVE>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, act, r0, rec, dump);
+                  epi_half<EXACT, SAVE>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump);
                 if (s == 6 && (lane & 3) == 0) {  // sigma = first column of the 16-column half
                   const float b = bias[128];
                   tile_raw[r0].w = acc_s[0] + b;

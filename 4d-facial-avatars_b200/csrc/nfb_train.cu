@@ -173,7 +173,8 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const CompBwdParams 
       const float dalpha = Ti * (dLdw - C);
       const float dsig = dalpha * (delta * e);  // d alpha / d sigma = delta exp(-sigma delta); (1e10 * 0) stays 0
       float4 d;
-      d.w = (r4.w > 0.f) ? dsig : 0.f;          // ReLU (the +1e-6 on the last sample is an additive constant)
+      // ReLU (the +1e-6 on the last sample is an additive constant); a NaN input passes its gradient, as torch's does
+      d.w = (r4.w <= 0.f) ? 0.f : dsig;
       if constexpr (kInputs) gdn = fmaf(dsig, fmaxf(r4.w, 0.f) + (i == S - 1 ? 1e-6f : 0.f), gdn);
       if (q.has_bg && i == S - 1) {
         d.x = d.y = d.z = 0.f;                  // background colour is data (train_background=False)

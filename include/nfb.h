@@ -196,7 +196,8 @@ typedef struct {
  * the sample depths carry no gradient (z_samples.detach(), train_utils.py:124).  Gradients are OVERWRITTEN, not accumulated.
  * The call may be repeated on one saved forward with other output gradients (each call starts from zeroed accumulators).
  * A non-finite output gradient gives non-finite parameter gradients, as autograd does; so does a loss-scaled FP16 gradient
- * that overflows inside the dX chain (it is not clamped).
+ * that overflows inside the dX chain (it is not clamped), and so does a hidden activation beyond what the forward's FP16
+ * records can hold (it is recorded as inf, not 65504).  Tile rows that hold no sample never contribute: their records are zero.
  * params_fine / grads_fine may be NULL when the forward had num_fine == 0.
  * Reproducibility: the path has no floating-point atomics; every sum over rays, tiles and CTAs runs in a fixed order.  Given the
  * same library build, device model (SM count), inputs (noise tensors included), sequence of calls and chunk plan, the forward
