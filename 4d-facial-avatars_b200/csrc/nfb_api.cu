@@ -62,6 +62,8 @@ struct NfbHandle {
     float* ray = nullptr; size_t cap_ray = 0;          // [n][7] = (o, d, v0), written by the SAVE forward
     float* rows = nullptr; size_t cap_rows = 0;        // [tiles][128][4]
     float *ray_dn = nullptr, *ray_bg = nullptr; size_t cap_rdn = 0, cap_rbg = 0;
+    // what the last one-launch backward of this forward left in ray_dn / ray_bg and rows (nfb_train_debug)
+    bool per_ray_formed = false, rows_formed = false;
     // chunked mode (the records of the whole call would exceed the memory budget): the forward only produced the outputs; the
     // backward re-runs the training forward chunk by chunk from the saved launch parameters (the caller keeps the inputs alive)
     bool chunked = false;
@@ -378,6 +380,7 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
     // Saved for nfb_render_backward: per-tile activation records, sample depths, (colour, ReLU input of sigma), |d|.
     NfbHandle::Train& tr = h->tr;
     tr.valid = false;
+    tr.per_ray_formed = tr.rows_formed = false;
     const size_t n = (size_t)rays->n_rays, tiles_per_unit = (size_t)(p.tiles_c + p.tiles_f), tiles = (size_t)p.n_units * tiles_per_unit;
     int rc;
     tr.chunked = tiles * nfb::kRecBytes > train_budget(h);
@@ -467,6 +470,7 @@ int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* con
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   NFB_CUDA(cudaMemsetAsync(tr.acc[0], 0, nfb::kAccFloats * sizeof(float), st));
   NFB_CUDA(cudaMemsetAsync(tr.acc[1], 0, nfb::kAccFloats * sizeof(float), st));
+  tr.per_ray_formed = tr.rows_formed = false;
 
   // compositing backward -> dX chain -> weight-gradient GEMMs -> fixed-order reduction for the rays [begin, begin + n) whose
   // training state the buffers hold; the FP32 accumulators tr.acc add up over chunks in chunk order (each chunk has its own
@@ -533,6 +537,8 @@ int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* con
   if (!tr.chunked) {
     int rc = backward_rays(0, tr.n_rays, tr.n_units);
     if (rc) return rc;
+    tr.per_ray_formed = per_ray;
+    tr.rows_formed = ray_grads;
   } else {
     const int R = tr.rays_per_unit;
     for (int begin = 0; begin < tr.n_rays; begin += tr.chunk_rays) {
@@ -582,6 +588,10 @@ int nfb_train_debug(NfbHandle* h, NfbTrainDebug* out) {
   out->d_raw = tr.draw; out->acc_coarse = tr.acc[0]; out->acc_fine = tr.acc[1]; out->acc_floats = nfb::kAccFloats;
   out->scale = tr.scal; out->z_coarse = tr.z_c; out->raw_coarse = tr.raw_c; out->z_fine = tr.z_f; out->raw_fine = tr.raw_f;
   out->tiles_coarse = tr.tiles_c; out->tiles_fine = tr.tiles_f; out->rays_per_unit = tr.rays_per_unit;
+  out->rays = tr.ray; out->dnorm = tr.dnorm;
+  out->rows = tr.rows_formed ? tr.rows : nullptr;
+  out->ray_dn = tr.per_ray_formed ? tr.ray_dn : nullptr;
+  out->ray_bg = (tr.per_ray_formed && tr.has_bg) ? tr.ray_bg : nullptr;
   return NFB_OK;
 }
 

@@ -76,7 +76,7 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const CompBwdParams 
     if (j < per && i < S) {
       zl[j] = z[i];
       const float delta = ((i < S - 1) ? (z[i + 1] - zl[j]) : 1e10f) * dn;
-      const float sig = fmaxf(raw[i].w, 0.f) + (i == S - 1 ? 1e-6f : 0.f);
+      const float sig = relu_nan(raw[i].w) + (i == S - 1 ? 1e-6f : 0.f);  // a NaN input stays NaN, as in the forward
       e_[j] = expf(-sig * delta);
       prod *= ((1.f - (1.f - e_[j])) + 1e-10f);
     }
@@ -108,11 +108,12 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const CompBwdParams 
     depth += __shfl_xor_sync(0xffffffffu, depth, o);
     acc += __shfl_xor_sync(0xffffffffu, acc, o);
   }
-  // disp = 1 / max(1e-10, depth / acc)  (volume_rendering_utils.py:69); rgb += 1 - acc with a white background (:71-72)
+  // disp = 1 / max(1e-10, depth / acc)  (volume_rendering_utils.py:69); rgb += 1 - acc with a white background (:71-72).
+  // A NaN depth / acc passes (torch.max keeps it, so its gradient is NaN); only the clamped branch has no gradient.
   float g_depth = 0.f;
   if (gdisp != 0.f) {
     const float qv = depth / acc;
-    if (qv > 1e-10f) {
+    if (!(qv <= 1e-10f)) {
       const float dq = -gdisp / (qv * qv);
       g_depth = dq / acc;
       g_acc += -dq * depth / (acc * acc);
@@ -175,7 +176,7 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const CompBwdParams 
       float4 d;
       // ReLU (the +1e-6 on the last sample is an additive constant); a NaN input passes its gradient, as torch's does
       d.w = (r4.w <= 0.f) ? 0.f : dsig;
-      if constexpr (kInputs) gdn = fmaf(dsig, fmaxf(r4.w, 0.f) + (i == S - 1 ? 1e-6f : 0.f), gdn);
+      if constexpr (kInputs) gdn = fmaf(dsig, relu_nan(r4.w) + (i == S - 1 ? 1e-6f : 0.f), gdn);
       if (q.has_bg && i == S - 1) {
         d.x = d.y = d.z = 0.f;                  // background colour is data (train_background=False)
         if constexpr (kInputs) {
@@ -924,7 +925,10 @@ __global__ void __launch_bounds__(kThreadsRow, 1) row_kernel(const InGradRowPara
     if (rr < p.rays_per_unit && g < p.n_rays) {
       const float z = zp[(size_t)g * S + i];
       const float* ray = p.ray + 7 * (size_t)g;
-      const float px = fmaf(ray[3], z, ray[0]), py = fmaf(ray[4], z, ray[1]), pz = fmaf(ray[5], z, ray[2]);
+      // p = o + d z rounded twice, exactly as the forward encoded it (one fused rounding moves p by an ulp at times, and the
+      // 2^9 frequency turns that into a phase error)
+      const float px = __fadd_rn(ray[0], __fmul_rn(ray[3], z)), py = __fadd_rn(ray[1], __fmul_rn(ray[4], z)),
+                  pz = __fadd_rn(ray[2], __fmul_rn(ray[5], z));
 #pragma unroll
       for (int kk = 0; kk < 16; ++kk) {
         const int k = 16 * kq + kk;

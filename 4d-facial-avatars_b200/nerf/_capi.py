@@ -61,7 +61,8 @@ class NfbTrainDebug(C.Structure):
     _fields_ = [("records", C.c_void_p), ("n_tiles", C.c_longlong), ("record_bytes", C.c_int32), ("d_raw", C.c_void_p),
                 ("acc_coarse", C.c_void_p), ("acc_fine", C.c_void_p), ("acc_floats", C.c_int32), ("scale", C.c_void_p),
                 ("z_coarse", C.c_void_p), ("raw_coarse", C.c_void_p), ("z_fine", C.c_void_p), ("raw_fine", C.c_void_p),
-                ("tiles_coarse", C.c_int32), ("tiles_fine", C.c_int32), ("rays_per_unit", C.c_int32)]
+                ("tiles_coarse", C.c_int32), ("tiles_fine", C.c_int32), ("rays_per_unit", C.c_int32), ("rays", C.c_void_p),
+                ("dnorm", C.c_void_p), ("rows", C.c_void_p), ("ray_dn", C.c_void_p), ("ray_bg", C.c_void_p)]
 
 
 class NfbAdam(C.Structure):

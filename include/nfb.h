@@ -338,7 +338,8 @@ int nfb_sample_rays(NfbHandle* h, const NfbRayMap* map, const double* draws, int
  * ascending flat indices zeroed_sorted set to zero.  No CUDA call. */
 int nfb_host_map_cdf(const NfbRayMap* map, const long long* zeroed_sorted, int n_zero, const long long* ks, int n, double* out);
 
-/* Test hook: device pointers of the training state (valid until the next forward_train on the handle). */
+/* Test hook: device pointers of the training state (valid until the next forward_train on the handle).  NFB_ERR_STATE after a
+ * chunked (over-budget) forward: its buffers only ever hold one chunk. */
 typedef struct {
   const uint8_t* records;      /* n_tiles records of record_bytes (layout: nfb_layout.h kRec*) */
   long long n_tiles;
@@ -350,6 +351,16 @@ typedef struct {
   const float* scale;          /* [0] loss scale, [1] its inverse */
   const float *z_coarse, *raw_coarse, *z_fine, *raw_fine;
   int32_t tiles_coarse, tiles_fine, rays_per_unit;
+  /* What the input gradients of nfb_render_backward_ex are formed from.  rays and dnorm are the training forward's: rays
+   * [n][7] = (o, d, v0) with v0 the direction encoder's first input (dir_z, else d_z), dnorm [n] = |d| in FP32.  The other three
+   * are NULL until a backward of this forward has formed per-ray terms, and stay NULL when that backward did not need them:
+   * rows [n_tiles][128][4] = (dp, d v0) per sample row, unscaled (written when a ray gradient was requested), ray_dn
+   * [passes][n] = dL/d|d| of each pass, ray_bg [passes][n][3] = dL/d background of each pass (only with a background). */
+  const float* rays;
+  const float* dnorm;
+  const float* rows;
+  const float* ray_dn;
+  const float* ray_bg;
 } NfbTrainDebug;
 int nfb_train_debug(NfbHandle* h, NfbTrainDebug* out);
 
