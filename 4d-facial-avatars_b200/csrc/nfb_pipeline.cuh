@@ -13,7 +13,7 @@ namespace nfb {
 
 constexpr int kThreads = 384;        // producer warpgroup + 2 consumer warpgroups
 constexpr int kRowThreads = 256;     // the two consumer warpgroups
-constexpr uint32_t kRowBarrier = 1;  // named barrier id of the eight consumer warps; 2 + w: warpgroup w alone
+constexpr uint32_t kRowBarrier = 1;  // named barrier id of the eight consumer warps; 2 + w: warpgroup w alone (render_kernel: 4 + w, its MMA ping-pong)
 constexpr int kRegsLight = 40, kRegsRow = 232;
 static_assert((4 * kRegsLight + 8 * kRegsRow) * 32 <= 65536, "register file");
 template <int N> __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }

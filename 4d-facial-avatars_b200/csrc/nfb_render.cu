@@ -22,8 +22,11 @@
 // activation buffers take the space.
 //
 // Warp roles (nfb_pipeline.cuh): warp 0 = weight producer, warpgroups 1 and 2 = "row" warps.  For the per-row work
-// (sampling, positional encoding, compositing, inverse-CDF resampling, the per-ray sort) thread <-> sample row, the two
-// warpgroups splitting the columns; for the MLP each warpgroup issues the wgmma of its 64 rows and runs their epilogues.
+// (sampling, positional encoding, compositing, inverse-CDF resampling, the per-ray sort) thread <-> sample row; for the MLP
+// each warpgroup issues the wgmma of its 64 rows and runs their epilogues.  Inside a pass each warpgroup runs the tiles on
+// its own rows (prologue, MLP, post-processing) under its own named barrier; in fast mode a ping-pong of two more named
+// barriers staggers their MMA issue by one step, so one's epilogue runs under the other's MMAs.  CTA-wide barriers remain at
+// unit and pass boundaries only.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 #include <math_constants.h>
@@ -37,7 +40,7 @@
 
 namespace nfb {
 
-constexpr int kRowsMax = 512;   // sample rows of one pass of one unit of work
+constexpr int kRowsMax = 512;  // sample rows of one pass of one unit of work
 
 // shared memory map (bytes from the 1024-aligned base).  Activation buffers (exact mode only; fast mode keeps the hidden
 // activations in registers): 4 K atoms x [128 rows x 128 B], swizzled.
@@ -58,7 +61,7 @@ struct SmemMap {
   static constexpr int kBins = kCdf + kRowsMax * 4;
   static constexpr int kSort = kBins + kRowsMax * 4;
   static constexpr int kDirBias = kSort + kRowsMax * 4;
-  static constexpr int kRay = kDirBias + 2 * 128 * 4;
+  static constexpr int kRay = kDirBias + 2 * 2 * 128 * 4;  // dirbias: [pass][ray][128]
   static constexpr int kTileRaw = kRay + 2 * kRayFloats * 4;  // [128] (rgb raw, sigma raw) of the current tile
   static constexpr int kBars = kTileRaw + kTileM * 16;
   static constexpr int kBytes = kBars + 2 * kSlots * 8;
@@ -68,6 +71,16 @@ struct SmemMap {
 
 constexpr int kTileUnits = prog_units(kFwdStream);
 __constant__ ProgTable c_prog = make_prog(kFwdStream);
+
+constexpr int max_step_units() {
+  int m = 0;
+  for (int s = 0; s < kNumSteps; ++s) m = step_info(s).k_atoms > m ? step_info(s).k_atoms : m;
+  return m;
+}
+// The two row warpgroups walk the same ring and may drift apart: the one ahead holds a step's units until the other has
+// consumed them too.  Each warpgroup waits for and releases every unit of a step before its epilogue, so both can always
+// finish a step when the ring holds all of its units at once.
+static_assert(max_step_units() <= SmemMap<false>::kSlots, "a fast-mode MLP step must fit in the weight ring");
 
 // A compile-time MLP step: converts to its index, and keeps it usable as a constant expression (Step::value).
 template <int V>
@@ -104,10 +117,11 @@ __device__ __forceinline__ void mma_rs(float (&d)[8], const uint32_t* a, uint64_
 // previous step's epilogue left in registers (fast mode: act[16 a + 4 ks + i] = fragment register i of K atom a, K slice ks).
 // `step` is a StepC in fast mode (the steps unrolled, each unit's wgmmas one straight-line batch) and a
 // runtime int in exact mode, whose steps stay a loop: exact mode gains nothing from the unrolling but code size.
-template <bool EXACT, class Step, class WeightRing>
+// `issued()` runs once the step's last batch is committed, before the wait for it.
+template <bool EXACT, class Step, class WeightRing, class Issued>
 __device__ __forceinline__ void mlp_step_mma(Step step, WeightRing& ring, uint32_t act_hi, uint32_t act_lo, uint32_t pe_hi, uint32_t pe_lo,
                                              uint32_t row_off, uint32_t (&act)[64], float (&acc0)[64], float (&acc1)[64],
-                                             float (&acc_s)[8], PhaseTimer& tm) {
+                                             float (&acc_s)[8], PhaseTimer& tm, Issued&& issued) {
   constexpr int NPART = EXACT ? 2 : 1;
   constexpr int kLag = WeightRing::kLag;
   const StepInfo si = step_info(step);
@@ -149,6 +163,7 @@ __device__ __forceinline__ void mlp_step_mma(Step step, WeightRing& ring, uint32
         }
       }
       wgmma_commit();
+      if (u == si.k_atoms - 1 && part == NPART - 1) issued();
       if (u * NPART + part >= kLag) {
         wgmma_wait<kLag>();
         reg_fence(acc0);
@@ -174,11 +189,12 @@ __device__ __forceinline__ void mlp_step_mma(Step step, WeightRing& ring, uint32
 // Epilogue of one 128-column accumulator half (columns [c_base, c_base + 128)) of a ReLU layer: + bias (+ the per-ray
 // direction term of step 6), ReLU, FP16 hi (and lo) written in place into the activation buffer (exact mode) or packed
 // into the A fragments of the next step (fast mode: act[c_base / 4 + 2 j + hh] holds columns c_base + 8 j + 2 c, +1 of
-// row r0 + 8 hh); the training record image and ReLU mask of the layer (SAVE), and the layer probe dump.
+// row r0 + 8 hh); the training record image and ReLU mask of the layer (SAVE), and the layer probe dump (PROBE, when `dump`
+// is set; the production instantiations carry no probe code, which ptxas would otherwise issue as predicated stores).
 // SAVE: bit hh of `live` is set when row r0 + 8 hh holds a sample of a valid ray.  The other rows (the tile's rows beyond
 // R*S, the rows of an invalid ray) still go through the MLP, at points no reference evaluates; their records and masks are
 // stored as zero, so that an out-of-range activation there cannot reach a weight gradient as 0 * inf.
-template <bool EXACT, bool SAVE>
+template <bool EXACT, bool SAVE, bool PROBE>
 __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_base, const float* __restrict__ bias,
                                          const float* dirb0, const float* dirb1, uint8_t* act_hi, uint8_t* act_lo,
                                          uint32_t (&act)[64], int r0, uint8_t* rec, uint32_t live, float* dump) {
@@ -208,7 +224,7 @@ __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_ba
       float x0 = __fadd_rn(acc[4 * j + 2 * hh], b.x), x1 = __fadd_rn(acc[4 * j + 2 * hh + 1], b.y);
       const float* db = hh ? dirb1 : dirb0;
       if (db) { x0 = __fadd_rn(x0, db[col]); x1 = __fadd_rn(x1, db[col + 1]); }
-      if (dump) { dump[R * 256 + col] = relu_nan(x0); dump[R * 256 + col + 1] = relu_nan(x1); }
+      if (PROBE && dump) { dump[R * 256 + col] = relu_nan(x0); dump[R * 256 + col + 1] = relu_nan(x1); }
       uint32_t hi, lo = 0u, saved;
       if constexpr (EXACT) {
         // NaN stays NaN; hi saturates at 65504 and lo carries the rest, so hi + lo reaches ~131008 and beyond that lo is
@@ -267,7 +283,9 @@ __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_ba
 }
 
 // ------------------------------------------------------------------------------------------------
-template <bool EXACT, bool SAVE>
+// PROBE: the instantiation that honours the activation probe (RenderParams::dbg_act); launch_render picks it only when the
+// probe is requested.
+template <bool EXACT, bool SAVE, bool PROBE>
 __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_constant__ RenderParams p) {
   using M = SmemMap<EXACT>;
   // Use the dynamic shared array directly (no integer round trip) so the compiler keeps the shared address
@@ -306,11 +324,12 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
     // ============================== row warps ==============================
     reg_inc<kRegsRow>();
     const int q = warp & 3;
-    const int row = q * 32 + lane;     // tile row of the per-row stages
-    const int ch = (warp - 4) >> 2;    // which half of the columns this warp of the quadrant pair handles == its warpgroup
-    const int ew = warp - 4;           // 0..7, ray index for per-ray stages
-    const int etid = ch * 128 + row;   // 0..255
-    const int wg = ch;
+    const int wg = (warp - 4) >> 2;        // row warpgroup: tile rows [64 wg, 64 wg + 64)
+    const int ew = warp - 4;               // 0..7, ray index for per-ray stages
+    const int etid = wg * 128 + q * 32 + lane;  // 0..255
+    // per-tile row stages (prologue, post-processing): the warpgroup's own rows, two threads per row, one PE half each
+    const int half = q >> 1;
+    const int row = 64 * wg + (q & 1) * 32 + lane;
     const int g = 16 * q + (lane >> 2);  // MLP: first of this thread's two accumulator rows within the warpgroup's 64
     const int r0 = 64 * wg + g;          // ... as a tile row (the other one is r0 + 8)
     uint8_t* pe_hi = smem + M::kPeHi;
@@ -328,7 +347,8 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
     float4* tile_raw = reinterpret_cast<float4*>(smem + M::kTileRaw);
     const int R = p.rays_per_unit;
     const bool has_bg = p.bg != nullptr;
-    PhaseTimer tm(p.prof, p.prof != nullptr && etid == 0);
+    // observers: the first thread of each row warpgroup, warpgroup w's laps at slot + kProfWgStride * w
+    PhaseTimer tm(p.prof ? p.prof + kProfWgStride * wg : nullptr, p.prof != nullptr && (etid & 127) == 0);
 
     for (int it = 0; it < n_iter; ++it) {
       const int unit = blockIdx.x + it * gridDim.x;
@@ -384,6 +404,21 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
         rp.ped[6 * f + 3 + c] = rp.valid ? cs : 0.f;
       }
       named_bar_sync(kRowBarrier, kRowThreads);
+      // per-ray additive term of layers_dir.0 for both passes: W[:, 256:280] . PE_dir (one output feature x ray per thread
+      // and pass), read by every tile's step-6 epilogue of either warpgroup
+      {
+        const int col = etid & 127, rr = etid >> 7;
+        const RayP& rq = rayp[rr < R ? rr : 0];
+#pragma unroll 1
+        for (int pass = 0; pass < 2; ++pass) {
+          const float* wt = p.wd0b_t[pass];
+          float acc0 = 0.f;
+#pragma unroll 8
+          for (int j = 0; j < kDimDir; ++j) acc0 = fmaf(wt[j * 128 + col], rq.ped[j], acc0);
+          dirbias[(2 * pass + rr) * 128 + col] = acc0;
+        }
+      }
+      named_bar_sync(kRowBarrier, kRowThreads);
       tm.lap(0);
 
 
@@ -421,7 +456,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
                 const float tr = rp.valid ? p.t_rand[(size_t)rp.gidx * p.nc + i] : 0.f;
                 z = __fadd_rn(lower, __fmul_rn(__fsub_rn(upper, lower), tr));
               }
-              if (ch == 0) carry_z[prow] = z;
+              if (half == 0) carry_z[prow] = z;
             } else {
               z = carry_z[prow];
             }
@@ -432,7 +467,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
           const float py = __fadd_rn(rp.o[1], __fmul_rn(rp.d[1], z));
           const float pz = __fadd_rn(rp.o[2], __fmul_rn(rp.d[2], z));
           float f[32];
-          if (ch == 0) {  // lanes 0..31: xyz, frequencies 0..3, sin of frequency 4, cos(x), cos(y) of frequency 4
+          if (half == 0) {  // lanes 0..31: xyz, frequencies 0..3, sin of frequency 4, cos(x), cos(y) of frequency 4
             f[0] = px; f[1] = py; f[2] = pz;
 #pragma unroll
             for (int fr = 0; fr < 4; ++fr) {
@@ -445,7 +480,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
             pe_sincos<EXACT>(px * 16.f, f[27], f[30]);
             pe_sincos<EXACT>(py * 16.f, f[28], f[31]);
             pe_sincos<EXACT>(pz * 16.f, f[29], cz);
-          } else {        // lanes 32..63: cos(z) of frequency 4, frequencies 5..9, zero pad
+          } else {          // lanes 32..63: cos(z) of frequency 4, frequencies 5..9, zero pad
             float sz;
             pe_sincos<EXACT>(pz * 16.f, sz, f[0]);
 #pragma unroll
@@ -470,13 +505,13 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
                 lo[e] = pack_f16x2(a - hf.x, b - hf.y);
               }
             }
-            const int off = row * 128 + (((ch * 4 + qq) ^ (row & 7)) << 4);
+            const int off = row * 128 + (((half * 4 + qq) ^ (row & 7)) << 4);
             *reinterpret_cast<uint4*>(pe_hi + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
             if constexpr (EXACT) *reinterpret_cast<uint4*>(pe_lo + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
           }
-          if (p.dbg_act && p.dbg_act_step == -1 && unit == 0 && pass == 0 && t == 0) {
+          if (PROBE && p.dbg_act && p.dbg_act_step == -1 && unit == 0 && pass == 0 && t == 0) {
 #pragma unroll
-            for (int k = 0; k < 32; ++k) p.dbg_act[row * 256 + ch * 32 + k] = f[k];
+            for (int k = 0; k < 32; ++k) p.dbg_act[row * 256 + half * 32 + k] = f[k];
           }
           if constexpr (SAVE) {  // FP16 encoding of this tile as a transposed image (input of layers_xyz.0 / .3 in dW)
             if (unit < p.n_units) {
@@ -484,7 +519,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
               uint32_t hh[16];
 #pragma unroll
               for (int e = 0; e < 16; ++e) hh[e] = pack_f16x2(f[2 * e], f[2 * e + 1]);
-              store_t32(rec + kRecPE + img_row_base(64, row), row, 32 * ch, hh);
+              store_t32(rec + kRecPE + img_row_base(64, row), row, 32 * half, hh);
             }
           }
           fence_proxy_async_smem();  // make the generic-proxy PE stores visible to the tensor core
@@ -493,15 +528,6 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
 
         for (int t = 0; t < n_tiles; ++t) {
           prologue(t);
-          if (t == 0) {
-            // per-ray additive term of layers_dir.0: W[:, 256:280] . PE_dir (one output feature x ray per thread)
-            const float* wt = p.wd0b_t[pass];
-            const RayP& rq = rayp[ch < R ? ch : 0];
-            float acc0 = 0.f;
-#pragma unroll 8
-            for (int j = 0; j < kDimDir; ++j) acc0 = fmaf(wt[j * 128 + row], rq.ped[j], acc0);
-            dirbias[ch * 128 + row] = acc0;
-          }
           uint8_t* rec = nullptr;  // this tile's training record (SAVE mode)
           if constexpr (SAVE) {
             if (unit < p.n_units) {
@@ -509,10 +535,10 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
               const bool live = prow < rows;
               const RayP& rp = rayp[live ? prow / S : 0];
               rec = p.save_rec + (size_t)(unit * tiles_per_unit + (pass ? p.tiles_c : 0) + t) * kRecBytes;
-              uint32_t hh[8];  // direction encoding of this row's ray: features [16*ch, 16*ch+16)
+              uint32_t hh[8];  // direction encoding of this row's ray: features [16*half, 16*half+16)
 #pragma unroll
               for (int e = 0; e < 8; ++e) {
-                const int k = 16 * ch + 2 * e;
+                const int k = 16 * half + 2 * e;
                 const float a = (live && rp.valid && k < kDimDir) ? rp.ped[k] : 0.f;
                 const float b = (live && rp.valid && k + 1 < kDimDir) ? rp.ped[k + 1] : 0.f;
                 hh[e] = pack_f16x2(a, b);
@@ -521,18 +547,20 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
               const uint32_t cr = (uint32_t)((row & 63) >> 3);
 #pragma unroll
               for (int e = 0; e < 8; ++e) {
-                const int ka = 16 * ch + 2 * e, kb = ka + 1;
+                const int ka = 16 * half + 2 * e, kb = ka + 1;
                 *reinterpret_cast<uint16_t*>(img + ka * 128 + ((cr ^ (uint32_t)(ka & 7)) << 4)) = (uint16_t)(hh[e] & 0xFFFFu);
                 *reinterpret_cast<uint16_t*>(img + kb * 128 + ((cr ^ (uint32_t)(kb & 7)) << 4)) = (uint16_t)(hh[e] >> 16);
               }
             }
           }
-          named_bar_sync(kRowBarrier, kRowThreads);  // PE buffer, carry_z and (t == 0) dirbias complete
+          // this warpgroup's PE rows complete.  Nothing else inside the tile is shared between the warpgroups: each reads
+          // and writes only its own 64 rows of the PE buffer, the activation buffers, tile_raw and the carry buffers.
+          named_bar_sync(2 + wg, 128);
           tm.lap(2);
 
           // ---- the MLP: this warpgroup's 64 rows
           {
-            const bool probe = p.dbg_act && unit == 0 && pass == 0 && t == 0;
+            const bool probe = PROBE && p.dbg_act && unit == 0 && pass == 0 && t == 0;
             float acc0[64], acc1[64], acc_s[8];
             uint32_t act[64];  // fast mode: this thread's part of the hidden activations, as the next step's A fragments
             const int prow0 = t * 128 + r0, prow1 = prow0 + 8;
@@ -543,16 +571,26 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
             auto mlp_step = [&](auto step) {
               const int s = step;
               const StepInfo si = step_info(s);
+              // Fast mode staggers the warpgroups (ping-pong): warpgroup 1 issues step s after warpgroup 0 has issued it, and
+              // warpgroup 0 issues step s + 1 after warpgroup 1 has issued step s, so one's epilogue runs under the other's
+              // MMAs.  Barrier 4 + w is the one warpgroup w waits on.  The pairs close within a pass: warpgroup 0 does not
+              // wait before the pass's first step, warpgroup 1 does not arrive after its last.  Exact mode's one-slot ring
+              // already keeps the warpgroups within one unit of each other, and a forced order there would deadlock it.
+              const bool pp_wait = !EXACT && (wg == 1 || s > 0 || t > 0);
+              const bool pp_arrive = !EXACT && (wg == 0 || s < kNumSteps - 1 || t < n_tiles - 1);
+              if (pp_wait) named_bar_sync(4 + wg, 256);
+              tm.lap(15);
+              auto issued = [&] { if (pp_arrive) named_bar_arrive(5 - wg, 256); };
               mlp_step_mma<EXACT>(step, ring, smem_base + M::kActHi, smem_base + M::kActLo, smem_base + M::kPeHi,
-                                     smem_base + M::kPeLo, (uint32_t)(64 * wg * 128), act, acc0, acc1, acc_s, tm);
+                                  smem_base + M::kPeLo, (uint32_t)(64 * wg * 128), act, acc0, acc1, acc_s, tm, issued);
               float* dump = (probe && p.dbg_act_step == s) ? p.dbg_act : nullptr;
               const float* bias = bias_n + si.bias_off;
               if (s <= 8) {
-                const float* db0 = (s == 6) ? dirbias + ray0 * 128 : nullptr;
-                const float* db1 = (s == 6) ? dirbias + ray1 * 128 : nullptr;
-                epi_half<EXACT, SAVE>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, act, r0, rec, live, dump);
+                const float* db0 = (s == 6) ? dirbias + (2 * pass + ray0) * 128 : nullptr;
+                const float* db1 = (s == 6) ? dirbias + (2 * pass + ray1) * 128 : nullptr;
+                epi_half<EXACT, SAVE, PROBE>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, act, r0, rec, live, dump);
                 if (si.nh1 == 128)
-                  epi_half<EXACT, SAVE>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump);
+                  epi_half<EXACT, SAVE, PROBE>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump);
                 if (s == 6 && (lane & 3) == 0) {  // sigma = first column of the 16-column half
                   const float b = bias[128];
                   tile_raw[r0].w = acc_s[0] + b;
@@ -581,11 +619,12 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
               static_for<0, kNumSteps>(mlp_step);
             }
           }
-          named_bar_sync(kRowBarrier, kRowThreads);  // tile_raw complete; PE and activation buffers free
+          named_bar_sync(2 + wg, 128);  // this warpgroup's rows of tile_raw complete
           tm.lap(14);
           // fc_rgb output.  Prepare what compositing needs per sample: colour and sigma (volume_rendering_utils.py:29-33,
-          // 41-53); the exp(-sigma*delta) needs the neighbour depth and stays in composite_ray.
-          if (ch == 0) {
+          // 41-53); the exp(-sigma*delta) needs the neighbour depth and stays in composite_ray.  One thread per row of the
+          // warpgroup's 64.
+          if (half == 0) {
             const int prow = t * 128 + row;
             const bool live = prow < rows;
             const int r = live ? prow / S : 0;
@@ -622,7 +661,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
           }
           tm.lap(13);
         }  // tiles
-        named_bar_sync(kRowBarrier, kRowThreads);
+        named_bar_sync(kRowBarrier, kRowThreads);  // carry_raw and carry_z of the pass complete
         tm.lap(3);
 
         // ---- debug dump of the sample depths
@@ -759,27 +798,43 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
   }
 }
 
+template <bool EXACT, bool SAVE, bool PROBE>
+static cudaError_t render_setup_one() {
+  return cudaFuncSetAttribute(render_kernel<EXACT, SAVE, PROBE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemMap<EXACT>::kBytes);
+}
+// The training forward takes no debug dumps (nfb_render_forward_train), so only the evaluation kernels have a probe
+// instantiation.
+template <bool EXACT, bool SAVE>
+static void render_launch(const RenderParams& p, bool probe, int grid, cudaStream_t st) {
+  if constexpr (!SAVE) {
+    if (probe) {
+      render_kernel<EXACT, false, true><<<grid, kThreads, SmemMap<EXACT>::kBytes, st>>>(p);
+      return;
+    }
+  }
+  render_kernel<EXACT, SAVE, false><<<grid, kThreads, SmemMap<EXACT>::kBytes, st>>>(p);
+}
+
 cudaError_t render_kernel_setup() {
-  cudaError_t e = cudaFuncSetAttribute(render_kernel<false, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemMap<false>::kBytes);
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(render_kernel<true, false>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemMap<true>::kBytes);
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(render_kernel<false, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemMap<false>::kBytes);
-  if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(render_kernel<true, true>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemMap<true>::kBytes);
+  const cudaError_t e[6] = {render_setup_one<false, false, false>(), render_setup_one<true, false, false>(),
+                            render_setup_one<false, true, false>(),  render_setup_one<true, true, false>(),
+                            render_setup_one<false, false, true>(),  render_setup_one<true, false, true>()};
+  for (const cudaError_t x : e)
+    if (x != cudaSuccess) return x;
+  return cudaSuccess;
 }
 
 cudaError_t launch_render(const RenderParams& p, int precision, int num_sms, cudaStream_t st, long long* launches) {
   const int grid = p.n_units < num_sms ? p.n_units : num_sms;
   if (grid <= 0) return cudaSuccess;
   const bool save = p.save_rec != nullptr;  // training forward: also writes the per-tile activation records
-  const size_t smem = precision == 1 ? SmemMap<true>::kBytes : SmemMap<false>::kBytes;
+  const bool probe = p.dbg_act != nullptr;  // the activation probe (evaluation only): its own instantiation
   if (precision == 1) {
-    if (save) render_kernel<true, true><<<grid, kThreads, smem, st>>>(p);
-    else render_kernel<true, false><<<grid, kThreads, smem, st>>>(p);
+    if (save) render_launch<true, true>(p, probe, grid, st);
+    else render_launch<true, false>(p, probe, grid, st);
   } else {
-    if (save) render_kernel<false, true><<<grid, kThreads, smem, st>>>(p);
-    else render_kernel<false, false><<<grid, kThreads, smem, st>>>(p);
+    if (save) render_launch<false, true>(p, probe, grid, st);
+    else render_launch<false, false>(p, probe, grid, st);
   }
   ++*launches;
   return cudaGetLastError();

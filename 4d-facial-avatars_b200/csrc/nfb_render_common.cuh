@@ -112,6 +112,7 @@ __device__ __forceinline__ float composite_ray(const float4* __restrict__ pre, c
 #ifndef NFB_TIMERS
 #define NFB_TIMERS 0
 #endif
+constexpr int kProfWgStride = 20;  // render kernel: row warpgroup w's observer writes its laps at slot + 20 w (slots < 40)
 #if NFB_TIMERS
 struct PhaseTimer {
   unsigned long long* dst;

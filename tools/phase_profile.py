@@ -1,9 +1,9 @@
 """Phase-cycle profile of the render kernels (NfbDebug.prof).  Usage: python tools/phase_profile.py [fast|exact] [H W [NC NF]]
 
 Needs a library with the timers compiled in: `python 4d-facial-avatars_b200/build.py --timers` (lib/libnfb_timers.so, picked
-up here unless NFB_LIB is set).  The observer is one row-warp thread per CTA (warpgroup 0); its cycles are summed over CTAs
-and reported per tile (MLP phases) and per unit of work (per-ray phases).  "wait MMAs" includes issuing them and releasing
-the weight slots."""
+up here unless NFB_LIB is set).  The observers are the first thread of each row warpgroup of every CTA (warpgroup w's laps at
+slot + 20 w); their cycles are summed over CTAs and reported per tile (MLP phases) and per unit of work (per-ray phases), one
+column per warpgroup.  "wait MMAs" includes issuing them and releasing the weight slots."""
 import os
 import sys
 
@@ -50,15 +50,17 @@ tiles_per_unit = -(-R * NC // 128) + (-(-R * (NC + NF) // 128) if NF > 0 else 0)
 units = -(-H * W // R)
 ctas = min(torch.cuda.get_device_properties(dev).multi_processor_count, units)
 tiles = units * tiles_per_unit
-per_tile = {2: "prologue (z + PE)", 10: "wait weights (wait_full)", 11: "wait MMAs", 12: "epilogue", 14: "end-of-MLP barrier",
-            13: "post-processing"}
+per_tile = {2: "prologue (z + PE)", 15: "ping-pong wait", 10: "wait weights (wait_full)", 11: "wait MMAs", 12: "epilogue",
+            14: "end-of-MLP barrier", 13: "post-processing"}
 per_unit = {39: "unit loop", 0: "ray setup", 3: "end-of-pass barrier", 4: "composite", 5: "cdf", 6: "inverse-cdf", 7: "sort"}
-total = sum(c[i] for i in list(per_tile) + list(per_unit))
+WG = 20  # slot stride between the two row warpgroups' observers (nfb_render_common.cuh: kProfWgStride)
+total = [sum(c[i + WG * w] for i in list(per_tile) + list(per_unit)) for w in (0, 1)]
 print(f"{prec} {H}x{W} {NC}c+{NF}f: {ms:.2f} ms, {H*W/ms*1e3:.3e} rays/s; {R} rays/unit, {tiles_per_unit} tiles/unit, "
-      f"{tiles/ctas:.0f} tiles per CTA; row-warp observer {total/ctas/1e6:.2f} Mcycles per CTA")
-print(f"{'phase':28s} {'cycles/tile':>12s} {'share':>7s}")
+      f"{tiles/ctas:.0f} tiles per CTA; observers {total[0]/ctas/1e6:.2f} / {total[1]/ctas/1e6:.2f} Mcycles per CTA")
+share = lambda v, w: 100 * v / total[w] if total[w] else 0.0  # noqa: E731
+print(f"{'phase':28s} {'wg0 cycles/tile':>16s} {'share':>7s} {'wg1 cycles/tile':>16s} {'share':>7s}")
 for i, name in per_tile.items():
-    print(f"{name:28s} {c[i]/tiles:12.0f} {100*c[i]/total:6.1f}%")
-print(f"{'phase':28s} {'cycles/unit':>12s} {'share':>7s}")
+    print(f"{name:28s} " + " ".join(f"{c[i + WG * w] / tiles:16.0f} {share(c[i + WG * w], w):6.1f}%" for w in (0, 1)))
+print(f"{'phase':28s} {'wg0 cycles/unit':>16s} {'share':>7s} {'wg1 cycles/unit':>16s} {'share':>7s}")
 for i, name in per_unit.items():
-    print(f"{name:28s} {c[i]/units:12.0f} {100*c[i]/total:6.1f}%")
+    print(f"{name:28s} " + " ".join(f"{c[i + WG * w] / units:16.0f} {share(c[i + WG * w], w):6.1f}%" for w in (0, 1)))
