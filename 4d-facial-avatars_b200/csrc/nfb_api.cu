@@ -25,10 +25,9 @@ int cuda_fail(cudaError_t e, const char* where) {
     cudaError_t e__ = (call);                            \
     if (e__ != cudaSuccess) return cuda_fail(e__, #call); \
   } while (0)
-
-template <class T>
-cudaError_t dev_alloc(T** p, size_t n) { return cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)); }
 }  // namespace
+
+using nfb::DevBuf;
 
 struct NfbHandle {
   int device = 0;
@@ -36,32 +35,30 @@ struct NfbHandle {
   nfb::NetBuffers net[2];
   bool frame_set = false;
   long long launches = 0;
-  // cached torch.linspace(0,1,n) tables on the device
-  float* lin_c = nullptr; int lin_c_n = 0;
-  float* lin_f = nullptr; int lin_f_n = 0;
+  // cached torch.linspace(0,1,n) tables on the device, and the n each was filled for
+  DevBuf<float> lin_c, lin_f;
+  int lin_c_n = 0, lin_f_n = 0;
   // staging for nfb_render_frame_host
-  float *d_expr = nullptr, *d_latent = nullptr, *d_bg = nullptr, *d_out = nullptr;
-  size_t bg_cap = 0, out_cap = 0;
+  DevBuf<float> d_expr, d_latent, d_bg, d_out;
   // training state: what nfb_render_forward_train saved for nfb_render_backward (grow-only buffers)
   struct Train {
-    uint8_t* rec = nullptr; size_t rec_tiles = 0;       // per-tile activation records (nfb_layout.h kRec*)
-    float* draw = nullptr; size_t draw_tiles = 0;       // [tiles][128][4]
-    float *z_c = nullptr, *raw_c = nullptr, *z_f = nullptr, *raw_f = nullptr, *dnorm = nullptr;
-    size_t cap_zc = 0, cap_rawc = 0, cap_zf = 0, cap_rawf = 0, cap_dn = 0;
-    float* acc[2] = {nullptr, nullptr};                 // kAccFloats each
+    DevBuf<uint8_t> rec;                                // per-tile activation records (nfb_layout.h kRec*)
+    DevBuf<float> draw;                                 // [tiles][128][4]
+    DevBuf<float> z_c, raw_c, z_f, raw_f, dnorm;
+    DevBuf<float> acc[2];                               // kAccFloats each
     // what the backward sums in a fixed order instead of with atomics: per-ray bias sums of the compositing backward
     // ([pass][ray][4]) and one weight-gradient partial per (network, part) (nfb::dw_workspace_floats)
-    float* bsum = nullptr; size_t cap_bsum = 0;
-    float* dw_ws = nullptr; size_t cap_ws = 0;
-    float* scal = nullptr;                              // [0] scale, [1] 1/scale, [2] max |d raw| (bits)
-    float* cond = nullptr;                              // [108] conditioning vector of the frame the forward rendered
-    int n_rays = 0, nc = 0, nf = 0, rays_per_unit = 0, tiles_c = 0, tiles_f = 0, n_units = 0, has_bg = 0, white_bkgd = 0;
+    DevBuf<float> bsum, dw_ws;
+    DevBuf<float> scal;                                 // [0] scale, [1] 1/scale, [2] max |d raw| (bits)
+    DevBuf<float> cond;                                 // [108] conditioning vector of the frame the forward rendered
+    nfb::TileGeom geom = {};                            // of the whole forward call
+    int has_bg = 0, white_bkgd = 0;
     bool valid = false;
     // for input gradients (nfb_render_backward_ex): the forward's rays (copied unless chunked), per-row / per-ray scratch
     bool has_rays = false, has_dir_z = false;
-    float* ray = nullptr; size_t cap_ray = 0;          // [n][7] = (o, d, v0), written by the SAVE forward
-    float* rows = nullptr; size_t cap_rows = 0;        // [tiles][128][4]
-    float *ray_dn = nullptr, *ray_bg = nullptr; size_t cap_rdn = 0, cap_rbg = 0;
+    DevBuf<float> ray;                                  // [n][7] = (o, d, v0), written by the SAVE forward
+    DevBuf<float> rows;                                 // [tiles][128][4]
+    DevBuf<float> ray_dn, ray_bg;
     // what the last one-launch backward of this forward left in ray_dn / ray_bg and rows (nfb_train_debug)
     bool per_ray_formed = false, rows_formed = false;
     // chunked mode (the records of the whole call would exceed the memory budget): the forward only produced the outputs; the
@@ -70,30 +67,19 @@ struct NfbHandle {
     nfb::RenderParams full;      // the forward call's parameters (pointers into caller memory)
     // handle-owned state `full` points at, copied at the forward: the folded per-frame biases (nfb_set_frame overwrites
     // bias_frame in place) and the linspace tables when they came from the handle's cache (a later sample count replaces it)
-    float* bias[2] = {nullptr, nullptr};
-    float *lin_c = nullptr, *lin_f = nullptr; size_t cap_lin_c = 0, cap_lin_f = 0;
+    DevBuf<float> bias[2];
+    DevBuf<float> lin_c, lin_f;
     int chunk_rays = 0, precision = 0;
-    float* scratch_out = nullptr; size_t scratch_cap = 0;   // [11 * chunk_rays] outputs of the re-run forwards (discarded)
+    DevBuf<float> scratch_out;   // [11 * chunk_rays] outputs of the re-run forwards (discarded)
   } tr;
   size_t train_budget = 0;       // bytes the per-tile records of one launch may take (0: not decided yet)
-  float* cond = nullptr;  // [108] = [expression / 3 ; latent] of the current frame
+  DevBuf<float> cond;            // [108] = [expression / 3 ; latent] of the current frame
   // scratch of the steps either side of the path
-  uint32_t* minmax = nullptr;                           // disparity-image min / max keys
-  nfb::smp::Run* smp_runs = nullptr; nfb::smp::Seg* smp_segs = nullptr; int* smp_first = nullptr; long long smp_first_n = 0;
+  DevBuf<uint32_t> minmax;       // disparity-image min / max keys
+  DevBuf<nfb::smp::Run> smp_runs;
+  DevBuf<nfb::smp::Seg> smp_segs;
+  DevBuf<int> smp_first;
 };
-
-namespace {
-template <class T>
-int ensure_cap(T** p, size_t* cap, size_t n) {
-  if (*cap >= n && *p) return NFB_OK;
-  if (*p) NFB_CUDA(cudaFree(*p));
-  *p = nullptr;
-  *cap = 0;
-  NFB_CUDA(cudaMalloc(reinterpret_cast<void**>(p), n * sizeof(T)));
-  *cap = n;
-  return NFB_OK;
-}
-}  // namespace
 
 extern "C" {
 
@@ -128,24 +114,24 @@ static int create_impl(NfbHandle* h, const cudaDeviceProp& prop) {
   h->num_sms = prop.multiProcessorCount;
   for (int n = 0; n < 2; ++n) {
     nfb::NetBuffers& nb = h->net[n];
-    NFB_CUDA(dev_alloc(&nb.stream_x1, nfb::kStreamBytesX1));
-    NFB_CUDA(dev_alloc(&nb.stream_x3, nfb::kStreamBytesX3));
-    NFB_CUDA(dev_alloc(&nb.w6, 144 * 256));
-    NFB_CUDA(dev_alloc(&nb.b6, 144));
-    NFB_CUDA(dev_alloc(&nb.bias_static, nfb::kBiasFloats));
-    NFB_CUDA(dev_alloc(&nb.bias_frame, nfb::kBiasFloats));
-    NFB_CUDA(dev_alloc(&nb.w0c, 256 * nfb::kDimCond));
-    NFB_CUDA(dev_alloc(&nb.w3c, 256 * nfb::kDimCond));
-    NFB_CUDA(dev_alloc(&nb.wd0b_t, nfb::kDimDir * 128));
-    NFB_CUDA(dev_alloc(&nb.stream_bwd, nfb::kBwdStreamBytes));
-    NFB_CUDA(dev_alloc(&h->tr.acc[n], nfb::kAccFloats));
+    NFB_CUDA(nb.stream_x1.reserve(nfb::kStreamBytesX1));
+    NFB_CUDA(nb.stream_x3.reserve(nfb::kStreamBytesX3));
+    NFB_CUDA(nb.w6.reserve(144 * 256));
+    NFB_CUDA(nb.b6.reserve(144));
+    NFB_CUDA(nb.bias_static.reserve(nfb::kBiasFloats));
+    NFB_CUDA(nb.bias_frame.reserve(nfb::kBiasFloats));
+    NFB_CUDA(nb.w0c.reserve(256 * nfb::kDimCond));
+    NFB_CUDA(nb.w3c.reserve(256 * nfb::kDimCond));
+    NFB_CUDA(nb.wd0b_t.reserve(nfb::kDimDir * 128));
+    NFB_CUDA(nb.stream_bwd.reserve(nfb::kBwdStreamBytes));
+    NFB_CUDA(h->tr.acc[n].reserve(nfb::kAccFloats));
   }
-  NFB_CUDA(dev_alloc(&h->tr.scal, 4));
-  NFB_CUDA(dev_alloc(&h->tr.cond, nfb::kDimCond));
-  NFB_CUDA(dev_alloc(&h->cond, nfb::kDimCond));
+  NFB_CUDA(h->tr.scal.reserve(4));
+  NFB_CUDA(h->tr.cond.reserve(nfb::kDimCond));
+  NFB_CUDA(h->cond.reserve(nfb::kDimCond));
   NFB_CUDA(nfb::train_kernels_setup());
-  NFB_CUDA(dev_alloc(&h->d_expr, nfb::kDimExpr));
-  NFB_CUDA(dev_alloc(&h->d_latent, nfb::kDimLatent));
+  NFB_CUDA(h->d_expr.reserve(nfb::kDimExpr));
+  NFB_CUDA(h->d_latent.reserve(nfb::kDimLatent));
   NFB_CUDA(nfb::render_kernel_setup());
   return NFB_OK;
 }
@@ -164,7 +150,7 @@ int nfb_create(const NfbModelDims* dims, int device, NfbHandle** out) {
   if (!h) return NFB_ERR_INVALID;
   h->device = device;
   const int rc = create_impl(h, prop);
-  if (rc != NFB_OK) {  // free whatever was allocated before the failure
+  if (rc != NFB_OK) {  // frees whatever was allocated before the failure
     nfb_destroy(h);
     return rc;
   }
@@ -175,18 +161,6 @@ int nfb_create(const NfbModelDims* dims, int device, NfbHandle** out) {
 int nfb_destroy(NfbHandle* h) {
   if (!h) return NFB_ERR_INVALID;
   cudaSetDevice(h->device);
-  for (int n = 0; n < 2; ++n) {
-    nfb::NetBuffers& nb = h->net[n];
-    cudaFree(nb.stream_x1); cudaFree(nb.stream_x3); cudaFree(nb.w6); cudaFree(nb.b6); cudaFree(nb.bias_static);
-    cudaFree(nb.bias_frame); cudaFree(nb.w0c); cudaFree(nb.w3c); cudaFree(nb.wd0b_t); cudaFree(nb.stream_bwd);
-    cudaFree(h->tr.acc[n]); cudaFree(h->tr.bias[n]);
-  }
-  cudaFree(h->tr.lin_c); cudaFree(h->tr.lin_f);
-  cudaFree(h->tr.rec); cudaFree(h->tr.draw); cudaFree(h->tr.z_c); cudaFree(h->tr.raw_c); cudaFree(h->tr.z_f); cudaFree(h->tr.raw_f);
-  cudaFree(h->tr.ray); cudaFree(h->tr.rows); cudaFree(h->tr.ray_dn); cudaFree(h->tr.ray_bg); cudaFree(h->tr.bsum); cudaFree(h->tr.dw_ws);
-  cudaFree(h->tr.dnorm); cudaFree(h->tr.scal); cudaFree(h->tr.cond); cudaFree(h->tr.scratch_out); cudaFree(h->cond);
-  cudaFree(h->minmax); cudaFree(h->smp_runs); cudaFree(h->smp_segs); cudaFree(h->smp_first);
-  cudaFree(h->lin_c); cudaFree(h->lin_f); cudaFree(h->d_expr); cudaFree(h->d_latent); cudaFree(h->d_bg); cudaFree(h->d_out);
   delete h;
   return NFB_OK;
 }
@@ -255,21 +229,19 @@ int nfb_set_frame(NfbHandle* h, const float* expression, const float* latent, vo
   NFB_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   nfb::NetBuffers* const nbs[2] = {&h->net[0], &h->net[1]};
-  NFB_CUDA(nfb::launch_frame_fold(nbs, h->net[1].loaded ? 2 : 1, expression, latent, h->cond, st, &h->launches));
+  NFB_CUDA(nfb::launch_frame_fold(nbs, h->net[1].loaded ? 2 : 1, expression, latent, h->cond.get(), st, &h->launches));
   h->frame_set = true;
   return NFB_OK;
 }
 
-static int ensure_linspace(float** buf, int* cached_n, int n, cudaStream_t st) {
-  if (*cached_n == n && *buf) return NFB_OK;
+static int ensure_linspace(DevBuf<float>& buf, int* cached_n, int n, cudaStream_t st) {
+  if (*cached_n == n && buf.get()) return NFB_OK;
   std::vector<float> host(n);
   nfb_host_linspace(host.data(), n);
-  if (*buf) NFB_CUDA(cudaFree(*buf));
-  *buf = nullptr;
   *cached_n = 0;
-  NFB_CUDA(dev_alloc(buf, (size_t)n));
+  NFB_CUDA(buf.reserve((size_t)n));
   // pageable source: the runtime stages it before returning, so `host` may die afterwards
-  NFB_CUDA(cudaMemcpyAsync(*buf, host.data(), n * sizeof(float), cudaMemcpyHostToDevice, st));
+  NFB_CUDA(cudaMemcpyAsync(buf.get(), host.data(), n * sizeof(float), cudaMemcpyHostToDevice, st));
   *cached_n = n;
   return NFB_OK;
 }
@@ -291,20 +263,20 @@ static size_t train_budget(NfbHandle* h) {
   return h->train_budget = budget;
 }
 
-// (Re)size the buffers a training launch over n rays / `tiles` tiles and its backward write.
-static int ensure_train_buffers(NfbHandle::Train& tr, size_t n, size_t tiles, int nc, int nf, int num_sms) {
-  int rc;
-  if ((rc = ensure_cap(&tr.rec, &tr.rec_tiles, tiles * nfb::kRecBytes))) return rc;
-  if ((rc = ensure_cap(&tr.draw, &tr.draw_tiles, tiles * 512))) return rc;
-  if ((rc = ensure_cap(&tr.bsum, &tr.cap_bsum, 8 * n))) return rc;
-  if ((rc = ensure_cap(&tr.dw_ws, &tr.cap_ws, nfb::dw_workspace_floats(num_sms)))) return rc;
-  if ((rc = ensure_cap(&tr.z_c, &tr.cap_zc, n * nc))) return rc;
-  if ((rc = ensure_cap(&tr.raw_c, &tr.cap_rawc, n * nc * 4))) return rc;
-  if ((rc = ensure_cap(&tr.dnorm, &tr.cap_dn, n))) return rc;
-  if ((rc = ensure_cap(&tr.ray, &tr.cap_ray, 7 * n))) return rc;
-  if (nf > 0) {
-    if ((rc = ensure_cap(&tr.z_f, &tr.cap_zf, n * (nc + nf)))) return rc;
-    if ((rc = ensure_cap(&tr.raw_f, &tr.cap_rawf, n * (nc + nf) * 4))) return rc;
+// (Re)size the buffers a training launch of geometry g and its backward write.
+static int ensure_train_buffers(NfbHandle::Train& tr, const nfb::TileGeom& g, int num_sms) {
+  const size_t n = (size_t)g.n_rays, tiles = g.tiles();
+  NFB_CUDA(tr.rec.reserve(tiles * nfb::kRecBytes));
+  NFB_CUDA(tr.draw.reserve(tiles * 512));
+  NFB_CUDA(tr.bsum.reserve(8 * n));
+  NFB_CUDA(tr.dw_ws.reserve(nfb::dw_workspace_floats(num_sms)));
+  NFB_CUDA(tr.z_c.reserve(n * g.samples(0)));
+  NFB_CUDA(tr.raw_c.reserve(n * g.samples(0) * 4));
+  NFB_CUDA(tr.dnorm.reserve(n));
+  NFB_CUDA(tr.ray.reserve(7 * n));
+  if (g.passes() == 2) {
+    NFB_CUDA(tr.z_f.reserve(n * g.samples(1)));
+    NFB_CUDA(tr.raw_f.reserve(n * g.samples(1) * 4));
   }
   return NFB_OK;
 }
@@ -330,7 +302,7 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
 
   nfb::RenderParams p;
   std::memset(&p, 0, sizeof(p));
-  p.o = rays->o; p.d = rays->d; p.n_rays = rays->n_rays;
+  p.o = rays->o; p.d = rays->d;
   for (int i = 0; i < 12; ++i) p.pose[i] = rays->pose[i];
   p.fx = static_cast<float>(rays->intrinsics[0]);
   p.fy = static_cast<float>(rays->intrinsics[1]);
@@ -340,34 +312,30 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
   p.row_begin = rays->row_begin;
   p.near_ = rays->near_; p.far_ = rays->far_;
   p.dir_z = rays->dir_z; p.bg = rays->background;
-  p.nc = nc; p.nf = nf; p.s_fine = nc + nf;
-  p.rays_per_unit = (2 * (nc + nf) <= 512) ? 2 : 1;
-  p.tiles_c = (p.rays_per_unit * nc + 127) / 128;
-  p.tiles_f = nf > 0 ? (p.rays_per_unit * (nc + nf) + 127) / 128 : 0;
-  p.n_units = (rays->n_rays + p.rays_per_unit - 1) / p.rays_per_unit;
+  p.geom = nfb::TileGeom::make(rays->n_rays, nc, nf);
   p.perturb = sm->perturb ? 1 : 0;
   p.noise_std = sm->noise_std;
   p.white_bkgd = sm->white_background ? 1 : 0;
   if (sm->t_coarse) p.t_coarse = sm->t_coarse;
   else {
-    int rc = ensure_linspace(&h->lin_c, &h->lin_c_n, nc, st);
+    int rc = ensure_linspace(h->lin_c, &h->lin_c_n, nc, st);
     if (rc) return rc;
-    p.t_coarse = h->lin_c;
+    p.t_coarse = h->lin_c.get();
   }
   if (nf > 0) {
     if (sm->u_fine) p.u_fine = sm->u_fine;
     else {
-      int rc = ensure_linspace(&h->lin_f, &h->lin_f_n, nf, st);
+      int rc = ensure_linspace(h->lin_f, &h->lin_f_n, nf, st);
       if (rc) return rc;
-      p.u_fine = h->lin_f;
+      p.u_fine = h->lin_f.get();
     }
   }
   if (noise) { p.t_rand = noise->t_rand; p.noise_c = noise->sigma_noise_c; p.u_rand = noise->u; p.noise_f = noise->sigma_noise_f; }
   const bool exact = sm->precision == NFB_PREC_EXACT;
   for (int n = 0; n < 2; ++n) {
-    p.wstream[n] = exact ? h->net[n].stream_x3 : h->net[n].stream_x1;
-    p.bias[n] = h->net[n].bias_frame;
-    p.wd0b_t[n] = h->net[n].wd0b_t;
+    p.wstream[n] = exact ? h->net[n].stream_x3.get() : h->net[n].stream_x1.get();
+    p.bias[n] = h->net[n].bias_frame.get();
+    p.wd0b_t[n] = h->net[n].wd0b_t.get();
   }
   if (nf == 0) { p.wstream[1] = p.wstream[0]; p.bias[1] = p.bias[0]; p.wd0b_t[1] = p.wd0b_t[0]; }
   p.rgb_c = out->rgb_coarse; p.disp_c = out->disp_coarse; p.acc_c = out->acc_coarse;
@@ -381,46 +349,44 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
     NfbHandle::Train& tr = h->tr;
     tr.valid = false;
     tr.per_ray_formed = tr.rows_formed = false;
-    const size_t n = (size_t)rays->n_rays, tiles_per_unit = (size_t)(p.tiles_c + p.tiles_f), tiles = (size_t)p.n_units * tiles_per_unit;
     int rc;
-    tr.chunked = tiles * nfb::kRecBytes > train_budget(h);
+    tr.chunked = p.geom.tiles() * nfb::kRecBytes > train_budget(h);
     if (tr.chunked) {
       // e.g. a whole frame rendered with gradients enabled: 1.5-2 MiB of records per ray.  Keep the launch parameters, produce
       // the outputs with the evaluation kernel now, and let the backward re-run the training forward in chunks that fit.
       if (!rays->o) { g_last_cuda_error = "training forward over budget needs explicit rays (o, d)"; return NFB_ERR_UNSUPPORTED; }
-      size_t units = train_budget(h) / nfb::kRecBytes / tiles_per_unit;
+      size_t units = train_budget(h) / nfb::kRecBytes / (size_t)p.geom.tiles_per_unit();
       if (units < 1) units = 1;
-      tr.chunk_rays = (int)(units * p.rays_per_unit);
+      tr.chunk_rays = (int)(units * p.geom.rays_per_unit);
       tr.full = p;
       tr.precision = exact ? 1 : 0;
       // the re-run forwards must read THIS call's frame and depth tables, whatever is rendered before the backward
       for (int n = 0; n < (nf > 0 ? 2 : 1); ++n) {
-        if (!tr.bias[n]) NFB_CUDA(dev_alloc(&tr.bias[n], nfb::kBiasFloats));
-        NFB_CUDA(cudaMemcpyAsync(tr.bias[n], h->net[n].bias_frame, nfb::kBiasFloats * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        tr.full.bias[n] = tr.bias[n];
+        NFB_CUDA(tr.bias[n].reserve(nfb::kBiasFloats));
+        NFB_CUDA(cudaMemcpyAsync(tr.bias[n].get(), h->net[n].bias_frame.get(), nfb::kBiasFloats * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        tr.full.bias[n] = tr.bias[n].get();
       }
       if (nf == 0) tr.full.bias[1] = tr.full.bias[0];
-      if (p.t_coarse == h->lin_c) {
-        if ((rc = ensure_cap(&tr.lin_c, &tr.cap_lin_c, (size_t)nc))) return rc;
-        NFB_CUDA(cudaMemcpyAsync(tr.lin_c, h->lin_c, nc * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        tr.full.t_coarse = tr.lin_c;
+      if (p.t_coarse == h->lin_c.get()) {
+        NFB_CUDA(tr.lin_c.reserve((size_t)nc));
+        NFB_CUDA(cudaMemcpyAsync(tr.lin_c.get(), h->lin_c.get(), nc * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        tr.full.t_coarse = tr.lin_c.get();
       }
-      if (nf > 0 && p.u_fine == h->lin_f) {
-        if ((rc = ensure_cap(&tr.lin_f, &tr.cap_lin_f, (size_t)nf))) return rc;
-        NFB_CUDA(cudaMemcpyAsync(tr.lin_f, h->lin_f, nf * sizeof(float), cudaMemcpyDeviceToDevice, st));
-        tr.full.u_fine = tr.lin_f;
+      if (nf > 0 && p.u_fine == h->lin_f.get()) {
+        NFB_CUDA(tr.lin_f.reserve((size_t)nf));
+        NFB_CUDA(cudaMemcpyAsync(tr.lin_f.get(), h->lin_f.get(), nf * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        tr.full.u_fine = tr.lin_f.get();
       }
-    } else if ((rc = ensure_train_buffers(tr, n, tiles, nc, nf, h->num_sms))) return rc;
+    } else if ((rc = ensure_train_buffers(tr, p.geom, h->num_sms))) return rc;
     // a later nfb_set_frame (e.g. a validation render before the backward) must not change what the backward differentiates
-    NFB_CUDA(cudaMemcpyAsync(tr.cond, h->cond, nfb::kDimCond * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    NFB_CUDA(cudaMemcpyAsync(tr.cond.get(), h->cond.get(), nfb::kDimCond * sizeof(float), cudaMemcpyDeviceToDevice, st));
     if (!tr.chunked) {
-      p.save_rec = tr.rec; p.save_dnorm = tr.dnorm; p.save_raw_c = tr.raw_c; p.save_raw_f = tr.raw_f;
-      p.dbg_z_c = tr.z_c; p.dbg_z_f = tr.z_f;
-      p.save_ray = tr.ray;  // the rays, for input gradients (the backward does not read the caller's buffers)
+      p.save_rec = tr.rec.get(); p.save_dnorm = tr.dnorm.get(); p.save_raw_c = tr.raw_c.get(); p.save_raw_f = tr.raw_f.get();
+      p.dbg_z_c = tr.z_c.get(); p.dbg_z_f = tr.z_f.get();
+      p.save_ray = tr.ray.get();  // the rays, for input gradients (the backward does not read the caller's buffers)
     }
     tr.has_rays = rays->o != nullptr; tr.has_dir_z = rays->dir_z != nullptr;
-    tr.n_rays = rays->n_rays; tr.nc = nc; tr.nf = nf; tr.rays_per_unit = p.rays_per_unit; tr.tiles_c = p.tiles_c;
-    tr.tiles_f = p.tiles_f; tr.n_units = p.n_units; tr.has_bg = rays->background != nullptr; tr.white_bkgd = p.white_bkgd;
+    tr.geom = p.geom; tr.has_bg = rays->background != nullptr; tr.white_bkgd = p.white_bkgd;
   }
   NFB_CUDA(nfb::launch_render(p, exact ? 1 : 0, h->num_sms, st, &h->launches));
   if (train) h->tr.valid = true;
@@ -450,7 +416,7 @@ int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* con
   if (!h || !og || !params_coarse) return NFB_ERR_INVALID;
   NfbHandle::Train& tr = h->tr;
   if (!tr.valid) return NFB_ERR_STATE;
-  const bool fine = tr.nf > 0;
+  const bool fine = tr.geom.passes() == 2;
   const bool input_only = !grads_coarse && !grads_fine;
   if (input_only && !in_grads) return NFB_ERR_INVALID;
   if (!input_only && !grads_coarse) return NFB_ERR_INVALID;
@@ -468,65 +434,63 @@ int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* con
   const bool per_ray = ray_grads || ig.background;
   NFB_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  NFB_CUDA(cudaMemsetAsync(tr.acc[0], 0, nfb::kAccFloats * sizeof(float), st));
-  NFB_CUDA(cudaMemsetAsync(tr.acc[1], 0, nfb::kAccFloats * sizeof(float), st));
+  float* const acc[2] = {tr.acc[0].get(), tr.acc[1].get()};
+  NFB_CUDA(cudaMemsetAsync(acc[0], 0, nfb::kAccFloats * sizeof(float), st));
+  NFB_CUDA(cudaMemsetAsync(acc[1], 0, nfb::kAccFloats * sizeof(float), st));
   tr.per_ray_formed = tr.rows_formed = false;
 
-  // compositing backward -> dX chain -> weight-gradient GEMMs -> fixed-order reduction for the rays [begin, begin + n) whose
-  // training state the buffers hold; the FP32 accumulators tr.acc add up over chunks in chunk order (each chunk has its own
-  // power-of-two loss scale, divided out again before the accumulation)
-  auto backward_rays = [&](int begin, int n, int n_units) -> int {
-    const size_t tiles = (size_t)n_units * (tr.tiles_c + tr.tiles_f);
-    NFB_CUDA(cudaMemsetAsync(tr.draw, 0, tiles * 512 * sizeof(float), st));
-    NFB_CUDA(cudaMemsetAsync(tr.scal, 0, 4 * sizeof(float), st));
+  // compositing backward -> dX chain -> weight-gradient GEMMs -> fixed-order reduction for the g.n_rays rays from `begin` on,
+  // whose training state the buffers hold; the FP32 accumulators tr.acc add up over chunks in chunk order (each chunk has its
+  // own power-of-two loss scale, divided out again before the accumulation)
+  auto backward_rays = [&](int begin, const nfb::TileGeom& g) -> int {
+    const size_t n = (size_t)g.n_rays, tiles = g.tiles();
+    float* const scal = tr.scal.get();
+    NFB_CUDA(cudaMemsetAsync(tr.draw.get(), 0, tiles * 512 * sizeof(float), st));
+    NFB_CUDA(cudaMemsetAsync(scal, 0, 4 * sizeof(float), st));
     nfb::CompBwdParams q;
     std::memset(&q, 0, sizeof(q));
-    q.n_rays = n; q.nc = tr.nc; q.nf = tr.nf; q.s_fine = tr.nc + tr.nf; q.rays_per_unit = tr.rays_per_unit;
-    q.tiles_c = tr.tiles_c; q.tiles_f = tr.tiles_f; q.has_bg = tr.has_bg; q.white_bkgd = tr.white_bkgd;
-    q.z_c = tr.z_c; q.raw_c = tr.raw_c; q.z_f = tr.z_f; q.raw_f = tr.raw_f; q.dnorm = tr.dnorm;
+    nfb::ChainParams c;
+    nfb::DwParams d = {};
+    nfb::InGradRowParams r = {};
+    nfb::InGradRayParams a = {};
+    q.geom = c.geom = d.geom = r.geom = a.geom = g;
+    q.has_bg = tr.has_bg; q.white_bkgd = tr.white_bkgd;
+    q.z_c = tr.z_c.get(); q.raw_c = tr.raw_c.get(); q.z_f = tr.z_f.get(); q.raw_f = tr.raw_f.get(); q.dnorm = tr.dnorm.get();
     auto off3 = [&](const float* p) { return p ? p + 3 * (size_t)begin : nullptr; };
     auto off1 = [&](const float* p) { return p ? p + (size_t)begin : nullptr; };
     q.g_rgb[0] = off3(og->rgb_coarse); q.g_disp[0] = off1(og->disp_coarse); q.g_acc[0] = off1(og->acc_coarse);
     q.g_rgb[1] = off3(og->rgb_fine); q.g_disp[1] = off1(og->disp_fine); q.g_acc[1] = off1(og->acc_fine); q.g_wlast = off1(og->w_last);
-    q.draw = tr.draw; q.bsum = tr.bsum;
-    q.absmax = reinterpret_cast<unsigned int*>(tr.scal + 2);
+    q.draw = tr.draw.get(); q.bsum = tr.bsum.get();
+    q.absmax = reinterpret_cast<unsigned int*>(scal + 2);
     if (per_ray) {
-      int rc;
-      if ((rc = ensure_cap(&tr.ray_dn, &tr.cap_rdn, 2 * (size_t)n)) || (rc = ensure_cap(&tr.ray_bg, &tr.cap_rbg, 6 * (size_t)n))) return rc;
-      if (ray_grads && (rc = ensure_cap(&tr.rows, &tr.cap_rows, tiles * 512))) return rc;
-      q.ray_dn = tr.ray_dn; q.ray_bg = tr.ray_bg;
+      NFB_CUDA(tr.ray_dn.reserve(2 * n));
+      NFB_CUDA(tr.ray_bg.reserve(6 * n));
+      if (ray_grads) NFB_CUDA(tr.rows.reserve(tiles * 512));
+      q.ray_dn = tr.ray_dn.get(); q.ray_bg = tr.ray_bg.get();
     }
-    NFB_CUDA(nfb::launch_composite_bwd(q, tr.scal, st, &h->launches));
+    NFB_CUDA(nfb::launch_composite_bwd(q, scal, st, &h->launches));
 
-    nfb::ChainParams c;
-    c.n_units = n_units; c.tiles_c = tr.tiles_c; c.tiles_f = tr.tiles_f;
-    c.rec = tr.rec; c.draw = tr.draw; c.scal = tr.scal;
-    c.wstream[0] = h->net[0].stream_bwd;
-    c.wstream[1] = fine ? h->net[1].stream_bwd : h->net[0].stream_bwd;
+    c.rec = tr.rec.get(); c.draw = tr.draw.get(); c.scal = scal;
+    c.wstream[0] = h->net[0].stream_bwd.get();
+    c.wstream[1] = h->net[fine ? 1 : 0].stream_bwd.get();
     NFB_CUDA(nfb::launch_chain(c, h->num_sms, st, &h->launches));
     const bool dw = !input_only || grad_latent || ig.expression;  // input-only: the PE jobs only serve d latent / d expression
-    nfb::DwParams d = {};
     if (dw) {
-      d.rec = tr.rec; d.n_units = n_units; d.tpu = tr.tiles_c + tr.tiles_f;
-      d.t_base[0] = 0; d.t_cnt[0] = tr.tiles_c;
-      d.t_base[1] = tr.tiles_c; d.t_cnt[1] = fine ? tr.tiles_f : 0;
-      d.ws = tr.dw_ws; d.scal = tr.scal;
+      d.rec = tr.rec.get(); d.ws = tr.dw_ws.get(); d.scal = scal;
       NFB_CUDA(nfb::launch_dw(d, h->num_sms, st, &h->launches, input_only));  // both networks in one launch
     }
-    NFB_CUDA(nfb::launch_grad_reduce(dw ? &d : nullptr, input_only, tr.bsum, n, fine ? 2 : 1, tr.acc, h->num_sms, st, &h->launches));
+    NFB_CUDA(nfb::launch_grad_reduce(dw ? &d : nullptr, input_only, tr.bsum.get(), g.n_rays, g.passes(), acc, h->num_sms, st,
+                                     &h->launches));
     if (per_ray) {
-      nfb::InGradRowParams r = {};
-      r.rec = tr.rec; r.n_units = n_units; r.tiles_c = tr.tiles_c; r.tiles_f = tr.tiles_f; r.rays_per_unit = tr.rays_per_unit;
-      r.nc = tr.nc; r.s_fine = tr.nc + tr.nf; r.n_rays = n;
-      r.z_c = tr.z_c; r.z_f = tr.z_f; r.ray = tr.ray; r.scal = tr.scal;
+      r.rec = tr.rec.get();
+      r.z_c = tr.z_c.get(); r.z_f = tr.z_f.get(); r.ray = tr.ray.get(); r.scal = scal;
       const float* const* pf = fine ? params_fine : params_coarse;
       r.w0[0] = params_coarse[0]; r.w3[0] = params_coarse[6]; r.wd0[0] = params_coarse[16];
       r.w0[1] = pf[0]; r.w3[1] = pf[6]; r.wd0[1] = pf[16];
-      r.out = tr.rows;
-      nfb::InGradRayParams a = {};
-      a.n_rays = n; a.nc = tr.nc; a.nf = tr.nf; a.s_fine = tr.nc + tr.nf; a.rays_per_unit = tr.rays_per_unit;
-      a.tiles_c = tr.tiles_c; a.tiles_f = tr.tiles_f; a.has_dir_z = tr.has_dir_z;
-      a.z_c = tr.z_c; a.z_f = tr.z_f; a.ray = tr.ray; a.dnorm = tr.dnorm; a.ray_dn = tr.ray_dn; a.ray_bg = tr.ray_bg;
+      r.out = tr.rows.get();
+      a.has_dir_z = tr.has_dir_z;
+      a.z_c = tr.z_c.get(); a.z_f = tr.z_f.get(); a.ray = tr.ray.get(); a.dnorm = tr.dnorm.get();
+      a.ray_dn = tr.ray_dn.get(); a.ray_bg = tr.ray_bg.get();
       auto at = [&](float* p, int w) { return p ? p + (size_t)w * begin : nullptr; };
       a.g_o = at(ig.ray_origins, 3); a.g_d = at(ig.ray_directions, 3); a.g_dir_z = at(ig.dir_z, 1); a.g_bg = at(ig.background, 3);
       NFB_CUDA(nfb::launch_input_grads(r, a, h->num_sms, st, &h->launches));
@@ -535,47 +499,41 @@ int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* con
   };
 
   if (!tr.chunked) {
-    int rc = backward_rays(0, tr.n_rays, tr.n_units);
+    int rc = backward_rays(0, tr.geom);
     if (rc) return rc;
     tr.per_ray_formed = per_ray;
     tr.rows_formed = ray_grads;
   } else {
-    const int R = tr.rays_per_unit;
-    for (int begin = 0; begin < tr.n_rays; begin += tr.chunk_rays) {
-      const int n = tr.n_rays - begin < tr.chunk_rays ? tr.n_rays - begin : tr.chunk_rays;
-      const int n_units = (n + R - 1) / R;
-      const size_t tiles = (size_t)n_units * (tr.tiles_c + tr.tiles_f);
-      int rc = ensure_train_buffers(tr, (size_t)n, tiles, tr.nc, tr.nf, h->num_sms);
+    const int n_rays = tr.geom.n_rays;
+    for (int begin = 0; begin < n_rays; begin += tr.chunk_rays) {
+      const nfb::TileGeom g = tr.geom.chunk(n_rays - begin < tr.chunk_rays ? n_rays - begin : tr.chunk_rays);
+      int rc = ensure_train_buffers(tr, g, h->num_sms);
       if (rc) return rc;
-      if (tr.scratch_cap < 11 * (size_t)tr.chunk_rays) {
-        if (tr.scratch_out) NFB_CUDA(cudaFree(tr.scratch_out));
-        tr.scratch_out = nullptr; tr.scratch_cap = 0;
-        NFB_CUDA(dev_alloc(&tr.scratch_out, 11 * (size_t)tr.chunk_rays));
-        tr.scratch_cap = 11 * (size_t)tr.chunk_rays;
-      }
+      const size_t cn = (size_t)tr.chunk_rays;
+      NFB_CUDA(tr.scratch_out.reserve(11 * cn));
       // the training forward of this chunk: the saved launch with every per-ray pointer advanced to `begin`
       nfb::RenderParams p = tr.full;
       const size_t b = (size_t)begin;
-      p.o += 3 * b; p.d += 3 * b; p.n_rays = n; p.n_units = n_units;
+      p.o += 3 * b; p.d += 3 * b; p.geom = g;
       if (p.dir_z) p.dir_z += b;
       if (p.bg) p.bg += 3 * b;
-      if (p.t_rand) p.t_rand += b * tr.nc;
-      if (p.noise_c) p.noise_c += b * tr.nc;
-      if (p.u_rand) p.u_rand += b * tr.nf;
-      if (p.noise_f) p.noise_f += b * (tr.nc + tr.nf);
-      float* so = tr.scratch_out;
-      const size_t cn = (size_t)tr.chunk_rays;
+      if (p.t_rand) p.t_rand += b * g.nc;
+      if (p.noise_c) p.noise_c += b * g.nc;
+      if (p.u_rand) p.u_rand += b * g.nf;
+      if (p.noise_f) p.noise_f += b * g.samples(1);
+      float* so = tr.scratch_out.get();
       p.rgb_c = so; p.disp_c = so + 3 * cn; p.acc_c = so + 4 * cn; p.rgb_f = so + 5 * cn; p.disp_f = so + 8 * cn; p.acc_f = so + 9 * cn;
       p.w_last = so + 10 * cn;
-      p.save_rec = tr.rec; p.save_dnorm = tr.dnorm; p.save_raw_c = tr.raw_c; p.save_raw_f = tr.raw_f; p.save_ray = tr.ray;
-      p.dbg_z_c = tr.z_c; p.dbg_z_f = tr.z_f;
+      p.save_rec = tr.rec.get(); p.save_dnorm = tr.dnorm.get(); p.save_raw_c = tr.raw_c.get(); p.save_raw_f = tr.raw_f.get();
+      p.save_ray = tr.ray.get();
+      p.dbg_z_c = tr.z_c.get(); p.dbg_z_f = tr.z_f.get();
       NFB_CUDA(nfb::launch_render(p, tr.precision, h->num_sms, st, &h->launches));
-      rc = backward_rays(begin, n, n_units);
+      rc = backward_rays(begin, g);
       if (rc) return rc;
     }
   }
-  NFB_CUDA(nfb::launch_finalize_all(params_coarse, input_only ? nullptr : grads_coarse, tr.acc[0], fine ? params_fine : nullptr,
-                                    (fine && !input_only) ? grads_fine : nullptr, tr.acc[1], tr.cond, grad_latent, st, &h->launches,
+  NFB_CUDA(nfb::launch_finalize_all(params_coarse, input_only ? nullptr : grads_coarse, acc[0], fine ? params_fine : nullptr,
+                                    (fine && !input_only) ? grads_fine : nullptr, acc[1], tr.cond.get(), grad_latent, st, &h->launches,
                                     ig.expression));
   return NFB_OK;
 }
@@ -584,14 +542,15 @@ int nfb_train_debug(NfbHandle* h, NfbTrainDebug* out) {
   if (!h || !out) return NFB_ERR_INVALID;
   if (!h->tr.valid || h->tr.chunked) return NFB_ERR_STATE;  // chunked: the buffers only ever hold one chunk
   const NfbHandle::Train& tr = h->tr;
-  out->records = tr.rec; out->n_tiles = (long long)tr.n_units * (tr.tiles_c + tr.tiles_f); out->record_bytes = nfb::kRecBytes;
-  out->d_raw = tr.draw; out->acc_coarse = tr.acc[0]; out->acc_fine = tr.acc[1]; out->acc_floats = nfb::kAccFloats;
-  out->scale = tr.scal; out->z_coarse = tr.z_c; out->raw_coarse = tr.raw_c; out->z_fine = tr.z_f; out->raw_fine = tr.raw_f;
-  out->tiles_coarse = tr.tiles_c; out->tiles_fine = tr.tiles_f; out->rays_per_unit = tr.rays_per_unit;
-  out->rays = tr.ray; out->dnorm = tr.dnorm;
-  out->rows = tr.rows_formed ? tr.rows : nullptr;
-  out->ray_dn = tr.per_ray_formed ? tr.ray_dn : nullptr;
-  out->ray_bg = (tr.per_ray_formed && tr.has_bg) ? tr.ray_bg : nullptr;
+  out->records = tr.rec.get(); out->n_tiles = (long long)tr.geom.tiles(); out->record_bytes = nfb::kRecBytes;
+  out->d_raw = tr.draw.get(); out->acc_coarse = tr.acc[0].get(); out->acc_fine = tr.acc[1].get(); out->acc_floats = nfb::kAccFloats;
+  out->scale = tr.scal.get(); out->z_coarse = tr.z_c.get(); out->raw_coarse = tr.raw_c.get(); out->z_fine = tr.z_f.get();
+  out->raw_fine = tr.raw_f.get();
+  out->tiles_coarse = tr.geom.tiles_c; out->tiles_fine = tr.geom.tiles_f; out->rays_per_unit = tr.geom.rays_per_unit;
+  out->rays = tr.ray.get(); out->dnorm = tr.dnorm.get();
+  out->rows = tr.rows_formed ? tr.rows.get() : nullptr;
+  out->ray_dn = tr.per_ray_formed ? tr.ray_dn.get() : nullptr;
+  out->ray_bg = (tr.per_ray_formed && tr.has_bg) ? tr.ray_bg.get() : nullptr;
   return NFB_OK;
 }
 
@@ -604,22 +563,12 @@ int nfb_render_frame_host(NfbHandle* h, const float pose[12], const double intri
   NFB_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const size_t n = (size_t)rows * width;
-  if (h->out_cap < 11 * n) {
-    if (h->d_out) NFB_CUDA(cudaFree(h->d_out));
-    h->d_out = nullptr; h->out_cap = 0;
-    NFB_CUDA(dev_alloc(&h->d_out, 11 * n));
-    h->out_cap = 11 * n;
-  }
-  if (background_host && h->bg_cap < 3 * n) {
-    if (h->d_bg) NFB_CUDA(cudaFree(h->d_bg));
-    h->d_bg = nullptr; h->bg_cap = 0;
-    NFB_CUDA(dev_alloc(&h->d_bg, 3 * n));
-    h->bg_cap = 3 * n;
-  }
-  NFB_CUDA(cudaMemcpyAsync(h->d_expr, expression_host, nfb::kDimExpr * sizeof(float), cudaMemcpyHostToDevice, st));
-  NFB_CUDA(cudaMemcpyAsync(h->d_latent, latent_host, nfb::kDimLatent * sizeof(float), cudaMemcpyHostToDevice, st));
-  if (background_host) NFB_CUDA(cudaMemcpyAsync(h->d_bg, background_host, 3 * n * sizeof(float), cudaMemcpyHostToDevice, st));
-  int rc = nfb_set_frame(h, h->d_expr, h->d_latent, stream);
+  NFB_CUDA(h->d_out.reserve(11 * n));
+  if (background_host) NFB_CUDA(h->d_bg.reserve(3 * n));
+  NFB_CUDA(cudaMemcpyAsync(h->d_expr.get(), expression_host, nfb::kDimExpr * sizeof(float), cudaMemcpyHostToDevice, st));
+  NFB_CUDA(cudaMemcpyAsync(h->d_latent.get(), latent_host, nfb::kDimLatent * sizeof(float), cudaMemcpyHostToDevice, st));
+  if (background_host) NFB_CUDA(cudaMemcpyAsync(h->d_bg.get(), background_host, 3 * n * sizeof(float), cudaMemcpyHostToDevice, st));
+  int rc = nfb_set_frame(h, h->d_expr.get(), h->d_latent.get(), stream);
   if (rc) return rc;
   NfbRays r;
   std::memset(&r, 0, sizeof(r));
@@ -628,14 +577,14 @@ int nfb_render_frame_host(NfbHandle* h, const float pose[12], const double intri
   for (int i = 0; i < 4; ++i) r.intrinsics[i] = intrinsics[i];
   r.height = height; r.width = width; r.row_begin = row_begin;
   r.near_ = near_; r.far_ = far_;
-  r.background = background_host ? h->d_bg : nullptr;
+  r.background = background_host ? h->d_bg.get() : nullptr;
   NfbOutputs o;
-  float* b = h->d_out;
+  float* b = h->d_out.get();
   o.rgb_coarse = b; o.disp_coarse = b + 3 * n; o.acc_coarse = b + 4 * n;
   o.rgb_fine = b + 5 * n; o.disp_fine = b + 8 * n; o.acc_fine = b + 9 * n; o.w_last = b + 10 * n;
   rc = nfb_render_forward(h, &r, sm, nullptr, &o, nullptr, stream);
   if (rc) return rc;
-  NFB_CUDA(cudaMemcpyAsync(out_host, h->d_out, 11 * n * sizeof(float), cudaMemcpyDeviceToHost, st));
+  NFB_CUDA(cudaMemcpyAsync(out_host, h->d_out.get(), 11 * n * sizeof(float), cudaMemcpyDeviceToHost, st));
   NFB_CUDA(cudaStreamSynchronize(st));
   return NFB_OK;
 }
@@ -646,8 +595,8 @@ int nfb_frame_products(NfbHandle* h, const float* rgb, const float* disparity, c
   if ((rgb_u8 && !rgb) || ((normals_u8 || disparity_u8) && !disparity)) return NFB_ERR_INVALID;
   if (normals_u8 && height != width) return NFB_ERR_UNSUPPORTED;  // the reference's expression only broadcasts for square frames
   NFB_CUDA(cudaSetDevice(h->device));
-  if (!h->minmax) NFB_CUDA(dev_alloc(&h->minmax, 2));
-  NFB_CUDA(nfb::launch_frame_products(rgb, disparity, w_last, intrinsics, height, width, rgb_u8, normals_u8, disparity_u8, h->minmax,
+  NFB_CUDA(h->minmax.reserve(2));
+  NFB_CUDA(nfb::launch_frame_products(rgb, disparity, w_last, intrinsics, height, width, rgb_u8, normals_u8, disparity_u8, h->minmax.get(),
                                       (flags & NFB_PRODUCTS_LIKE_TORCH_CPU) ? 1 : 0, static_cast<cudaStream_t>(stream), &h->launches));
   return NFB_OK;
 }
@@ -662,22 +611,18 @@ int nfb_sample_rays(NfbHandle* h, const NfbRayMap* map, const double* draws, int
   NFB_CUDA(cudaSetDevice(h->device));
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const long long N = (long long)map->height * map->width;
-  if (!h->smp_runs) NFB_CUDA(dev_alloc(&h->smp_runs, nfb::smp::kMaxRuns));
-  if (!h->smp_segs) NFB_CUDA(dev_alloc(&h->smp_segs, nfb::smp::kMaxSegs));
-  if (h->smp_first_n < N) {
-    if (h->smp_first) NFB_CUDA(cudaFree(h->smp_first));
-    h->smp_first = nullptr; h->smp_first_n = 0;
-    NFB_CUDA(dev_alloc(&h->smp_first, (size_t)N));
-    h->smp_first_n = N;
-    NFB_CUDA(nfb::launch_fill_int(h->smp_first, N, 0x7FFFFFFF, st, &h->launches));
-  }
+  NFB_CUDA(h->smp_runs.reserve(nfb::smp::kMaxRuns));
+  NFB_CUDA(h->smp_segs.reserve(nfb::smp::kMaxSegs));
+  bool fresh = false;  // a new first_pos starts all INT_MAX (SampleArgs::first_pos)
+  NFB_CUDA(h->smp_first.reserve((size_t)N, &fresh));
+  if (fresh) NFB_CUDA(nfb::launch_fill_int(h->smp_first.get(), N, 0x7FFFFFFF, st, &h->launches));
   nfb::SampleArgs a;
   std::memset(&a, 0, sizeof(a));
   a.map.H = map->height; a.map.W = map->width;
   a.map.b0 = map->bbox[0]; a.map.b1 = map->bbox[1]; a.map.b2 = map->bbox[2]; a.map.b3 = map->bbox[3];
   a.map.q_out = map->q_out; a.map.q_in = map->q_in;
   a.draws = draws; a.size = size; a.max_rounds = max_rounds; a.found = indices; a.state = state;
-  a.runs = h->smp_runs; a.segs = h->smp_segs; a.first_pos = h->smp_first;
+  a.runs = h->smp_runs.get(); a.segs = h->smp_segs.get(); a.first_pos = h->smp_first.get();
   if (g) {
     if ((g->target && !g->image) || (g->background_out && !g->background) || (g->ray_origins && !g->ray_directions)) return NFB_ERR_INVALID;
     for (int i = 0; i < 12; ++i) a.pose[i] = g->pose[i];

@@ -1,25 +1,54 @@
-// nfb_internal.h — structures shared between the C-ABI layer (nfb_api.cu), the preparation kernels
-// (nfb_pack.cu) and the render kernel (nfb_render.cu).  Not part of the public interface.
+// nfb_internal.h — what the C-ABI layer (nfb_api.cu) and the kernel files share: the handle's device buffers, the parameter
+// blocks of the preparation (nfb_pack.cu), render (nfb_render.cu), training (nfb_train.cu, nfb_optim.cu) and post-processing
+// (nfb_post.cu) kernels, and their launchers.  Not part of the public interface.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 
+#include "nfb_layout.h"
 #include "nfb_sampler.h"
 
 namespace nfb {
 
+// A device allocation its owner frees.  Grow-only; what it held is gone once it has grown.
+template <class T>
+class DevBuf {
+ public:
+  DevBuf() = default;
+  DevBuf(const DevBuf&) = delete;
+  DevBuf& operator=(const DevBuf&) = delete;
+  ~DevBuf() { cudaFree(p_); }
+  T* get() const { return p_; }
+  // Room for n elements: allocates anew only when there is none or less.  *grew, when asked for, says whether it did.
+  cudaError_t reserve(size_t n, bool* grew = nullptr) {
+    if (grew) *grew = false;
+    if (p_ && cap_ >= n) return cudaSuccess;
+    cudaError_t e = p_ ? cudaFree(p_) : cudaSuccess;
+    p_ = nullptr; cap_ = 0;
+    if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&p_), n * sizeof(T));
+    if (e != cudaSuccess) return e;
+    cap_ = n;
+    if (grew) *grew = true;
+    return cudaSuccess;
+  }
+
+ private:
+  T* p_ = nullptr;
+  size_t cap_ = 0;
+};
+
 // Device buffers of one loaded network.
 struct NetBuffers {
-  uint8_t* stream_x1 = nullptr;  // kStreamBytesX1: FP16 weights, swizzled units in execution order
-  uint8_t* stream_x3 = nullptr;  // kStreamBytesX3: hi unit, lo unit, ...
-  float* w6 = nullptr;           // [144,256] folded layers_dir.0 / fc_alpha
-  float* b6 = nullptr;           // [144]
-  float* bias_static = nullptr;  // [kBiasFloats]
-  float* bias_frame = nullptr;   // [kBiasFloats] bias_static + per-frame fold (what the kernel reads)
-  float* w0c = nullptr;          // [256,108] conditioning columns of layers_xyz.0
-  float* w3c = nullptr;          // [256,108] conditioning columns of layers_xyz.3
-  float* wd0b_t = nullptr;       // [24,128] direction columns of layers_dir.0, transposed
-  uint8_t* stream_bwd = nullptr; // kBwdStreamBytes: transposed FP16 weights for the backward chain (nfb_train.cu)
+  DevBuf<uint8_t> stream_x1;  // kStreamBytesX1: FP16 weights, swizzled units in execution order
+  DevBuf<uint8_t> stream_x3;  // kStreamBytesX3: hi unit, lo unit, ...
+  DevBuf<float> w6;           // [144,256] folded layers_dir.0 / fc_alpha
+  DevBuf<float> b6;           // [144]
+  DevBuf<float> bias_static;  // [kBiasFloats]
+  DevBuf<float> bias_frame;   // [kBiasFloats] bias_static + per-frame fold (what the kernel reads)
+  DevBuf<float> w0c;          // [256,108] conditioning columns of layers_xyz.0
+  DevBuf<float> w3c;          // [256,108] conditioning columns of layers_xyz.3
+  DevBuf<float> wd0b_t;       // [24,128] direction columns of layers_dir.0, transposed
+  DevBuf<uint8_t> stream_bwd; // kBwdStreamBytes: transposed FP16 weights for the backward chain (nfb_train.cu)
   bool loaded = false;
 };
 
@@ -28,7 +57,6 @@ struct RenderParams {
   // rays
   const float* o;
   const float* d;
-  int n_rays;
   float pose[12];
   float fx, fy, wcx, hcy;  // intrinsics as FP32; wcx = width*cx, hcy = height*cy (rounded like torch does)
   int width, row_begin;
@@ -36,10 +64,7 @@ struct RenderParams {
   const float* dir_z;
   const float* bg;
   // sampling
-  int nc, nf, s_fine;     // s_fine = nc + nf
-  int rays_per_unit;      // R
-  int tiles_c, tiles_f;   // 128-row tiles per coarse / fine pass of one unit
-  int n_units;
+  TileGeom geom;          // rays, samples per ray, and how they are cut into units and tiles
   int perturb;
   float noise_std;
   int white_bkgd;
@@ -66,7 +91,8 @@ struct RenderParams {
 
 // ---- training (nfb_train.cu)
 struct CompBwdParams {
-  int n_rays, nc, nf, s_fine, rays_per_unit, tiles_c, tiles_f, has_bg, white_bkgd;
+  TileGeom geom;
+  int has_bg, white_bkgd;
   const float *z_c, *raw_c, *z_f, *raw_f, *dnorm;                       // saved by the training forward
   const float *g_rgb[2], *g_disp[2], *g_acc[2], *g_wlast;               // dL/d outputs (coarse, fine); any may be null
   float* draw;                                                          // [tiles][128][4] dL/d(rgb_raw, sigma_raw), zero-initialised
@@ -77,7 +103,7 @@ struct CompBwdParams {
 // Input gradients (nfb_render_backward_ex): per-row (dp, d v0) of every tile, then per-ray sums.
 struct InGradRowParams {
   const uint8_t* rec;
-  int n_units, tiles_c, tiles_f, rays_per_unit, nc, s_fine, n_rays;
+  TileGeom geom;
   int parts[2];                       // CTAs working on network 0 / network 1
   const float *z_c, *z_f, *ray;        // ray: the training forward's [n][7] = (o, d, v0)
   const float* scal;
@@ -85,12 +111,13 @@ struct InGradRowParams {
   float* out;                         // [tiles][128] float4
 };
 struct InGradRayParams {
-  int n_rays, nc, nf, s_fine, rays_per_unit, tiles_c, tiles_f, has_dir_z;
+  TileGeom geom;
+  int has_dir_z;
   const float *rows, *z_c, *z_f, *ray, *dnorm, *ray_dn, *ray_bg;
   float *g_o, *g_d, *g_dir_z, *g_bg;  // any may be null
 };
 struct ChainParams {
-  int n_units, tiles_c, tiles_f;
+  TileGeom geom;
   uint8_t* rec;
   const float* draw;
   const float* scal;            // [0] = loss scale, [1] = 1 / scale
@@ -98,8 +125,7 @@ struct ChainParams {
 };
 struct DwParams {  // ONE launch covers both networks: the first parts[0] * groups CTAs work on network 0, the rest on network 1
   const uint8_t* rec;
-  int n_units, tpu;
-  int t_base[2], t_cnt[2];  // tiles of network i: unit * tpu + t_base[i] + [0, t_cnt[i])
+  TileGeom geom;
   int parts[2];             // CTAs per job group of network i (set by launch_dw, proportional to the tile counts)
   float* ws;                // partial sums: slot (network 0's parts, then network 1's) of ws_stride floats per part
   int ws_stride;            // set by launch_dw: kAccBRaw, or the compact PE-only slot (nfb_train.cu dw::kPeSlotFloats)

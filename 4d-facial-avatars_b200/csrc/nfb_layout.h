@@ -23,6 +23,7 @@
 // The accumulator is kept in two column halves ("half 0" = output columns [0,128) = K atoms 0,1 of the next step,
 // "half 1" = [128,256) = atoms 2,3), one m64n128 (or n16) wgmma accumulator each.
 #pragma once
+#include <stddef.h>
 #include <stdint.h>
 
 #if defined(__CUDACC__)
@@ -65,6 +66,82 @@ constexpr int kBiasFloats = 1952;  // 6*256 + 144 + 128 + 128 + 16
 // XORed with (row & 7) — the SWIZZLE_128B pattern the wgmma shared-memory descriptor expects.
 NFB_HD constexpr int sw128_offset(int n, int k) { return n * 128 + ((((k >> 3) ^ (n & 7)) & 7) << 4) + ((k & 7) << 1); }
 
+// ------------------------------------------------------------------------------------------------
+// How a call's rays are cut into work.  A unit is R = rays_per_unit consecutive rays (two when both fit the 512 sample rows a
+// unit's pass may hold, else one).  A unit's pass p (0 coarse, 1 fine; network p evaluates it) is the R * samples(p) rows
+// "ray rr, sample i" -> rr * samples(p) + i, cut into 128-row tiles; a unit's tiles are its coarse ones, then its fine ones,
+// and units follow each other.  Every per-tile array (the activation records, d raw, the input-gradient rows) is indexed by
+// that global tile.  The only definition: the kernels that write such an array and the ones that read it all ask here.
+struct TileGeom {
+  int n_rays, nc, nf;      // rays of the launch; coarse samples per ray; additional fine samples per ray (0: no fine pass)
+  int rays_per_unit;       // R
+  int tiles_c, tiles_f;    // 128-row tiles per coarse / fine pass of one unit
+  int n_units;
+
+  static NFB_HD constexpr TileGeom make(int n_rays, int nc, int nf) {
+    const int R = 2 * (nc + nf) <= 512 ? 2 : 1;
+    return TileGeom{n_rays, nc, nf, R, (R * nc + kTileM - 1) / kTileM, nf > 0 ? (R * (nc + nf) + kTileM - 1) / kTileM : 0,
+                    (n_rays + R - 1) / R};
+  }
+  // The same cut for a chunk of n of the rays (a chunk that starts at a multiple of R holds whole units of the full call).
+  NFB_HD constexpr TileGeom chunk(int n) const { return make(n, nc, nf); }
+
+  NFB_HD constexpr int passes() const { return nf > 0 ? 2 : 1; }
+  NFB_HD constexpr int samples(int pass) const { return pass ? nc + nf : nc; }
+  NFB_HD constexpr int tile_count(int net) const { return net ? tiles_f : tiles_c; }
+  NFB_HD constexpr int tile_base(int net) const { return net ? tiles_c : 0; }  // first tile of the network within a unit
+  NFB_HD constexpr int tiles_per_unit() const { return tiles_c + tiles_f; }
+  NFB_HD constexpr size_t tiles() const { return (size_t)n_units * tiles_per_unit(); }
+  NFB_HD constexpr int net_of(int unit_tile) const { return unit_tile < tiles_c ? 0 : 1; }  // unit_tile in [0, tiles_per_unit)
+  NFB_HD constexpr size_t global_tile(int unit, int unit_tile) const { return (size_t)unit * tiles_per_unit() + unit_tile; }
+  NFB_HD constexpr size_t global_tile(int unit, int net, int local_tile) const { return global_tile(unit, tile_base(net) + local_tile); }
+  // Index of sample i of ray g in pass `pass` within a [tiles][128] array: row (prow & 127) of the pass's tile (prow >> 7),
+  // prow = rr * samples(pass) + i for ray rr of the unit.  A kernel that sweeps a ray's samples asks for ray_rows once.
+  struct RayRows {
+    int tile0, rr, S;  // global tile of the unit's pass, ray within the unit, samples per ray
+    NFB_HD constexpr size_t slot(int i) const { return (size_t)(tile0 + ((rr * S + i) >> 7)) * 128 + ((rr * S + i) & 127); }
+  };
+  NFB_HD constexpr RayRows ray_rows(int pass, int g) const {
+    const int unit = g / rays_per_unit;
+    return RayRows{(int)global_tile(unit, pass, 0), g - unit * rays_per_unit, samples(pass)};
+  }
+  NFB_HD constexpr size_t slot(int pass, int g, int i) const { return ray_rows(pass, g).slot(i); }
+  // The inverse for one row of a tile.  used: the row holds a sample of one of the unit's R rays (else ray = sample = 0);
+  // whether that ray exists is ray_index(unit, ray) < n_rays.
+  struct Row { int pass_row, ray, sample; bool used; };  // row within the unit's pass, ray within the unit, sample of the ray
+  NFB_HD constexpr Row row(int pass, int local_tile, int tile_row) const {
+    const int S = samples(pass), prow = local_tile * kTileM + tile_row;
+    const bool used = prow < rays_per_unit * S;
+    const int ray = used ? prow / S : 0;
+    return Row{prow, ray, used ? prow - ray * S : 0, used};
+  }
+  NFB_HD constexpr int ray_index(int unit, int ray) const { return unit * rays_per_unit + ray; }
+};
+
+namespace geom_check {
+constexpr bool cut(int nc, int nf, int R, int tc, int tf) {
+  const TileGeom g = TileGeom::make(5, nc, nf);
+  return g.rays_per_unit == R && g.tiles_c == tc && g.tiles_f == tf && g.n_units == (5 + R - 1) / R &&
+         g.chunk(3).n_units == (3 + R - 1) / R && g.chunk(3).tiles_f == tf;
+}
+// row() takes every sample's slot() back to that sample, in a tile of the sample's own network, inside the array.
+constexpr bool round_trip(int n_rays, int nc, int nf) {
+  const TileGeom g = TileGeom::make(n_rays, nc, nf);
+  for (int pass = 0; pass < g.passes(); ++pass)
+    for (int r = 0; r < n_rays; ++r)
+      for (int i = 0; i < g.samples(pass); ++i) {
+        const size_t s = g.slot(pass, r, i);
+        const int unit = (int)((s >> 7) / g.tiles_per_unit()), lt = (int)((s >> 7) % g.tiles_per_unit()) - g.tile_base(pass);
+        if (lt < 0 || lt >= g.tile_count(pass) || g.net_of(g.tile_base(pass) + lt) != pass) return false;
+        const TileGeom::Row w = g.row(pass, lt, (int)(s & 127));
+        if (!w.used || w.sample != i || g.ray_index(unit, w.ray) != r || s >= g.tiles() * 128) return false;
+      }
+  return true;
+}
+static_assert(cut(64, 128, 2, 1, 3) && cut(128, 256, 1, 1, 3) && cut(64, 0, 2, 1, 0) && cut(256, 256, 1, 2, 4), "tile cut");
+static_assert(round_trip(5, 64, 128) && round_trip(3, 128, 256) && round_trip(5, 64, 0) && round_trip(2, 256, 256) &&
+              round_trip(5, 3, 7), "slot / row round trip");
+}  // namespace geom_check
 
 // ------------------------------------------------------------------------------------------------
 // Training: per-tile activation record (written by the forward kernel in SAVE mode and by the backward chain kernel,

@@ -237,10 +237,10 @@ cudaError_t launch_repack(NetBuffers* const nb[2], const float* const* const par
   for (int n = 0; n < n_nets; ++n) {
     for (int i = 0; i < 26; ++i) { a.net[n].p[i] = params[n][i]; f.net[n].p[i] = params[n][i]; }
     f.net[n].w6 = f.net[n].b6 = nullptr;
-    f.w6[n] = nb[n]->w6; f.b6[n] = nb[n]->b6;
-    a.net[n].w6 = nb[n]->w6; a.net[n].b6 = nb[n]->b6;
-    a.x1[n] = nb[n]->stream_x1; a.x3[n] = nb[n]->stream_x3; a.bwd[n] = nb[n]->stream_bwd;
-    a.bias_static[n] = nb[n]->bias_static; a.w0c[n] = nb[n]->w0c; a.w3c[n] = nb[n]->w3c; a.wd0b_t[n] = nb[n]->wd0b_t;
+    f.w6[n] = nb[n]->w6.get(); f.b6[n] = nb[n]->b6.get();
+    a.net[n].w6 = nb[n]->w6.get(); a.net[n].b6 = nb[n]->b6.get();
+    a.x1[n] = nb[n]->stream_x1.get(); a.x3[n] = nb[n]->stream_x3.get(); a.bwd[n] = nb[n]->stream_bwd.get();
+    a.bias_static[n] = nb[n]->bias_static.get(); a.w0c[n] = nb[n]->w0c.get(); a.w3c[n] = nb[n]->w3c.get(); a.wd0b_t[n] = nb[n]->wd0b_t.get();
   }
   fold_feat_kernel<<<dim3(144, 4, n_nets), 256, 0, st>>>(f);
   ++*launches;
@@ -253,7 +253,7 @@ cudaError_t launch_frame_fold(NetBuffers* const nb[2], int n_nets, const float* 
                               cudaStream_t st, long long* launches) {
   FrameFoldArgs a;
   for (int n = 0; n < n_nets; ++n) {
-    a.bias_static[n] = nb[n]->bias_static; a.w0c[n] = nb[n]->w0c; a.w3c[n] = nb[n]->w3c; a.bias_frame[n] = nb[n]->bias_frame;
+    a.bias_static[n] = nb[n]->bias_static.get(); a.w0c[n] = nb[n]->w0c.get(); a.w3c[n] = nb[n]->w3c.get(); a.bias_frame[n] = nb[n]->bias_frame.get();
   }
   a.cond = cond;
   a.n_nets = n_nets;

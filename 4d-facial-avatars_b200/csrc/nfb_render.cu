@@ -299,8 +299,9 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
   if (threadIdx.x == 0) ring.init();
   __syncthreads();
 
-  const int n_iter = (p.n_units - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-  const int tiles_per_unit = p.tiles_c + p.tiles_f;
+  const TileGeom& geom = p.geom;
+  const int n_iter = (geom.n_units - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  const int tiles_per_unit = geom.tiles_per_unit();
 
   if (warp < 4) {
     // ============================== weight producer ==============================
@@ -309,7 +310,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
     if (warp == 0) {
       for (int it = 0; it < n_iter; ++it) {
         for (int t = 0; t < tiles_per_unit; ++t) {
-          const uint8_t* base = p.wstream[t < p.tiles_c ? 0 : 1];
+          const uint8_t* base = p.wstream[geom.net_of(t)];
           for (int i = 0; i < kTileUnits; ++i) {
             const uint32_t w = c_prog.e[i].w;
             const uint32_t off = (w & 0xFFFFFu) << 4, bytes = (w >> 20) * 128u;
@@ -345,7 +346,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
     float* dirbias = reinterpret_cast<float*>(smem + M::kDirBias);
     RayP* rayp = reinterpret_cast<RayP*>(smem + M::kRay);
     float4* tile_raw = reinterpret_cast<float4*>(smem + M::kTileRaw);
-    const int R = p.rays_per_unit;
+    const int R = geom.rays_per_unit;
     const bool has_bg = p.bg != nullptr;
     // observers: the first thread of each row warpgroup, warpgroup w's laps at slot + kProfWgStride * w
     PhaseTimer tm(p.prof ? p.prof + kProfWgStride * wg : nullptr, p.prof != nullptr && (etid & 127) == 0);
@@ -356,8 +357,8 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
       // ---- per-ray constants
       if (etid < R) {
         RayP& rp = rayp[etid];
-        const int g = unit * R + etid;
-        rp.valid = g < p.n_rays;
+        const int g = geom.ray_index(unit, etid);
+        rp.valid = g < geom.n_rays;
         rp.gidx = g;
         if (rp.valid) {
           float o0, o1, o2, d0, d1, d2;
@@ -423,19 +424,18 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
 
 
       for (int pass = 0; pass < 2; ++pass) {
-        if (pass == 1 && p.nf == 0) break;
-        const int S = pass ? p.s_fine : p.nc;
+        if (pass == 1 && geom.nf == 0) break;
+        const int S = geom.samples(pass);
         const int rows = R * S;
-        const int n_tiles = pass ? p.tiles_f : p.tiles_c;
+        const int n_tiles = geom.tile_count(pass);
         const float* bias_n = p.bias[pass];
 
         // ---- prologue of tile t: sample depth + positional encoding -> PE buffer.
         auto prologue = [&](int t) {
-          const int prow = t * 128 + row;
-          const bool live = prow < rows;
-          const int r = live ? prow / S : 0;
-          const int i = live ? prow - r * S : 0;
-          const RayP& rp = rayp[r];
+          const TileGeom::Row rw = geom.row(pass, t, row);
+          const int prow = rw.pass_row, i = rw.sample;
+          const bool live = rw.used;
+          const RayP& rp = rayp[rw.ray];
           float z = 0.f;
           if (live) {
             if (pass == 0) {
@@ -453,7 +453,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
                   const float zn = __fadd_rn(__fmul_rn(p.near_, __fsub_rn(1.f, tn)), __fmul_rn(p.far_, tn));
                   upper = __fmul_rn(0.5f, __fadd_rn(zn, z));
                 }
-                const float tr = rp.valid ? p.t_rand[(size_t)rp.gidx * p.nc + i] : 0.f;
+                const float tr = rp.valid ? p.t_rand[(size_t)rp.gidx * geom.nc + i] : 0.f;
                 z = __fadd_rn(lower, __fmul_rn(__fsub_rn(upper, lower), tr));
               }
               if (half == 0) carry_z[prow] = z;
@@ -514,8 +514,8 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
             for (int k = 0; k < 32; ++k) p.dbg_act[row * 256 + half * 32 + k] = f[k];
           }
           if constexpr (SAVE) {  // FP16 encoding of this tile as a transposed image (input of layers_xyz.0 / .3 in dW)
-            if (unit < p.n_units) {
-              uint8_t* rec = p.save_rec + (size_t)(unit * tiles_per_unit + (pass ? p.tiles_c : 0) + t) * kRecBytes;
+            if (unit < geom.n_units) {
+              uint8_t* rec = p.save_rec + geom.global_tile(unit, pass, t) * kRecBytes;
               uint32_t hh[16];
 #pragma unroll
               for (int e = 0; e < 16; ++e) hh[e] = pack_f16x2(f[2 * e], f[2 * e + 1]);
@@ -530,11 +530,11 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
           prologue(t);
           uint8_t* rec = nullptr;  // this tile's training record (SAVE mode)
           if constexpr (SAVE) {
-            if (unit < p.n_units) {
-              const int prow = t * 128 + row;
-              const bool live = prow < rows;
-              const RayP& rp = rayp[live ? prow / S : 0];
-              rec = p.save_rec + (size_t)(unit * tiles_per_unit + (pass ? p.tiles_c : 0) + t) * kRecBytes;
+            if (unit < geom.n_units) {
+              const TileGeom::Row rw = geom.row(pass, t, row);
+              const bool live = rw.used;
+              const RayP& rp = rayp[rw.ray];
+              rec = p.save_rec + geom.global_tile(unit, pass, t) * kRecBytes;
               uint32_t hh[8];  // direction encoding of this row's ray: features [16*half, 16*half+16)
 #pragma unroll
               for (int e = 0; e < 8; ++e) {
@@ -563,11 +563,10 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
             const bool probe = PROBE && p.dbg_act && unit == 0 && pass == 0 && t == 0;
             float acc0[64], acc1[64], acc_s[8];
             uint32_t act[64];  // fast mode: this thread's part of the hidden activations, as the next step's A fragments
-            const int prow0 = t * 128 + r0, prow1 = prow0 + 8;
-            const int ray0 = prow0 < rows ? prow0 / S : 0, ray1 = prow1 < rows ? prow1 / S : 0;
+            const TileGeom::Row rw0 = geom.row(pass, t, r0), rw1 = geom.row(pass, t, r0 + 8);
+            const int ray0 = rw0.ray, ray1 = rw1.ray;
             uint32_t live = 0u;  // SAVE: which of this thread's two rows hold a sample (see epi_half)
-            if constexpr (SAVE)
-              live = ((prow0 < rows && rayp[ray0].valid) ? 1u : 0u) | ((prow1 < rows && rayp[ray1].valid) ? 2u : 0u);
+            if constexpr (SAVE) live = ((rw0.used && rayp[ray0].valid) ? 1u : 0u) | ((rw1.used && rayp[ray1].valid) ? 2u : 0u);
             auto mlp_step = [&](auto step) {
               const int s = step;
               const StepInfo si = step_info(s);
@@ -625,12 +624,10 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
           // 41-53); the exp(-sigma*delta) needs the neighbour depth and stays in composite_ray.  One thread per row of the
           // warpgroup's 64.
           if (half == 0) {
-            const int prow = t * 128 + row;
-            const bool live = prow < rows;
-            const int r = live ? prow / S : 0;
-            const int i = live ? prow - r * S : 0;
-            const RayP& rp = rayp[r];
-            if (live) {
+            const TileGeom::Row rw = geom.row(pass, t, row);
+            const int prow = rw.pass_row, i = rw.sample;
+            const RayP& rp = rayp[rw.ray];
+            if (rw.used) {
               const float4 v = tile_raw[row];
               const float r0_ = v.x, r1 = v.y, r2 = v.z, sigma_raw = v.w;
               if (rp.valid) {
@@ -685,10 +682,10 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
           const float wl = composite_ray(carry_raw + ew * S, carry_z + ew * S, scr_w + ew * S, S, rp.dnorm, p.white_bkgd != 0,
                                          o_rgb ? o_rgb + 3 * (size_t)g : nullptr, o_disp ? o_disp + g : nullptr,
                                          o_acc ? o_acc + g : nullptr, lane);
-          const bool last_pass = (pass == 1) || (p.nf == 0);
+          const bool last_pass = (pass == 1) || (geom.nf == 0);
           if (last_pass && lane == 0 && p.w_last) p.w_last[g] = wl;
         }
-        if (pass == 1 || p.nf == 0) {
+        if (pass == 1 || geom.nf == 0) {
           named_bar_sync(kRowBarrier, kRowThreads);  // carry buffers are reused by the next unit
           tm.lap(4);
           continue;
@@ -697,13 +694,13 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
 
         // ---- inverse-CDF resampling (nerf_helpers.py:344-387) on weights[1:-1] over the mid-point bins
         __syncwarp();
-        const int nb = p.nc - 1;   // bins / cdf entries
-        const int nw = p.nc - 2;   // interior weights
+        const int nb = geom.nc - 1;   // bins / cdf entries
+        const int nw = geom.nc - 2;   // interior weights
         if (ew < R) {
-          const float* w = scr_w + ew * p.nc;
-          const float* zc = carry_z + ew * p.nc;
-          float* cdf = scr_cdf + ew * p.nc;
-          float* bins = scr_bins + ew * p.nc;
+          const float* w = scr_w + ew * geom.nc;
+          const float* zc = carry_z + ew * geom.nc;
+          float* cdf = scr_cdf + ew * geom.nc;
+          float* bins = scr_bins + ew * geom.nc;
           for (int k = lane; k < nb; k += 32) bins[k] = __fmul_rn(0.5f, __fadd_rn(zc[k + 1], zc[k]));
           const int per = (nw + 31) >> 5;
           const int k0 = lane * per;
@@ -731,17 +728,17 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
         named_bar_sync(kRowBarrier, kRowThreads);
         tm.lap(5);
         // cat(z_coarse, z_samples) per ray into scr_sort (stride s_fine)
-        const int SF = p.s_fine;
+        const int SF = geom.samples(1);
         for (int k = etid; k < R * SF; k += kRowThreads) {
           const int rr = k / SF, i = k - rr * SF;
           float val;
-          if (i < p.nc) {
-            val = carry_z[rr * p.nc + i];
+          if (i < geom.nc) {
+            val = carry_z[rr * geom.nc + i];
           } else {
-            const int j = i - p.nc;
-            const float* cdf = scr_cdf + rr * p.nc;
-            const float* bins = scr_bins + rr * p.nc;
-            const float u = p.perturb ? (rayp[rr].valid ? p.u_rand[(size_t)rayp[rr].gidx * p.nf + j] : 0.f) : p.u_fine[j];
+            const int j = i - geom.nc;
+            const float* cdf = scr_cdf + rr * geom.nc;
+            const float* bins = scr_bins + rr * geom.nc;
+            const float u = p.perturb ? (rayp[rr].valid ? p.u_rand[(size_t)rayp[rr].gidx * geom.nf + j] : 0.f) : p.u_fine[j];
             int lo = 0, hi = nb;  // searchsorted(..., right=True): number of cdf entries <= u
             while (lo < hi) {
               const int mid = (lo + hi) >> 1;
@@ -766,25 +763,25 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
         for (int k = etid; k < R * SF; k += kRowThreads) {
           const int rr = k / SF, i = k - rr * SF;
           const float* zc = scr_sort + rr * SF;
-          const float* zs = zc + p.nc;
+          const float* zs = zc + geom.nc;
           const float v = zc[i];
           int rank;
-          if (i < p.nc) {
+          if (i < geom.nc) {
             rank = i;
-            for (int j = 0; j < p.nf; ++j) rank += (zs[j] < v) ? 1 : 0;
+            for (int j = 0; j < geom.nf; ++j) rank += (zs[j] < v) ? 1 : 0;
           } else if (v != v) {
-            const int jm = i - p.nc;
-            rank = p.nc;
-            for (int j = 0; j < p.nf; ++j) rank += (zs[j] == zs[j] || j < jm) ? 1 : 0;
+            const int jm = i - geom.nc;
+            rank = geom.nc;
+            for (int j = 0; j < geom.nf; ++j) rank += (zs[j] == zs[j] || j < jm) ? 1 : 0;
           } else {
-            const int jm = i - p.nc;
-            int lo = 0, hi = p.nc;  // # coarse depths <= v
+            const int jm = i - geom.nc;
+            int lo = 0, hi = geom.nc;  // # coarse depths <= v
             while (lo < hi) {
               const int mid = (lo + hi) >> 1;
               if (zc[mid] <= v) lo = mid + 1; else hi = mid;
             }
             rank = lo;
-            for (int j = 0; j < p.nf; ++j) {
+            for (int j = 0; j < geom.nf; ++j) {
               const float y = zs[j];
               rank += (y < v || (y == v && j < jm)) ? 1 : 0;
             }
@@ -825,7 +822,7 @@ cudaError_t render_kernel_setup() {
 }
 
 cudaError_t launch_render(const RenderParams& p, int precision, int num_sms, cudaStream_t st, long long* launches) {
-  const int grid = p.n_units < num_sms ? p.n_units : num_sms;
+  const int grid = p.geom.n_units < num_sms ? p.geom.n_units : num_sms;
   if (grid <= 0) return cudaSuccess;
   const bool save = p.save_rec != nullptr;  // training forward: also writes the per-tile activation records
   const bool probe = p.dbg_act != nullptr;  // the activation probe (evaluation only): its own instantiation

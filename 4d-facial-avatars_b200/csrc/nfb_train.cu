@@ -49,11 +49,11 @@ template <bool kInputs>
 __global__ void __launch_bounds__(256) composite_bwd_kernel(const CompBwdParams q) {
   const int lane = threadIdx.x & 31;
   const int idx = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int npass = q.nf > 0 ? 2 : 1;
-  if (idx >= npass * q.n_rays) return;  // whole warps
-  const int pass = idx / q.n_rays;
-  const int g = idx - pass * q.n_rays;
-  const int S = pass ? q.s_fine : q.nc;
+  const int npass = q.geom.passes(), n_rays = q.geom.n_rays;
+  if (idx >= npass * n_rays) return;  // whole warps
+  const int pass = idx / n_rays;
+  const int g = idx - pass * n_rays;
+  const int S = q.geom.samples(pass);
   const float* __restrict__ z = (pass ? q.z_f : q.z_c) + (size_t)g * S;
   const float4* __restrict__ raw = reinterpret_cast<const float4*>(pass ? q.raw_f : q.raw_c) + (size_t)g * S;
   const float dn = q.dnorm[g];
@@ -146,8 +146,7 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const CompBwdParams 
   float C = __shfl_down_sync(0xffffffffu, SA, 1);  // composed map of all higher lanes applied to C = 0
   if (lane == 31) C = 0.f;
 
-  const int unit = g / q.rays_per_unit, rr = g - unit * q.rays_per_unit;
-  const int tile0 = unit * (q.tiles_c + q.tiles_f) + (pass ? q.tiles_c : 0);
+  const TileGeom::RayRows rows = q.geom.ray_rows(pass, g);
   float s0 = 0.f, s1 = 0.f, s2 = 0.f, s3 = 0.f, amax = 0.f;
   float gdn = 0.f;  // kInputs: sum of dsig_i sigma_i over this lane's samples
   // transmittance in front of each sample of this block, walking down from the block's end
@@ -180,7 +179,7 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const CompBwdParams 
       if (q.has_bg && i == S - 1) {
         d.x = d.y = d.z = 0.f;                  // background colour is data (train_background=False)
         if constexpr (kInputs) {
-          float* bgo = q.ray_bg + ((size_t)pass * q.n_rays + g) * 3;
+          float* bgo = q.ray_bg + ((size_t)pass * n_rays + g) * 3;
           bgo[0] = w * G0; bgo[1] = w * G1; bgo[2] = w * G2;
         }
       } else {
@@ -189,8 +188,7 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const CompBwdParams 
         d.z = w * G2 * r4.z * (1.f - r4.z);
       }
       C = fmaf(e + 1e-10f, C, dLdw * alpha);
-      const int prow = rr * S + i;
-      reinterpret_cast<float4*>(q.draw)[(size_t)(tile0 + (prow >> 7)) * 128 + (prow & 127)] = d;
+      reinterpret_cast<float4*>(q.draw)[rows.slot(i)] = d;
       s0 += d.x; s1 += d.y; s2 += d.z; s3 += d.w;
       amax = fmaxf(amax, fmaxf(fmaxf(fabsf(d.x), fabsf(d.y)), fmaxf(fabsf(d.z), fabsf(d.w))));
     }
@@ -204,10 +202,10 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(const CompBwdParams 
     if constexpr (kInputs) gdn += __shfl_xor_sync(0xffffffffu, gdn, o);
   }
   if constexpr (kInputs) {
-    if (lane == 0) q.ray_dn[(size_t)pass * q.n_rays + g] = gdn / dn;
+    if (lane == 0) q.ray_dn[(size_t)pass * n_rays + g] = gdn / dn;
   }
   if (lane == 0) {
-    reinterpret_cast<float4*>(q.bsum)[(size_t)pass * q.n_rays + g] = make_float4(s0, s1, s2, s3);  // summed by grad_reduce_kernel
+    reinterpret_cast<float4*>(q.bsum)[(size_t)pass * n_rays + g] = make_float4(s0, s1, s2, s3);  // summed by grad_reduce_kernel
     if (amax == amax && amax < 3.0e38f) atomicMax(q.absmax, __float_as_uint(amax));  // a max: independent of the order
   }
 }
@@ -286,8 +284,8 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
     reinterpret_cast<uint4*>(smem + kOffOp)[i] = make_uint4(0u, 0u, 0u, 0u);
   __syncthreads();
 
-  const int n_iter = (p.n_units - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-  const int tpu = p.tiles_c + p.tiles_f;
+  const int n_iter = (p.geom.n_units - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
+  const int tpu = p.geom.tiles_per_unit();
   const int n_tiles_cta = n_iter * tpu;
 
   if (warp < 4) {
@@ -295,8 +293,7 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
     reg_dec<kRegsLight>();
     if (warp == 0) {
       for (int j = 0; j < n_tiles_cta; ++j) {
-        const int t = j % tpu;
-        const uint8_t* base = p.wstream[t < p.tiles_c ? 0 : 1];
+        const uint8_t* base = p.wstream[p.geom.net_of(j % tpu)];
         for (int i = 0; i < kTileUnits; ++i) {
           const uint32_t w = c_prog.e[i].w;
           ring.produce(base + ((w & 0xFFFFFu) << 4), (w >> 20) * 128u);
@@ -316,8 +313,8 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
 
     for (int j = 0; j < n_tiles_cta; ++j) {
       const int unit = blockIdx.x + (j / tpu) * gridDim.x;
-      const bool real = unit < p.n_units;
-      const size_t gt = (size_t)unit * tpu + (j % tpu);
+      const bool real = unit < p.geom.n_units;
+      const size_t gt = p.geom.global_tile(unit, j % tpu);
       uint8_t* rec = real ? p.rec + gt * kRecBytes : nullptr;
       // d raw of tile j -> FP16 operand row in shared memory (+ its transposed image for the weight-gradient kernel)
       if (ch == 0) {
@@ -545,8 +542,8 @@ __global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__
   const int net = (part >= p.parts[0]) ? 1 : 0;
   if (net) part -= p.parts[0];
   const int parts = p.parts[net];
-  const int t_cnt = p.t_cnt[net], t_base = p.t_base[net];
-  const int total = p.n_units * t_cnt;
+  const int t_cnt = p.geom.tile_count(net);
+  const int total = p.geom.n_units * t_cnt;
   const int per = (total + parts - 1) / parts;
   const int j0 = part * per;
   const int j1 = min(total, j0 + per);
@@ -562,7 +559,7 @@ __global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__
 
   auto tile_rec = [&](int j) -> const uint8_t* {
     const int u = j / t_cnt, t = j - u * t_cnt;
-    return p.rec + ((size_t)u * p.tpu + t_base + t) * kRecBytes;
+    return p.rec + p.geom.global_tile(u, net, t) * kRecBytes;
   };
 
   if (warp < 4) {
@@ -883,13 +880,13 @@ __global__ void __launch_bounds__(kThreadsRow, 1) row_kernel(const InGradRowPara
   __syncthreads();
   const int row = threadIdx.x & 127, kq = threadIdx.x >> 7;
   const float inv = p.scal[1];
-  const int t_cnt = net ? p.tiles_f : p.tiles_c, t_base = net ? p.tiles_c : 0;
-  const int S = net ? p.s_fine : p.nc;
+  const int t_cnt = p.geom.tile_count(net);
+  const int S = p.geom.samples(net);
   const float* zp = net ? p.z_f : p.z_c;
-  const int total = p.n_units * t_cnt;
+  const int total = p.geom.n_units * t_cnt;
   for (int j = part; j < total; j += parts) {
     const int unit = j / t_cnt, tl = j - unit * t_cnt;
-    const size_t gt = (size_t)unit * (p.tiles_c + p.tiles_f) + t_base + tl;
+    const size_t gt = p.geom.global_tile(unit, net, tl);
     const uint8_t* rec = p.rec + gt * kRecBytes;
     float acc[16];
 #pragma unroll
@@ -921,9 +918,10 @@ __global__ void __launch_bounds__(kThreadsRow, 1) row_kernel(const InGradRowPara
       }
     }
     float4 r = make_float4(0.f, 0.f, 0.f, 0.f);
-    const int prow = tl * 128 + row, rr = prow / S, i = prow - rr * S, g = unit * p.rays_per_unit + rr;
-    if (rr < p.rays_per_unit && g < p.n_rays) {
-      const float z = zp[(size_t)g * S + i];
+    const TileGeom::Row rw = p.geom.row(net, tl, row);
+    const int g = p.geom.ray_index(unit, rw.ray);
+    if (rw.used && g < p.geom.n_rays) {
+      const float z = zp[(size_t)g * S + rw.sample];
       const float* ray = p.ray + 7 * (size_t)g;
       // p = o + d z rounded twice, exactly as the forward encoded it (one fused rounding moves p by an ulp at times, and the
       // 2^9 frequency turns that into a phase error)
@@ -968,18 +966,16 @@ __global__ void __launch_bounds__(kThreadsRow, 1) row_kernel(const InGradRowPara
 __global__ void __launch_bounds__(256) ray_kernel(const InGradRayParams p) {
   const int lane = threadIdx.x & 31;
   const int g = (blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  if (g >= p.n_rays) return;  // whole warps
-  const int npass = p.nf > 0 ? 2 : 1;
+  if (g >= p.geom.n_rays) return;  // whole warps
+  const int npass = p.geom.passes();
   float so0 = 0.f, so1 = 0.f, so2 = 0.f, sd0 = 0.f, sd1 = 0.f, sd2 = 0.f, sv = 0.f;
   if (p.rows) {
-    const int unit = g / p.rays_per_unit, rr = g - unit * p.rays_per_unit;
     for (int pass = 0; pass < npass; ++pass) {
-      const int S = pass ? p.s_fine : p.nc;
+      const int S = p.geom.samples(pass);
       const float* z = (pass ? p.z_f : p.z_c) + (size_t)g * S;
-      const size_t tile0 = (size_t)unit * (p.tiles_c + p.tiles_f) + (pass ? p.tiles_c : 0);
+      const TileGeom::RayRows rows = p.geom.ray_rows(pass, g);
       for (int i = lane; i < S; i += 32) {
-        const int prow = rr * S + i;
-        const float4 v = reinterpret_cast<const float4*>(p.rows)[(tile0 + (prow >> 7)) * 128 + (prow & 127)];
+        const float4 v = reinterpret_cast<const float4*>(p.rows)[rows.slot(i)];
         const float zi = z[i];
         so0 += v.x; so1 += v.y; so2 += v.z;
         sd0 = fmaf(zi, v.x, sd0); sd1 = fmaf(zi, v.y, sd1); sd2 = fmaf(zi, v.z, sd2);
@@ -998,7 +994,7 @@ __global__ void __launch_bounds__(256) ray_kernel(const InGradRayParams p) {
   if (p.g_o) { p.g_o[3 * g] = so0; p.g_o[3 * g + 1] = so1; p.g_o[3 * g + 2] = so2; }
   if (p.g_d) {
     float gdn = p.ray_dn[g];
-    if (npass == 2) gdn += p.ray_dn[p.n_rays + g];
+    if (npass == 2) gdn += p.ray_dn[p.geom.n_rays + g];
     const float* ray = p.ray + 7 * (size_t)g;
     const float dx = ray[3], dy = ray[4], dz = ray[5];
     const float s = gdn / p.dnorm[g];
@@ -1011,7 +1007,7 @@ __global__ void __launch_bounds__(256) ray_kernel(const InGradRayParams p) {
 #pragma unroll
     for (int c = 0; c < 3; ++c) {
       float b = p.ray_bg[3 * g + c];
-      if (npass == 2) b += p.ray_bg[3 * ((size_t)p.n_rays + g) + c];
+      if (npass == 2) b += p.ray_bg[3 * ((size_t)p.geom.n_rays + g) + c];
       p.g_bg[3 * g + c] = b;
     }
   }
@@ -1045,7 +1041,7 @@ cudaError_t train_kernels_setup() {
 }
 
 cudaError_t launch_composite_bwd(const CompBwdParams& q, float* scal, cudaStream_t st, long long* launches) {
-  const int n = (q.nf > 0 ? 2 : 1) * q.n_rays;
+  const int n = q.geom.passes() * q.geom.n_rays;
   if (q.ray_dn) composite_bwd_kernel<true><<<(n + 7) / 8, 256, 0, st>>>(q);  // one warp per (ray, pass)
   else composite_bwd_kernel<false><<<(n + 7) / 8, 256, 0, st>>>(q);
   ++*launches;
@@ -1055,7 +1051,7 @@ cudaError_t launch_composite_bwd(const CompBwdParams& q, float* scal, cudaStream
 }
 
 cudaError_t launch_chain(const ChainParams& p, int num_sms, cudaStream_t st, long long* launches) {
-  const int grid = p.n_units < num_sms ? p.n_units : num_sms;
+  const int grid = p.geom.n_units < num_sms ? p.geom.n_units : num_sms;
   if (grid <= 0) return cudaSuccess;
   chain::chain_kernel<<<grid, kThreads, chain::kSmemBytes, st>>>(p);
   ++*launches;
@@ -1097,7 +1093,7 @@ size_t dw_workspace_floats(int num_sms) {  // the most parts dw_split deals out 
 cudaError_t launch_dw(DwParams& p, int num_sms, cudaStream_t st, long long* launches, bool pe_only) {
   p.parts[0] = p.parts[1] = 0;
   p.ws_stride = pe_only ? dw::kPeSlotFloats : kAccBRaw;
-  const long long tot0 = (long long)p.n_units * p.t_cnt[0], tot1 = (long long)p.n_units * p.t_cnt[1];
+  const long long tot0 = (long long)p.geom.n_units * p.geom.tiles_c, tot1 = (long long)p.geom.n_units * p.geom.tiles_f;
   if (tot0 + tot1 <= 0) return cudaSuccess;
   dw_split(dw_split_sms(num_sms, pe_only), tot0, tot1, &p.parts[0], &p.parts[1]);
   if (p.parts[0] + p.parts[1] < 1) return cudaSuccess;
@@ -1118,7 +1114,7 @@ cudaError_t launch_grad_reduce(const DwParams* d, bool pe_only, const float* bsu
     r.ws = d->ws;
     r.stride = d->ws_stride;
     for (int net = 0; net < 2; ++net) {  // the parts dw_kernel gave tiles: the leading ones (j0 = part * per)
-      const long long total = (long long)d->n_units * d->t_cnt[net];
+      const long long total = (long long)d->geom.n_units * d->geom.tile_count(net);
       const int parts = d->parts[net];
       if (parts > 0 && total > 0) {
         const long long per = (total + parts - 1) / parts;
@@ -1173,7 +1169,7 @@ cudaError_t launch_input_grads(const InGradRowParams& r_in, const InGradRayParam
   InGradRayParams q = q_in;
   if (q.g_o || q.g_d || q.g_dir_z) {
     InGradRowParams r = r_in;
-    const long long tot0 = (long long)r.n_units * r.tiles_c, tot1 = q.nf > 0 ? (long long)r.n_units * r.tiles_f : 0;
+    const long long tot0 = (long long)r.geom.n_units * r.geom.tiles_c, tot1 = (long long)r.geom.n_units * r.geom.tiles_f;
     dw_split(num_sms * dw::kGroups, tot0, tot1, &r.parts[0], &r.parts[1]);  // num_sms CTAs, split by tile counts
     ing::row_kernel<<<r.parts[0] + r.parts[1], ing::kThreadsRow, ing::kSmemBytes, st>>>(r);
     ++*launches;
@@ -1181,7 +1177,7 @@ cudaError_t launch_input_grads(const InGradRowParams& r_in, const InGradRayParam
   } else {
     q.rows = nullptr;
   }
-  ing::ray_kernel<<<(q.n_rays + 7) / 8, 256, 0, st>>>(q);  // one warp per ray
+  ing::ray_kernel<<<(q.geom.n_rays + 7) / 8, 256, 0, st>>>(q);  // one warp per ray
   ++*launches;
   return cudaGetLastError();
 }

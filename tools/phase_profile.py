@@ -44,7 +44,7 @@ torch.cuda.synchronize()
 ms = e0.elapsed_time(e1)
 c = prof.cpu().tolist()
 
-# the kernel's work decomposition (nfb_api.cu): R rays per unit, tiles_c + tiles_f 128-row tiles per unit
+# the kernel's work decomposition (TileGeom::make in csrc/nfb_layout.h): R rays per unit, tiles_c + tiles_f 128-row tiles per unit
 R = 2 if 2 * (NC + NF) <= 512 else 1
 tiles_per_unit = -(-R * NC // 128) + (-(-R * (NC + NF) // 128) if NF > 0 else 0)
 units = -(-H * W // R)
