@@ -143,6 +143,59 @@ static_assert(round_trip(5, 64, 128) && round_trip(3, 128, 256) && round_trip(5,
               round_trip(5, 3, 7), "slot / row round trip");
 }  // namespace geom_check
 
+// The order in which one CTA of the render kernel runs the tiles of its n_iter units (its "tile stream"; the weight producer
+// and the row warps both walk it).  With C(u) = the coarse tiles of the CTA's u-th unit and F(u) = its fine tiles:
+//   C(0), [C(u+1), F(u)] for u = 0 .. n_iter-2, F(n_iter-1)        (nf == 0: C(0), C(1), ...)
+// so the per-ray stages of unit u (compositing, resampling, sorting) run on other warps while the tensor cores run C(u+1)
+// and the fine tiles of u-1.  Only the order changes: global_tile(unit, pass, t) still names each tile's record.
+struct StreamTile { int it, pass, t; };  // the CTA's unit iteration, pass (= network), tile within the pass
+NFB_HD constexpr int stream_tiles(const TileGeom& g, int n_iter) { return n_iter * g.tiles_per_unit(); }
+NFB_HD constexpr StreamTile stream_tile(const TileGeom& g, int n_iter, int k) {
+  const int tc = g.tiles_c, tpu = g.tiles_per_unit();
+  if (g.nf == 0) return StreamTile{k / tc, 0, k - (k / tc) * tc};
+  if (k < tc) return StreamTile{0, 0, k};
+  const int b = (k - tc) / tpu, r = (k - tc) - b * tpu;
+  if (b == n_iter - 1) return StreamTile{b, 1, r};
+  return r < tc ? StreamTile{b + 1, 0, r} : StreamTile{b, 1, r - tc};
+}
+
+namespace geom_check {
+// Every tile of every unit appears once, in its own network; C(u) precedes F(u); and the first tile of C(u) comes after
+// every tile of C(v <= u-1) and F(v <= u-2), the first tile of F(u) after every tile of C(v <= u) and F(v <= u-1): what
+// the render kernel's hand-offs wait for before those tiles (nfb_render.cu) is produced from strictly earlier tiles.
+constexpr bool stream_order(int nc, int nf, int n_iter) {
+  const TileGeom g = TileGeom::make(2 * n_iter, nc, nf);
+  constexpr int kMaxIt = 4, kMaxT = 8;
+  int pos[kMaxIt][2][kMaxT] = {};
+  int seen[kMaxIt][2][kMaxT] = {};
+  const int n = stream_tiles(g, n_iter);
+  for (int k = 0; k < n; ++k) {
+    const StreamTile s = stream_tile(g, n_iter, k);
+    if (s.it < 0 || s.it >= n_iter || s.pass < 0 || s.pass >= g.passes() || s.t < 0 || s.t >= g.tile_count(s.pass)) return false;
+    if (g.net_of(g.tile_base(s.pass) + s.t) != s.pass) return false;
+    ++seen[s.it][s.pass][s.t];
+    pos[s.it][s.pass][s.t] = k;
+  }
+  for (int u = 0; u < n_iter; ++u)
+    for (int pass = 0; pass < g.passes(); ++pass)
+      for (int t = 0; t < g.tile_count(pass); ++t) {
+        if (seen[u][pass][t] != 1) return false;
+        const int first = pos[u][pass][0];
+        for (int v = 0; v < n_iter; ++v)
+          for (int q = 0; q < g.passes(); ++q)
+            for (int x = 0; x < g.tile_count(q); ++x) {
+              const bool before = pass == 0 ? (q == 0 ? v <= u - 1 : v <= u - 2) : (q == 0 ? v <= u : v <= u - 1);
+              if (before && pos[v][q][x] >= first) return false;
+            }
+      }
+  return true;
+}
+static_assert(stream_order(64, 128, 1) && stream_order(64, 128, 2) && stream_order(64, 128, 3) && stream_order(128, 256, 3) &&
+              stream_order(256, 256, 1) && stream_order(256, 256, 2) && stream_order(256, 256, 3) && stream_order(64, 0, 1) &&
+              stream_order(64, 0, 3) && stream_order(3, 7, 1) && stream_order(3, 7, 2) && stream_order(3, 7, 3),
+              "render tile stream order");
+}  // namespace geom_check
+
 // ------------------------------------------------------------------------------------------------
 // Training: per-tile activation record (written by the forward kernel in SAVE mode and by the backward chain kernel,
 // read by the weight-gradient kernel).  Every entry is a TRANSPOSED image of a [128 sample rows x C features] FP16

@@ -2,7 +2,8 @@
 // dw::dw_kernel): the thread roles, the register split between them, and the ring of shared-memory slots that the producer
 // warp fills with bulk copies and the consumer warpgroups drain, under full / empty mbarriers.
 //
-// Roles (384 threads): warpgroup 0 is the producer side (warp 0 issues the copies; warps 1..3 idle), warpgroups 1 and 2 are
+// Roles (384 threads): warpgroup 0 is the producer side (warp 0 issues the copies; warps 1..3 idle, except in render_kernel,
+// where they run the per-ray stages), warpgroups 1 and 2 are
 // the consumers ("row" warps), each issuing the wgmma of 64 tile rows.  The register file is re-partitioned per warpgroup.
 #pragma once
 #include <stdint.h>
@@ -13,9 +14,16 @@ namespace nfb {
 
 constexpr int kThreads = 384;        // producer warpgroup + 2 consumer warpgroups
 constexpr int kRowThreads = 256;     // the two consumer warpgroups
+constexpr int kRayThreads = 96;      // render_kernel: warps 1..3 of the producer warpgroup, its per-ray stages
 constexpr uint32_t kRowBarrier = 1;  // named barrier id of the eight consumer warps; 2 + w: warpgroup w alone (render_kernel: 4 + w, its MMA ping-pong)
 constexpr int kRegsLight = 40, kRegsRow = 232;
 static_assert((4 * kRegsLight + 8 * kRegsRow) * 32 <= 65536, "register file");
+// render_kernel's producer warpgroup also runs the per-ray stages (warps 1..3), which spill at 40 registers.  setmaxnreg.inc
+// takes registers only from those the CTA's other warps released, so a split must fit the kernel's own allocation (384
+// threads x 168 registers under __launch_bounds__(384, 1)), not just the register file: the row warps give up 8.
+constexpr int kRegsRenderLight = 56, kRegsRenderRow = 224;
+static_assert(4 * kRegsLight + 8 * kRegsRow <= 12 * 168 && 4 * kRegsRenderLight + 8 * kRegsRenderRow <= 12 * 168,
+              "a register split must fit the 168 registers per thread a 384-thread kernel is compiled for");
 template <int N> __device__ __forceinline__ void reg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
 template <int N> __device__ __forceinline__ void reg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
 

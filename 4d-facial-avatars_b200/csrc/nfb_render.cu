@@ -54,19 +54,23 @@ struct SmemMap {
   static constexpr int kActLo = kActHi + kActBytes;
   static constexpr int kPeHi = kActLo + kActBytes;
   static constexpr int kPeLo = kPeHi + kTileM * 128;
-  static constexpr int kRaw = kPeLo + (EXACT ? kTileM * 128 : 0);
-  static constexpr int kZ = kRaw + kRowsMax * 16;
-  static constexpr int kW = kZ + kRowsMax * 4;
+  // Per-unit buffers, one copy each unless noted (the table in DESIGN §4 gives each one's writer, reader and lifetime):
+  static constexpr int kRaw = kPeLo + (EXACT ? kTileM * 128 : 0);  // coarse carry: (colour, sigma) per sample row
+  static constexpr int kRawF = kRaw + kRowsMax * 16;                  // fine carry (nf == 0: the second coarse copy)
+  static constexpr int kZ = kRawF + kRowsMax * 16;                    // coarse depths
+  static constexpr int kZF = kZ + kRowsMax * 4;                       // fine depths (nf == 0: the second coarse copy)
+  static constexpr int kW = kZF + kRowsMax * 4;                       // ray warps' scratch: [ray][kRowsMax / 2] each
   static constexpr int kCdf = kW + kRowsMax * 4;
   static constexpr int kBins = kCdf + kRowsMax * 4;
   static constexpr int kSort = kBins + kRowsMax * 4;
-  static constexpr int kDirBias = kSort + kRowsMax * 4;
-  static constexpr int kRay = kDirBias + 2 * 2 * 128 * 4;  // dirbias: [pass][ray][128]
-  static constexpr int kTileRaw = kRay + 2 * kRayFloats * 4;  // [128] (rgb raw, sigma raw) of the current tile
+  static constexpr int kDirBias = kSort + kRowsMax * 4;  // [coarse of an even unit, coarse of an odd unit, fine][ray][128]
+  static constexpr int kRay = kDirBias + 3 * 2 * 128 * 4;            // RayP [unit % 3][ray]
+  static constexpr int kTileRaw = kRay + 3 * 2 * kRayFloats * 4;  // [128] (rgb raw, sigma raw) of the current tile
   static constexpr int kBars = kTileRaw + kTileM * 16;
-  static constexpr int kBytes = kBars + 2 * kSlots * 8;
+  static constexpr int kHand = kBars + 2 * kSlots * 8;  // the hand-off mbarriers (Hand)
+  static constexpr int kBytes = kHand + 9 * 8;
   static_assert(kBytes <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
-  static_assert(kRaw % 16 == 0 && kBars % 8 == 0, "alignment");
+  static_assert(kRaw % 16 == 0 && kBars % 8 == 0 && kHand % 8 == 0, "alignment");
 };
 
 constexpr int kTileUnits = prog_units(kFwdStream);
@@ -283,8 +287,52 @@ __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_ba
 }
 
 // ------------------------------------------------------------------------------------------------
+// Hand-offs between the row warps (tiles) and the ray warps (per-ray stages), one mbarrier each, phases counted per unit:
+//   cdone[b]  row warps -> ray warps: the coarse tiles of the unit in coarse buffer b are done (arrivals: every row thread)
+//   cfree[b]  ray warps -> row warps: coarse buffer b has been read (arrivals: every ray-warp thread)
+//   fdone     row warps -> ray warps: the unit's fine tiles are done
+//   fready    ray warps -> row warps: the unit's fine depths and fine direction term are written, and the fine carry of the
+//             unit before it has been read
+//   sready[s] ray warps -> row warps: RayP slot s and the coarse direction term of its unit are written
+// A unit's coarse buffer is it % nb, nb = 1 with a fine pass (its slack is the fine tiles of the unit before) and 2
+// without one; its RayP slot is it % 3.
+struct Hand {
+  uint32_t base;
+  __device__ __forceinline__ uint32_t cdone(int b) const { return base + 8 * b; }
+  __device__ __forceinline__ uint32_t cfree(int b) const { return base + 16 + 8 * b; }
+  __device__ __forceinline__ uint32_t fdone() const { return base + 32; }
+  __device__ __forceinline__ uint32_t fready() const { return base + 40; }
+  __device__ __forceinline__ uint32_t sready(int s) const { return base + 48 + 8 * s; }
+  __device__ __forceinline__ void init() const {
+    for (int b = 0; b < 2; ++b) { mbar_init(cdone(b), kRowThreads); mbar_init(cfree(b), kRayThreads); }
+    mbar_init(fdone(), kRowThreads);
+    mbar_init(fready(), kRayThreads);
+    for (int s = 0; s < 3; ++s) mbar_init(sready(s), kRayThreads);
+    mbar_fence_init();
+  }
+};
+
 // PROBE: the instantiation that honours the activation probe (RenderParams::dbg_act); launch_render picks it only when the
 // probe is requested.
+//
+// Roles.  Warp 0 streams the weights; warps 1..3 (the "ray warps") run the per-ray stages, warp 1 + rr those of ray rr of
+// each unit (warp 3 only keeps the arrival counts); warpgroups 1 and 2 (the "row warps") run the tiles.  The producer and
+// the row warps walk the CTA's tile stream (stream_tile, nfb_layout.h): C(0), C(1), F(0), C(2), F(1), ...  The ray warps
+// run, for unit it: wait cdone(it); composite the coarse pass, CDF, inverse-CDF samples; arrive cfree; wait fdone(it-1),
+// composite the fine pass of it-1; merge-sort the fine depths of it, its fine direction term; arrive fready; set up unit
+// it+2 (RayP, direction encoding, coarse direction term); arrive sready.  The row warps wait sready(it) and cfree(it-nb)
+// before the first tile of C(it), fready(it) before that of F(it), and arrive cdone / fdone after the last tile of a pass.
+//
+// Deadlock freedom.  Every arrival above is made by every thread of its side on every path: for invalid rays, for the warp
+// without a ray, for n_iter = 1 and for the CTA's last unit (the loops run the same n_iter on both sides, n_iter >= 1); no
+// arrival sits under a data-dependent condition.  What the ray warps arrive for unit it depends only on cdone(v <= it) and
+// fdone(v <= it-1) (they run their units in order), so cfree(it - nb) and sready(it) depend on the tiles of C(v <= it-1)
+// and F(v <= it-2), fready(it) on those of C(v <= it) and F(v <= it-1), and stream_order (nfb_layout.h) asserts that all
+// of these come before the tile that waits.  Induction over the stream position: no wait depends on itself.  No barrier
+// runs more than one phase ahead of a waiter, which the parity waits need: cdone(b)'s next phase needs C(it + nb), after
+// cfree(it); fdone's needs fready(it + 1), after the ray warps' wait for fdone(it); cfree and fready need cdone / fdone of
+// the next unit, after the row warps' waits; sready(s)'s needs cdone(it + 1).  The producer depends on the row warps
+// only through the weight ring, which both walk in stream order.
 template <bool EXACT, bool SAVE, bool PROBE>
 __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_constant__ RenderParams p) {
   using M = SmemMap<EXACT>;
@@ -296,37 +344,302 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
   constexpr int NPART = EXACT ? 2 : 1;
 
   typename M::WeightRing ring(smem_base + M::kRing, smem_base + M::kBars);
-  if (threadIdx.x == 0) ring.init();
+  const Hand hand{smem_base + M::kHand};
+  if (threadIdx.x == 0) {
+    ring.init();
+    hand.init();
+  }
   __syncthreads();
 
   const TileGeom& geom = p.geom;
   const int n_iter = (geom.n_units - (int)blockIdx.x + (int)gridDim.x - 1) / (int)gridDim.x;
-  const int tiles_per_unit = geom.tiles_per_unit();
+  const int n_stream = stream_tiles(geom, n_iter);
+  const int nb = geom.nf > 0 ? 1 : 2;  // coarse buffers
+  const int R = geom.rays_per_unit;
+  float4* raw_c = reinterpret_cast<float4*>(smem + M::kRaw);
+  float4* raw_f = reinterpret_cast<float4*>(smem + M::kRawF);
+  float* z_c = reinterpret_cast<float*>(smem + M::kZ);
+  float* z_f = reinterpret_cast<float*>(smem + M::kZF);
+  float* dirbias = reinterpret_cast<float*>(smem + M::kDirBias);
+  RayP* rayp_all = reinterpret_cast<RayP*>(smem + M::kRay);
 
   if (warp < 4) {
-    // ============================== weight producer ==============================
-    // The whole warp runs the (warp-uniform) loop; one elected lane issues the copies.
-    reg_dec<kRegsLight>();
+    reg_dec<kRegsRenderLight>();
     if (warp == 0) {
-      for (int it = 0; it < n_iter; ++it) {
-        for (int t = 0; t < tiles_per_unit; ++t) {
-          const uint8_t* base = p.wstream[geom.net_of(t)];
-          for (int i = 0; i < kTileUnits; ++i) {
-            const uint32_t w = c_prog.e[i].w;
-            const uint32_t off = (w & 0xFFFFFu) << 4, bytes = (w >> 20) * 128u;
+      // ============================== weight producer ==============================
+      // The whole warp runs the (warp-uniform) loop; one elected lane issues the copies.
+      for (int k = 0; k < n_stream; ++k) {
+        const uint8_t* base = p.wstream[stream_tile(geom, n_iter, k).pass];
+        for (int i = 0; i < kTileUnits; ++i) {
+          const uint32_t w = c_prog.e[i].w;
+          const uint32_t off = (w & 0xFFFFFu) << 4, bytes = (w >> 20) * 128u;
 #pragma unroll
-            for (int part = 0; part < NPART; ++part)  // exact mode: the hi unit, then the lo unit
-              ring.produce(EXACT ? base + 2 * (size_t)off + part * bytes : base + off, bytes);
+          for (int part = 0; part < NPART; ++part)  // exact mode: the hi unit, then the lo unit
+            ring.produce(EXACT ? base + 2 * (size_t)off + part * bytes : base + off, bytes);
+        }
+      }
+    } else {
+      // ============================== ray warps ==============================
+      const int rr = warp - 1;  // this warp's ray within each unit
+      const bool mine = rr < R;
+      const int rs = rr * (kRowsMax / 2);  // this ray's part of the scratch buffers (R == 1: ray 0, all of them)
+      float* scr_w = reinterpret_cast<float*>(smem + M::kW) + rs;
+      float* scr_cdf = reinterpret_cast<float*>(smem + M::kCdf) + rs;
+      float* scr_bins = reinterpret_cast<float*>(smem + M::kBins) + rs;
+      float* scr_sort = reinterpret_cast<float*>(smem + M::kSort) + rs;
+      const bool has_bg = p.bg != nullptr;
+      const int nc = geom.nc, nf = geom.nf, SF = geom.samples(1);
+      // observer: lane 0 of warp 1, laps at kProfRay + slot
+      PhaseTimer tm(p.prof ? p.prof + kProfRay : nullptr, p.prof != nullptr && threadIdx.x == 32);
+      // The CDF of an invalid ray reads weights no compositing wrote: give them a value.
+      if (mine)
+        for (int k = lane; k < kRowsMax / R; k += 32) scr_w[k] = 0.f;
+
+      // per-ray term of layers_dir.0 of network `pass`: W[:, 256:280] . PE_dir (one output feature per lane and step), read by
+      // every step-6 epilogue of the unit's tiles of that network
+      auto dir_term = [&](const RayP& rq, int pass, float* dst) {
+        const float* wt = p.wd0b_t[pass];
+        for (int col = lane; col < 128; col += 32) {
+          float acc0 = 0.f;
+#pragma unroll 8
+          for (int j = 0; j < kDimDir; ++j) acc0 = fmaf(wt[j * 128 + col], rq.ped[j], acc0);
+          dst[rr * 128 + col] = acc0;
+        }
+      };
+      // ---- per-ray constants of unit `it`, its direction encoding and its coarse direction term
+      auto setup = [&](int it) {
+        if (mine) {
+          const int unit = blockIdx.x + it * gridDim.x;
+          RayP& rp = rayp_all[(it % 3) * 2 + rr];
+          if (lane == 0) {
+            const int g = geom.ray_index(unit, rr);
+            rp.valid = g < geom.n_rays;
+            rp.gidx = g;
+            if (rp.valid) {
+              float o0, o1, o2, d0, d1, d2;
+              if (p.o) {
+                o0 = p.o[3 * g]; o1 = p.o[3 * g + 1]; o2 = p.o[3 * g + 2];
+                d0 = p.d[3 * g]; d1 = p.d[3 * g + 1]; d2 = p.d[3 * g + 2];
+              } else {  // get_ray_bundle (nerf_helpers.py:111-122), same operation order in FP32
+                const int pj = p.row_begin + g / p.width, pi = g % p.width;
+                const float cx = __fdiv_rn(__fsub_rn((float)pi, p.wcx), p.fx);
+                const float cy = -__fdiv_rn(__fsub_rn((float)pj, p.hcy), p.fy);
+                d0 = __fadd_rn(__fadd_rn(__fmul_rn(cx, p.pose[0]), __fmul_rn(cy, p.pose[1])), __fmul_rn(-1.f, p.pose[2]));
+                d1 = __fadd_rn(__fadd_rn(__fmul_rn(cx, p.pose[4]), __fmul_rn(cy, p.pose[5])), __fmul_rn(-1.f, p.pose[6]));
+                d2 = __fadd_rn(__fadd_rn(__fmul_rn(cx, p.pose[8]), __fmul_rn(cy, p.pose[9])), __fmul_rn(-1.f, p.pose[10]));
+                o0 = p.pose[3]; o1 = p.pose[7]; o2 = p.pose[11];
+              }
+              rp.o[0] = o0; rp.o[1] = o1; rp.o[2] = o2;
+              rp.d[0] = d0; rp.d[1] = d1; rp.d[2] = d2;
+              rp.dnorm = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(d0, d0), __fmul_rn(d1, d1)), __fmul_rn(d2, d2)));
+              if (has_bg) { rp.bg[0] = p.bg[3 * g]; rp.bg[1] = p.bg[3 * g + 1]; rp.bg[2] = p.bg[3 * g + 2]; }
+              rp.dz = p.dir_z ? p.dir_z[g] : d2;
+              if constexpr (SAVE) {
+                p.save_dnorm[g] = rp.dnorm;
+                if (p.save_ray) {  // the ray as the input gradients need it: o, d, direction-encoder input
+                  float* sr = p.save_ray + 7 * (size_t)g;
+                  sr[0] = o0; sr[1] = o1; sr[2] = o2; sr[3] = d0; sr[4] = d1; sr[5] = d2; sr[6] = rp.dz;
+                }
+              }
+            } else {
+              for (int k = 0; k < 3; ++k) { rp.o[k] = 0.f; rp.d[k] = 0.f; rp.bg[k] = 0.f; }
+              rp.dnorm = 0.f;
+              rp.dz = 0.f;
+            }
+          }
+          __syncwarp();
+          // direction encoder input is (d_z, near, far): run_network reads ray_batch[..., -3:] (train_utils.py:14);
+          // one accurate sincos per lane
+          if (lane < 12) {
+            const int f = lane / 3, c = lane - f * 3;
+            const float v = (c == 0) ? rp.dz : (c == 1 ? p.near_ : p.far_);
+            float sn, cs;
+            sincosf(v * (float)(1 << f), &sn, &cs);
+            rp.ped[6 * f + c] = rp.valid ? sn : 0.f;
+            rp.ped[6 * f + 3 + c] = rp.valid ? cs : 0.f;
+          }
+          __syncwarp();
+          dir_term(rp, 0, dirbias + (it & 1) * 256);
+        }
+        __syncwarp();
+        mbar_arrive(hand.sready(it % 3));
+      };
+      // ---- compositing of this warp's ray in pass `pass` of unit `it`
+      auto composite = [&](int it, int pass, const float4* carry_raw, const float* carry_z) {
+        const RayP& rp = rayp_all[(it % 3) * 2 + rr];
+        const int S = geom.samples(pass);
+        float* dz = pass ? p.dbg_z_f : p.dbg_z_c;  // debug dump of the sample depths
+        if (dz && rp.valid)
+          for (int i = lane; i < S; i += 32) dz[(size_t)rp.gidx * S + i] = carry_z[rr * S + i];
+        if (rp.valid) {
+          const int g = rp.gidx;
+          float* o_rgb = pass ? p.rgb_f : p.rgb_c;
+          float* o_disp = pass ? p.disp_f : p.disp_c;
+          float* o_acc = pass ? p.acc_f : p.acc_c;
+          const float wl = composite_ray(carry_raw + rr * S, carry_z + rr * S, scr_w, S, rp.dnorm, p.white_bkgd != 0,
+                                         o_rgb ? o_rgb + 3 * (size_t)g : nullptr, o_disp ? o_disp + g : nullptr,
+                                         o_acc ? o_acc + g : nullptr, lane);
+          const bool last_pass = (pass == 1) || (nf == 0);
+          if (last_pass && lane == 0 && p.w_last) p.w_last[g] = wl;
+        }
+        __syncwarp();
+      };
+
+      setup(0);
+      if (n_iter > 1) setup(1);
+      tm.lap(7);
+      for (int it = 0; it < n_iter; ++it) {
+        const int cb = it % nb;
+        const float4* craw = cb ? raw_f : raw_c;
+        const float* cz = cb ? z_f : z_c;
+        mbar_wait(hand.cdone(cb), (uint32_t)(it / nb) & 1u);
+        tm.lap(0);
+        if (mine) {
+          composite(it, 0, craw, cz);
+          tm.lap(1);
+          if (nf > 0) {
+            // ---- inverse-CDF resampling (nerf_helpers.py:344-387) on weights[1:-1] over the mid-point bins
+            const RayP& rp = rayp_all[(it % 3) * 2 + rr];
+            const int nb_ = nc - 1;  // bins / cdf entries
+            const int nw = nc - 2;   // interior weights
+            {
+              const float* w = scr_w;
+              const float* zc = cz + rr * nc;
+              float* cdf = scr_cdf;
+              float* bins = scr_bins;
+              for (int k = lane; k < nb_; k += 32) bins[k] = __fmul_rn(0.5f, __fadd_rn(zc[k + 1], zc[k]));
+              const int per = (nw + 31) >> 5;
+              const int k0 = lane * per;
+              float part = 0.f;
+              for (int j = 0; j < per; ++j)
+                if (k0 + j < nw) part += __fadd_rn(w[k0 + j + 1], 1e-5f);
+              const float total = warp_sum(part);
+              float psum = 0.f;
+              for (int j = 0; j < per; ++j)
+                if (k0 + j < nw) psum += __fdiv_rn(__fadd_rn(w[k0 + j + 1], 1e-5f), total);
+              float incl = psum;
+#pragma unroll
+              for (int o = 1; o < 32; o <<= 1) {
+                const float tt = __shfl_up_sync(0xffffffffu, incl, o);
+                if (lane >= o) incl += tt;
+              }
+              float run = incl - psum;  // exclusive prefix of this lane's block
+              if (lane == 0) cdf[0] = 0.f;
+              for (int j = 0; j < per; ++j)
+                if (k0 + j < nw) {
+                  run += __fdiv_rn(__fadd_rn(w[k0 + j + 1], 1e-5f), total);
+                  cdf[k0 + j + 1] = run;
+                }
+            }
+            __syncwarp();
+            tm.lap(2);
+            // cat(z_coarse, z_samples) of the ray into scr_sort
+            for (int i = lane; i < SF; i += 32) {
+              float val;
+              if (i < nc) {
+                val = cz[rr * nc + i];
+              } else {
+                const int j = i - nc;
+                const float* cdf = scr_cdf;
+                const float* bins = scr_bins;
+                const float u = p.perturb ? (rp.valid ? p.u_rand[(size_t)rp.gidx * nf + j] : 0.f) : p.u_fine[j];
+                int lo = 0, hi = nb_;  // searchsorted(..., right=True): number of cdf entries <= u
+                while (lo < hi) {
+                  const int mid = (lo + hi) >> 1;
+                  if (cdf[mid] <= u) lo = mid + 1; else hi = mid;
+                }
+                const int below = max(0, lo - 1), above = min(nb_ - 1, lo);
+                const float cb_ = cdf[below], ca = cdf[above];
+                float den = __fsub_rn(ca, cb_);
+                if (den < 1e-5f) den = 1.f;
+                const float tt = __fdiv_rn(__fsub_rn(u, cb_), den);
+                val = __fadd_rn(bins[below], __fmul_rn(tt, __fsub_rn(bins[above], bins[below])));
+              }
+              scr_sort[i] = val;
+            }
+            tm.lap(3);
           }
         }
+        __syncwarp();
+        mbar_arrive(hand.cfree(cb));  // the coarse carry of unit it is read
+        if (nf > 0) {
+          if (it > 0) {
+            mbar_wait(hand.fdone(), (uint32_t)(it - 1) & 1u);
+            tm.lap(4);
+            if (mine) composite(it - 1, 1, raw_f, z_f);
+            tm.lap(5);
+          }
+          if (mine) {
+            // ---- torch.sort(cat(z, z_samples)) (train_utils.py:126) as a rank merge: the coarse depths are sorted, the
+            //      samples need not be (stochastic u), so an element's rank = (# coarse before it, by binary search)
+            //      + (# samples before it, counted).  Ties: coarse first, then samples by index — equal values make any
+            //      tie order give the same sorted array.  A NaN sample (from non-finite weights) goes after every number,
+            //      by index, as torch.sort places it; no comparison with a NaN counts, so the other ranks stay as they are.
+            //      When the samples are already sorted and hold no NaN (deterministic u), the same ranks follow from binary
+            //      searches alone: # samples < v for a coarse depth, and j itself for sample j.
+            __syncwarp();
+            bool sorted = true;
+            for (int j = lane; j < nf; j += 32) {
+              const float y = scr_sort[nc + j];
+              sorted = sorted && y == y && (j + 1 == nf || y <= scr_sort[nc + j + 1]);
+            }
+            sorted = __all_sync(0xffffffffu, sorted);
+            for (int i = lane; i < SF; i += 32) {
+              const float* zc = scr_sort;
+              const float* zs = zc + nc;
+              const float v = zc[i];
+              int rank;
+              if (sorted) {
+                const float* a = i < nc ? zs : zc;
+                int lo = 0, hi = i < nc ? nf : nc;  // coarse: # samples < v; sample: # coarse depths <= v
+                while (lo < hi) {
+                  const int mid = (lo + hi) >> 1;
+                  if (i < nc ? a[mid] < v : a[mid] <= v) lo = mid + 1; else hi = mid;
+                }
+                rank = lo + (i < nc ? i : i - nc);
+              } else if (i < nc) {
+                rank = i;
+                for (int j = 0; j < nf; ++j) rank += (zs[j] < v) ? 1 : 0;
+              } else if (v != v) {
+                const int jm = i - nc;
+                rank = nc;
+                for (int j = 0; j < nf; ++j) rank += (zs[j] == zs[j] || j < jm) ? 1 : 0;
+              } else {
+                const int jm = i - nc;
+                int lo = 0, hi = nc;  // # coarse depths <= v
+                while (lo < hi) {
+                  const int mid = (lo + hi) >> 1;
+                  if (zc[mid] <= v) lo = mid + 1; else hi = mid;
+                }
+                rank = lo;
+                for (int j = 0; j < nf; ++j) {
+                  const float y = zs[j];
+                  rank += (y < v || (y == v && j < jm)) ? 1 : 0;
+                }
+              }
+              z_f[rr * SF + rank] = v;
+            }
+            tm.lap(6);
+            dir_term(rayp_all[(it % 3) * 2 + rr], 1, dirbias + 512);
+          }
+          __syncwarp();
+          mbar_arrive(hand.fready());
+        }
+        if (it + 2 < n_iter) setup(it + 2);
+        tm.lap(7);
+      }
+      if (nf > 0) {
+        mbar_wait(hand.fdone(), (uint32_t)(n_iter - 1) & 1u);
+        tm.lap(4);
+        if (mine) composite(n_iter - 1, 1, raw_f, z_f);
+        tm.lap(5);
       }
     }
   } else {
     // ============================== row warps ==============================
-    reg_inc<kRegsRow>();
+    reg_inc<kRegsRenderRow>();
     const int q = warp & 3;
     const int wg = (warp - 4) >> 2;        // row warpgroup: tile rows [64 wg, 64 wg + 64)
-    const int ew = warp - 4;               // 0..7, ray index for per-ray stages
     const int etid = wg * 128 + q * 32 + lane;  // 0..255
     // per-tile row stages (prologue, post-processing): the warpgroup's own rows, two threads per row, one PE half each
     const int half = q >> 1;
@@ -337,461 +650,263 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
     uint8_t* pe_lo = smem + M::kPeLo;
     uint8_t* act_hi = smem + M::kActHi;
     uint8_t* act_lo = smem + M::kActLo;
-    float4* carry_raw = reinterpret_cast<float4*>(smem + M::kRaw);
-    float* carry_z = reinterpret_cast<float*>(smem + M::kZ);
-    float* scr_w = reinterpret_cast<float*>(smem + M::kW);
-    float* scr_cdf = reinterpret_cast<float*>(smem + M::kCdf);
-    float* scr_bins = reinterpret_cast<float*>(smem + M::kBins);
-    float* scr_sort = reinterpret_cast<float*>(smem + M::kSort);
-    float* dirbias = reinterpret_cast<float*>(smem + M::kDirBias);
-    RayP* rayp = reinterpret_cast<RayP*>(smem + M::kRay);
     float4* tile_raw = reinterpret_cast<float4*>(smem + M::kTileRaw);
-    const int R = geom.rays_per_unit;
     const bool has_bg = p.bg != nullptr;
     // observers: the first thread of each row warpgroup, warpgroup w's laps at slot + kProfWgStride * w
     PhaseTimer tm(p.prof ? p.prof + kProfWgStride * wg : nullptr, p.prof != nullptr && (etid & 127) == 0);
 
-    for (int it = 0; it < n_iter; ++it) {
+    for (int k = 0; k < n_stream; ++k) {
+      const StreamTile stile = stream_tile(geom, n_iter, k);
+      const int it = stile.it, pass = stile.pass, t = stile.t;
       const int unit = blockIdx.x + it * gridDim.x;
-      tm.lap(39);
-      // ---- per-ray constants
-      if (etid < R) {
-        RayP& rp = rayp[etid];
-        const int g = geom.ray_index(unit, etid);
-        rp.valid = g < geom.n_rays;
-        rp.gidx = g;
-        if (rp.valid) {
-          float o0, o1, o2, d0, d1, d2;
-          if (p.o) {
-            o0 = p.o[3 * g]; o1 = p.o[3 * g + 1]; o2 = p.o[3 * g + 2];
-            d0 = p.d[3 * g]; d1 = p.d[3 * g + 1]; d2 = p.d[3 * g + 2];
-          } else {  // get_ray_bundle (nerf_helpers.py:111-122), same operation order in FP32
-            const int pj = p.row_begin + g / p.width, pi = g % p.width;
-            const float cx = __fdiv_rn(__fsub_rn((float)pi, p.wcx), p.fx);
-            const float cy = -__fdiv_rn(__fsub_rn((float)pj, p.hcy), p.fy);
-            d0 = __fadd_rn(__fadd_rn(__fmul_rn(cx, p.pose[0]), __fmul_rn(cy, p.pose[1])), __fmul_rn(-1.f, p.pose[2]));
-            d1 = __fadd_rn(__fadd_rn(__fmul_rn(cx, p.pose[4]), __fmul_rn(cy, p.pose[5])), __fmul_rn(-1.f, p.pose[6]));
-            d2 = __fadd_rn(__fadd_rn(__fmul_rn(cx, p.pose[8]), __fmul_rn(cy, p.pose[9])), __fmul_rn(-1.f, p.pose[10]));
-            o0 = p.pose[3]; o1 = p.pose[7]; o2 = p.pose[11];
+      const int S = geom.samples(pass);
+      const int n_tiles = geom.tile_count(pass);
+      const float* bias_n = p.bias[pass];
+      const int cb = it % nb;
+      float4* carry_raw = (pass || cb) ? raw_f : raw_c;
+      float* carry_z = (pass || cb) ? z_f : z_c;
+      const RayP* rayp = rayp_all + (it % 3) * 2;
+      const float* dirb = dirbias + (pass ? 512 : (it & 1) * 256);  // [ray][128]
+      if (t == 0) {  // the pass's inputs from the ray warps, and its carry buffer free
+        if (pass == 0) {
+          mbar_wait(hand.sready(it % 3), (uint32_t)(it / 3) & 1u);
+          if (it >= nb) mbar_wait(hand.cfree(cb), (uint32_t)((it - nb) / nb) & 1u);
+        } else {
+          mbar_wait(hand.fready(), (uint32_t)it & 1u);
+        }
+        tm.lap(16);
+      }
+
+      // ---- prologue of tile t: sample depth + positional encoding -> PE buffer.
+      auto prologue = [&](int t) {
+        const TileGeom::Row rw = geom.row(pass, t, row);
+        const int prow = rw.pass_row, i = rw.sample;
+        const bool live = rw.used;
+        const RayP& rp = rayp[rw.ray];
+        float z = 0.f;
+        if (live) {
+          if (pass == 0) {
+            const float tc = p.t_coarse[i];
+            z = __fadd_rn(__fmul_rn(p.near_, __fsub_rn(1.f, tc)), __fmul_rn(p.far_, tc));
+            if (p.perturb) {  // stratified jitter (train_utils.py:69-76)
+              float lower = z, upper = z;
+              if (i > 0) {
+                const float tp = p.t_coarse[i - 1];
+                const float zp = __fadd_rn(__fmul_rn(p.near_, __fsub_rn(1.f, tp)), __fmul_rn(p.far_, tp));
+                lower = __fmul_rn(0.5f, __fadd_rn(z, zp));
+              }
+              if (i < S - 1) {
+                const float tn = p.t_coarse[i + 1];
+                const float zn = __fadd_rn(__fmul_rn(p.near_, __fsub_rn(1.f, tn)), __fmul_rn(p.far_, tn));
+                upper = __fmul_rn(0.5f, __fadd_rn(zn, z));
+              }
+              const float tr = rp.valid ? p.t_rand[(size_t)rp.gidx * geom.nc + i] : 0.f;
+              z = __fadd_rn(lower, __fmul_rn(__fsub_rn(upper, lower), tr));
+            }
+            if (half == 0) carry_z[prow] = z;
+          } else {
+            z = carry_z[prow];
           }
-          rp.o[0] = o0; rp.o[1] = o1; rp.o[2] = o2;
-          rp.d[0] = d0; rp.d[1] = d1; rp.d[2] = d2;
-          rp.dnorm = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(d0, d0), __fmul_rn(d1, d1)), __fmul_rn(d2, d2)));
-          if (has_bg) { rp.bg[0] = p.bg[3 * g]; rp.bg[1] = p.bg[3 * g + 1]; rp.bg[2] = p.bg[3 * g + 2]; }
-          rp.dz = p.dir_z ? p.dir_z[g] : d2;
-          if constexpr (SAVE) {
-            p.save_dnorm[g] = rp.dnorm;
-            if (p.save_ray) {  // the ray as the input gradients need it: o, d, direction-encoder input
-              float* sr = p.save_ray + 7 * (size_t)g;
-              sr[0] = o0; sr[1] = o1; sr[2] = o2; sr[3] = d0; sr[4] = d1; sr[5] = d2; sr[6] = rp.dz;
+        }
+        // positional encoding of o + d*z: 63 lanes + 1 zero pad, FP16 (hi[,lo]) into the swizzled PE buffer.
+        // The two threads of a row write lanes [0,32) and [32,64) respectively.
+        const float px = __fadd_rn(rp.o[0], __fmul_rn(rp.d[0], z));
+        const float py = __fadd_rn(rp.o[1], __fmul_rn(rp.d[1], z));
+        const float pz = __fadd_rn(rp.o[2], __fmul_rn(rp.d[2], z));
+        float f[32];
+        if (half == 0) {  // lanes 0..31: xyz, frequencies 0..3, sin of frequency 4, cos(x), cos(y) of frequency 4
+          f[0] = px; f[1] = py; f[2] = pz;
+#pragma unroll
+          for (int fr = 0; fr < 4; ++fr) {
+            const float sc = (float)(1 << fr);
+            pe_sincos<EXACT>(px * sc, f[3 + 6 * fr + 0], f[3 + 6 * fr + 3]);
+            pe_sincos<EXACT>(py * sc, f[3 + 6 * fr + 1], f[3 + 6 * fr + 4]);
+            pe_sincos<EXACT>(pz * sc, f[3 + 6 * fr + 2], f[3 + 6 * fr + 5]);
+          }
+          float cz;
+          pe_sincos<EXACT>(px * 16.f, f[27], f[30]);
+          pe_sincos<EXACT>(py * 16.f, f[28], f[31]);
+          pe_sincos<EXACT>(pz * 16.f, f[29], cz);
+        } else {          // lanes 32..63: cos(z) of frequency 4, frequencies 5..9, zero pad
+          float sz;
+          pe_sincos<EXACT>(pz * 16.f, sz, f[0]);
+#pragma unroll
+          for (int fr = 5; fr < 10; ++fr) {
+            const float sc = (float)(1 << fr);
+            const int b = 6 * fr - 29;  // lane 3 + 6*fr, minus 32
+            pe_sincos<EXACT>(px * sc, f[b + 0], f[b + 3]);
+            pe_sincos<EXACT>(py * sc, f[b + 1], f[b + 4]);
+            pe_sincos<EXACT>(pz * sc, f[b + 2], f[b + 5]);
+          }
+          f[31] = 0.f;
+        }
+#pragma unroll
+        for (int qq = 0; qq < 4; ++qq) {
+          uint32_t hi[4], lo[4];
+#pragma unroll
+          for (int e = 0; e < 4; ++e) {
+            const float a = f[qq * 8 + 2 * e], b = f[qq * 8 + 2 * e + 1];
+            hi[e] = pack_f16x2(a, b);
+            if constexpr (EXACT) {
+              const float2 hf = unpack_f16x2(hi[e]);
+              lo[e] = pack_f16x2(a - hf.x, b - hf.y);
             }
           }
-        } else {
-          for (int k = 0; k < 3; ++k) { rp.o[k] = 0.f; rp.d[k] = 0.f; rp.bg[k] = 0.f; }
-          rp.dnorm = 0.f;
-          rp.dz = 0.f;
+          const int off = row * 128 + (((half * 4 + qq) ^ (row & 7)) << 4);
+          *reinterpret_cast<uint4*>(pe_hi + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
+          if constexpr (EXACT) *reinterpret_cast<uint4*>(pe_lo + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
         }
-      }
-      named_bar_sync(kRowBarrier, kRowThreads);
-      // direction encoder input is (d_z, near, far): run_network reads ray_batch[..., -3:] (train_utils.py:14);
-      // one accurate sincos per thread
-      if (etid < R * 12) {
-        const int rr = etid / 12, k = etid - rr * 12, f = k / 3, c = k - f * 3;
-        RayP& rp = rayp[rr];
-        const float v = (c == 0) ? rp.dz : (c == 1 ? p.near_ : p.far_);
-        float sn, cs;
-        sincosf(v * (float)(1 << f), &sn, &cs);
-        rp.ped[6 * f + c] = rp.valid ? sn : 0.f;
-        rp.ped[6 * f + 3 + c] = rp.valid ? cs : 0.f;
-      }
-      named_bar_sync(kRowBarrier, kRowThreads);
-      // per-ray additive term of layers_dir.0 for both passes: W[:, 256:280] . PE_dir (one output feature x ray per thread
-      // and pass), read by every tile's step-6 epilogue of either warpgroup
+        if (PROBE && p.dbg_act && p.dbg_act_step == -1 && unit == 0 && pass == 0 && t == 0) {
+#pragma unroll
+          for (int k = 0; k < 32; ++k) p.dbg_act[row * 256 + half * 32 + k] = f[k];
+        }
+        if constexpr (SAVE) {  // FP16 encoding of this tile as a transposed image (input of layers_xyz.0 / .3 in dW)
+          if (unit < geom.n_units) {
+            uint8_t* rec = p.save_rec + geom.global_tile(unit, pass, t) * kRecBytes;
+            uint32_t hh[16];
+#pragma unroll
+            for (int e = 0; e < 16; ++e) hh[e] = pack_f16x2(f[2 * e], f[2 * e + 1]);
+            store_t32(rec + kRecPE + img_row_base(64, row), row, 32 * half, hh);
+          }
+        }
+        fence_proxy_async_smem();  // make the generic-proxy PE stores visible to the tensor core
+      };
+
+
       {
-        const int col = etid & 127, rr = etid >> 7;
-        const RayP& rq = rayp[rr < R ? rr : 0];
-#pragma unroll 1
-        for (int pass = 0; pass < 2; ++pass) {
-          const float* wt = p.wd0b_t[pass];
-          float acc0 = 0.f;
-#pragma unroll 8
-          for (int j = 0; j < kDimDir; ++j) acc0 = fmaf(wt[j * 128 + col], rq.ped[j], acc0);
-          dirbias[(2 * pass + rr) * 128 + col] = acc0;
+        prologue(t);
+        uint8_t* rec = nullptr;  // this tile's training record (SAVE mode)
+        if constexpr (SAVE) {
+          if (unit < geom.n_units) {
+            const TileGeom::Row rw = geom.row(pass, t, row);
+            const bool live = rw.used;
+            const RayP& rp = rayp[rw.ray];
+            rec = p.save_rec + geom.global_tile(unit, pass, t) * kRecBytes;
+            uint32_t hh[8];  // direction encoding of this row's ray: features [16*half, 16*half+16)
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              const int k = 16 * half + 2 * e;
+              const float a = (live && rp.valid && k < kDimDir) ? rp.ped[k] : 0.f;
+              const float b = (live && rp.valid && k + 1 < kDimDir) ? rp.ped[k + 1] : 0.f;
+              hh[e] = pack_f16x2(a, b);
+            }
+            uint8_t* img = rec + kRecPEd + img_row_base(32, row);
+            const uint32_t cr = (uint32_t)((row & 63) >> 3);
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+              const int ka = 16 * half + 2 * e, kb = ka + 1;
+              *reinterpret_cast<uint16_t*>(img + ka * 128 + ((cr ^ (uint32_t)(ka & 7)) << 4)) = (uint16_t)(hh[e] & 0xFFFFu);
+              *reinterpret_cast<uint16_t*>(img + kb * 128 + ((cr ^ (uint32_t)(kb & 7)) << 4)) = (uint16_t)(hh[e] >> 16);
+            }
+          }
         }
-      }
-      named_bar_sync(kRowBarrier, kRowThreads);
-      tm.lap(0);
+        // this warpgroup's PE rows complete.  Nothing else inside the tile is shared between the warpgroups: each reads
+        // and writes only its own 64 rows of the PE buffer, the activation buffers, tile_raw and the carry buffers.
+        named_bar_sync(2 + wg, 128);
+        tm.lap(2);
 
-
-      for (int pass = 0; pass < 2; ++pass) {
-        if (pass == 1 && geom.nf == 0) break;
-        const int S = geom.samples(pass);
-        const int rows = R * S;
-        const int n_tiles = geom.tile_count(pass);
-        const float* bias_n = p.bias[pass];
-
-        // ---- prologue of tile t: sample depth + positional encoding -> PE buffer.
-        auto prologue = [&](int t) {
+        // ---- the MLP: this warpgroup's 64 rows
+        {
+          const bool probe = PROBE && p.dbg_act && unit == 0 && pass == 0 && t == 0;
+          float acc0[64], acc1[64], acc_s[8];
+          uint32_t act[64];  // fast mode: this thread's part of the hidden activations, as the next step's A fragments
+          const TileGeom::Row rw0 = geom.row(pass, t, r0), rw1 = geom.row(pass, t, r0 + 8);
+          const int ray0 = rw0.ray, ray1 = rw1.ray;
+          uint32_t live = 0u;  // SAVE: which of this thread's two rows hold a sample (see epi_half)
+          if constexpr (SAVE) live = ((rw0.used && rayp[ray0].valid) ? 1u : 0u) | ((rw1.used && rayp[ray1].valid) ? 2u : 0u);
+          auto mlp_step = [&](auto step) {
+            const int s = step;
+            const StepInfo si = step_info(s);
+            // Fast mode staggers the warpgroups (ping-pong): warpgroup 1 issues step s after warpgroup 0 has issued it, and
+            // warpgroup 0 issues step s + 1 after warpgroup 1 has issued step s, so one's epilogue runs under the other's
+            // MMAs.  Barrier 4 + w is the one warpgroup w waits on.  The pairs close over the CTA's tile stream: warpgroup 0
+            // does not wait before its first step, warpgroup 1 does not arrive after its last.  Exact mode's one-slot ring
+            // already keeps the warpgroups within one unit of each other, and a forced order there would deadlock it.
+            const bool pp_wait = !EXACT && (wg == 1 || s > 0 || k > 0);
+            const bool pp_arrive = !EXACT && (wg == 0 || s < kNumSteps - 1 || k < n_stream - 1);
+            if (pp_wait) named_bar_sync(4 + wg, 256);
+            tm.lap(15);
+            auto issued = [&] { if (pp_arrive) named_bar_arrive(5 - wg, 256); };
+            mlp_step_mma<EXACT>(step, ring, smem_base + M::kActHi, smem_base + M::kActLo, smem_base + M::kPeHi,
+                                smem_base + M::kPeLo, (uint32_t)(64 * wg * 128), act, acc0, acc1, acc_s, tm, issued);
+            float* dump = (probe && p.dbg_act_step == s) ? p.dbg_act : nullptr;
+            const float* bias = bias_n + si.bias_off;
+            if (s <= 8) {
+              const float* db0 = (s == 6) ? dirb + ray0 * 128 : nullptr;
+              const float* db1 = (s == 6) ? dirb + ray1 * 128 : nullptr;
+              epi_half<EXACT, SAVE, PROBE>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, act, r0, rec, live, dump);
+              if (si.nh1 == 128)
+                epi_half<EXACT, SAVE, PROBE>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump);
+              if (s == 6 && (lane & 3) == 0) {  // sigma = first column of the 16-column half
+                const float b = bias[128];
+                tile_raw[r0].w = acc_s[0] + b;
+                tile_raw[r0 + 8].w = acc_s[2] + b;
+              }
+              if constexpr (EXACT) {
+                fence_proxy_async_smem();  // generic-proxy activation stores -> the next step's wgmma
+                named_bar_sync(2 + wg, 128);
+              }
+            } else {  // fc_rgb: raw colour of columns 0..2
+              const int c = lane & 3;
+              if (c == 0) {
+                tile_raw[r0].x = acc_s[0] + bias[0]; tile_raw[r0].y = acc_s[1] + bias[1];
+                tile_raw[r0 + 8].x = acc_s[2] + bias[0]; tile_raw[r0 + 8].y = acc_s[3] + bias[1];
+              } else if (c == 1) {
+                tile_raw[r0].z = acc_s[0] + bias[2];
+                tile_raw[r0 + 8].z = acc_s[2] + bias[2];
+              }
+            }
+            tm.lap(12);
+          };
+          if constexpr (EXACT) {
+#pragma unroll 1
+            for (int s = 0; s < kNumSteps; ++s) mlp_step(s);
+          } else {
+            static_for<0, kNumSteps>(mlp_step);
+          }
+        }
+        named_bar_sync(2 + wg, 128);  // this warpgroup's rows of tile_raw complete
+        tm.lap(14);
+        // fc_rgb output.  Prepare what compositing needs per sample: colour and sigma (volume_rendering_utils.py:29-33,
+        // 41-53); the exp(-sigma*delta) needs the neighbour depth and stays in composite_ray.  One thread per row of the
+        // warpgroup's 64.
+        if (half == 0) {
           const TileGeom::Row rw = geom.row(pass, t, row);
           const int prow = rw.pass_row, i = rw.sample;
-          const bool live = rw.used;
           const RayP& rp = rayp[rw.ray];
-          float z = 0.f;
-          if (live) {
-            if (pass == 0) {
-              const float tc = p.t_coarse[i];
-              z = __fadd_rn(__fmul_rn(p.near_, __fsub_rn(1.f, tc)), __fmul_rn(p.far_, tc));
-              if (p.perturb) {  // stratified jitter (train_utils.py:69-76)
-                float lower = z, upper = z;
-                if (i > 0) {
-                  const float tp = p.t_coarse[i - 1];
-                  const float zp = __fadd_rn(__fmul_rn(p.near_, __fsub_rn(1.f, tp)), __fmul_rn(p.far_, tp));
-                  lower = __fmul_rn(0.5f, __fadd_rn(z, zp));
-                }
-                if (i < S - 1) {
-                  const float tn = p.t_coarse[i + 1];
-                  const float zn = __fadd_rn(__fmul_rn(p.near_, __fsub_rn(1.f, tn)), __fmul_rn(p.far_, tn));
-                  upper = __fmul_rn(0.5f, __fadd_rn(zn, z));
-                }
-                const float tr = rp.valid ? p.t_rand[(size_t)rp.gidx * geom.nc + i] : 0.f;
-                z = __fadd_rn(lower, __fmul_rn(__fsub_rn(upper, lower), tr));
-              }
-              if (half == 0) carry_z[prow] = z;
-            } else {
-              z = carry_z[prow];
+          if (rw.used) {
+            const float4 v = tile_raw[row];
+            const float r0_ = v.x, r1 = v.y, r2 = v.z, sigma_raw = v.w;
+            if (rp.valid) {
+              float* dr = pass ? p.dbg_raw_f : p.dbg_raw_c;
+              if (dr) reinterpret_cast<float4*>(dr)[(size_t)rp.gidx * S + i] = make_float4(r0_, r1, r2, sigma_raw);
             }
-          }
-          // positional encoding of o + d*z: 63 lanes + 1 zero pad, FP16 (hi[,lo]) into the swizzled PE buffer.
-          // The two threads of a row write lanes [0,32) and [32,64) respectively.
-          const float px = __fadd_rn(rp.o[0], __fmul_rn(rp.d[0], z));
-          const float py = __fadd_rn(rp.o[1], __fmul_rn(rp.d[1], z));
-          const float pz = __fadd_rn(rp.o[2], __fmul_rn(rp.d[2], z));
-          float f[32];
-          if (half == 0) {  // lanes 0..31: xyz, frequencies 0..3, sin of frequency 4, cos(x), cos(y) of frequency 4
-            f[0] = px; f[1] = py; f[2] = pz;
-#pragma unroll
-            for (int fr = 0; fr < 4; ++fr) {
-              const float sc = (float)(1 << fr);
-              pe_sincos<EXACT>(px * sc, f[3 + 6 * fr + 0], f[3 + 6 * fr + 3]);
-              pe_sincos<EXACT>(py * sc, f[3 + 6 * fr + 1], f[3 + 6 * fr + 4]);
-              pe_sincos<EXACT>(pz * sc, f[3 + 6 * fr + 2], f[3 + 6 * fr + 5]);
+            float sig = sigma_raw;
+            if (p.noise_std > 0.f && rp.valid)
+              sig = __fadd_rn(sig, __fmul_rn((pass ? p.noise_f : p.noise_c)[(size_t)rp.gidx * S + i], p.noise_std));
+            const float sig_in = sig;  // what the ReLU sees (volume_rendering_utils.py:52)
+            sig = relu_nan(sig);
+            float4 pre;
+            if (i == S - 1) {
+              sig = __fadd_rn(sig, 1e-6f);
+              if (has_bg) { pre.x = rp.bg[0]; pre.y = rp.bg[1]; pre.z = rp.bg[2]; }
             }
-            float cz;
-            pe_sincos<EXACT>(px * 16.f, f[27], f[30]);
-            pe_sincos<EXACT>(py * 16.f, f[28], f[31]);
-            pe_sincos<EXACT>(pz * 16.f, f[29], cz);
-          } else {          // lanes 32..63: cos(z) of frequency 4, frequencies 5..9, zero pad
-            float sz;
-            pe_sincos<EXACT>(pz * 16.f, sz, f[0]);
-#pragma unroll
-            for (int fr = 5; fr < 10; ++fr) {
-              const float sc = (float)(1 << fr);
-              const int b = 6 * fr - 29;  // lane 3 + 6*fr, minus 32
-              pe_sincos<EXACT>(px * sc, f[b + 0], f[b + 3]);
-              pe_sincos<EXACT>(py * sc, f[b + 1], f[b + 4]);
-              pe_sincos<EXACT>(pz * sc, f[b + 2], f[b + 5]);
+            if (!(has_bg && i == S - 1)) {
+              pre.x = 1.f / (1.f + expf(-r0_));
+              pre.y = 1.f / (1.f + expf(-r1));
+              pre.z = 1.f / (1.f + expf(-r2));
             }
-            f[31] = 0.f;
-          }
-#pragma unroll
-          for (int qq = 0; qq < 4; ++qq) {
-            uint32_t hi[4], lo[4];
-#pragma unroll
-            for (int e = 0; e < 4; ++e) {
-              const float a = f[qq * 8 + 2 * e], b = f[qq * 8 + 2 * e + 1];
-              hi[e] = pack_f16x2(a, b);
-              if constexpr (EXACT) {
-                const float2 hf = unpack_f16x2(hi[e]);
-                lo[e] = pack_f16x2(a - hf.x, b - hf.y);
-              }
-            }
-            const int off = row * 128 + (((half * 4 + qq) ^ (row & 7)) << 4);
-            *reinterpret_cast<uint4*>(pe_hi + off) = make_uint4(hi[0], hi[1], hi[2], hi[3]);
-            if constexpr (EXACT) *reinterpret_cast<uint4*>(pe_lo + off) = make_uint4(lo[0], lo[1], lo[2], lo[3]);
-          }
-          if (PROBE && p.dbg_act && p.dbg_act_step == -1 && unit == 0 && pass == 0 && t == 0) {
-#pragma unroll
-            for (int k = 0; k < 32; ++k) p.dbg_act[row * 256 + half * 32 + k] = f[k];
-          }
-          if constexpr (SAVE) {  // FP16 encoding of this tile as a transposed image (input of layers_xyz.0 / .3 in dW)
-            if (unit < geom.n_units) {
-              uint8_t* rec = p.save_rec + geom.global_tile(unit, pass, t) * kRecBytes;
-              uint32_t hh[16];
-#pragma unroll
-              for (int e = 0; e < 16; ++e) hh[e] = pack_f16x2(f[2 * e], f[2 * e + 1]);
-              store_t32(rec + kRecPE + img_row_base(64, row), row, 32 * half, hh);
-            }
-          }
-          fence_proxy_async_smem();  // make the generic-proxy PE stores visible to the tensor core
-        };
-
-
-        for (int t = 0; t < n_tiles; ++t) {
-          prologue(t);
-          uint8_t* rec = nullptr;  // this tile's training record (SAVE mode)
-          if constexpr (SAVE) {
-            if (unit < geom.n_units) {
-              const TileGeom::Row rw = geom.row(pass, t, row);
-              const bool live = rw.used;
-              const RayP& rp = rayp[rw.ray];
-              rec = p.save_rec + geom.global_tile(unit, pass, t) * kRecBytes;
-              uint32_t hh[8];  // direction encoding of this row's ray: features [16*half, 16*half+16)
-#pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                const int k = 16 * half + 2 * e;
-                const float a = (live && rp.valid && k < kDimDir) ? rp.ped[k] : 0.f;
-                const float b = (live && rp.valid && k + 1 < kDimDir) ? rp.ped[k + 1] : 0.f;
-                hh[e] = pack_f16x2(a, b);
-              }
-              uint8_t* img = rec + kRecPEd + img_row_base(32, row);
-              const uint32_t cr = (uint32_t)((row & 63) >> 3);
-#pragma unroll
-              for (int e = 0; e < 8; ++e) {
-                const int ka = 16 * half + 2 * e, kb = ka + 1;
-                *reinterpret_cast<uint16_t*>(img + ka * 128 + ((cr ^ (uint32_t)(ka & 7)) << 4)) = (uint16_t)(hh[e] & 0xFFFFu);
-                *reinterpret_cast<uint16_t*>(img + kb * 128 + ((cr ^ (uint32_t)(kb & 7)) << 4)) = (uint16_t)(hh[e] >> 16);
-              }
-            }
-          }
-          // this warpgroup's PE rows complete.  Nothing else inside the tile is shared between the warpgroups: each reads
-          // and writes only its own 64 rows of the PE buffer, the activation buffers, tile_raw and the carry buffers.
-          named_bar_sync(2 + wg, 128);
-          tm.lap(2);
-
-          // ---- the MLP: this warpgroup's 64 rows
-          {
-            const bool probe = PROBE && p.dbg_act && unit == 0 && pass == 0 && t == 0;
-            float acc0[64], acc1[64], acc_s[8];
-            uint32_t act[64];  // fast mode: this thread's part of the hidden activations, as the next step's A fragments
-            const TileGeom::Row rw0 = geom.row(pass, t, r0), rw1 = geom.row(pass, t, r0 + 8);
-            const int ray0 = rw0.ray, ray1 = rw1.ray;
-            uint32_t live = 0u;  // SAVE: which of this thread's two rows hold a sample (see epi_half)
-            if constexpr (SAVE) live = ((rw0.used && rayp[ray0].valid) ? 1u : 0u) | ((rw1.used && rayp[ray1].valid) ? 2u : 0u);
-            auto mlp_step = [&](auto step) {
-              const int s = step;
-              const StepInfo si = step_info(s);
-              // Fast mode staggers the warpgroups (ping-pong): warpgroup 1 issues step s after warpgroup 0 has issued it, and
-              // warpgroup 0 issues step s + 1 after warpgroup 1 has issued step s, so one's epilogue runs under the other's
-              // MMAs.  Barrier 4 + w is the one warpgroup w waits on.  The pairs close within a pass: warpgroup 0 does not
-              // wait before the pass's first step, warpgroup 1 does not arrive after its last.  Exact mode's one-slot ring
-              // already keeps the warpgroups within one unit of each other, and a forced order there would deadlock it.
-              const bool pp_wait = !EXACT && (wg == 1 || s > 0 || t > 0);
-              const bool pp_arrive = !EXACT && (wg == 0 || s < kNumSteps - 1 || t < n_tiles - 1);
-              if (pp_wait) named_bar_sync(4 + wg, 256);
-              tm.lap(15);
-              auto issued = [&] { if (pp_arrive) named_bar_arrive(5 - wg, 256); };
-              mlp_step_mma<EXACT>(step, ring, smem_base + M::kActHi, smem_base + M::kActLo, smem_base + M::kPeHi,
-                                  smem_base + M::kPeLo, (uint32_t)(64 * wg * 128), act, acc0, acc1, acc_s, tm, issued);
-              float* dump = (probe && p.dbg_act_step == s) ? p.dbg_act : nullptr;
-              const float* bias = bias_n + si.bias_off;
-              if (s <= 8) {
-                const float* db0 = (s == 6) ? dirbias + (2 * pass + ray0) * 128 : nullptr;
-                const float* db1 = (s == 6) ? dirbias + (2 * pass + ray1) * 128 : nullptr;
-                epi_half<EXACT, SAVE, PROBE>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, act, r0, rec, live, dump);
-                if (si.nh1 == 128)
-                  epi_half<EXACT, SAVE, PROBE>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump);
-                if (s == 6 && (lane & 3) == 0) {  // sigma = first column of the 16-column half
-                  const float b = bias[128];
-                  tile_raw[r0].w = acc_s[0] + b;
-                  tile_raw[r0 + 8].w = acc_s[2] + b;
-                }
-                if constexpr (EXACT) {
-                  fence_proxy_async_smem();  // generic-proxy activation stores -> the next step's wgmma
-                  named_bar_sync(2 + wg, 128);
-                }
-              } else {  // fc_rgb: raw colour of columns 0..2
-                const int c = lane & 3;
-                if (c == 0) {
-                  tile_raw[r0].x = acc_s[0] + bias[0]; tile_raw[r0].y = acc_s[1] + bias[1];
-                  tile_raw[r0 + 8].x = acc_s[2] + bias[0]; tile_raw[r0 + 8].y = acc_s[3] + bias[1];
-                } else if (c == 1) {
-                  tile_raw[r0].z = acc_s[0] + bias[2];
-                  tile_raw[r0 + 8].z = acc_s[2] + bias[2];
-                }
-              }
-              tm.lap(12);
-            };
-            if constexpr (EXACT) {
-#pragma unroll 1
-              for (int s = 0; s < kNumSteps; ++s) mlp_step(s);
-            } else {
-              static_for<0, kNumSteps>(mlp_step);
-            }
-          }
-          named_bar_sync(2 + wg, 128);  // this warpgroup's rows of tile_raw complete
-          tm.lap(14);
-          // fc_rgb output.  Prepare what compositing needs per sample: colour and sigma (volume_rendering_utils.py:29-33,
-          // 41-53); the exp(-sigma*delta) needs the neighbour depth and stays in composite_ray.  One thread per row of the
-          // warpgroup's 64.
-          if (half == 0) {
-            const TileGeom::Row rw = geom.row(pass, t, row);
-            const int prow = rw.pass_row, i = rw.sample;
-            const RayP& rp = rayp[rw.ray];
-            if (rw.used) {
-              const float4 v = tile_raw[row];
-              const float r0_ = v.x, r1 = v.y, r2 = v.z, sigma_raw = v.w;
-              if (rp.valid) {
-                float* dr = pass ? p.dbg_raw_f : p.dbg_raw_c;
-                if (dr) reinterpret_cast<float4*>(dr)[(size_t)rp.gidx * S + i] = make_float4(r0_, r1, r2, sigma_raw);
-              }
-              float sig = sigma_raw;
-              if (p.noise_std > 0.f && rp.valid)
-                sig = __fadd_rn(sig, __fmul_rn((pass ? p.noise_f : p.noise_c)[(size_t)rp.gidx * S + i], p.noise_std));
-              const float sig_in = sig;  // what the ReLU sees (volume_rendering_utils.py:52)
-              sig = relu_nan(sig);
-              float4 pre;
-              if (i == S - 1) {
-                sig = __fadd_rn(sig, 1e-6f);
-                if (has_bg) { pre.x = rp.bg[0]; pre.y = rp.bg[1]; pre.z = rp.bg[2]; }
-              }
-              if (!(has_bg && i == S - 1)) {
-                pre.x = 1.f / (1.f + expf(-r0_));
-                pre.y = 1.f / (1.f + expf(-r1));
-                pre.z = 1.f / (1.f + expf(-r2));
-              }
-              pre.w = sig;
-              carry_raw[prow] = pre;
-              if constexpr (SAVE) {  // what the compositing backward needs: colour (or bg) and the ReLU input
-                if (rp.valid) reinterpret_cast<float4*>(pass ? p.save_raw_f : p.save_raw_c)[(size_t)rp.gidx * S + i] = make_float4(pre.x, pre.y, pre.z, sig_in);
-              }
-            }
-          }
-          tm.lap(13);
-        }  // tiles
-        named_bar_sync(kRowBarrier, kRowThreads);  // carry_raw and carry_z of the pass complete
-        tm.lap(3);
-
-        // ---- debug dump of the sample depths
-        {
-          float* dz = pass ? p.dbg_z_f : p.dbg_z_c;
-          if (dz) {
-            for (int k = etid; k < rows; k += kRowThreads) {
-              const int rr = k / S;
-              if (rayp[rr].valid) dz[(size_t)rayp[rr].gidx * S + (k - rr * S)] = carry_z[k];
+            pre.w = sig;
+            carry_raw[prow] = pre;
+            if constexpr (SAVE) {  // what the compositing backward needs: colour (or bg) and the ReLU input
+              if (rp.valid) reinterpret_cast<float4*>(pass ? p.save_raw_f : p.save_raw_c)[(size_t)rp.gidx * S + i] = make_float4(pre.x, pre.y, pre.z, sig_in);
             }
           }
         }
-
-        // ---- compositing: warp `ew` renders ray `ew`
-        if (ew < R && rayp[ew].valid) {
-          const RayP& rp = rayp[ew];
-          const int g = rp.gidx;
-          float* o_rgb = pass ? p.rgb_f : p.rgb_c;
-          float* o_disp = pass ? p.disp_f : p.disp_c;
-          float* o_acc = pass ? p.acc_f : p.acc_c;
-          const float wl = composite_ray(carry_raw + ew * S, carry_z + ew * S, scr_w + ew * S, S, rp.dnorm, p.white_bkgd != 0,
-                                         o_rgb ? o_rgb + 3 * (size_t)g : nullptr, o_disp ? o_disp + g : nullptr,
-                                         o_acc ? o_acc + g : nullptr, lane);
-          const bool last_pass = (pass == 1) || (geom.nf == 0);
-          if (last_pass && lane == 0 && p.w_last) p.w_last[g] = wl;
-        }
-        if (pass == 1 || geom.nf == 0) {
-          named_bar_sync(kRowBarrier, kRowThreads);  // carry buffers are reused by the next unit
-          tm.lap(4);
-          continue;
-        }
-        tm.lap(4);
-
-        // ---- inverse-CDF resampling (nerf_helpers.py:344-387) on weights[1:-1] over the mid-point bins
-        __syncwarp();
-        const int nb = geom.nc - 1;   // bins / cdf entries
-        const int nw = geom.nc - 2;   // interior weights
-        if (ew < R) {
-          const float* w = scr_w + ew * geom.nc;
-          const float* zc = carry_z + ew * geom.nc;
-          float* cdf = scr_cdf + ew * geom.nc;
-          float* bins = scr_bins + ew * geom.nc;
-          for (int k = lane; k < nb; k += 32) bins[k] = __fmul_rn(0.5f, __fadd_rn(zc[k + 1], zc[k]));
-          const int per = (nw + 31) >> 5;
-          const int k0 = lane * per;
-          float part = 0.f;
-          for (int j = 0; j < per; ++j)
-            if (k0 + j < nw) part += __fadd_rn(w[k0 + j + 1], 1e-5f);
-          const float total = warp_sum(part);
-          float psum = 0.f;
-          for (int j = 0; j < per; ++j)
-            if (k0 + j < nw) psum += __fdiv_rn(__fadd_rn(w[k0 + j + 1], 1e-5f), total);
-          float incl = psum;
-#pragma unroll
-          for (int o = 1; o < 32; o <<= 1) {
-            const float tt = __shfl_up_sync(0xffffffffu, incl, o);
-            if (lane >= o) incl += tt;
-          }
-          float run = incl - psum;  // exclusive prefix of this lane's block
-          if (lane == 0) cdf[0] = 0.f;
-          for (int j = 0; j < per; ++j)
-            if (k0 + j < nw) {
-              run += __fdiv_rn(__fadd_rn(w[k0 + j + 1], 1e-5f), total);
-              cdf[k0 + j + 1] = run;
-            }
-        }
-        named_bar_sync(kRowBarrier, kRowThreads);
-        tm.lap(5);
-        // cat(z_coarse, z_samples) per ray into scr_sort (stride s_fine)
-        const int SF = geom.samples(1);
-        for (int k = etid; k < R * SF; k += kRowThreads) {
-          const int rr = k / SF, i = k - rr * SF;
-          float val;
-          if (i < geom.nc) {
-            val = carry_z[rr * geom.nc + i];
-          } else {
-            const int j = i - geom.nc;
-            const float* cdf = scr_cdf + rr * geom.nc;
-            const float* bins = scr_bins + rr * geom.nc;
-            const float u = p.perturb ? (rayp[rr].valid ? p.u_rand[(size_t)rayp[rr].gidx * geom.nf + j] : 0.f) : p.u_fine[j];
-            int lo = 0, hi = nb;  // searchsorted(..., right=True): number of cdf entries <= u
-            while (lo < hi) {
-              const int mid = (lo + hi) >> 1;
-              if (cdf[mid] <= u) lo = mid + 1; else hi = mid;
-            }
-            const int below = max(0, lo - 1), above = min(nb - 1, lo);
-            const float cb = cdf[below], ca = cdf[above];
-            float den = __fsub_rn(ca, cb);
-            if (den < 1e-5f) den = 1.f;
-            const float tt = __fdiv_rn(__fsub_rn(u, cb), den);
-            val = __fadd_rn(bins[below], __fmul_rn(tt, __fsub_rn(bins[above], bins[below])));
-          }
-          scr_sort[k] = val;
-        }
-        named_bar_sync(kRowBarrier, kRowThreads);
-        tm.lap(6);
-        // ---- torch.sort(cat(z, z_samples)) (train_utils.py:126) as a rank merge: the coarse depths are sorted, the
-        //      samples need not be (stochastic u), so an element's rank = (# coarse before it, by binary search)
-        //      + (# samples before it, counted).  Ties: coarse first, then samples by index — equal values make any
-        //      tie order give the same sorted array.  A NaN sample (from non-finite weights) goes after every number, by
-        //      index, as torch.sort places it; no comparison with a NaN counts, so the other ranks stay as they are.
-        for (int k = etid; k < R * SF; k += kRowThreads) {
-          const int rr = k / SF, i = k - rr * SF;
-          const float* zc = scr_sort + rr * SF;
-          const float* zs = zc + geom.nc;
-          const float v = zc[i];
-          int rank;
-          if (i < geom.nc) {
-            rank = i;
-            for (int j = 0; j < geom.nf; ++j) rank += (zs[j] < v) ? 1 : 0;
-          } else if (v != v) {
-            const int jm = i - geom.nc;
-            rank = geom.nc;
-            for (int j = 0; j < geom.nf; ++j) rank += (zs[j] == zs[j] || j < jm) ? 1 : 0;
-          } else {
-            const int jm = i - geom.nc;
-            int lo = 0, hi = geom.nc;  // # coarse depths <= v
-            while (lo < hi) {
-              const int mid = (lo + hi) >> 1;
-              if (zc[mid] <= v) lo = mid + 1; else hi = mid;
-            }
-            rank = lo;
-            for (int j = 0; j < geom.nf; ++j) {
-              const float y = zs[j];
-              rank += (y < v || (y == v && j < jm)) ? 1 : 0;
-            }
-          }
-          carry_z[rr * SF + rank] = v;
-        }
-        named_bar_sync(kRowBarrier, kRowThreads);
-        tm.lap(7);
-      }  // pass
-    }    // units
+        tm.lap(13);
+        if (t == n_tiles - 1) mbar_arrive(pass ? hand.fdone() : hand.cdone(cb));  // the pass's carry complete
+      }
+    }  // tile stream
   }
 }
 

@@ -113,6 +113,7 @@ __device__ __forceinline__ float composite_ray(const float4* __restrict__ pre, c
 #define NFB_TIMERS 0
 #endif
 constexpr int kProfWgStride = 20;  // render kernel: row warpgroup w's observer writes its laps at slot + 20 w (slots < 40)
+constexpr int kProfRay = 40;       // ... and the ray warps' observer at slot + 40 (slots 40..59)
 #if NFB_TIMERS
 struct PhaseTimer {
   unsigned long long* dst;

@@ -2,8 +2,9 @@
 
 Needs a library with the timers compiled in: `python 4d-facial-avatars_b200/build.py --timers` (lib/libnfb_timers.so, picked
 up here unless NFB_LIB is set).  The observers are the first thread of each row warpgroup of every CTA (warpgroup w's laps at
-slot + 20 w); their cycles are summed over CTAs and reported per tile (MLP phases) and per unit of work (per-ray phases), one
-column per warpgroup.  "wait MMAs" includes issuing them and releasing the weight slots."""
+slot + 20 w) and the first thread of the ray warps (slots 40..59); their cycles are summed over CTAs and reported per tile
+(MLP phases, one column per row warpgroup), per unit of work for the row warps' wait for the ray warps, and per unit for the
+ray warps' per-ray stages.  "wait MMAs" includes issuing them and releasing the weight slots."""
 import os
 import sys
 
@@ -52,9 +53,14 @@ ctas = min(torch.cuda.get_device_properties(dev).multi_processor_count, units)
 tiles = units * tiles_per_unit
 per_tile = {2: "prologue (z + PE)", 15: "ping-pong wait", 10: "wait weights (wait_full)", 11: "wait MMAs", 12: "epilogue",
             14: "end-of-MLP barrier", 13: "post-processing"}
-per_unit = {39: "unit loop", 0: "ray setup", 3: "end-of-pass barrier", 4: "composite", 5: "cdf", 6: "inverse-cdf", 7: "sort"}
+per_unit = {16: "wait for ray warps"}
+# the ray warps' observer (lane 0 of warp 1, slots 40..59): the per-ray stages of a unit, beside the row warps' tiles
+RAY = 40  # nfb_render_common.cuh: kProfRay
+per_unit_ray = {0: "wait coarse tiles", 1: "composite coarse", 2: "cdf", 3: "inverse-cdf", 4: "wait fine tiles",
+                5: "composite fine", 6: "sort", 7: "ray setup + dir terms"}
 WG = 20  # slot stride between the two row warpgroups' observers (nfb_render_common.cuh: kProfWgStride)
 total = [sum(c[i + WG * w] for i in list(per_tile) + list(per_unit)) for w in (0, 1)]
+total_ray = sum(c[RAY + i] for i in per_unit_ray)
 print(f"{prec} {H}x{W} {NC}c+{NF}f: {ms:.2f} ms, {H*W/ms*1e3:.3e} rays/s; {R} rays/unit, {tiles_per_unit} tiles/unit, "
       f"{tiles/ctas:.0f} tiles per CTA; observers {total[0]/ctas/1e6:.2f} / {total[1]/ctas/1e6:.2f} Mcycles per CTA")
 share = lambda v, w: 100 * v / total[w] if total[w] else 0.0  # noqa: E731
@@ -64,3 +70,6 @@ for i, name in per_tile.items():
 print(f"{'phase':28s} {'wg0 cycles/unit':>16s} {'share':>7s} {'wg1 cycles/unit':>16s} {'share':>7s}")
 for i, name in per_unit.items():
     print(f"{name:28s} " + " ".join(f"{c[i + WG * w] / units:16.0f} {share(c[i + WG * w], w):6.1f}%" for w in (0, 1)))
+print(f"{'ray warps':28s} {'cycles/unit':>16s} {'share':>7s}   (observer {total_ray / ctas / 1e6:.2f} Mcycles per CTA)")
+for i, name in per_unit_ray.items():
+    print(f"{name:28s} {c[RAY + i] / units:16.0f} {100 * c[RAY + i] / total_ray if total_ray else 0.0:6.1f}%")
