@@ -28,6 +28,7 @@ int cuda_fail(cudaError_t e, const char* where) {
 }  // namespace
 
 using nfb::DevBuf;
+static_assert(NFB_MAX_FRAMES == nfb::kMaxFrames, "frame bound");
 
 struct NfbHandle {
   int device = 0;
@@ -71,9 +72,20 @@ struct NfbHandle {
     DevBuf<float> lin_c, lin_f;
     int chunk_rays = 0, precision = 0;
     DevBuf<float> scratch_out;   // [11 * chunk_rays] outputs of the re-run forwards (discarded)
+    // multi-frame forward (nfb_render_forward_frames_train): the frame table and conditioning vectors it rendered with (copied,
+    // as bias / cond are), the frame slot of every ray (written by the forward), and the backward's per-ray / per-frame sums
+    bool multi = false;
+    int n_frames = 0;
+    DevBuf<float> ftab[2], fcond;
+    DevBuf<int> frame;
+    DevBuf<float> raysum, fsum;
   } tr;
   size_t train_budget = 0;       // bytes the per-tile records of one launch may take (0: not decided yet)
   DevBuf<float> cond;            // [108] = [expression / 3 ; latent] of the current frame
+  // nfb_set_frames: per network [n_frames + 1][kFrameRows] folded rows (the last NaN), and [n_frames][108] conditioning vectors;
+  // independent of the single frame above
+  DevBuf<float> ftab[2], fcond;
+  int n_frames = 0;
   // scratch of the steps either side of the path
   DevBuf<uint32_t> minmax;       // disparity-image min / max keys
   DevBuf<nfb::smp::Run> smp_runs;
@@ -177,6 +189,7 @@ int nfb_load_weights(NfbHandle* h, int which, const float* const params[26], voi
   NFB_CUDA(nfb::launch_repack(nbs, ps, 1, st, &h->launches));  // forward streams, transposed backward stream, bias / column blocks
   nb.loaded = true;
   h->frame_set = false;  // folded biases are stale
+  h->n_frames = 0;
   return NFB_OK;
 }
 
@@ -191,6 +204,7 @@ int nfb_repack(NfbHandle* h, const float* const params_coarse[26], const float* 
   h->net[0].loaded = true;
   if (params_fine) h->net[1].loaded = true;
   h->frame_set = false;  // folded biases are stale
+  h->n_frames = 0;
   return NFB_OK;
 }
 
@@ -234,6 +248,23 @@ int nfb_set_frame(NfbHandle* h, const float* expression, const float* latent, vo
   return NFB_OK;
 }
 
+int nfb_set_frames(NfbHandle* h, const float* expressions, const float* latents, int n_frames, void* stream) {
+  if (!h || !expressions || !latents || n_frames < 1) return NFB_ERR_INVALID;
+  if (n_frames > NFB_MAX_FRAMES) return NFB_ERR_UNSUPPORTED;
+  if (!h->net[0].loaded) return NFB_ERR_STATE;
+  NFB_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const int nets = h->net[1].loaded ? 2 : 1;
+  for (int n = 0; n < nets; ++n) NFB_CUDA(h->ftab[n].reserve((size_t)(n_frames + 1) * nfb::kFrameRows));
+  NFB_CUDA(h->fcond.reserve((size_t)n_frames * nfb::kDimCond));
+  nfb::NetBuffers* const nbs[2] = {&h->net[0], &h->net[1]};
+  float* const tab[2] = {h->ftab[0].get(), h->ftab[1].get()};
+  h->n_frames = 0;
+  NFB_CUDA(nfb::launch_frames_fold(nbs, nets, n_frames, expressions, latents, tab, h->fcond.get(), st, &h->launches));
+  h->n_frames = n_frames;
+  return NFB_OK;
+}
+
 static int ensure_linspace(DevBuf<float>& buf, int* cached_n, int n, cudaStream_t st) {
   if (*cached_n == n && buf.get()) return NFB_OK;
   std::vector<float> host(n);
@@ -274,6 +305,10 @@ static int ensure_train_buffers(NfbHandle::Train& tr, const nfb::TileGeom& g, in
   NFB_CUDA(tr.raw_c.reserve(n * g.samples(0) * 4));
   NFB_CUDA(tr.dnorm.reserve(n));
   NFB_CUDA(tr.ray.reserve(7 * n));
+  if (tr.multi) {
+    NFB_CUDA(tr.frame.reserve(n));
+    NFB_CUDA(tr.raysum.reserve(2 * n * nfb::kFrameRows));
+  }
   if (g.passes() == 2) {
     NFB_CUDA(tr.z_f.reserve(n * g.samples(1)));
     NFB_CUDA(tr.raw_f.reserve(n * g.samples(1) * 4));
@@ -281,9 +316,11 @@ static int ensure_train_buffers(NfbHandle::Train& tr, const nfb::TileGeom& g, in
   return NFB_OK;
 }
 
+// frame_index non-null: a multi-frame call (the frame table of nfb_set_frames instead of the frame of nfb_set_frame).
 static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm, const NfbNoise* noise, const NfbOutputs* out,
-                       const NfbDebug* dbg, void* stream, bool train) {
+                       const NfbDebug* dbg, void* stream, bool train, const int32_t* frame_index = nullptr) {
   if (!h || !rays || !sm || !out) return NFB_ERR_INVALID;
+  const bool multi = frame_index != nullptr;
   if (rays->n_rays < 0) return NFB_ERR_INVALID;
   if ((rays->o == nullptr) != (rays->d == nullptr)) return NFB_ERR_INVALID;
   if (!rays->o && (rays->width <= 0 || rays->height <= 0)) return NFB_ERR_INVALID;
@@ -291,7 +328,8 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
   if (nc < 3 || nf < 0 || nc + nf > 512) return NFB_ERR_UNSUPPORTED;
   if (sm->lindisp) return NFB_ERR_UNSUPPORTED;
   if (sm->precision != NFB_PREC_FAST && sm->precision != NFB_PREC_EXACT) return NFB_ERR_INVALID;
-  if (!h->net[0].loaded || (nf > 0 && !h->net[1].loaded) || !h->frame_set) return NFB_ERR_STATE;
+  if (multi && !rays->o) return NFB_ERR_UNSUPPORTED;  // in-kernel ray generation is one pose per call
+  if (!h->net[0].loaded || (nf > 0 && !h->net[1].loaded) || (multi ? h->n_frames < 1 : !h->frame_set)) return NFB_ERR_STATE;
   if (!out->rgb_coarse || !out->disp_coarse || !out->acc_coarse) return NFB_ERR_INVALID;
   if (nf > 0 && (!out->rgb_fine || !out->disp_fine || !out->acc_fine)) return NFB_ERR_INVALID;
   if (sm->perturb && (!noise || !noise->t_rand || (nf > 0 && !noise->u))) return NFB_ERR_INVALID;
@@ -334,10 +372,13 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
   const bool exact = sm->precision == NFB_PREC_EXACT;
   for (int n = 0; n < 2; ++n) {
     p.wstream[n] = exact ? h->net[n].stream_x3.get() : h->net[n].stream_x1.get();
-    p.bias[n] = h->net[n].bias_frame.get();
+    // a multi-frame call takes the folded rows of steps 0 and 3 from the frame table; its other bias entries are the static ones
+    p.bias[n] = multi ? h->net[n].bias_static.get() : h->net[n].bias_frame.get();
     p.wd0b_t[n] = h->net[n].wd0b_t.get();
+    p.fbias[n] = multi ? h->ftab[n].get() : nullptr;
   }
-  if (nf == 0) { p.wstream[1] = p.wstream[0]; p.bias[1] = p.bias[0]; p.wd0b_t[1] = p.wd0b_t[0]; }
+  if (nf == 0) { p.wstream[1] = p.wstream[0]; p.bias[1] = p.bias[0]; p.wd0b_t[1] = p.wd0b_t[0]; p.fbias[1] = p.fbias[0]; }
+  if (multi) { p.frame = frame_index; p.n_frames = h->n_frames; }
   p.rgb_c = out->rgb_coarse; p.disp_c = out->disp_coarse; p.acc_c = out->acc_coarse;
   p.rgb_f = out->rgb_fine; p.disp_f = out->disp_fine; p.acc_f = out->acc_fine; p.w_last = out->w_last;
   if (dbg) {
@@ -350,12 +391,30 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
     tr.valid = false;
     tr.per_ray_formed = tr.rows_formed = false;
     int rc;
-    tr.chunked = p.geom.tiles() * nfb::kRecBytes > train_budget(h);
+    // a multi-frame backward also keeps per-ray dY0 / dY3 sums: 2 passes x kFrameRows floats = 4 KiB per ray, in the budget too
+    const size_t ray_bytes = multi ? 2 * nfb::kFrameRows * sizeof(float) : 0;
+    tr.chunked = p.geom.tiles() * nfb::kRecBytes + (size_t)p.geom.n_rays * ray_bytes > train_budget(h);
+    tr.multi = multi;
+    if (multi) {
+      // the frame table and conditioning vectors this forward rendered with: a later nfb_set_frames must not change them
+      const int nets = nf > 0 ? 2 : 1, F = h->n_frames;
+      tr.n_frames = F;
+      for (int n = 0; n < nets; ++n) {
+        NFB_CUDA(tr.ftab[n].reserve((size_t)(F + 1) * nfb::kFrameRows));
+        NFB_CUDA(cudaMemcpyAsync(tr.ftab[n].get(), h->ftab[n].get(), (size_t)(F + 1) * nfb::kFrameRows * sizeof(float),
+                                 cudaMemcpyDeviceToDevice, st));
+        p.fbias[n] = tr.ftab[n].get();
+      }
+      if (nf == 0) p.fbias[1] = p.fbias[0];
+      NFB_CUDA(tr.fcond.reserve((size_t)F * nfb::kDimCond));
+      NFB_CUDA(cudaMemcpyAsync(tr.fcond.get(), h->fcond.get(), (size_t)F * nfb::kDimCond * sizeof(float), cudaMemcpyDeviceToDevice, st));
+      NFB_CUDA(tr.fsum.reserve((size_t)F * 2 * nfb::kFrameRows));
+    }
     if (tr.chunked) {
       // e.g. a whole frame rendered with gradients enabled: 1.5-2 MiB of records per ray.  Keep the launch parameters, produce
       // the outputs with the evaluation kernel now, and let the backward re-run the training forward in chunks that fit.
       if (!rays->o) { g_last_cuda_error = "training forward over budget needs explicit rays (o, d)"; return NFB_ERR_UNSUPPORTED; }
-      size_t units = train_budget(h) / nfb::kRecBytes / (size_t)p.geom.tiles_per_unit();
+      size_t units = train_budget(h) / ((size_t)p.geom.tiles_per_unit() * nfb::kRecBytes + (size_t)p.geom.rays_per_unit * ray_bytes);
       if (units < 1) units = 1;
       tr.chunk_rays = (int)(units * p.geom.rays_per_unit);
       tr.full = p;
@@ -363,7 +422,7 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
       // the re-run forwards must read THIS call's frame and depth tables, whatever is rendered before the backward
       for (int n = 0; n < (nf > 0 ? 2 : 1); ++n) {
         NFB_CUDA(tr.bias[n].reserve(nfb::kBiasFloats));
-        NFB_CUDA(cudaMemcpyAsync(tr.bias[n].get(), h->net[n].bias_frame.get(), nfb::kBiasFloats * sizeof(float), cudaMemcpyDeviceToDevice, st));
+        NFB_CUDA(cudaMemcpyAsync(tr.bias[n].get(), p.bias[n], nfb::kBiasFloats * sizeof(float), cudaMemcpyDeviceToDevice, st));
         tr.full.bias[n] = tr.bias[n].get();
       }
       if (nf == 0) tr.full.bias[1] = tr.full.bias[0];
@@ -379,18 +438,33 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
       }
     } else if ((rc = ensure_train_buffers(tr, p.geom, h->num_sms))) return rc;
     // a later nfb_set_frame (e.g. a validation render before the backward) must not change what the backward differentiates
-    NFB_CUDA(cudaMemcpyAsync(tr.cond.get(), h->cond.get(), nfb::kDimCond * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    if (!multi) NFB_CUDA(cudaMemcpyAsync(tr.cond.get(), h->cond.get(), nfb::kDimCond * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    else NFB_CUDA(cudaMemsetAsync(tr.cond.get(), 0, nfb::kDimCond * sizeof(float), st));
     if (!tr.chunked) {
       p.save_rec = tr.rec.get(); p.save_dnorm = tr.dnorm.get(); p.save_raw_c = tr.raw_c.get(); p.save_raw_f = tr.raw_f.get();
       p.dbg_z_c = tr.z_c.get(); p.dbg_z_f = tr.z_f.get();
       p.save_ray = tr.ray.get();  // the rays, for input gradients (the backward does not read the caller's buffers)
+      if (multi) p.save_frame = tr.frame.get();
     }
     tr.has_rays = rays->o != nullptr; tr.has_dir_z = rays->dir_z != nullptr;
     tr.geom = p.geom; tr.has_bg = rays->background != nullptr; tr.white_bkgd = p.white_bkgd;
   }
-  NFB_CUDA(nfb::launch_render(p, exact ? 1 : 0, h->num_sms, st, &h->launches));
+  if (multi) NFB_CUDA(nfb::launch_render_frames(p, exact ? 1 : 0, h->num_sms, st, &h->launches));
+  else NFB_CUDA(nfb::launch_render(p, exact ? 1 : 0, h->num_sms, st, &h->launches));
   if (train) h->tr.valid = true;
   return NFB_OK;
+}
+
+int nfb_render_forward_frames(NfbHandle* h, const NfbRays* rays, const int32_t* frame_index, const NfbSampling* sm, const NfbNoise* noise,
+                              const NfbOutputs* out, void* stream) {
+  if (!frame_index) return NFB_ERR_INVALID;
+  return render_impl(h, rays, sm, noise, out, nullptr, stream, false, frame_index);
+}
+
+int nfb_render_forward_frames_train(NfbHandle* h, const NfbRays* rays, const int32_t* frame_index, const NfbSampling* sm,
+                                    const NfbNoise* noise, const NfbOutputs* out, void* stream) {
+  if (!frame_index) return NFB_ERR_INVALID;
+  return render_impl(h, rays, sm, noise, out, nullptr, stream, true, frame_index);
 }
 
 int nfb_render_forward(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm, const NfbNoise* noise, const NfbOutputs* out,
@@ -410,15 +484,24 @@ int nfb_render_backward(NfbHandle* h, const NfbOutGrads* og, const float* const 
   return nfb_render_backward_ex(h, og, params_coarse, params_fine, grads_coarse, grads_fine, grad_latent, nullptr, stream);
 }
 
-int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* const params_coarse[26],
-                           const float* const params_fine[26], float* const grads_coarse[26], float* const grads_fine[26],
-                           float* grad_latent, const NfbInputGrads* in_grads, void* stream) {
+// The backward of both kinds of training forward.  frames: a multi-frame backward (grad_latent / in_grads->expression unused;
+// the per-frame gradients go to frame_latent / frame_expr, either may be null).
+static int backward_impl(NfbHandle* h, const NfbOutGrads* og, const float* const params_coarse[26], const float* const params_fine[26],
+                         float* const grads_coarse[26], float* const grads_fine[26], float* grad_latent, const NfbInputGrads* in_grads,
+                         bool frames, float* frame_latent, float* frame_expr, void* stream) {
   if (!h || !og || !params_coarse) return NFB_ERR_INVALID;
   NfbHandle::Train& tr = h->tr;
   if (!tr.valid) return NFB_ERR_STATE;
+  if (frames != tr.multi) {
+    // a single-frame backward of a multi-frame forward has no one latent / expression to differentiate: refuse rather than sum
+    if (!frames && (grad_latent || (in_grads && in_grads->expression))) return NFB_ERR_STATE;
+    if (frames) return NFB_ERR_STATE;
+  }
+  if (frames && in_grads && in_grads->expression) return NFB_ERR_INVALID;  // per-frame expression gradients: frame_expr
+  const bool frame_grads = tr.multi && (frame_latent || frame_expr || grads_coarse);
   const bool fine = tr.geom.passes() == 2;
   const bool input_only = !grads_coarse && !grads_fine;
-  if (input_only && !in_grads) return NFB_ERR_INVALID;
+  if (input_only && !in_grads && !(frames && (frame_latent || frame_expr))) return NFB_ERR_INVALID;
   if (!input_only && !grads_coarse) return NFB_ERR_INVALID;
   if (fine && (!params_fine || (!input_only && !grads_fine))) return NFB_ERR_INVALID;
   for (int i = 0; i < 26; ++i) {
@@ -437,6 +520,7 @@ int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* con
   float* const acc[2] = {tr.acc[0].get(), tr.acc[1].get()};
   NFB_CUDA(cudaMemsetAsync(acc[0], 0, nfb::kAccFloats * sizeof(float), st));
   NFB_CUDA(cudaMemsetAsync(acc[1], 0, nfb::kAccFloats * sizeof(float), st));
+  if (frame_grads) NFB_CUDA(cudaMemsetAsync(tr.fsum.get(), 0, (size_t)tr.n_frames * 2 * nfb::kFrameRows * sizeof(float), st));
   tr.per_ray_formed = tr.rows_formed = false;
 
   // compositing backward -> dX chain -> weight-gradient GEMMs -> fixed-order reduction for the g.n_rays rays from `begin` on,
@@ -474,10 +558,17 @@ int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* con
     c.wstream[0] = h->net[0].stream_bwd.get();
     c.wstream[1] = h->net[fine ? 1 : 0].stream_bwd.get();
     NFB_CUDA(nfb::launch_chain(c, h->num_sms, st, &h->launches));
-    const bool dw = !input_only || grad_latent || ig.expression;  // input-only: the PE jobs only serve d latent / d expression
+    // input-only: the PE jobs only serve d latent / d expression (a multi-frame backward forms those from the per-frame sums)
+    const bool dw = !input_only || (!tr.multi && (grad_latent || ig.expression));
     if (dw) {
       d.rec = tr.rec.get(); d.ws = tr.dw_ws.get(); d.scal = scal;
       NFB_CUDA(nfb::launch_dw(d, h->num_sms, st, &h->launches, input_only));  // both networks in one launch
+    }
+    if (frame_grads) {
+      nfb::FrameSumParams fs = {};
+      fs.rec = tr.rec.get(); fs.geom = g; fs.scal = scal; fs.frame = tr.frame.get(); fs.n_frames = tr.n_frames;
+      fs.raysum = tr.raysum.get(); fs.fsum = tr.fsum.get();
+      NFB_CUDA(nfb::launch_frame_sums(fs, st, &h->launches));
     }
     NFB_CUDA(nfb::launch_grad_reduce(dw ? &d : nullptr, input_only, tr.bsum.get(), g.n_rays, g.passes(), acc, h->num_sms, st,
                                      &h->launches));
@@ -527,15 +618,46 @@ int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* con
       p.save_rec = tr.rec.get(); p.save_dnorm = tr.dnorm.get(); p.save_raw_c = tr.raw_c.get(); p.save_raw_f = tr.raw_f.get();
       p.save_ray = tr.ray.get();
       p.dbg_z_c = tr.z_c.get(); p.dbg_z_f = tr.z_f.get();
-      NFB_CUDA(nfb::launch_render(p, tr.precision, h->num_sms, st, &h->launches));
+      if (tr.multi) {
+        p.frame += b;
+        p.save_frame = tr.frame.get();
+        NFB_CUDA(nfb::launch_render_frames(p, tr.precision, h->num_sms, st, &h->launches));
+      } else {
+        NFB_CUDA(nfb::launch_render(p, tr.precision, h->num_sms, st, &h->launches));
+      }
       rc = backward_rays(begin, g);
       if (rc) return rc;
     }
+  }
+  if (tr.multi) {  // no single latent / expression: the conditioning columns and the per-frame gradients come from the per-frame sums
+    // finalize writes db (x) 0 into the conditioning columns (tr.cond is zeroed by a multi-frame forward); frames_grad_kernel,
+    // next on the stream, overwrites them with sum_f db_f (x) c_f
+    if (!input_only)
+      NFB_CUDA(nfb::launch_finalize_all(params_coarse, grads_coarse, acc[0], fine ? params_fine : nullptr, fine ? grads_fine : nullptr,
+                                        acc[1], tr.cond.get(), nullptr, st, &h->launches));
+    if (frame_grads)
+      NFB_CUDA(nfb::launch_frames_grad(params_coarse, input_only ? nullptr : grads_coarse, fine ? params_fine : nullptr,
+                                       (fine && !input_only) ? grads_fine : nullptr, tr.fsum.get(), tr.fcond.get(), tr.n_frames,
+                                       frame_latent, frame_expr, st, &h->launches));
+    return NFB_OK;
   }
   NFB_CUDA(nfb::launch_finalize_all(params_coarse, input_only ? nullptr : grads_coarse, acc[0], fine ? params_fine : nullptr,
                                     (fine && !input_only) ? grads_fine : nullptr, acc[1], tr.cond.get(), grad_latent, st, &h->launches,
                                     ig.expression));
   return NFB_OK;
+}
+
+int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* og, const float* const params_coarse[26],
+                           const float* const params_fine[26], float* const grads_coarse[26], float* const grads_fine[26],
+                           float* grad_latent, const NfbInputGrads* in_grads, void* stream) {
+  return backward_impl(h, og, params_coarse, params_fine, grads_coarse, grads_fine, grad_latent, in_grads, false, nullptr, nullptr, stream);
+}
+
+int nfb_render_backward_frames(NfbHandle* h, const NfbOutGrads* out_grads, const float* const params_coarse[26],
+                               const float* const params_fine[26], float* const grads_coarse[26], float* const grads_fine[26],
+                               float* grad_latents, float* grad_expressions, const NfbInputGrads* in_grads, void* stream) {
+  return backward_impl(h, out_grads, params_coarse, params_fine, grads_coarse, grads_fine, nullptr, in_grads, true, grad_latents,
+                       grad_expressions, stream);
 }
 
 int nfb_train_debug(NfbHandle* h, NfbTrainDebug* out) {

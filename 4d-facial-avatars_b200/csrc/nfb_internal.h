@@ -87,6 +87,12 @@ struct RenderParams {
   float *dbg_z_c, *dbg_raw_c, *dbg_z_f, *dbg_raw_f, *dbg_act;
   int dbg_act_step;
   unsigned long long* prof;  // optional [64] phase-cycle counters (see PhaseTimer in nfb_render.cu)
+  // multi-frame call (render_frames_kernel; unused by render_kernel): per-ray frame index and the folded rows of steps 0 and 3 per
+  // (network, frame) — kFrameRows floats per frame, then the NaN row an out-of-range index selects (nfb_pack.cu: frames_fold_kernel)
+  const int* frame;
+  int n_frames;
+  const float* fbias[2];
+  int* save_frame;  // training forward: [n] the frame slot each ray was rendered with (n_frames when out of range)
 };
 
 // ---- training (nfb_train.cu)
@@ -131,6 +137,16 @@ struct DwParams {  // ONE launch covers both networks: the first parts[0] * grou
   int ws_stride;            // set by launch_dw: kAccBRaw, or the compact PE-only slot (nfb_train.cu dw::kPeSlotFloats)
   const float* scal;
 };
+// Multi-frame backward (nfb_render_backward_frames): per-ray sums of dY0 and dY3 from the tile records, then per-frame sums.
+struct FrameSumParams {
+  const uint8_t* rec;
+  TileGeom geom;
+  const float* scal;
+  const int* frame;  // [n] frame slot per ray, saved by the training forward
+  int n_frames;
+  float* raysum;     // [passes][n][kFrameRows] scratch
+  float* fsum;       // [n_frames][2][kFrameRows]: += this chunk's per-frame sums (zeroed before the first chunk)
+};
 // host copies of the compile-time schedules (nfb_debug_schedule); index < 0: number of entries; else words written or -1
 int debug_jobs_dw(int index, uint32_t* out);
 int debug_dw_split(uint32_t* io);  // io: {num_sms, tiles net 0, tiles net 1} -> {parts0, parts1, groups}
@@ -144,10 +160,17 @@ size_t dw_workspace_floats(int num_sms);  // floats of DwParams::ws that either 
 // and acc[pass][kAccBRaw..+4] += the compositing backward's per-ray sums bsum[pass][0..n_rays) in a fixed order.
 cudaError_t launch_grad_reduce(const DwParams* d, bool pe_only, const float* bsum, int n_rays, int npass, float* const acc[2], int num_sms,
                                cudaStream_t st, long long* launches);
-// grads_c == nullptr: input-gradient-only backward (d latent and d expression alone, one small launch).
+// grads_c == nullptr: input-gradient-only backward (d latent and d expression alone, one small launch).  cond == nullptr: the
+// conditioning columns of dW0 / dW3 are left to launch_frames_grad.
 cudaError_t launch_finalize_all(const float* const params_c[26], float* const grads_c[26], const float* acc_c,
                                 const float* const params_f[26], float* const grads_f[26], const float* acc_f, const float* cond,
                                 float* latent_out, cudaStream_t st, long long* launches, float* expr_out = nullptr);
+cudaError_t launch_frame_sums(const FrameSumParams& p, cudaStream_t st, long long* launches);
+// d latent_f, d expression_f [n_frames][32 / 76] from the per-frame sums, and (grads_* non-null) the conditioning columns of dW0 / dW3
+// as sum_f db_f (x) c_f.  One launch.
+cudaError_t launch_frames_grad(const float* const params_c[26], float* const grads_c[26], const float* const params_f[26],
+                               float* const grads_f[26], const float* fsum, const float* fcond, int n_frames, float* latent_out,
+                               float* expr_out, cudaStream_t st, long long* launches);
 cudaError_t launch_input_grads(const InGradRowParams& r, const InGradRayParams& q, int num_sms, cudaStream_t st, long long* launches);
 
 // Two launches (fold, pack): FP32 parameters of n_nets (1 or 2) networks -> forward / backward weight streams, bias block, conditioning and
@@ -156,6 +179,9 @@ cudaError_t launch_repack(NetBuffers* const nb[2], const float* const* const par
 // One launch: per-frame bias fold of the loaded networks + cond[108] = [expr / 3 ; latent].
 cudaError_t launch_frame_fold(NetBuffers* const nb[2], int n_nets, const float* expr, const float* latent, float* cond,
                               cudaStream_t st, long long* launches);
+// One launch: the fold of n_frames frames into table[net] ([n_frames + 1][kFrameRows], the last row NaN) + cond[n_frames][108].
+cudaError_t launch_frames_fold(NetBuffers* const nb[2], int n_nets, int n_frames, const float* expr, const float* latent,
+                               float* const table[2], float* cond, cudaStream_t st, long long* launches);
 // Training-step tail (nfb_optim.cu): d mse / d rgb (+ loss sums), Adam over a flat bucket with zero_grad fused.
 cudaError_t launch_loss_grad(const float* rgb_c, const float* rgb_f, const float* target, int n_rays, long long n_total, float* g_c,
                              float* g_f, float* loss, cudaStream_t st, long long* launches);
@@ -164,6 +190,8 @@ cudaError_t launch_adam(float* p, float* g, float* m, float* v, long long n, flo
                         float grad_scale, long long reg_off, float reg_w, cudaStream_t st, long long* launches);
 // precision: 0 = fast (x1), 1 = exact (x3).  num_sms = CTAs to launch at most.
 cudaError_t launch_render(const RenderParams& p, int precision, int num_sms, cudaStream_t st, long long* launches);
+// The multi-frame instantiations (render_frames_kernel): p.frame and p.fbias select each ray's rows of steps 0 and 3.
+cudaError_t launch_render_frames(const RenderParams& p, int precision, int num_sms, cudaStream_t st, long long* launches);
 cudaError_t render_kernel_setup();  // opt-in to the large dynamic shared memory size
 
 // ---- either side of the path (nfb_post.cu)

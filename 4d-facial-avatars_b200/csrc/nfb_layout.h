@@ -61,6 +61,9 @@ NFB_HD constexpr StepInfo step_info(int s) {
                   : StepInfo{16, 0, 2, 0, 1936, 16};
 }
 constexpr int kBiasFloats = 1952;  // 6*256 + 144 + 128 + 128 + 16
+// Multi-frame conditioning: per (network, frame) the folded bias rows of step 0 (256) then of step 3 (256); nfb.h NFB_MAX_FRAMES frames.
+constexpr int kFrameRows = 512;
+constexpr int kMaxFrames = 1024;
 
 // Byte offset of element (row n, k in [0,64)) inside one swizzled unit: 128-byte rows, 16-byte chunks
 // XORed with (row & 7) — the SWIZZLE_128B pattern the wgmma shared-memory descriptor expects.

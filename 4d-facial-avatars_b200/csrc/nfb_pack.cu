@@ -5,9 +5,11 @@
 //                        biases, conditioning columns, transposed direction columns.  Units land at nfb_layout.h unit_offset,
 //                        the function the kernels' unit programs are built from.
 //   * frame_fold_kernel: per-frame expression/latent fold into the layer-0 / layer-3 biases
+//   * frames_fold_kernel: the same fold for F frames at once, into the table the multi-frame render kernel reads
 // Reference semantics: nerf/models.py:236-261 (forward), :218-233 (parameter shapes).
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
+#include <math_constants.h>
 
 #include "nfb_internal.h"
 #include "nfb_layout.h"
@@ -192,27 +194,23 @@ struct FrameFoldArgs {
   int n_nets;
 };
 constexpr int kFoldSlabs = 8;  // blocks per network: 64 of the 512 folded bias rows each (one warp per row, lanes over the 108 columns)
-__global__ void __launch_bounds__(256) frame_fold_kernel(const float* __restrict__ expr, const float* __restrict__ latent, const FrameFoldArgs a) {
-  __shared__ float c[kDimCond];
+// c[108] = [expr / 3 ; latent] in shared memory (expr * 1 / 3, models.py:241); threads 0..107 write, the caller synchronises.
+__device__ __forceinline__ void fold_cond(const float* __restrict__ expr, const float* __restrict__ latent, float* c) {
   const int t = threadIdx.x;
-  if (t < kDimExpr) c[t] = __fdiv_rn(expr[t], 3.0f);  // (expr * 1 / 3), models.py:241
+  if (t < kDimExpr) c[t] = __fdiv_rn(expr[t], 3.0f);
   else if (t < kDimCond) c[t] = latent[t - kDimExpr];
-  __syncthreads();
-  const int net = blockIdx.x / kFoldSlabs, slab = blockIdx.x % kFoldSlabs;
-  if (net >= a.n_nets) {
-    if (slab == 0 && t < kDimCond) a.cond[t] = c[t];
-    return;
-  }
-  const float* __restrict__ bias_static = a.bias_static[net];
-  float* __restrict__ bias_frame = a.bias_frame[net];
-  if (slab == 0)  // the entries no fold touches: steps 1, 2 and 4..9
-    for (int i = t; i < kBiasFloats; i += blockDim.x)
-      if (!(i < 256 || (i >= 768 && i < 1024))) bias_frame[i] = bias_static[i];
-  const int warp = t >> 5, lane = t & 31;
+}
+// The 64 folded bias rows of slab `slab` (0..255: layers_xyz.0, 256..511: layers_xyz.3): out(bi) = bias_static[bi] + W[n, 63:171] . c
+// with bi = n (step 0) or 768 + n (step 3) and the accumulation order of a scalar loop.  Every fold (nfb_set_frame, nfb_set_frames)
+// runs this routine, so a frame's rows are the same bits whichever entry folded them.
+template <class Out>
+__device__ __forceinline__ void fold_slab(const float* __restrict__ bias_static, const float* __restrict__ w0c, const float* __restrict__ w3c,
+                                          const float* c, int slab, Out&& out) {
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (int r = warp; r < 64; r += 8) {
     const int row = slab * 64 + r;                 // 0..255: layers_xyz.0, 256..511: layers_xyz.3
     const int n = row & 255;
-    const float* __restrict__ w = (row < 256 ? a.w0c[net] : a.w3c[net]) + n * kDimCond;
+    const float* __restrict__ w = (row < 256 ? w0c : w3c) + n * kDimCond;
     // the same left-to-right fma chain a single thread would run (j ascending), split over lanes would change the rounding of
     // the per-frame bias by ~1 ulp; keep the sequential order: lane 0 accumulates, the other lanes only prefetch into registers
     float wv[4];
@@ -226,8 +224,54 @@ __global__ void __launch_bounds__(256) frame_fold_kernel(const float* __restrict
         if (l + 32 * q < kDimCond) acc = fmaf(x, c[l + 32 * q], acc);
       }
     const int bi = (row < 256) ? n : 768 + n;
-    if (lane == 0) bias_frame[bi] = bias_static[bi] + acc;
+    if (lane == 0) out(row, bias_static[bi] + acc);
   }
+}
+__global__ void __launch_bounds__(256) frame_fold_kernel(const float* __restrict__ expr, const float* __restrict__ latent, const FrameFoldArgs a) {
+  __shared__ float c[kDimCond];
+  const int t = threadIdx.x;
+  fold_cond(expr, latent, c);
+  __syncthreads();
+  const int net = blockIdx.x / kFoldSlabs, slab = blockIdx.x % kFoldSlabs;
+  if (net >= a.n_nets) {
+    if (slab == 0 && t < kDimCond) a.cond[t] = c[t];
+    return;
+  }
+  const float* __restrict__ bias_static = a.bias_static[net];
+  float* __restrict__ bias_frame = a.bias_frame[net];
+  if (slab == 0)  // the entries no fold touches: steps 1, 2 and 4..9
+    for (int i = t; i < kBiasFloats; i += blockDim.x)
+      if (!(i < 256 || (i >= 768 && i < 1024))) bias_frame[i] = bias_static[i];
+  fold_slab(bias_static, a.w0c[net], a.w3c[net], c, slab, [&](int row, float v) { bias_frame[row < 256 ? row : 768 + (row & 255)] = v; });
+}
+
+// Several frames in ONE launch (nfb_set_frames): block (slab of a network, frame f).  Per network the table holds kFrameRows floats per
+// frame — the folded rows of step 0 then those of step 3 — and one more row of NaN after the last frame, which the multi-frame render
+// kernel reads for a ray whose frame index is out of range (its conditioning behaves as NaN).  The extra slab per frame writes
+// cond[f][108].
+struct FramesFoldArgs {
+  const float *bias_static[2], *w0c[2], *w3c[2];
+  float* table[2];  // [n_frames + 1][kFrameRows]
+  float* cond;      // [n_frames][108]
+  int n_nets, n_frames;
+};
+__global__ void __launch_bounds__(256) frames_fold_kernel(const float* __restrict__ expr, const float* __restrict__ latent, const FramesFoldArgs a) {
+  __shared__ float c[kDimCond];
+  const int f = blockIdx.y, t = threadIdx.x;
+  const int net = blockIdx.x / kFoldSlabs, slab = blockIdx.x % kFoldSlabs;
+  if (f == a.n_frames) {  // the NaN row
+    if (net < a.n_nets && slab == 0)
+      for (int i = t; i < kFrameRows; i += blockDim.x) a.table[net][(size_t)f * kFrameRows + i] = CUDART_NAN_F;
+    return;
+  }
+  fold_cond(expr + (size_t)f * kDimExpr, latent + (size_t)f * kDimLatent, c);
+  __syncthreads();
+  if (net >= a.n_nets) {
+    if (slab == 0 && t < kDimCond) a.cond[(size_t)f * kDimCond + t] = c[t];
+    return;
+  }
+  float* __restrict__ row_out = a.table[net] + (size_t)f * kFrameRows;
+  fold_slab(a.bias_static[net], a.w0c[net], a.w3c[net], c, slab, [&](int row, float v) { row_out[row] = v; });
 }
 
 cudaError_t launch_repack(NetBuffers* const nb[2], const float* const* const params[2], int n_nets, cudaStream_t st,
@@ -258,6 +302,20 @@ cudaError_t launch_frame_fold(NetBuffers* const nb[2], int n_nets, const float* 
   a.cond = cond;
   a.n_nets = n_nets;
   frame_fold_kernel<<<(n_nets + 1) * kFoldSlabs, 256, 0, st>>>(expr, latent, a);
+  ++*launches;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_frames_fold(NetBuffers* const nb[2], int n_nets, int n_frames, const float* expr, const float* latent,
+                               float* const table[2], float* cond, cudaStream_t st, long long* launches) {
+  FramesFoldArgs a = {};
+  for (int n = 0; n < n_nets; ++n) {
+    a.bias_static[n] = nb[n]->bias_static.get(); a.w0c[n] = nb[n]->w0c.get(); a.w3c[n] = nb[n]->w3c.get(); a.table[n] = table[n];
+  }
+  a.cond = cond;
+  a.n_nets = n_nets;
+  a.n_frames = n_frames;
+  frames_fold_kernel<<<dim3((n_nets + 1) * kFoldSlabs, n_frames + 1), 256, 0, st>>>(expr, latent, a);
   ++*launches;
   return cudaGetLastError();
 }

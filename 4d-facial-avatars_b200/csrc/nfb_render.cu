@@ -198,10 +198,12 @@ __device__ __forceinline__ void mlp_step_mma(Step step, WeightRing& ring, uint32
 // SAVE: bit hh of `live` is set when row r0 + 8 hh holds a sample of a valid ray.  The other rows (the tile's rows beyond
 // R*S, the rows of an invalid ray) still go through the MLP, at points no reference evaluates; their records and masks are
 // stored as zero, so that an out-of-range activation there cannot reach a weight gradient as 0 * inf.
-template <bool EXACT, bool SAVE, bool PROBE>
+// ROWB (multi-frame kernels): row r0 + 8 adds bias1 instead of bias, as rows of two rays add their own direction terms.
+template <bool EXACT, bool SAVE, bool PROBE, bool ROWB = false>
 __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_base, const float* __restrict__ bias,
                                          const float* dirb0, const float* dirb1, uint8_t* act_hi, uint8_t* act_lo,
-                                         uint32_t (&act)[64], int r0, uint8_t* rec, uint32_t live, float* dump) {
+                                         uint32_t (&act)[64], int r0, uint8_t* rec, uint32_t live, float* dump,
+                                         const float* __restrict__ bias1 = nullptr) {
   int c = threadIdx.x & 3;
   // Fast mode unrolls the steps: without this the compiler hoists the per-thread addresses of all ten epilogues out of the
   // tile loop and keeps them in registers (spilling) across the MMAs.
@@ -222,10 +224,13 @@ __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_ba
   for (int j = 0; j < 16; ++j) {
     const int col = c_base + 8 * j + 2 * c;
     const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col));
+    float2 b1 = b;
+    if constexpr (ROWB) b1 = __ldg(reinterpret_cast<const float2*>(bias1 + col));
 #pragma unroll
     for (int hh = 0; hh < 2; ++hh) {
       const int R = r0 + 8 * hh;
-      float x0 = __fadd_rn(acc[4 * j + 2 * hh], b.x), x1 = __fadd_rn(acc[4 * j + 2 * hh + 1], b.y);
+      const float2 bb = hh ? b1 : b;
+      float x0 = __fadd_rn(acc[4 * j + 2 * hh], bb.x), x1 = __fadd_rn(acc[4 * j + 2 * hh + 1], bb.y);
       const float* db = hh ? dirb1 : dirb0;
       if (db) { x0 = __fadd_rn(x0, db[col]); x1 = __fadd_rn(x1, db[col + 1]); }
       if (PROBE && dump) { dump[R * 256 + col] = relu_nan(x0); dump[R * 256 + col + 1] = relu_nan(x1); }
@@ -333,8 +338,12 @@ struct Hand {
 // cfree(it); fdone's needs fready(it + 1), after the ray warps' wait for fdone(it); cfree and fready need cdone / fdone of
 // the next unit, after the row warps' waits; sready(s)'s needs cdone(it + 1).  The producer depends on the row warps
 // only through the weight ring, which both walk in stream order.
-template <bool EXACT, bool SAVE, bool PROBE>
-__global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_constant__ RenderParams p) {
+//
+// MULTI: the multi-frame kernel (render_frames_kernel).  Each ray carries a frame index (RenderParams::frame); the epilogues of
+// steps 0 and 3 add the folded bias row of the ray's own frame (RenderParams::fbias) instead of the call's one frame bias, per
+// accumulator row as the direction term of step 6 is.  Everything else is the same code.
+template <bool EXACT, bool SAVE, bool PROBE, bool MULTI>
+__device__ __forceinline__ void render_body(const RenderParams& p) {
   using M = SmemMap<EXACT>;
   // Use the dynamic shared array directly (no integer round trip) so the compiler keeps the shared address
   // space and emits LDS/STS instead of generic loads; the swizzled operands need 1024-byte alignment.
@@ -434,6 +443,11 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
               rp.dnorm = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(d0, d0), __fmul_rn(d1, d1)), __fmul_rn(d2, d2)));
               if (has_bg) { rp.bg[0] = p.bg[3 * g]; rp.bg[1] = p.bg[3 * g + 1]; rp.bg[2] = p.bg[3 * g + 2]; }
               rp.dz = p.dir_z ? p.dir_z[g] : d2;
+              if constexpr (MULTI) {  // an index out of range selects the NaN row after the last frame: no out-of-bounds read
+                const int f = p.frame[g];
+                rp.frame = (f >= 0 && f < p.n_frames) ? f : p.n_frames;
+                if (SAVE && p.save_frame) p.save_frame[g] = rp.frame;
+              }
               if constexpr (SAVE) {
                 p.save_dnorm[g] = rp.dnorm;
                 if (p.save_ray) {  // the ray as the input gradients need it: o, d, direction-encoder input
@@ -445,6 +459,7 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
               for (int k = 0; k < 3; ++k) { rp.o[k] = 0.f; rp.d[k] = 0.f; rp.bg[k] = 0.f; }
               rp.dnorm = 0.f;
               rp.dz = 0.f;
+              if constexpr (MULTI) rp.frame = 0;
             }
           }
           __syncwarp();
@@ -834,9 +849,30 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
             if (s <= 8) {
               const float* db0 = (s == 6) ? dirb + ray0 * 128 : nullptr;
               const float* db1 = (s == 6) ? dirb + ray1 * 128 : nullptr;
-              epi_half<EXACT, SAVE, PROBE>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, act, r0, rec, live, dump);
-              if (si.nh1 == 128)
-                epi_half<EXACT, SAVE, PROBE>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump);
+              if constexpr (MULTI) {
+                // steps 0 and 3, whose bias carries the conditioning fold: the rows of the frames of this thread's two
+                // accumulator rows (step 0 at +0, step 3 at +256), looked up here rather than held in registers across the tile.
+                // In fast mode (steps unrolled) the other steps run the single-frame epilogue.  Exact mode's steps are a runtime
+                // loop: there one row-bias epilogue serves every step (b0 == b1 outside steps 0 and 3), since a second copy of the
+                // epilogue in the loop costs registers (ptxas: 40 bytes of spill in the training forward).
+                if (EXACT || s == 0 || s == 3) {
+                  const bool cond = s == 0 || s == 3;
+                  const float* fb = p.fbias[pass] + (s == 3 ? 256 : 0);
+                  const float* b0 = cond ? fb + (size_t)rayp[ray0].frame * kFrameRows : bias;
+                  const float* b1 = cond ? fb + (size_t)rayp[ray1].frame * kFrameRows : bias;
+                  epi_half<EXACT, SAVE, PROBE, true>(acc0, s, 0, b0, db0, db1, act_hi, act_lo, act, r0, rec, live, dump, b1);
+                  if (si.nh1 == 128)
+                    epi_half<EXACT, SAVE, PROBE, true>(acc1, s, 128, b0, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump, b1);
+                } else {
+                  epi_half<EXACT, SAVE, PROBE>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, act, r0, rec, live, dump);
+                  if (si.nh1 == 128)
+                    epi_half<EXACT, SAVE, PROBE>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump);
+                }
+              } else {
+                epi_half<EXACT, SAVE, PROBE>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, act, r0, rec, live, dump);
+                if (si.nh1 == 128)
+                  epi_half<EXACT, SAVE, PROBE>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump);
+              }
               if (s == 6 && (lane & 3) == 0) {  // sigma = first column of the 16-column half
                 const float b = bias[128];
                 tile_raw[r0].w = acc_s[0] + b;
@@ -911,8 +947,23 @@ __global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_consta
 }
 
 template <bool EXACT, bool SAVE, bool PROBE>
+__global__ void __launch_bounds__(kThreads, 1) render_kernel(const __grid_constant__ RenderParams p) {
+  render_body<EXACT, SAVE, PROBE, false>(p);
+}
+// The multi-frame instantiations: a kernel of their own (not a fourth template parameter of render_kernel), so that each
+// single-frame instantiation keeps its name and its code.  No probe instantiation.
+template <bool EXACT, bool SAVE>
+__global__ void __launch_bounds__(kThreads, 1) render_frames_kernel(const __grid_constant__ RenderParams p) {
+  render_body<EXACT, SAVE, false, true>(p);
+}
+
+template <bool EXACT, bool SAVE, bool PROBE>
 static cudaError_t render_setup_one() {
   return cudaFuncSetAttribute(render_kernel<EXACT, SAVE, PROBE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemMap<EXACT>::kBytes);
+}
+template <bool EXACT, bool SAVE>
+static cudaError_t render_frames_setup_one() {
+  return cudaFuncSetAttribute(render_frames_kernel<EXACT, SAVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemMap<EXACT>::kBytes);
 }
 // The training forward takes no debug dumps (nfb_render_forward_train), so only the evaluation kernels have a probe
 // instantiation.
@@ -928,9 +979,11 @@ static void render_launch(const RenderParams& p, bool probe, int grid, cudaStrea
 }
 
 cudaError_t render_kernel_setup() {
-  const cudaError_t e[6] = {render_setup_one<false, false, false>(), render_setup_one<true, false, false>(),
-                            render_setup_one<false, true, false>(),  render_setup_one<true, true, false>(),
-                            render_setup_one<false, false, true>(),  render_setup_one<true, false, true>()};
+  const cudaError_t e[10] = {render_setup_one<false, false, false>(), render_setup_one<true, false, false>(),
+                             render_setup_one<false, true, false>(),  render_setup_one<true, true, false>(),
+                             render_setup_one<false, false, true>(),  render_setup_one<true, false, true>(),
+                             render_frames_setup_one<false, false>(), render_frames_setup_one<true, false>(),
+                             render_frames_setup_one<false, true>(),  render_frames_setup_one<true, true>()};
   for (const cudaError_t x : e)
     if (x != cudaSuccess) return x;
   return cudaSuccess;
@@ -947,6 +1000,22 @@ cudaError_t launch_render(const RenderParams& p, int precision, int num_sms, cud
   } else {
     if (save) render_launch<false, true>(p, probe, grid, st);
     else render_launch<false, false>(p, probe, grid, st);
+  }
+  ++*launches;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_render_frames(const RenderParams& p, int precision, int num_sms, cudaStream_t st, long long* launches) {
+  const int grid = p.geom.n_units < num_sms ? p.geom.n_units : num_sms;
+  if (grid <= 0) return cudaSuccess;
+  const bool save = p.save_rec != nullptr;
+  constexpr int B = SmemMap<true>::kBytes, F = SmemMap<false>::kBytes;
+  if (precision == 1) {
+    if (save) render_frames_kernel<true, true><<<grid, kThreads, B, st>>>(p);
+    else render_frames_kernel<true, false><<<grid, kThreads, B, st>>>(p);
+  } else {
+    if (save) render_frames_kernel<false, true><<<grid, kThreads, F, st>>>(p);
+    else render_frames_kernel<false, false><<<grid, kThreads, F, st>>>(p);
   }
   ++*launches;
   return cudaGetLastError();

@@ -9,7 +9,7 @@
 
 namespace nfb {
 
-constexpr int kRayFloats = 40;  // o[3] d[3] dnorm valid bg[3] gidx PEd[24] dz pad[3]
+constexpr int kRayFloats = 40;  // o[3] d[3] dnorm valid bg[3] gidx PEd[24] dz frame pad[2]
 struct RayP {  // per-ray constants in shared memory (kRayFloats floats)
   float o[3], d[3];
   float dnorm;
@@ -18,7 +18,8 @@ struct RayP {  // per-ray constants in shared memory (kRayFloats floats)
   int gidx;
   float ped[24];
   float dz;
-  float pad[3];
+  int frame;  // multi-frame kernels only: the ray's row of the frame table
+  float pad[2];
 };
 static_assert(sizeof(RayP) == kRayFloats * 4, "RayP size");
 

@@ -843,6 +843,105 @@ __global__ void __launch_bounds__(256) cond_grad_kernel(const FinAll f) {
 }
 
 // ================================================================================================
+// 4b. multi-frame conditioning (nfb_render_backward_frames)
+// ================================================================================================
+// Per-frame bias sums db0_f, db3_f = the sums of dY0, dY3 over the sample rows of frame f's rays, in a fixed order and without
+// atomics: per ray (samples ascending) from the dY images the dX chain left in the tile records, then per frame over the rays in
+// ascending order, added to the running sums of earlier chunks.
+// raysum_kernel: block = (ray, pass), thread = column (0..255: dY0, 256..511: dY3).
+__global__ void __launch_bounds__(kFrameRows) raysum_kernel(const FrameSumParams p) {
+  const int g = blockIdx.x, pass = blockIdx.y, t = threadIdx.x;
+  const int L = t < 256 ? 0 : 3, n = t & 255;
+  const TileGeom::RayRows rows = p.geom.ray_rows(pass, g);
+  float s = 0.f;
+  for (int i = 0; i < rows.S; ++i) {
+    const size_t slot = rows.slot(i);
+    const uint8_t* img = p.rec + (slot >> 7) * kRecBytes + rec_dy_off(L);
+    s += __half2float(*reinterpret_cast<const __half*>(img + img_offset(256, n, (int)(slot & 127))));
+  }
+  p.raysum[((size_t)pass * p.geom.n_rays + g) * kFrameRows + t] = s * p.scal[1];
+}
+// framesum_kernel: block = (frame, pass), thread = column.  Per batch of 512 rays the block first compacts the frame's rays into a
+// list (ballot + warp prefix: ascending ray order, no atomics), then every thread adds its column over that list.  A block reads
+// each frame slot once (n / 512 steps) and sums only its own frame's rays, so the launch costs O(F n / 512 + 512 n), not O(F n 512).
+__global__ void __launch_bounds__(kFrameRows) framesum_kernel(const FrameSumParams p) {
+  constexpr int kWarps = kFrameRows / 32;
+  __shared__ int list[kFrameRows];
+  __shared__ int wcount[kWarps];
+  const int f = blockIdx.x, pass = blockIdx.y, t = threadIdx.x, n = p.geom.n_rays, lane = t & 31, w = t >> 5;
+  const float* rs = p.raysum + (size_t)pass * n * kFrameRows + t;
+  float s = 0.f;
+  for (int b = 0; b < n; b += kFrameRows) {
+    const bool hit = b + t < n && p.frame[b + t] == f;
+    const unsigned m = __ballot_sync(0xffffffffu, hit);
+    if (lane == 0) wcount[w] = __popc(m);
+    __syncthreads();
+    int before = 0, total = 0;
+    for (int i = 0; i < kWarps; ++i) {
+      const int c = wcount[i];
+      before += i < w ? c : 0;
+      total += c;
+    }
+    if (hit) list[before + __popc(m & ((1u << lane) - 1u))] = b + t;
+    __syncthreads();
+    for (int i = 0; i < total; ++i) s += rs[(size_t)list[i] * kFrameRows];
+    __syncthreads();
+  }
+  float* out = p.fsum + ((size_t)f * 2 + pass) * kFrameRows + t;
+  *out = *out + s;
+}
+
+// From the per-frame sums, blockIdx.y selects the work:
+//   y = 0: block f = frame f's d latent [32] and d expression [76] (the sums latent_grad_block / expr_grad_block form from the totals)
+//   y = 1 + net: the conditioning columns of network net, W0[:, 63:171] and W3[:, 63:171]: sum_f db_f[n] c_f[j], frames ascending
+struct FramesGradArgs {
+  const float* p[2][2];  // [net] = {layers_xyz.0.weight, layers_xyz.3.weight}
+  float* g[2][2];        // [net] = their gradients (null: no parameter gradients)
+  const float *fsum, *fcond;
+  int n_frames, nets;
+  float *latent_out, *expr_out;
+};
+__global__ void __launch_bounds__(256) frames_grad_kernel(const FramesGradArgs a) {
+  const int t = threadIdx.x;
+  if (blockIdx.y == 0) {
+    const int f = blockIdx.x;
+    if (f >= a.n_frames) return;
+    __shared__ float part[2][128];
+    // thread = (half c of the 256 rows, j < 108 of [expression ; latent]), then the two halves in a fixed order
+    const int j = t & 127, c = t >> 7;
+    float s = 0.f;
+    if (j < kDimCond)
+      for (int net = 0; net < a.nets; ++net) {
+        const float* b0 = a.fsum + ((size_t)f * 2 + net) * kFrameRows;
+        const float* b3 = b0 + 256;
+        const float* w0 = a.p[net][0];
+        const float* w3 = a.p[net][1];
+        for (int n = c * 128; n < c * 128 + 128; ++n) {
+          s = fmaf(w0[n * 171 + kDimXyz + j], b0[n], s);
+          s = fmaf(w3[(size_t)n * 427 + kDimXyz + j], b3[n], s);
+        }
+      }
+    part[c][j] = s;
+    __syncthreads();
+    if (c == 0 && j < kDimCond) {
+      const float v = part[0][j] + part[1][j];
+      if (j < kDimExpr) { if (a.expr_out) a.expr_out[(size_t)f * kDimExpr + j] = v * (1.f / 3.f); }
+      else if (a.latent_out) a.latent_out[(size_t)f * kDimLatent + j - kDimExpr] = v;
+    }
+    return;
+  }
+  const int net = blockIdx.y - 1;
+  const int e = blockIdx.x * 256 + t;  // (layer L of {0, 3}, row n, column j)
+  if (net >= a.nets || e >= 2 * 256 * kDimCond || !a.g[net][0]) return;
+  const int L = e / (256 * kDimCond), r = e - L * 256 * kDimCond, n = r / kDimCond, j = r - n * kDimCond;
+  float v = 0.f;
+  for (int f = 0; f < a.n_frames; ++f)
+    v = fmaf(a.fsum[((size_t)f * 2 + net) * kFrameRows + 256 * L + n], a.fcond[(size_t)f * kDimCond + j], v);
+  if (L == 0) a.g[net][0][n * 171 + kDimXyz + j] = v;
+  else a.g[net][1][(size_t)n * 427 + kDimXyz + j] = v;
+}
+
+// ================================================================================================
 // 5. input gradients (rays, direction, background; nfb_render_backward_ex)
 // ================================================================================================
 // Per sample row of every tile (after the dX chain, which left dY0, dY3 and dY6 in the tile record):
@@ -1161,6 +1260,35 @@ cudaError_t launch_finalize_all(const float* const params_c[26], float* const gr
   finalize_kernel<<<dim3(blocks, f.nets), 256, 0, st>>>(f);
   ++*launches;
   fin_dir0_kernel<<<dim3((128 * 256 + 256) * 32 / 256, f.nets), 256, 0, st>>>(f);
+  ++*launches;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_frame_sums(const FrameSumParams& p, cudaStream_t st, long long* launches) {
+  if (p.geom.n_rays <= 0) return cudaSuccess;
+  raysum_kernel<<<dim3(p.geom.n_rays, p.geom.passes()), kFrameRows, 0, st>>>(p);
+  ++*launches;
+  framesum_kernel<<<dim3(p.n_frames, p.geom.passes()), kFrameRows, 0, st>>>(p);
+  ++*launches;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_frames_grad(const float* const params_c[26], float* const grads_c[26], const float* const params_f[26],
+                               float* const grads_f[26], const float* fsum, const float* fcond, int n_frames, float* latent_out,
+                               float* expr_out, cudaStream_t st, long long* launches) {
+  FramesGradArgs a = {};
+  a.nets = params_f ? 2 : 1;
+  const float* const* ps[2] = {params_c, params_f};
+  float* const* gs[2] = {grads_c, grads_f};
+  for (int n = 0; n < a.nets; ++n) {
+    a.p[n][0] = ps[n][0]; a.p[n][1] = ps[n][6];
+    if (gs[n]) { a.g[n][0] = gs[n][0]; a.g[n][1] = gs[n][6]; }
+  }
+  a.fsum = fsum; a.fcond = fcond; a.n_frames = n_frames; a.latent_out = latent_out; a.expr_out = expr_out;
+  const int col_blocks = grads_c ? (2 * 256 * kDimCond + 255) / 256 : 0;
+  const int bx = n_frames > col_blocks ? n_frames : col_blocks;
+  if (bx <= 0) return cudaSuccess;
+  frames_grad_kernel<<<dim3(bx, grads_c ? 1 + a.nets : 1), 256, 0, st>>>(a);
   ++*launches;
   return cudaGetLastError();
 }

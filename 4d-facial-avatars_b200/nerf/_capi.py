@@ -13,7 +13,9 @@ NFB_PREC_FAST, NFB_PREC_EXACT = 0, 1
 EXPORTS = ["nfb_version", "nfb_strerror", "nfb_last_cuda_error", "nfb_create", "nfb_destroy", "nfb_load_weights",
            "nfb_set_frame", "nfb_render_forward", "nfb_render_frame_host", "nfb_launch_count", "nfb_host_linspace",
            "nfb_render_forward_train", "nfb_render_backward", "nfb_render_backward_ex", "nfb_train_debug", "nfb_debug_schedule", "nfb_loss_mse_grad",
-           "nfb_adam_step", "nfb_adam_step_dev", "nfb_repack", "nfb_frame_products", "nfb_sample_rays", "nfb_host_map_cdf"]
+           "nfb_adam_step", "nfb_adam_step_dev", "nfb_repack", "nfb_frame_products", "nfb_sample_rays", "nfb_host_map_cdf",
+           "nfb_set_frames", "nfb_render_forward_frames", "nfb_render_forward_frames_train", "nfb_render_backward_frames"]
+NFB_MAX_FRAMES = 1024
 
 
 class NfbModelDims(C.Structure):
@@ -124,12 +126,20 @@ def _load():
                                     C.POINTER(NfbRayGather), C.c_void_p]
     lib.nfb_host_map_cdf.argtypes = [C.POINTER(NfbRayMap), C.POINTER(C.c_longlong), C.c_int, C.POINTER(C.c_longlong), C.c_int,
                                      C.POINTER(C.c_double)]
+    lib.nfb_set_frames.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p]
+    for fn in ("nfb_render_forward_frames", "nfb_render_forward_frames_train"):
+        getattr(lib, fn).argtypes = [C.c_void_p, C.POINTER(NfbRays), C.c_void_p, C.POINTER(NfbSampling), C.POINTER(NfbNoise),
+                                     C.POINTER(NfbOutputs), C.c_void_p]
+    lib.nfb_render_backward_frames.argtypes = [C.c_void_p, C.POINTER(NfbOutGrads), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                               C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p,
+                                               C.POINTER(NfbInputGrads), C.c_void_p]
     lib.nfb_launch_count.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
     lib.nfb_host_linspace.argtypes = [C.POINTER(C.c_float), C.c_int]
     for fn in ("nfb_create", "nfb_destroy", "nfb_load_weights", "nfb_set_frame", "nfb_render_forward",
                "nfb_render_frame_host", "nfb_launch_count", "nfb_host_linspace", "nfb_render_forward_train",
                "nfb_render_backward", "nfb_render_backward_ex", "nfb_train_debug", "nfb_loss_mse_grad", "nfb_adam_step", "nfb_adam_step_dev", "nfb_repack", "nfb_frame_products",
-               "nfb_sample_rays", "nfb_host_map_cdf"):
+               "nfb_sample_rays", "nfb_host_map_cdf", "nfb_set_frames", "nfb_render_forward_frames",
+               "nfb_render_forward_frames_train", "nfb_render_backward_frames"):
         getattr(lib, fn).restype = C.c_int
     return lib
 

@@ -63,6 +63,8 @@ class Renderer:
         self._keep = [None, None]  # contiguous FP32 copies handed to the pack kernels
         self.train_token = 0       # bumped by every training forward: the handle keeps ONE saved state
         self.train_rays = 0        # rays of that forward
+        self.n_frames = 0          # frames of the last set_frames
+        self.train_frames = None   # frames of the last training forward when it was a multi-frame one
         weakref.finalize(self, capi.lib.nfb_destroy, h)
 
     def _params(self, model):
@@ -118,6 +120,16 @@ class Renderer:
         capi.check(capi.lib.nfb_set_frame(self._h, _ptr(e), _ptr(l), _stream()), "set_frame")
         self._frame = (e, l)
 
+    def set_frames(self, expressions, latent_codes):
+        """nfb_set_frames: expressions [F,76], latent_codes [F,32] -> the frame table a `frame_index` render reads."""
+        e = _f32c(expressions, self.device).reshape(-1, 76)
+        l = _f32c(latent_codes, self.device).reshape(-1, 32)
+        if e.shape[0] != l.shape[0] or e.shape[0] < 1:
+            raise ValueError("expressions [F,76] and latent_codes [F,32] must have the same F >= 1")
+        capi.check(capi.lib.nfb_set_frames(self._h, _ptr(e), _ptr(l), e.shape[0], _stream()), "set_frames")
+        self._frames = (e, l)
+        self.n_frames = e.shape[0]
+
     def kernel_info(self, precision="fast"):
         """Which render kernel an evaluation call runs (bench.py): one kernel, both precision modes."""
         return dict(name="nfb::render_kernel", block_size=384)
@@ -128,10 +140,11 @@ class Renderer:
         return n.value
 
     def render(self, ro, rd, near, far, num_coarse, num_fine, perturb=False, noise_std=0.0, white_bkgd=False,
-               background=None, dir_z=None, noise=None, precision=None, debug=False, act_step=None, train=False):
+               background=None, dir_z=None, noise=None, precision=None, debug=False, act_step=None, train=False, frame_index=None):
         """ro, rd: [N,3] CUDA FP32.  noise: dict with t_rand, n_c, u, n_f (any may be None).  Returns a dict
         with the seven outputs (+ per-sample dumps when debug).  train=True: nfb_render_forward_train (the handle keeps
-        the state `backward` consumes)."""
+        the state `backward` consumes).  frame_index: [N] int32-convertible CUDA tensor -> a multi-frame call over the frames of
+        set_frames (nfb_render_forward_frames[_train]; no debug dumps)."""
         dev = self.device
         ro, rd = _f32c(ro, dev), _f32c(rd, dev)
         n = ro.shape[0]
@@ -176,9 +189,22 @@ class Renderer:
             if act_step is not None:
                 out["act"] = torch.zeros((128, 256), device=dev)
                 dbg.act_dump, dbg.act_step = out["act"].data_ptr(), int(act_step)
-        if train:
+        if frame_index is not None:
+            if dbg is not None:
+                raise ValueError("a multi-frame render takes no debug dumps")
+            fi = frame_index.detach().to(device=dev, dtype=torch.int32).reshape(n).contiguous()
+            keep.append(fi)
+            fn = capi.lib.nfb_render_forward_frames_train if train else capi.lib.nfb_render_forward_frames
+            if train:
+                self.train_token += 1
+                self.train_rays = n
+                self.train_frames = self.n_frames
+            capi.check(fn(self._h, C.byref(rays), _ptr(fi), C.byref(sm), C.byref(nz) if noise else None, C.byref(o), _stream()),
+                       "render_forward_frames")
+        elif train:
             self.train_token += 1
             self.train_rays = n
+            self.train_frames = None
             capi.check(capi.lib.nfb_render_forward_train(self._h, C.byref(rays), C.byref(sm), C.byref(nz) if noise else None,
                                                          C.byref(o), _stream()), "render_forward_train")
         else:
@@ -241,13 +267,14 @@ class Renderer:
                                                 _ptr(grad_latent), _stream()), "render_backward")
         self._bwd_keep = keep
 
-    def backward(self, out_grads, params_c, params_f, want_latent=True, want_params=True, inputs=None):
+    def backward(self, out_grads, params_c, params_f, want_latent=True, want_params=True, inputs=None, frames=False):
         """nfb_render_backward_ex for the last training forward.  out_grads: 7 CUDA tensors or None (rgb_c, disp_c, acc_c,
         rgb_f, disp_f, acc_f, w_last); params_*: the 26 FP32 parameter tensors in PARAM_ORDER (params_f None without a
         fine network).  Returns (grads_c, grads_f, grad_latent) — lists aligned with PARAM_ORDER, None for layers_dir.3.*.
         inputs: names of the input gradients wanted, out of INPUT_GRADS ("ray_origins", "ray_directions", "dir_z", "background",
         "expression"); then a 4th element, a dict name -> tensor, is returned.  want_params=False: input-only backward (no
-        parameter gradient is formed; grads_c / grads_f are None)."""
+        parameter gradient is formed; grads_c / grads_f are None).  frames=True: nfb_render_backward_frames after a multi-frame
+        forward; grad_latent is then [F,32], and "expression" in `inputs` yields [F,76]."""
         dev = self.device
         keep = []
         og = capi.NfbOutGrads()
@@ -270,6 +297,26 @@ class Renderer:
         pf, gf, grads_f = pack(params_f)
         if not want_params:
             gc = gf = grads_c = grads_f = None
+        if frames:
+            if self.train_frames is None:
+                raise RuntimeError("backward(frames=True) needs a multi-frame training forward (render(..., train=True, "
+                                   "frame_index=...)); the last training forward was a single-frame one")
+            nfr = self.train_frames
+            glat = torch.empty((nfr, 32), device=dev, dtype=torch.float32) if want_latent else None
+            gexp = torch.empty((nfr, 76), device=dev, dtype=torch.float32) if inputs and "expression" in inputs else None
+            ig, ing = capi.NfbInputGrads(), {}
+            n = self.train_rays
+            shapes = dict(ray_origins=(n, 3), ray_directions=(n, 3), dir_z=(n,), background=(n, 3))
+            for name in (inputs or ()):
+                if name != "expression":
+                    ing[name] = torch.empty(shapes[name], device=dev, dtype=torch.float32)
+                    setattr(ig, name, ing[name].data_ptr())
+            if gexp is not None:
+                ing["expression"] = gexp
+            capi.check(capi.lib.nfb_render_backward_frames(self._h, C.byref(og), pc, pf, gc, gf, _ptr(glat), _ptr(gexp), C.byref(ig),
+                                                           _stream()), "render_backward_frames")
+            self._bwd_keep = keep
+            return (grads_c, grads_f, glat, ing) if inputs is not None else (grads_c, grads_f, glat)
         glat = torch.empty(32, device=dev, dtype=torch.float32) if want_latent else None
         ig, ing = None, {}
         if inputs is not None:

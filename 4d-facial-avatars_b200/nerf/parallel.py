@@ -103,7 +103,11 @@ def data_parallel(run_fn, group=None):
 
     Noise: every rank draws the noise of the WHOLE call in the reference's order and keeps its shard's slice
     (train_utils._shard_ctx), so a seeded multi-rank run renders exactly what the seeded single-process run renders and the
-    ranks' RNG streams stay in lock-step for the caller's own draws (ray selection)."""
+    ranks' RNG streams stay in lock-step for the caller's own draws (ray selection).
+
+    Multi-frame calls (nerf.render_frames) are not sharded: NotImplementedError."""
+    if getattr(run_fn, "multi_frame", False):
+        raise NotImplementedError("data_parallel does not shard multi-frame calls (nerf.render_frames): run them in one process")
     def wrapped(height, width, focal_length, model_coarse, model_fine, ray_origins, ray_directions, options, mode="train",
                 encode_position_fn=None, encode_direction_fn=None, expressions=None, background_prior=None, latent_code=None,
                 ray_directions_ablation=None):

@@ -147,6 +147,57 @@ def run_one_iter_of_nerf(height, width, focal_length, model_coarse, model_fine, 
     return tuple(outs)
 
 
+def render_frames(ray_origins, ray_directions, frame_index, expressions, latent_codes, model_coarse, model_fine, options, mode="train",
+                  background_prior=None):
+    """Render rays of several frames in ONE kernel launch, each ray conditioned on its own frame: ray i uses expressions[frame_index[i]]
+    ([F,76]) and latent_codes[frame_index[i]] ([F,32]).  Options as run_one_iter_of_nerf handles them (near/far from
+    options.dataset, the noise of the whole call drawn in the reference's chunk order).  Returns the 7-tuple of
+    run_one_iter_of_nerf's training mode for the flattened rays.  Differentiable with respect to the parameters, every frame's
+    expression and latent (pass `latent_table[ids]` to route the gradients back into a table), the rays and the background: a
+    loss over several frames is one forward and one backward (the renderer keeps one saved training state).  frame_index outside
+    [0, F) gives NaN outputs for those rays only.  Up to 1024 frames per call."""
+    if options.dataset.no_ndc is False:
+        raise NotImplementedError("NDC rays are not implemented (every shipped config sets no_ndc: True)")
+    opts = _mode_opts(options, mode)
+    _check_models(model_coarse, model_fine)
+    if opts["lindisp"]:
+        raise NotImplementedError("lindisp sampling is not implemented (every shipped config sets it to False)")
+    has_fine = bool(model_fine) and opts["num_fine"] > 0
+    ro = ray_origins.reshape(-1, 3)
+    rd = ray_directions.reshape(-1, 3)
+    n = rd.shape[0]
+    fi = frame_index.reshape(-1)
+    if fi.shape[0] != n:
+        raise ValueError(f"frame_index has {fi.shape[0]} entries for {n} rays")
+    if expressions.dim() != 2 or latent_codes.dim() != 2 or expressions.shape[0] != latent_codes.shape[0]:
+        raise ValueError("expressions [F,76] and latent_codes [F,32] must share F")
+    near, far = options.dataset.near, options.dataset.far
+    rays = torch.cat((ro, rd, near * torch.ones_like(rd[..., :1]), far * torch.ones_like(rd[..., :1])), dim=-1)
+    noise = None
+    if opts["perturb"] or opts["noise_std"] > 0.0:
+        chunk = opts["chunksize"]
+        noise = _cat_noise([_draw_noise(min(chunk, n - st), opts, rays.device, has_fine) for st in range(0, n, chunk)])
+    bg = background_prior.reshape(-1, 3) if background_prior is not None else None
+    eng = _engine.renderer_for(rays.device)
+    eng.sync_weights(model_coarse, model_fine if has_fine else None)
+    needs_grad = torch.is_grad_enabled() and (
+        any(p.requires_grad for p in model_coarse.parameters())
+        or (has_fine and any(p.requires_grad for p in model_fine.parameters()))
+        or any(t is not None and t.requires_grad for t in (latent_codes, rays, expressions, bg)))
+    args = dict(near=float(near), far=float(far), num_coarse=opts["num_coarse"], num_fine=opts["num_fine"] if has_fine else 0,
+                perturb=opts["perturb"], noise_std=opts["noise_std"], white_bkgd=opts["white_bkgd"], background=bg, noise=noise)
+    if needs_grad:
+        from ._autograd import render_frames_with_grad
+        return render_frames_with_grad(eng, rays, fi, model_coarse, model_fine if has_fine else None, expressions, latent_codes, args)
+    eng.set_frames(expressions, latent_codes)
+    out = eng.render(rays[:, :3], rays[:, 3:6], frame_index=fi, **args)
+    return (out["rgb_coarse"], out["disp_coarse"], out["acc_coarse"], out.get("rgb_fine"), out.get("disp_fine"),
+            out.get("acc_fine"), out["w_last"])
+
+
+render_frames.multi_frame = True  # nerf.parallel.data_parallel refuses it
+
+
 class GaussianSmoothing(torch.nn.Module):
     """Depth-wise Gaussian blur (nerf/train_utils.py:379-442); only reachable in the reference when two
     hard-coded flags are edited.  Kept so `from nerf import GaussianSmoothing` works."""

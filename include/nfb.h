@@ -29,6 +29,10 @@ extern "C" {
 /* Defined when the backward and the loss repeat bit for bit (no floating-point atomics; see nfb_render_backward).  The
  * version number stayed 130 for this addition, so test this macro rather than the version. */
 #define NFB_REPRODUCIBLE_BACKWARD 1
+/* Defined when the multi-frame entries exist (nfb_set_frames, nfb_render_forward_frames[_train], nfb_render_backward_frames): one
+ * call renders and differentiates rays of up to NFB_MAX_FRAMES frames, each ray conditioned on its own frame.  Test this macro. */
+#define NFB_MULTI_FRAME 1
+#define NFB_MAX_FRAMES 1024
 
 typedef struct NfbHandle NfbHandle;
 
@@ -240,6 +244,51 @@ typedef struct {
 int nfb_render_backward_ex(NfbHandle* h, const NfbOutGrads* out_grads, const float* const params_coarse[26],
                            const float* const params_fine[26], float* const grads_coarse[26], float* const grads_fine[26],
                            float* grad_latent, const NfbInputGrads* in_grads, void* stream);
+
+/* ---- Several frames in one call (NFB_MULTI_FRAME) ----
+ * A loss over rays of several frames (one latent code fitted to several frames, a clip's per-frame expressions in one step,
+ * training batches drawn from several images) as ONE forward with ONE saved training state and ONE backward: every ray names its
+ * frame, and the kernel adds that frame's folded layer-0 / layer-3 biases to the ray's rows.  Each frame's folded rows are the
+ * bits nfb_set_frame would fold for it alone, so a ray renders exactly as a single-frame call of its frame renders it.
+ *
+ * State.  The frames of nfb_set_frames and the frame of nfb_set_frame are independent: each leaves the other as it was, and the
+ * single-frame entries keep using the frame of nfb_set_frame.  Loading weights (nfb_load_weights, nfb_repack) makes both stale.
+ * A multi-frame training forward replaces the handle's saved training state like nfb_render_forward_train does, and copies the
+ * frame table and conditioning vectors: a later nfb_set_frame(s) or evaluation render does not change what is differentiated.
+ *
+ * nfb_set_frames: expressions [n_frames,76] and latents [n_frames,32], DEVICE, row-major.  Folds each (expression / 3, latent) pair
+ * into the layer-0 / layer-3 biases of both loaded networks, about 4 KB per frame.  1 <= n_frames <= NFB_MAX_FRAMES, else
+ * NFB_ERR_INVALID / NFB_ERR_UNSUPPORTED.  1 launch. */
+int nfb_set_frames(NfbHandle* h, const float* expressions, const float* latents, int n_frames, void* stream);
+
+/* nfb_render_forward / nfb_render_forward_train with a per-ray frame: frame_index is a DEVICE int32 [n_rays] in [0, n_frames) of
+ * the last nfb_set_frames.  Explicit rays only (rays->o, d): in-kernel generation is one pose per call, so o == NULL gives
+ * NFB_ERR_UNSUPPORTED.  A ray whose index is out of range (negative or >= n_frames) reads nothing out of bounds: it renders as if
+ * its conditioning were NaN, so its outputs are NaN and gradients that reach it are non-finite; no other ray is affected.
+ * Without nfb_set_frames first: NFB_ERR_STATE.  The chunked training forward (over the memory budget, see
+ * nfb_render_forward_train) also re-reads frame_index in the backward: keep it alive with the rays.  1 launch each (the training
+ * forward copies the frame table first). */
+int nfb_render_forward_frames(NfbHandle* h, const NfbRays* rays, const int32_t* frame_index, const NfbSampling* sampling,
+                              const NfbNoise* noise /* nullable */, const NfbOutputs* out, void* stream);
+int nfb_render_forward_frames_train(NfbHandle* h, const NfbRays* rays, const int32_t* frame_index, const NfbSampling* sampling,
+                                    const NfbNoise* noise /* nullable */, const NfbOutputs* out, void* stream);
+
+/* Backward of the last nfb_render_forward_frames_train: nfb_render_backward_ex's parameter and input gradients (in_grads may be
+ * NULL; its `expression` member must be NULL: NFB_ERR_INVALID), plus per-frame conditioning gradients grad_latents [n_frames,32]
+ * and grad_expressions [n_frames,76] (device; either may be NULL), dL/d the rows given to nfb_set_frames (the expression before its
+ * division by 3).  A frame without rays gets exactly zero.  The conditioning columns of layers_xyz.0 / .3 become
+ * sum_f db_f (x) c_f, with db_f the layer's bias gradient summed over frame f's rays; the bias gradients themselves are the totals
+ * as always.  Input-only mode (grads_coarse and grads_fine NULL) forms no parameter gradient, as in nfb_render_backward_ex; with
+ * neither conditioning nor input gradients requested it is NFB_ERR_INVALID.  The per-frame sums are taken per ray, then per frame
+ * over the rays in ascending order, and across chunks in chunk order: the reproducibility of nfb_render_backward holds.
+ * nfb_render_backward_frames after a single-frame training forward is NFB_ERR_STATE; nfb_render_backward(_ex) after a multi-frame
+ * forward is NFB_ERR_STATE when it is asked for grad_latent or in_grads->expression (there is no one latent to return; the other
+ * gradients are formed as here).
+ * Launches: nfb_render_backward_ex's (without the weight-gradient launch in input-only mode), plus two per chunk for the per-frame
+ * sums, and one for the per-frame gradients. */
+int nfb_render_backward_frames(NfbHandle* h, const NfbOutGrads* out_grads, const float* const params_coarse[26],
+                               const float* const params_fine[26], float* const grads_coarse[26], float* const grads_fine[26],
+                               float* grad_latents, float* grad_expressions, const NfbInputGrads* in_grads, void* stream);
 
 /* ---- Training-step tail: loss, optimizer, re-pack (replaces train_transformed_rays.py:355-400 for callers that adopt it;
  * the drop-in Python surface keeps working with torch.nn.functional.mse_loss + torch.optim.Adam) ----
