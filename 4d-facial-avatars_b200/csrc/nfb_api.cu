@@ -60,8 +60,8 @@ struct NfbHandle {
     DevBuf<float> ray;                                  // [n][7] = (o, d, v0), written by the SAVE forward
     DevBuf<float> rows;                                 // [tiles][128][4]
     DevBuf<float> ray_dn, ray_bg;
-    // what the last one-launch backward of this forward left in ray_dn / ray_bg and rows (nfb_train_debug)
-    bool per_ray_formed = false, rows_formed = false;
+    // what the last one-launch backward of this forward left in ray_dn / ray_bg, rows and raysum / fsum (nfb_train_debug)
+    bool per_ray_formed = false, rows_formed = false, frame_sums_formed = false;
     // chunked mode (the records of the whole call would exceed the memory budget): the forward only produced the outputs; the
     // backward re-runs the training forward chunk by chunk from the saved launch parameters (the caller keeps the inputs alive)
     bool chunked = false;
@@ -389,7 +389,7 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
     // Saved for nfb_render_backward: per-tile activation records, sample depths, (colour, ReLU input of sigma), |d|.
     NfbHandle::Train& tr = h->tr;
     tr.valid = false;
-    tr.per_ray_formed = tr.rows_formed = false;
+    tr.per_ray_formed = tr.rows_formed = tr.frame_sums_formed = false;
     int rc;
     // a multi-frame backward also keeps per-ray dY0 / dY3 sums: 2 passes x kFrameRows floats = 4 KiB per ray, in the budget too
     const size_t ray_bytes = multi ? 2 * nfb::kFrameRows * sizeof(float) : 0;
@@ -521,7 +521,7 @@ static int backward_impl(NfbHandle* h, const NfbOutGrads* og, const float* const
   NFB_CUDA(cudaMemsetAsync(acc[0], 0, nfb::kAccFloats * sizeof(float), st));
   NFB_CUDA(cudaMemsetAsync(acc[1], 0, nfb::kAccFloats * sizeof(float), st));
   if (frame_grads) NFB_CUDA(cudaMemsetAsync(tr.fsum.get(), 0, (size_t)tr.n_frames * 2 * nfb::kFrameRows * sizeof(float), st));
-  tr.per_ray_formed = tr.rows_formed = false;
+  tr.per_ray_formed = tr.rows_formed = tr.frame_sums_formed = false;
 
   // compositing backward -> dX chain -> weight-gradient GEMMs -> fixed-order reduction for the g.n_rays rays from `begin` on,
   // whose training state the buffers hold; the FP32 accumulators tr.acc add up over chunks in chunk order (each chunk has its
@@ -594,6 +594,7 @@ static int backward_impl(NfbHandle* h, const NfbOutGrads* og, const float* const
     if (rc) return rc;
     tr.per_ray_formed = per_ray;
     tr.rows_formed = ray_grads;
+    tr.frame_sums_formed = frame_grads;
   } else {
     const int n_rays = tr.geom.n_rays;
     for (int begin = 0; begin < n_rays; begin += tr.chunk_rays) {
@@ -673,6 +674,14 @@ int nfb_train_debug(NfbHandle* h, NfbTrainDebug* out) {
   out->rows = tr.rows_formed ? tr.rows.get() : nullptr;
   out->ray_dn = tr.per_ray_formed ? tr.ray_dn.get() : nullptr;
   out->ray_bg = (tr.per_ray_formed && tr.has_bg) ? tr.ray_bg.get() : nullptr;
+  const bool multi = tr.multi;
+  out->n_frames = multi ? tr.n_frames : 0;
+  out->frame = multi ? tr.frame.get() : nullptr;
+  out->frame_table[0] = multi ? tr.ftab[0].get() : nullptr;
+  out->frame_table[1] = (multi && tr.geom.passes() == 2) ? tr.ftab[1].get() : nullptr;
+  out->frame_cond = multi ? tr.fcond.get() : nullptr;
+  out->ray_sums = (multi && tr.frame_sums_formed) ? tr.raysum.get() : nullptr;
+  out->frame_sums = (multi && tr.frame_sums_formed) ? tr.fsum.get() : nullptr;
   return NFB_OK;
 }
 

@@ -64,7 +64,9 @@ class NfbTrainDebug(C.Structure):
                 ("acc_coarse", C.c_void_p), ("acc_fine", C.c_void_p), ("acc_floats", C.c_int32), ("scale", C.c_void_p),
                 ("z_coarse", C.c_void_p), ("raw_coarse", C.c_void_p), ("z_fine", C.c_void_p), ("raw_fine", C.c_void_p),
                 ("tiles_coarse", C.c_int32), ("tiles_fine", C.c_int32), ("rays_per_unit", C.c_int32), ("rays", C.c_void_p),
-                ("dnorm", C.c_void_p), ("rows", C.c_void_p), ("ray_dn", C.c_void_p), ("ray_bg", C.c_void_p)]
+                ("dnorm", C.c_void_p), ("rows", C.c_void_p), ("ray_dn", C.c_void_p), ("ray_bg", C.c_void_p),
+                ("n_frames", C.c_int32), ("frame", C.c_void_p), ("frame_table", C.c_void_p * 2), ("frame_cond", C.c_void_p),
+                ("ray_sums", C.c_void_p), ("frame_sums", C.c_void_p)]
 
 
 class NfbAdam(C.Structure):

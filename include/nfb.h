@@ -410,6 +410,18 @@ typedef struct {
   const float* rows;
   const float* ray_dn;
   const float* ray_bg;
+  /* What a multi-frame forward (nfb_render_forward_frames_train) saved; n_frames is 0 and the pointers NULL after a single-frame
+   * one.  frame [n] = the slot each ray rendered with (n_frames where its index was out of range); frame_table[net]
+   * [n_frames + 1][512] = the folded rows of steps 0 and 3 per frame, the last row NaN ([1] NULL without a fine pass);
+   * frame_cond [n_frames][108] = [expression / 3 ; latent] per frame.  ray_sums [passes][n][512] (dY0 | dY3 summed over each
+   * ray's samples, unscaled) and frame_sums [n_frames][2][512] (those summed over each frame's rays) are NULL until a backward of
+   * this forward has formed them. */
+  int32_t n_frames;
+  const int32_t* frame;
+  const float* frame_table[2];
+  const float* frame_cond;
+  const float* ray_sums;
+  const float* frame_sums;
 } NfbTrainDebug;
 int nfb_train_debug(NfbHandle* h, NfbTrainDebug* out);
 

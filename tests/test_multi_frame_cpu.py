@@ -64,3 +64,25 @@ def test_no_global_store_in_the_multi_frame_fast_epilogues(built_lib):
     epi = frames_epilogue_stores(built_lib)
     assert epi, "render_frames_kernel<false, false> not found in the library"
     assert sum(epi) == 0, epi
+
+
+def test_train_debug_struct_matches_header(capi):
+    """nerf._capi.NfbTrainDebug declares the fields of include/nfb.h's NfbTrainDebug, in the header's order, at offsets that
+    only grow: a field appended to one but not the other, or two swapped, reads the wrong device pointer."""
+    h = open(os.path.join(ROOT, "include", "nfb.h")).read()
+    body = re.search(r"typedef struct \{([^{}]*)\} NfbTrainDebug;", h).group(1)
+    body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
+    names = []
+    for decl in body.split(";"):
+        decl = decl.strip()
+        if not decl:
+            continue
+        for part in decl.split(","):
+            m = re.search(r"(\w+)\s*(\[\d+\])?\s*$", part.strip())
+            names.append(m.group(1))
+    fields = [f[0] for f in capi.NfbTrainDebug._fields_]
+    assert fields == names
+    offsets = [getattr(capi.NfbTrainDebug, f).offset for f in fields]
+    assert offsets == sorted(offsets) and len(set(offsets)) == len(offsets)
+    assert fields[-6:] == ["n_frames", "frame", "frame_table", "frame_cond", "ray_sums", "frame_sums"]
+    assert C.sizeof(dict(capi.NfbTrainDebug._fields_)["frame_table"]) == 2 * C.sizeof(C.c_void_p)

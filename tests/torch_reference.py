@@ -17,12 +17,16 @@ def _posenc(x, n_freq, include_input):
     return torch.cat(parts, dim=-1)
 
 
-def _mlp(p, x, expr, latent, taps=None):
-    """taps (dict): receives the post-activation outputs h0..h5, g0..g2 and the pre-activations a0..a8 (retain_grad)."""
+def _mlp(p, x, expr, latent, taps=None, per_row=False):
+    """taps (dict): receives the post-activation outputs h0..h5, g0..g2 and the pre-activations a0..a8 (retain_grad).
+    per_row: expr [rows,76] and latent [rows,32] condition each row on its own (a multi-frame call)."""
     F = torch.nn.functional
     xyz, dirs = x[..., :63], x[..., 63:]
     rows = xyz.shape[0]
-    cond = torch.cat(((expr * 1 / 3).reshape(1, -1).expand(rows, -1), latent.reshape(1, -1).expand(rows, -1)), dim=1)
+    if per_row:
+        cond = torch.cat((expr * 1 / 3, latent), dim=1)
+    else:
+        cond = torch.cat(((expr * 1 / 3).reshape(1, -1).expand(rows, -1), latent.reshape(1, -1).expand(rows, -1)), dim=1)
     initial = torch.cat((xyz, cond), dim=1)
 
     def act(a, name_pre, name_post):
@@ -74,12 +78,15 @@ def _composite(raw, z, rd, noise_std, noise, white_bkgd, bg):
     return rgb, disp, acc, w
 
 
-def _pass(p, z, rays, dir_cols, expr, latent, noise_std, noise, white_bkgd, bg, taps=None):
+def _pass(p, z, rays, dir_cols, expr, latent, noise_std, noise, white_bkgd, bg, taps=None, per_ray_cond=False):
     ro, rd = rays[:, :3], rays[:, 3:6]
     n, s = z.shape
     pts = ro[:, None, :] + rd[:, None, :] * z[:, :, None]
     x = torch.cat((_posenc(pts.reshape(-1, 3), 10, True), _posenc(dir_cols[:, None, :].expand(n, s, 3).reshape(-1, 3), 4, False)), dim=-1)
-    raw = _mlp(p, x, expr, latent, taps).reshape(n, s, 4)
+    if per_ray_cond:  # [n,76] / [n,32] -> one row per sample
+        expr = expr[:, None, :].expand(n, s, expr.shape[1]).reshape(n * s, -1)
+        latent = latent[:, None, :].expand(n, s, latent.shape[1]).reshape(n * s, -1)
+    raw = _mlp(p, x, expr, latent, taps, per_row=per_ray_cond).reshape(n, s, 4)
     if taps is not None:
         raw.retain_grad()
         taps["raw"] = raw
@@ -87,17 +94,20 @@ def _pass(p, z, rays, dir_cols, expr, latent, noise_std, noise, white_bkgd, bg, 
 
 
 def render_at_depths(rays, params_c, params_f, expr, latent, z_c, z_f, near, far, noise_std=0.0, noise=None,
-                     white_bkgd=False, bg=None, dir_z=None, taps=None):
+                     white_bkgd=False, bg=None, dir_z=None, taps=None, per_ray_cond=False):
     """rays [N,8]; params_*: dict name -> tensor (requires_grad leaves).  Returns the 7-tuple as differentiable tensors.
-    `taps` (dict): receives per-pass intermediate tensors under "coarse"/"fine"."""
+    `taps` (dict): receives per-pass intermediate tensors under "coarse"/"fine".  per_ray_cond: expr [N,76] and latent [N,32]
+    hold each ray's own frame (a multi-frame call); otherwise one expression [76] and latent [32] for all rays."""
     dir_cols = torch.cat((dir_z.reshape(-1, 1) if dir_z is not None else rays[:, 5:6],
                           torch.full_like(rays[:, :1], near), torch.full_like(rays[:, :1], far)), dim=-1)
     nz = noise or {}
     tc = taps.setdefault("coarse", {}) if taps is not None else None
-    rgb_c, disp_c, acc_c, w = _pass(params_c, z_c, rays, dir_cols, expr, latent, noise_std, nz.get("n_c"), white_bkgd, bg, tc)
+    rgb_c, disp_c, acc_c, w = _pass(params_c, z_c, rays, dir_cols, expr, latent, noise_std, nz.get("n_c"), white_bkgd, bg, tc,
+                                per_ray_cond)
     outs = [rgb_c, disp_c, acc_c, None, None, None, w[:, -1]]
     if params_f is not None:
         tf = taps.setdefault("fine", {}) if taps is not None else None
-        rgb_f, disp_f, acc_f, w = _pass(params_f, z_f, rays, dir_cols, expr, latent, noise_std, nz.get("n_f"), white_bkgd, bg, tf)
+        rgb_f, disp_f, acc_f, w = _pass(params_f, z_f, rays, dir_cols, expr, latent, noise_std, nz.get("n_f"), white_bkgd, bg, tf,
+                                    per_ray_cond)
         outs[3:7] = [rgb_f, disp_f, acc_f, w[:, -1]]
     return outs
