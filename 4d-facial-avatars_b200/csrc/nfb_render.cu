@@ -68,9 +68,12 @@ struct SmemMap {
   static constexpr int kTileRaw = kRay + 3 * 2 * kRayFloats * 4;  // [128] (rgb raw, sigma raw) of the current tile
   static constexpr int kBars = kTileRaw + kTileM * 16;
   static constexpr int kHand = kBars + 2 * kSlots * 8;  // the hand-off mbarriers (Hand)
-  static constexpr int kBytes = kHand + 9 * 8;
+  // Fast mode: both networks' bias blocks, copied once per CTA, so the epilogues read them from shared memory.  Exact mode has
+  // no room for them and reads them from global memory.
+  static constexpr int kBias = (kHand + 9 * 8 + 15) / 16 * 16;
+  static constexpr int kBytes = kBias + (EXACT ? 0 : 2 * kBiasFloats * 4);
   static_assert(kBytes <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
-  static_assert(kRaw % 16 == 0 && kBars % 8 == 0 && kHand % 8 == 0, "alignment");
+  static_assert(kRaw % 16 == 0 && kBars % 8 == 0 && kHand % 8 == 0 && kBias % 16 == 0, "alignment");
 };
 
 constexpr int kTileUnits = prog_units(kFwdStream);
@@ -223,7 +226,10 @@ __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_ba
 #pragma unroll
   for (int j = 0; j < 16; ++j) {
     const int col = c_base + 8 * j + 2 * c;
-    const float2 b = __ldg(reinterpret_cast<const float2*>(bias + col));
+    // fast mode: `bias` is the shared-memory copy, except for ROWB's per-frame rows (global)
+    float2 b;
+    if constexpr (EXACT || ROWB) b = __ldg(reinterpret_cast<const float2*>(bias + col));
+    else b = *reinterpret_cast<const float2*>(bias + col);
     float2 b1 = b;
     if constexpr (ROWB) b1 = __ldg(reinterpret_cast<const float2*>(bias1 + col));
 #pragma unroll
@@ -357,6 +363,11 @@ __device__ __forceinline__ void render_body(const RenderParams& p) {
   if (threadIdx.x == 0) {
     ring.init();
     hand.init();
+  }
+  float* sbias = reinterpret_cast<float*>(smem + M::kBias);
+  if constexpr (!EXACT) {
+    for (int i = threadIdx.x; i < 2 * kBiasFloats; i += kThreads)
+      sbias[i] = p.bias[i / kBiasFloats][i % kBiasFloats];
   }
   __syncthreads();
 
@@ -676,7 +687,7 @@ __device__ __forceinline__ void render_body(const RenderParams& p) {
       const int unit = blockIdx.x + it * gridDim.x;
       const int S = geom.samples(pass);
       const int n_tiles = geom.tile_count(pass);
-      const float* bias_n = p.bias[pass];
+      const float* bias_n = EXACT ? p.bias[pass] : sbias + pass * kBiasFloats;
       const int cb = it % nb;
       float4* carry_raw = (pass || cb) ? raw_f : raw_c;
       float* carry_z = (pass || cb) ? z_f : z_c;
