@@ -62,6 +62,9 @@ struct NfbHandle {
     DevBuf<float> ray_dn, ray_bg;
     // what the last one-launch backward of this forward left in ray_dn / ray_bg, rows and raysum / fsum (nfb_train_debug)
     bool per_ray_formed = false, rows_formed = false, frame_sums_formed = false;
+    // ... and in dw_ws / bsum: the split and slot size of its weight-gradient launch (dw_parts 0, 0: none ran)
+    bool bwd_formed = false, dw_pe_only = false;
+    int dw_parts[2] = {0, 0}, dw_stride = 0;
     // chunked mode (the records of the whole call would exceed the memory budget): the forward only produced the outputs; the
     // backward re-runs the training forward chunk by chunk from the saved launch parameters (the caller keeps the inputs alive)
     bool chunked = false;
@@ -389,7 +392,7 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
     // Saved for nfb_render_backward: per-tile activation records, sample depths, (colour, ReLU input of sigma), |d|.
     NfbHandle::Train& tr = h->tr;
     tr.valid = false;
-    tr.per_ray_formed = tr.rows_formed = tr.frame_sums_formed = false;
+    tr.per_ray_formed = tr.rows_formed = tr.frame_sums_formed = tr.bwd_formed = false;
     int rc;
     // a multi-frame backward also keeps per-ray dY0 / dY3 sums: 2 passes x kFrameRows floats = 4 KiB per ray, in the budget too
     const size_t ray_bytes = multi ? 2 * nfb::kFrameRows * sizeof(float) : 0;
@@ -521,7 +524,9 @@ static int backward_impl(NfbHandle* h, const NfbOutGrads* og, const float* const
   NFB_CUDA(cudaMemsetAsync(acc[0], 0, nfb::kAccFloats * sizeof(float), st));
   NFB_CUDA(cudaMemsetAsync(acc[1], 0, nfb::kAccFloats * sizeof(float), st));
   if (frame_grads) NFB_CUDA(cudaMemsetAsync(tr.fsum.get(), 0, (size_t)tr.n_frames * 2 * nfb::kFrameRows * sizeof(float), st));
-  tr.per_ray_formed = tr.rows_formed = tr.frame_sums_formed = false;
+  tr.per_ray_formed = tr.rows_formed = tr.frame_sums_formed = tr.bwd_formed = false;
+  tr.dw_parts[0] = tr.dw_parts[1] = tr.dw_stride = 0;
+  tr.dw_pe_only = false;
 
   // compositing backward -> dX chain -> weight-gradient GEMMs -> fixed-order reduction for the g.n_rays rays from `begin` on,
   // whose training state the buffers hold; the FP32 accumulators tr.acc add up over chunks in chunk order (each chunk has its
@@ -563,6 +568,8 @@ static int backward_impl(NfbHandle* h, const NfbOutGrads* og, const float* const
     if (dw) {
       d.rec = tr.rec.get(); d.ws = tr.dw_ws.get(); d.scal = scal;
       NFB_CUDA(nfb::launch_dw(d, h->num_sms, st, &h->launches, input_only));  // both networks in one launch
+      tr.dw_parts[0] = d.parts[0]; tr.dw_parts[1] = d.parts[1]; tr.dw_stride = d.ws_stride;
+      tr.dw_pe_only = input_only;
     }
     if (frame_grads) {
       nfb::FrameSumParams fs = {};
@@ -595,6 +602,7 @@ static int backward_impl(NfbHandle* h, const NfbOutGrads* og, const float* const
     tr.per_ray_formed = per_ray;
     tr.rows_formed = ray_grads;
     tr.frame_sums_formed = frame_grads;
+    tr.bwd_formed = true;
   } else {
     const int n_rays = tr.geom.n_rays;
     for (int begin = 0; begin < n_rays; begin += tr.chunk_rays) {
@@ -682,6 +690,13 @@ int nfb_train_debug(NfbHandle* h, NfbTrainDebug* out) {
   out->frame_cond = multi ? tr.fcond.get() : nullptr;
   out->ray_sums = (multi && tr.frame_sums_formed) ? tr.raysum.get() : nullptr;
   out->frame_sums = (multi && tr.frame_sums_formed) ? tr.fsum.get() : nullptr;
+  const bool dw = tr.bwd_formed && tr.dw_parts[0] + tr.dw_parts[1] > 0;
+  out->dw_partials = dw ? tr.dw_ws.get() : nullptr;
+  out->dw_slot_floats = dw ? tr.dw_stride : 0;
+  out->dw_parts[0] = dw ? tr.dw_parts[0] : 0;
+  out->dw_parts[1] = dw ? tr.dw_parts[1] : 0;
+  out->dw_pe_only = (dw && tr.dw_pe_only) ? 1 : 0;
+  out->ray_bias_sums = tr.bwd_formed ? tr.bsum.get() : nullptr;
   return NFB_OK;
 }
 

@@ -66,7 +66,8 @@ class NfbTrainDebug(C.Structure):
                 ("tiles_coarse", C.c_int32), ("tiles_fine", C.c_int32), ("rays_per_unit", C.c_int32), ("rays", C.c_void_p),
                 ("dnorm", C.c_void_p), ("rows", C.c_void_p), ("ray_dn", C.c_void_p), ("ray_bg", C.c_void_p),
                 ("n_frames", C.c_int32), ("frame", C.c_void_p), ("frame_table", C.c_void_p * 2), ("frame_cond", C.c_void_p),
-                ("ray_sums", C.c_void_p), ("frame_sums", C.c_void_p)]
+                ("ray_sums", C.c_void_p), ("frame_sums", C.c_void_p), ("dw_partials", C.c_void_p), ("dw_slot_floats", C.c_int32),
+                ("dw_parts", C.c_int32 * 2), ("dw_pe_only", C.c_int32), ("ray_bias_sums", C.c_void_p)]
 
 
 class NfbAdam(C.Structure):

@@ -422,6 +422,18 @@ typedef struct {
   const float* frame_cond;
   const float* ray_sums;
   const float* frame_sums;
+  /* What the parameter-gradient backward summed, NULL / 0 until a backward of this forward has run.  dw_partials = the
+   * weight-gradient partials of the last backward: slot (network 0 parts first, then network 1's) of dw_slot_floats floats
+   * each, filled by the parts that got tiles (part p of a network owns its tiles [p per, (p + 1) per), per = ceil(tiles /
+   * parts)); dw_slot_floats is the accumulator range below the raw-output biases (kAccBRaw, nfb_layout.h) after a full launch,
+   * the compact [dW0 | dW3a | db0 | db3] slot after a PE-only one (dw_pe_only = 1: an input-only backward that formed d latent
+   * or d expression); dw_parts = parts per network of that launch (0, 0 and dw_partials NULL when the backward ran no
+   * weight-gradient launch).  ray_bias_sums [passes][n][4] = each ray's sums of d raw over its samples, unscaled. */
+  const float* dw_partials;
+  int32_t dw_slot_floats;
+  int32_t dw_parts[2];
+  int32_t dw_pe_only;
+  const float* ray_bias_sums;
 } NfbTrainDebug;
 int nfb_train_debug(NfbHandle* h, NfbTrainDebug* out);
 

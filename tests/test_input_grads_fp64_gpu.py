@@ -129,9 +129,11 @@ def check_saved_rays(c, s, tag):
 
 # ---------------------------------------------------------------------------------------------------------------- (b)
 def composite_terms64(c, s, pas, gouts):
-    """float64 dL/d|d| and dL/d background of one pass's compositing, at the kernel's saved sigma inputs, colours, depths."""
+    """float64 dL/d|d|, dL/d background and d raw [n, S, 4] = (dL/d rgb_raw, dL/d sigma_raw) of one pass's compositing, at
+    the kernel's saved sigma inputs, colours, depths: d rgb_raw = dL/dc c (1 - c) from the saved colour c, d sigma_raw through
+    the ReLU of the saved input."""
     z = (s.z_f if pas else s.z_c).double()
-    raw = s.raw[pas].double()
+    raw = s.raw[pas].double().requires_grad_(True)
     dn = s.dnorm.double().requires_grad_(True)
     bg = c.bg.double().requires_grad_(True) if c.bg is not None else None
     col = raw[..., :3] if bg is None else torch.cat((raw[:, :-1, :3], bg[:, None, :]), dim=1)
@@ -152,13 +154,15 @@ def composite_terms64(c, s, pas, gouts):
         outs.append((w[:, -1], gouts[6]))
     loss = sum((o * g.double()).sum() for o, g in outs if g is not None)
     loss.backward()
-    return dn.grad, (bg.grad if bg is not None else None)
+    col = raw.detach()[..., :3]
+    d_raw = torch.cat((raw.grad[..., :3] * col * (1.0 - col), raw.grad[..., 3:]), dim=-1)
+    return dn.grad, (bg.grad if bg is not None else None), d_raw
 
 
 def check_compositing_terms(c, s, t, gouts, tag):
     worst = [0.0, 0.0]
     for pas in range(2 if c.nf else 1):
-        gdn, gbg = composite_terms64(c, s, pas, gouts)
+        gdn, gbg, _ = composite_terms64(c, s, pas, gouts)
         pairs = [("ray_dn", t.ray_dn[pas], gdn)] + ([("ray_bg", t.ray_bg[pas], gbg)] if gbg is not None else [])
         for name, got, ref in pairs:
             assert bool(torch.isfinite(got).all()), (tag, pas, name)

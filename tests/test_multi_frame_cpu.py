@@ -66,9 +66,10 @@ def test_no_global_store_in_the_multi_frame_fast_epilogues(built_lib):
     assert sum(epi) == 0, epi
 
 
-def test_train_debug_struct_matches_header(capi):
+def test_train_debug_struct_matches_header_appended_fields(capi):
     """nerf._capi.NfbTrainDebug declares the fields of include/nfb.h's NfbTrainDebug, in the header's order, at offsets that
-    only grow: a field appended to one but not the other, or two swapped, reads the wrong device pointer."""
+    only grow: a field appended to one but not the other, or two swapped, reads the wrong device pointer.  The last eleven
+    fields are the six multi-frame ones, followed by the five parameter-gradient ones appended after them."""
     h = open(os.path.join(ROOT, "include", "nfb.h")).read()
     body = re.search(r"typedef struct \{([^{}]*)\} NfbTrainDebug;", h).group(1)
     body = re.sub(r"/\*.*?\*/", "", body, flags=re.S)
@@ -84,5 +85,7 @@ def test_train_debug_struct_matches_header(capi):
     assert fields == names
     offsets = [getattr(capi.NfbTrainDebug, f).offset for f in fields]
     assert offsets == sorted(offsets) and len(set(offsets)) == len(offsets)
-    assert fields[-6:] == ["n_frames", "frame", "frame_table", "frame_cond", "ray_sums", "frame_sums"]
+    assert fields[-11:] == ["n_frames", "frame", "frame_table", "frame_cond", "ray_sums", "frame_sums", "dw_partials",
+                            "dw_slot_floats", "dw_parts", "dw_pe_only", "ray_bias_sums"]
     assert C.sizeof(dict(capi.NfbTrainDebug._fields_)["frame_table"]) == 2 * C.sizeof(C.c_void_p)
+    assert C.sizeof(dict(capi.NfbTrainDebug._fields_)["dw_parts"]) == 2 * C.sizeof(C.c_int32)
