@@ -1,6 +1,8 @@
 """Multi-GPU checks of the split `north_star` names (SURVEY.md §8e) on real devices: launched as one torch.distributed.run job
 with one rank per visible GPU (NCCL over NVLink); skipped below 2 devices.  The world_size-2 gloo tests on CPU
-(test_parallel_gloo.py, test_data_parallel_gloo.py) cover the same host logic without GPUs."""
+(test_parallel_gloo.py, test_data_parallel_gloo.py) cover the same host logic without GPUs.  On one GPU,
+test_sharded_fp64_gpu.py plays the ranks in one process: row shards and the drop-in wrapper's shards bit for bit against the
+unsharded call, the sharded training batch's loss gradient, shard gradients, their sum and the regulariser against float64."""
 import os
 import subprocess
 import sys
