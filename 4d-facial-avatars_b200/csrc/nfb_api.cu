@@ -2,6 +2,7 @@
 // translation of the public structs into kernel launches.  No torch, no exceptions across the boundary.
 #include <cuda_runtime.h>
 
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -29,6 +30,9 @@ int cuda_fail(cudaError_t e, const char* where) {
 
 using nfb::DevBuf;
 static_assert(NFB_MAX_FRAMES == nfb::kMaxFrames, "frame bound");
+static_assert(NFB_MAX_STEP_IMAGES == nfb::kMaxStepImages, "image bound");
+static_assert(sizeof(NfbRayMap) == sizeof(nfb::RayMapRec) && offsetof(NfbRayMap, q_out) == offsetof(nfb::RayMapRec, q_out),
+              "NfbRayMap mirror");
 
 struct NfbHandle {
   int device = 0;
@@ -94,6 +98,11 @@ struct NfbHandle {
   DevBuf<nfb::smp::Run> smp_runs;
   DevBuf<nfb::smp::Seg> smp_segs;
   DevBuf<int> smp_first;
+  // nfb_sample_rays_images: per-image copies of the above, and the selected indices
+  DevBuf<nfb::smp::Run> smpi_runs;
+  DevBuf<nfb::smp::Seg> smpi_segs;
+  DevBuf<int> smpi_first;
+  DevBuf<long long> smpi_found;
 };
 
 extern "C" {
@@ -780,6 +789,51 @@ int nfb_sample_rays(NfbHandle* h, const NfbRayMap* map, const double* draws, int
     a.target = g->target; a.bg_out = g->background_out; a.pixel_rc = g->pixel_rc;
   }
   NFB_CUDA(nfb::launch_sample_rays(a, st, &h->launches));
+  return NFB_OK;
+}
+
+int nfb_sample_rays_images(NfbHandle* h, const NfbTrainImages* d, const int32_t* image_index, int K, int n, const double* draws,
+                           int max_rounds, const float* latent_table, const NfbImageBatch* out, void* stream) {
+  if (!h || !d || !image_index || !draws || !latent_table || !out || K < 1 || n < 1 || n > nfb::kSmpMax || max_rounds < 1)
+    return NFB_ERR_INVALID;
+  if (K > NFB_MAX_STEP_IMAGES) return NFB_ERR_UNSUPPORTED;
+  if (!d->maps || !d->poses || !d->expressions || !d->images || d->n_images < 1 || d->height < 1 || d->width < 1 ||
+      (long long)d->height * d->width < n)
+    return NFB_ERR_INVALID;
+  if (out->background && !d->background) return NFB_ERR_INVALID;
+  NFB_CUDA(cudaSetDevice(h->device));
+  cudaStream_t st = static_cast<cudaStream_t>(stream);
+  const size_t hw = (size_t)d->height * d->width;
+  NFB_CUDA(h->smpi_runs.reserve((size_t)K * nfb::smp::kMaxRuns));
+  NFB_CUDA(h->smpi_segs.reserve((size_t)K * nfb::smp::kMaxSegs));
+  NFB_CUDA(h->smpi_found.reserve((size_t)K * n));
+  bool fresh = false;  // a new first-occurrence table starts all INT_MAX (the kernel leaves it so)
+  NFB_CUDA(h->smpi_first.reserve((size_t)K * hw, &fresh));
+  if (fresh) NFB_CUDA(nfb::launch_fill_int(h->smpi_first.get(), (long long)(K * hw), 0x7FFFFFFF, st, &h->launches));
+  nfb::ImageSampleArgs a = {};
+  a.maps = reinterpret_cast<const nfb::RayMapRec*>(d->maps);
+  a.poses = d->poses; a.expr_table = d->expressions; a.images = d->images; a.background = d->background;
+  a.n_images = d->n_images; a.H = d->height; a.W = d->width;
+  a.fx = static_cast<float>(d->intrinsics[0]);
+  a.fy = static_cast<float>(d->intrinsics[1]);
+  a.wcx = static_cast<float>(static_cast<double>(d->width) * d->intrinsics[2]);
+  a.hcy = static_cast<float>(static_cast<double>(d->height) * d->intrinsics[3]);
+  a.image_index = image_index; a.K = K; a.size = n; a.max_rounds = max_rounds; a.draws = draws; a.latent_table = latent_table;
+  a.runs = h->smpi_runs.get(); a.segs = h->smpi_segs.get(); a.first_pos = h->smpi_first.get(); a.found = h->smpi_found.get();
+  a.ray_o = out->ray_origins; a.ray_d = out->ray_directions; a.target = out->target; a.bg_out = out->background;
+  a.pixel_rc = out->pixel_rc; a.indices = out->indices; a.frame = out->frame_index;
+  a.expr_out = out->expressions; a.latent_out = out->latents; a.state = out->state; a.shortfall = out->shortfall;
+  NFB_CUDA(nfb::launch_sample_images(a, st, &h->launches));
+  return NFB_OK;
+}
+
+int nfb_latent_rows_grad(NfbHandle* h, const float* grad_latents, const int32_t* image_index, int K, const float* latent_table, int n_rows,
+                         float* table_grads, float reg_weight, void* stream) {
+  if (!h || !grad_latents || !image_index || !latent_table || !table_grads || K < 1 || n_rows < 1) return NFB_ERR_INVALID;
+  if (K > NFB_MAX_STEP_IMAGES) return NFB_ERR_UNSUPPORTED;
+  NFB_CUDA(cudaSetDevice(h->device));
+  NFB_CUDA(nfb::launch_latent_rows(grad_latents, image_index, K, latent_table, n_rows, table_grads, reg_weight,
+                                   static_cast<cudaStream_t>(stream), &h->launches));
   return NFB_OK;
 }
 

@@ -218,6 +218,44 @@ struct SampleArgs {
 };
 
 cudaError_t launch_sample_rays(const SampleArgs& a, cudaStream_t st, long long* launches);
+
+// Training rays of K images in one launch (nfb_sample_rays_images): block k selects n = size pixels of image image_index[k] as
+// sample_rays_kernel does (draws [K][max_rounds * size], block k reads its own slice) and writes rays k*size.. of the batch.
+constexpr int kMaxStepImages = 64;
+struct RayMapRec { int H, W; int bbox[4]; double q_out, q_in; };  // mirrors NfbRayMap (include/nfb.h)
+struct ImageSampleArgs {
+  // dataset (device tables; images and background may be pinned host memory)
+  const RayMapRec* maps;     // [n_images]
+  const float* poses;        // [n_images][12]
+  const float* expr_table;   // [n_images][kDimExpr]
+  const float* images;       // [n_images][H][W][3]
+  const float* background;   // [H][W][3] or null
+  int n_images, H, W;
+  float fx, fy, wcx, hcy;
+  // this step
+  const int* image_index;    // [K]
+  int K, size, max_rounds;
+  const double* draws;       // [K][max_rounds * size]
+  const float* latent_table; // [n_images][kDimLatent]
+  // per-image scratch: [K][kMaxRuns], [K][kMaxSegs], [K][H * W] (all INT_MAX between calls), [K][size]
+  smp::Run* runs;
+  smp::Seg* segs;
+  int* first_pos;
+  long long* found;
+  // outputs, any may be null: [K * size] rows of the batch, [K] conditioning rows, [K][3] state, [K] running shortfall
+  float *ray_o, *ray_d, *target, *bg_out;
+  int* pixel_rc;
+  long long* indices;
+  int* frame;
+  float *expr_out, *latent_out;
+  int* state;
+  long long* shortfall;
+};
+cudaError_t launch_sample_images(const ImageSampleArgs& a, cudaStream_t st, long long* launches);
+// One launch (nfb_optim.cu): the latent-table rows of the bucket gradient for a step over K images (order: include/nfb.h,
+// nfb_latent_rows_grad).
+cudaError_t launch_latent_rows(const float* grad_latents, const int* image_index, int K, const float* table, int n_rows, float* table_grads,
+                               float reg_w, cudaStream_t st, long long* launches);
 cudaError_t launch_fill_int(int* p, long long n, int v, cudaStream_t st, long long* launches);
 
 }  // namespace nfb

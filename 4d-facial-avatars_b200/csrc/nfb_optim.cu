@@ -147,6 +147,43 @@ cudaError_t launch_adam_dev(float* p, float* g, float* m, float* v, long long n,
   return cudaGetLastError();
 }
 
+// The latent-table rows of the bucket gradient for one step over K images (nfb_latent_rows_grad).  ONE warp, lane c = column c of
+// every row, so each element's sum runs in one fixed order with integer indexing and no atomics:
+//   for k = 0..K-1:  G[img[k]][c] += grad_latents[k][c]                                   (the per-frame d latent)
+//   for k = 0..K-1:  G[img[k]][c] += (reg_w * (1 / sqrt(s))) * T[img[k]][c],  s = sum_c T[img[k]][c]^2
+// each a separately rounded FP32 multiply and add; s is the lanes' squares summed by the xor butterfly (offsets 16, 8, 4, 2, 1);
+// the term is skipped at s == 0 (torch.norm's subgradient at 0) and for reg_w == 0.  A row named twice gets both frames'
+// terms in that order; an index outside [0, n_rows) adds nothing and reads nothing.
+__global__ void __launch_bounds__(32) latent_rows_kernel(const float* __restrict__ glat, const int* __restrict__ img, int K,
+                                                         const float* __restrict__ table, int n_rows, float* __restrict__ tgrad, float reg_w) {
+  const int c = threadIdx.x;
+  for (int k = 0; k < K; ++k) {
+    const int r = img[k];
+    if (r < 0 || r >= n_rows) continue;
+    float* g = tgrad + (size_t)r * kDimLatent + c;
+    *g = __fadd_rn(*g, glat[(size_t)k * kDimLatent + c]);
+  }
+  if (reg_w == 0.f) return;
+  for (int k = 0; k < K; ++k) {
+    const int r = img[k];
+    if (r < 0 || r >= n_rows) continue;
+    const float l = table[(size_t)r * kDimLatent + c];
+    float s = __fmul_rn(l, l);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) s = __fadd_rn(s, __shfl_xor_sync(0xffffffffu, s, o));
+    if (s == 0.f) continue;  // uniform: every lane holds the same s
+    float* g = tgrad + (size_t)r * kDimLatent + c;
+    *g = __fadd_rn(*g, __fmul_rn(__fmul_rn(reg_w, __fdiv_rn(1.f, __fsqrt_rn(s))), l));
+  }
+}
+
+cudaError_t launch_latent_rows(const float* grad_latents, const int* image_index, int K, const float* table, int n_rows, float* table_grads,
+                               float reg_w, cudaStream_t st, long long* launches) {
+  latent_rows_kernel<<<1, kDimLatent, 0, st>>>(grad_latents, image_index, K, table, n_rows, table_grads, reg_w);
+  ++*launches;
+  return cudaGetLastError();
+}
+
 cudaError_t launch_loss_grad(const float* rgb_c, const float* rgb_f, const float* target, int n_rays, long long n_total, float* g_c,
                              float* g_f, float* loss, cudaStream_t st, long long* launches) {
   const int n = 3 * n_rays;

@@ -154,7 +154,8 @@ cudaError_t launch_frame_products(const float* rgb, const float* disp, const flo
 // (ray origin / direction, target colour, background colour) including the reference's index quirk: flat index k addresses the
 // PROBABILITY map row-major (k = row * W + col) but the PIXEL (row = k % H, col = k / H) — coords is built from a transposed
 // meshgrid (:303-316) — so the box of probable pixels is the transposed bounding box.
-// One thread block does the whole selection: the cdf is never materialised (nfb_sampler.h evaluates any entry exactly).
+// One thread block does the whole selection of one image: the cdf is never materialised (nfb_sampler.h evaluates any entry
+// exactly).  sample_rays_kernel selects for one image; sample_images_kernel for K images of a training step, one block each.
 // ================================================================================================
 #include "nfb_sampler.h"
 
@@ -162,7 +163,21 @@ namespace nfb {
 
 constexpr int kSmpThreads = 1024;
 
-__global__ void __launch_bounds__(kSmpThreads, 1) sample_rays_kernel(const SampleArgs a) {
+// One image's selection, run by one thread block of kSmpThreads threads.
+struct SelectArgs {
+  smp::Map map;
+  const double* draws;   // consumed like RandomState.rand: round r takes (size - n_found) values
+  int size, max_rounds;
+  long long* found;      // [size] selected flat indices in selection order
+  smp::Run* runs;
+  smp::Seg* segs;
+  int* first_pos;        // [H * W] scratch, all INT_MAX before and after
+};
+struct SelectState { int n_found, rounds, consumed; };
+
+// numpy's choice loop (nfb_sampler.h) from `resume` ({n_found, rounds, consumed}; null: from the start) until `size` indices are
+// found or max_rounds rounds ran.  Every thread of the block returns the same state.
+__device__ __forceinline__ SelectState select_pixels(const SelectArgs& a, const int* resume) {
   __shared__ long long sorted[kSmpMax];
   __shared__ long long cand[kSmpMax];
   __shared__ int warp_sums[kSmpThreads / 32];
@@ -170,7 +185,7 @@ __global__ void __launch_bounds__(kSmpThreads, 1) sample_rays_kernel(const Sampl
   __shared__ int n_runs_s, n_found_s, consumed_s;
   const int tid = threadIdx.x;
   const long long N = (long long)a.map.H * a.map.W;
-  if (tid == 0) { n_found_s = a.state[0]; consumed_s = a.state[2]; }
+  if (tid == 0) { n_found_s = resume ? resume[0] : 0; consumed_s = resume ? resume[2] : 0; }
   __syncthreads();
   int rounds = 0;
   while (rounds < a.max_rounds && n_found_s < a.size) {
@@ -244,13 +259,35 @@ __global__ void __launch_bounds__(kSmpThreads, 1) sample_rays_kernel(const Sampl
     ++rounds;
     __syncthreads();
   }
-  if (tid == 0) { a.state[0] = n_found_s; a.state[1] += rounds; a.state[2] = consumed_s; }
-  // ---- gathers (train_transformed_rays.py:323-331) for the indices selected so far
-  const int H = a.map.H, W = a.map.W;
-  for (int i = tid; i < n_found_s; i += kSmpThreads) {
-    const long long k = a.found[i];
+  const SelectState r = {n_found_s, rounds, consumed_s};
+  __syncthreads();  // every thread has read the state before a later call may reset it
+  return r;
+}
+
+// Where the gathers of one image go (any output may be null).
+struct GatherArgs {
+  const float* pose;        // [12] camera-to-world 3x4
+  float fx, fy, wcx, hcy;
+  int H, W;
+  const float* image;       // [H, W, 3]
+  const float* background;  // [H, W, 3]
+  float *ray_o, *ray_d, *target, *bg_out;  // [count, 3] each
+  int* pixel_rc;            // [count, 2]
+  long long* indices;       // [count]
+  int* frame;               // [count] <- frame_value
+  int frame_value;
+};
+
+// Gathers (train_transformed_rays.py:323-331) into output slots [0, count): slot i takes found[i] while i < n_found and
+// found[i % n_found] after (an incomplete selection repeats its first pixels).
+__device__ __forceinline__ void gather_pixels(const GatherArgs& a, const long long* found, int n_found, int count) {
+  const int H = a.H, W = a.W;
+  for (int i = threadIdx.x; i < count; i += kSmpThreads) {
+    const long long k = found[i < n_found ? i : i % n_found];
     const int row = (int)(k % H), col = (int)(k / H);  // coords[k]: the transposed-meshgrid quirk
     if (a.pixel_rc) { a.pixel_rc[2 * i] = row; a.pixel_rc[2 * i + 1] = col; }
+    if (a.indices) a.indices[i] = k;
+    if (a.frame) a.frame[i] = a.frame_value;
     if (a.ray_d) {  // get_ray_bundle (nerf_helpers.py:111-122) at pixel (row, col), same FP32 operation order as the render kernels
       const float cx = __fdiv_rn(__fsub_rn((float)col, a.wcx), a.fx);
       const float cy = -__fdiv_rn(__fsub_rn((float)row, a.hcy), a.fy);
@@ -262,6 +299,74 @@ __global__ void __launch_bounds__(kSmpThreads, 1) sample_rays_kernel(const Sampl
     if (a.target) for (int q = 0; q < 3; ++q) a.target[3 * i + q] = a.image[px + q];
     if (a.bg_out) for (int q = 0; q < 3; ++q) a.bg_out[3 * i + q] = a.background[px + q];
   }
+}
+
+__global__ void __launch_bounds__(kSmpThreads, 1) sample_rays_kernel(const SampleArgs a) {
+  const SelectArgs s = {a.map, a.draws, a.size, a.max_rounds, a.found, a.runs, a.segs, a.first_pos};
+  const SelectState r = select_pixels(s, a.state);
+  if (threadIdx.x == 0) { a.state[0] = r.n_found; a.state[1] += r.rounds; a.state[2] = r.consumed; }
+  GatherArgs g = {};
+  g.pose = a.pose; g.fx = a.fx; g.fy = a.fy; g.wcx = a.wcx; g.hcy = a.hcy; g.H = a.map.H; g.W = a.map.W;
+  g.image = a.image; g.background = a.background;
+  g.ray_o = a.ray_o; g.ray_d = a.ray_d; g.target = a.target; g.bg_out = a.bg_out; g.pixel_rc = a.pixel_rc;
+  gather_pixels(g, a.found, r.n_found, r.n_found);
+}
+
+// Several images in one launch, block k = image image_index[k] (see ImageSampleArgs).  Everything per step comes from device
+// memory, so a captured launch samples whatever images the index table names at replay.
+__global__ void __launch_bounds__(kSmpThreads, 1) sample_images_kernel(const ImageSampleArgs a) {
+  const int k = blockIdx.x, tid = threadIdx.x, n = a.size;
+  const int img = a.image_index[k];
+  const size_t slot = (size_t)k * n;
+  bool ok = img >= 0 && img < a.n_images;
+  smp::Map m = {};
+  if (ok) {
+    const RayMapRec r = a.maps[img];
+    m.H = r.H; m.W = r.W; m.b0 = r.bbox[0]; m.b1 = r.bbox[1]; m.b2 = r.bbox[2]; m.b3 = r.bbox[3]; m.q_out = r.q_out; m.q_in = r.q_in;
+    // a map the selection cannot follow reads nothing: the batch's shape, a box inside the frame, positive weights, room for its runs
+    ok = m.H == a.H && m.W == a.W && m.b0 >= 0 && m.b1 <= m.H && m.b2 >= 0 && m.b3 <= m.W && m.q_out > 0.0 && m.q_in > 0.0 &&
+         smp::num_runs(m) <= smp::kMaxRuns;
+  }
+  if (!ok) {  // out-of-range index: NaN rays and rows, frame slot K (out of range for nfb_set_frames of K frames: renders NaN)
+    const float nan = __int_as_float(0x7FC00000);
+    for (int i = tid; i < n; i += kSmpThreads) {
+      for (int q = 0; q < 3; ++q) {
+        if (a.ray_o) a.ray_o[3 * (slot + i) + q] = nan;
+        if (a.ray_d) a.ray_d[3 * (slot + i) + q] = nan;
+        if (a.target) a.target[3 * (slot + i) + q] = nan;
+        if (a.bg_out) a.bg_out[3 * (slot + i) + q] = nan;
+      }
+      if (a.pixel_rc) { a.pixel_rc[2 * (slot + i)] = -1; a.pixel_rc[2 * (slot + i) + 1] = -1; }
+      if (a.indices) a.indices[slot + i] = -1;
+      if (a.frame) a.frame[slot + i] = a.K;
+    }
+    if (a.expr_out) for (int i = tid; i < kDimExpr; i += kSmpThreads) a.expr_out[(size_t)k * kDimExpr + i] = nan;
+    if (a.latent_out) for (int i = tid; i < kDimLatent; i += kSmpThreads) a.latent_out[(size_t)k * kDimLatent + i] = nan;
+    if (tid == 0 && a.state) { a.state[3 * k] = 0; a.state[3 * k + 1] = 0; a.state[3 * k + 2] = 0; }
+    return;
+  }
+  const size_t hw = (size_t)a.H * a.W;
+  const SelectArgs s = {m, a.draws + (size_t)k * a.max_rounds * n, n, a.max_rounds, a.found + slot, a.runs + (size_t)k * smp::kMaxRuns,
+                        a.segs + (size_t)k * smp::kMaxSegs, a.first_pos + k * hw};
+  const SelectState r = select_pixels(s, nullptr);
+  if (tid == 0) {
+    if (a.state) { a.state[3 * k] = r.n_found; a.state[3 * k + 1] = r.rounds; a.state[3 * k + 2] = r.consumed; }
+    if (a.shortfall) a.shortfall[k] += n - r.n_found;  // slot k is this block's alone: no atomic
+  }
+  GatherArgs g = {};
+  g.pose = a.poses + 12 * (size_t)img; g.fx = a.fx; g.fy = a.fy; g.wcx = a.wcx; g.hcy = a.hcy; g.H = a.H; g.W = a.W;
+  g.image = a.images + 3 * hw * img; g.background = a.background;
+  auto at3 = [&](float* p) { return p ? p + 3 * slot : nullptr; };
+  g.ray_o = at3(a.ray_o); g.ray_d = at3(a.ray_d); g.target = at3(a.target); g.bg_out = at3(a.bg_out);
+  g.pixel_rc = a.pixel_rc ? a.pixel_rc + 2 * slot : nullptr;
+  g.indices = a.indices ? a.indices + slot : nullptr;
+  g.frame = a.frame ? a.frame + slot : nullptr;
+  g.frame_value = k;
+  gather_pixels(g, a.found + slot, r.n_found, n);
+  // the conditioning rows nfb_set_frames reads: frame k = (expressions[img], latent_table[img])
+  if (a.expr_out) for (int i = tid; i < kDimExpr; i += kSmpThreads) a.expr_out[(size_t)k * kDimExpr + i] = a.expr_table[(size_t)img * kDimExpr + i];
+  if (a.latent_out)
+    for (int i = tid; i < kDimLatent; i += kSmpThreads) a.latent_out[(size_t)k * kDimLatent + i] = a.latent_table[(size_t)img * kDimLatent + i];
 }
 
 __global__ void fill_int_kernel(int* p, long long n, int v) {
@@ -276,6 +381,12 @@ cudaError_t launch_fill_int(int* p, long long n, int v, cudaStream_t st, long lo
 
 cudaError_t launch_sample_rays(const SampleArgs& a, cudaStream_t st, long long* launches) {
   sample_rays_kernel<<<1, kSmpThreads, 0, st>>>(a);
+  ++*launches;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_sample_images(const ImageSampleArgs& a, cudaStream_t st, long long* launches) {
+  sample_images_kernel<<<a.K, kSmpThreads, 0, st>>>(a);
   ++*launches;
   return cudaGetLastError();
 }

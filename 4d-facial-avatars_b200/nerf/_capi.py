@@ -14,8 +14,10 @@ EXPORTS = ["nfb_version", "nfb_strerror", "nfb_last_cuda_error", "nfb_create", "
            "nfb_set_frame", "nfb_render_forward", "nfb_render_frame_host", "nfb_launch_count", "nfb_host_linspace",
            "nfb_render_forward_train", "nfb_render_backward", "nfb_render_backward_ex", "nfb_train_debug", "nfb_debug_schedule", "nfb_loss_mse_grad",
            "nfb_adam_step", "nfb_adam_step_dev", "nfb_repack", "nfb_frame_products", "nfb_sample_rays", "nfb_host_map_cdf",
-           "nfb_set_frames", "nfb_render_forward_frames", "nfb_render_forward_frames_train", "nfb_render_backward_frames"]
+           "nfb_set_frames", "nfb_render_forward_frames", "nfb_render_forward_frames_train", "nfb_render_backward_frames",
+           "nfb_sample_rays_images", "nfb_latent_rows_grad"]
 NFB_MAX_FRAMES = 1024
+NFB_MAX_STEP_IMAGES = 64
 
 
 class NfbModelDims(C.Structure):
@@ -92,6 +94,18 @@ class NfbRayGather(C.Structure):
                 ("pixel_rc", C.c_void_p)]
 
 
+class NfbTrainImages(C.Structure):
+    _fields_ = [("maps", C.c_void_p), ("poses", C.c_void_p), ("expressions", C.c_void_p), ("images", C.c_void_p),
+                ("background", C.c_void_p), ("n_images", C.c_int32), ("height", C.c_int32), ("width", C.c_int32), ("pad", C.c_int32),
+                ("intrinsics", C.c_double * 4)]
+
+
+class NfbImageBatch(C.Structure):
+    _fields_ = [("ray_origins", C.c_void_p), ("ray_directions", C.c_void_p), ("target", C.c_void_p), ("background", C.c_void_p),
+                ("pixel_rc", C.c_void_p), ("indices", C.c_void_p), ("frame_index", C.c_void_p), ("expressions", C.c_void_p),
+                ("latents", C.c_void_p), ("state", C.c_void_p), ("shortfall", C.c_void_p)]
+
+
 def _load():
     if not os.path.exists(LIB_PATH):
         raise ImportError(f"{LIB_PATH} not found: build it with `python 4d-facial-avatars_b200/build.py` "
@@ -136,13 +150,17 @@ def _load():
     lib.nfb_render_backward_frames.argtypes = [C.c_void_p, C.POINTER(NfbOutGrads), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                                C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p,
                                                C.POINTER(NfbInputGrads), C.c_void_p]
+    lib.nfb_sample_rays_images.argtypes = [C.c_void_p, C.POINTER(NfbTrainImages), C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int,
+                                           C.c_void_p, C.POINTER(NfbImageBatch), C.c_void_p]
+    lib.nfb_latent_rows_grad.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float,
+                                         C.c_void_p]
     lib.nfb_launch_count.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
     lib.nfb_host_linspace.argtypes = [C.POINTER(C.c_float), C.c_int]
     for fn in ("nfb_create", "nfb_destroy", "nfb_load_weights", "nfb_set_frame", "nfb_render_forward",
                "nfb_render_frame_host", "nfb_launch_count", "nfb_host_linspace", "nfb_render_forward_train",
                "nfb_render_backward", "nfb_render_backward_ex", "nfb_train_debug", "nfb_loss_mse_grad", "nfb_adam_step", "nfb_adam_step_dev", "nfb_repack", "nfb_frame_products",
                "nfb_sample_rays", "nfb_host_map_cdf", "nfb_set_frames", "nfb_render_forward_frames",
-               "nfb_render_forward_frames_train", "nfb_render_backward_frames"):
+               "nfb_render_forward_frames_train", "nfb_render_backward_frames", "nfb_sample_rays_images", "nfb_latent_rows_grad"):
         getattr(lib, fn).restype = C.c_int
     return lib
 

@@ -267,6 +267,39 @@ class Renderer:
                                                 _ptr(grad_latent), _stream()), "render_backward")
         self._bwd_keep = keep
 
+    def backward_frames_into(self, out_grads, params_c, params_f, grads_c, grads_f, grad_latents):
+        """nfb_render_backward_frames after a multi-frame training forward, writing straight into caller-owned tensors as
+        backward_into does: parameter gradients into the 26 + 26 views, per-frame d latent into grad_latents [F,32]."""
+        og = capi.NfbOutGrads()
+        keep = []
+        for field, g in zip(("rgb_coarse", "disp_coarse", "acc_coarse", "rgb_fine", "disp_fine", "acc_fine", "w_last"), out_grads):
+            if g is not None:
+                keep.append(g)
+                setattr(og, field, g.data_ptr())
+        arr = lambda ts: (C.c_void_p * 26)(*[(t.data_ptr() if t is not None else None) for t in ts]) if ts is not None else None  # noqa: E731
+        capi.check(capi.lib.nfb_render_backward_frames(self._h, C.byref(og), arr(params_c), arr(params_f), arr(grads_c), arr(grads_f),
+                                                       _ptr(grad_latents), None, None, _stream()), "render_backward_frames")
+        self._bwd_keep = keep
+
+    def sample_images(self, data, image_index, n, draws, max_rounds, latent_table, out):
+        """nfb_sample_rays_images: data = ray_sampler.TrainImages, image_index = int32 CUDA [K], draws = float64 CUDA
+        [K * max_rounds * n], latent_table = [n_images,32] CUDA; out = dict of CUDA tensors named like NfbImageBatch's members
+        (missing keys: not written)."""
+        b = capi.NfbImageBatch()
+        for name, _ in capi.NfbImageBatch._fields_:
+            t = out.get(name)
+            if t is not None:
+                setattr(b, name, t.data_ptr())
+        capi.check(capi.lib.nfb_sample_rays_images(self._h, C.byref(data.desc), _ptr(image_index), image_index.numel(), int(n),
+                                                   _ptr(draws), int(max_rounds), _ptr(latent_table), C.byref(b), _stream()),
+                   "sample_rays_images")
+
+    def latent_rows_grad(self, grad_latents, image_index, table, table_grads, reg_weight):
+        """nfb_latent_rows_grad: table_grads[image_index[k]] += grad_latents[k] in ascending k, then the regulariser terms
+        reg_weight * l / ||l|| in ascending k (all CUDA tensors; image_index int32 [K])."""
+        capi.check(capi.lib.nfb_latent_rows_grad(self._h, _ptr(grad_latents), _ptr(image_index), image_index.numel(), _ptr(table),
+                                                 table.shape[0], _ptr(table_grads), float(reg_weight), _stream()), "latent_rows_grad")
+
     def backward(self, out_grads, params_c, params_f, want_latent=True, want_params=True, inputs=None, frames=False):
         """nfb_render_backward_ex for the last training forward.  out_grads: 7 CUDA tensors or None (rgb_c, disp_c, acc_c,
         rgb_f, disp_f, acc_f, w_last); params_*: the 26 FP32 parameter tensors in PARAM_ORDER (params_f None without a

@@ -59,6 +59,8 @@ class FusedTrainer:
         self._gc = [None if s else g for s, g in zip(skip, self._gviews[:npar])]
         self._gf = [None if s else g for s, g in zip(skip, self._gviews[npar:])] if model_fine is not None else None
         self.loss = torch.zeros(4, device=dev, dtype=torch.float32)
+        # pixels the K-image sampler repeated because an image's selection came up short, per batch slot, since construction
+        self.shortfall = torch.zeros(64, device=dev, dtype=torch.int64)
         self._g_rgb = {}
         self._own_engine()
 
@@ -215,3 +217,181 @@ class FusedTrainer:
         loss = self.gradients(*args, **kwargs)
         self.update()
         return loss
+
+    # ---- steps over rays of several training images (DESIGN.md 8c): sample, gather, fold, forward, loss, backward, latent rows,
+    # Adam and re-pack from K image indices alone
+    def _images_buffers(self, data, k, n):
+        """Per-step buffers of a K-image step (cached per shape: the chunked backward re-reads rays and frame indices)."""
+        key = (k, n, data.background is not None)
+        sb = self._image_bufs.get(key) if hasattr(self, "_image_bufs") else None
+        if sb is None:
+            if not hasattr(self, "_image_bufs"):
+                self._image_bufs = {}
+            N, dev = k * n, self.dev
+            z = lambda *shape, dt=torch.float32: torch.zeros(shape, device=dev, dtype=dt)  # noqa: E731
+            sb = self._image_bufs[key] = dict(
+                img=z(k, dt=torch.int32), ray_origins=z(N, 3), ray_directions=z(N, 3), target=z(N, 3),
+                background=z(N, 3) if data.background is not None else None, frame_index=z(N, dt=torch.int32),
+                expressions=z(k, 76), latents=z(k, 32), state=z(k, 3, dt=torch.int32), shortfall=self.shortfall[:k],
+                glat=z(k, 32), g0=z(N, 3), g1=z(N, 3))
+        return sb
+
+    def _images_sample(self, data, sb, n, draws, max_rounds):
+        self.eng.sample_images(data, sb["img"], n, draws, max_rounds, self.latent_codes, sb)
+
+    def _images_gradients(self, sb, k, n):
+        """Forward, loss and backward of the sampled batch into the flat bucket, then the latent-table rows.  K = 1 takes the
+        single-frame kernels (its regulariser stays in Adam, as in step()); K >= 2 one multi-frame forward and backward."""
+        eng, o = self.eng, self.opts
+        N = k * n
+        noise = self._draw_noise(N)
+        kw = dict(perturb=o["perturb"], noise_std=o["noise_std"], white_bkgd=o["white_bkgd"], background=sb["background"], noise=noise,
+                  precision=o["precision"], train=True)
+        if k == 1:
+            eng.set_frame(sb["expressions"][0], sb["latents"][0])
+            out = eng.render(sb["ray_origins"], sb["ray_directions"], o["near"], o["far"], o["num_coarse"], o["num_fine"], **kw)
+        else:
+            eng.set_frames(sb["expressions"], sb["latents"])
+            out = eng.render(sb["ray_origins"], sb["ray_directions"], o["near"], o["far"], o["num_coarse"], o["num_fine"],
+                             frame_index=sb["frame_index"], **kw)
+        has_fine = o["num_fine"] > 0
+        self.loss.zero_()
+        eng.loss_mse_grad(out["rgb_coarse"], out["rgb_fine"] if has_fine else None, sb["target"], N, sb["g0"],
+                          sb["g1"] if has_fine else None, self.loss)
+        og = (sb["g0"], None, None, sb["g1"] if has_fine else None, None, None, None)
+        if k == 1:
+            eng.backward_into(og, self._pc, self._pf, self._gc, self._gf, sb["glat"][0])
+        else:
+            eng.backward_frames_into(og, self._pc, self._pf, self._gc, self._gf, sb["glat"])
+        eng.latent_rows_grad(sb["glat"], sb["img"], self.latent_codes, self.grads[self.lat_off:].view(-1, 32),
+                             0.0 if k == 1 else self.latent_reg / k)
+        return out
+
+    def _adam_dev_state(self, k, row_ptr=None):
+        """NfbAdamDev for a K-image step: from this trainer's step counter; the regulariser on the row at row_ptr (K = 1) or off
+        (K >= 2: nfb_latent_rows_grad added it)."""
+        from . import _capi as capi
+        reg = k == 1 and self.latent_reg > 0.0
+        st = capi.NfbAdamDev(step=self.iter, pad=0, lr0=self.lr0, decay_factor=self.decay_factor, decay_steps=self.decay_steps,
+                             beta1=self.betas[0], beta2=self.betas[1], eps=self.eps, grad_scale=1.0, reg_weight=self.latent_reg,
+                             table_offset=self.lat_off if reg else -1, row=row_ptr if reg else None, lr_over_bc1=0.0, sqrt_bc2=1.0,
+                             reg_offset=-1)
+        return torch.frombuffer(bytearray(bytes(st)), dtype=torch.uint8).to(self.dev)
+
+    def _check_images(self, data, k, n, world):
+        if world != 1:
+            raise NotImplementedError("steps over several images are single-rank: world must be 1")
+        if not 1 <= k <= 64:
+            raise ValueError("1 <= K <= 64 images per step")
+        if not 1 <= n <= 2048 or n > data.H * data.W:
+            raise ValueError("1 <= n_per_image <= 2048 rays per image (and no more than the frame's pixels)")
+        if data.n_images > self.latent_codes.shape[0]:
+            raise ValueError("the latent table has fewer rows than the training set has images")
+
+    def step_images(self, data, image_index, n_per_image, draws=None, max_rounds=32, world=1):
+        """One optimizer step on n_per_image rays of each of the K images image_index (host ints, repeats allowed; image i
+        conditions on expressions[i] and latent row i).  data: ray_sampler.TrainImages.  draws: float64 CUDA [K * max_rounds * n]
+        (image k consumes slice k as RandomState.rand inside np.random.choice); None: torch.rand on the device.  The loss is
+        mse(rgb_c, t) + mse(rgb_f, t) + (latent_reg / K) * sum_k ||latent[image_index[k]]|| over all K * n rays.  K = 1 is step()
+        on the sampled rays, bit for bit.  Raises RuntimeError, before any gradient is formed, when an image's selection came
+        up short of n distinct pixels within max_rounds rounds.
+        Launches (within the memory budget; +1 the first time the sampler's scratch grows): K = 1: 15 = sample 1, set_frame 1,
+        forward 1, loss 1, backward 7, latent rows 1, Adam 1, re-pack 2; K >= 2: 19 = sample 1, set_frames 1, forward 1, loss 1,
+        backward 10, latent rows 1, Adam 2 (device-side schedule, as in the graph), re-pack 2.  Returns the device tensor
+        [mse_coarse, mse_fine]."""
+        k, n = len(image_index), int(n_per_image)
+        self._check_images(data, k, n, world)
+        if any(not 0 <= int(i) < data.n_images for i in image_index):
+            raise ValueError("image index out of range")
+        sb = self._images_buffers(data, k, n)
+        sb["img"].copy_(torch.tensor([int(i) for i in image_index], dtype=torch.int32))
+        if draws is None:
+            draws = torch.rand(k * max_rounds * n, dtype=torch.float64, device=self.dev)
+        elif draws.numel() < k * max_rounds * n:
+            raise ValueError("draws must hold K * max_rounds * n_per_image values")
+        self._own_engine()
+        self._images_sample(data, sb, n, draws, max_rounds)
+        found = sb["state"][:, 0].cpu()
+        if bool((found < n).any()):
+            short = [(int(image_index[j]), int(found[j])) for j in range(k) if int(found[j]) < n]
+            raise RuntimeError(f"ray sampler: {max_rounds} rounds of draws found fewer than {n} distinct pixels for (image, found) "
+                               f"{short}; raise max_rounds")
+        self._images_gradients(sb, k, n)
+        if k == 1:
+            self._reg_row = int(image_index[0])
+            self.update()
+        else:
+            eng = self.eng
+            st = self._adam_dev_state(k)
+            eng.adam_step_dev(self.params, self.grads, self.exp_avg, self.exp_avg_sq, st)
+            self.iter += 1
+            eng.repack(self._pc, self._pf)
+            eng.mark_synced(self.mc, self.mf)
+            eng.packed_owner = self
+        return self.loss[:2]
+
+    def capture_images(self, data, k, n_per_image, has_background=True, max_rounds=32, device_draws=True, world=1):
+        """Capture a whole K-image step into a CUDA graph: sampler (draws from torch.rand(float64) inside the graph, or with
+        device_draws=False from a static buffer step_images_graph fills), fold, noise, forward, loss, backward, latent rows, Adam
+        with its device-side schedule, re-pack.  Only the K image indices change between replays.  An incomplete selection does
+        not stop the graph: the image's missing slots repeat its first pixels and self.shortfall[k] counts them (include/nfb.h,
+        nfb_sample_rays_images).  Launches per replay: 16 at K = 1, 19 at K >= 2.
+        The graph holds the renderer's device buffers as sized at capture, and they only grow: a later call on the same device
+        that needs more room (more images or rays per step, a larger render with gradients) re-allocates them and leaves this
+        graph pointing at freed memory.  Run the largest step first, or capture again after it."""
+        n = int(n_per_image)
+        self._check_images(data, k, n, world)
+        if has_background != (data.background is not None):
+            raise ValueError("has_background must say whether the training set has a background")
+        dev, eng = self.dev, self.eng
+        sb = dict(self._images_buffers(data, k, n))  # own copies of the per-step buffers: eager steps must not write into them
+        for name, t in list(sb.items()):
+            if t is not None and name != "shortfall":
+                sb[name] = torch.zeros_like(t)
+        sb["idx64"] = torch.zeros(1, device=dev, dtype=torch.int64)
+        sb["draws"] = None if device_draws else torch.zeros(k * max_rounds * n, device=dev, dtype=torch.float64)
+        sb["adam"] = self._adam_dev_state(k, sb["idx64"].data_ptr())
+
+        def body():
+            if k == 1:
+                sb["idx64"].copy_(sb["img"])  # the Adam regulariser's row
+            draws = torch.rand(k * max_rounds * n, dtype=torch.float64, device=dev) if device_draws else sb["draws"]
+            self._images_sample(data, sb, n, draws, max_rounds)
+            return self._images_gradients(sb, k, n), draws
+
+        self._own_engine()
+        sb["img"].copy_(torch.arange(k, dtype=torch.int32) % data.n_images)
+        if not device_draws:
+            sb["draws"].uniform_()
+        body()                      # eager warm-up: sizes the library's buffers (cudaMalloc is not capturable)
+        self.grads.zero_()
+        torch.cuda.synchronize()
+        before = self.shortfall.clone()
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            keep = body()
+            eng.adam_step_dev(self.params, self.grads, self.exp_avg, self.exp_avg_sq, sb["adam"])
+            eng.repack(self._pc, self._pf)
+        self.shortfall.copy_(before)  # the warm-up's selections are not a step's
+        self._igraph = dict(graph=graph, sb=sb, k=k, n=n, max_rounds=max_rounds, keep=keep)
+        return self
+
+    def step_images_graph(self, image_index, draws=None):
+        """One optimizer step by replaying the graph of capture_images: copies the K image indices (host ints, or an int32 CUDA /
+        pinned tensor: no host sync) and, when captured with device_draws=False, the draws, then replays."""
+        g = self._igraph
+        sb = g["sb"]
+        if len(image_index) != g["k"]:
+            raise ValueError(f"the graph was captured for {g['k']} images per step")
+        idx = image_index if torch.is_tensor(image_index) else torch.tensor([int(i) for i in image_index], dtype=torch.int32)
+        sb["img"].copy_(idx, non_blocking=True)
+        if sb["draws"] is not None:
+            if draws is None:
+                raise ValueError("the graph was captured with device_draws=False: pass the draws")
+            sb["draws"].copy_(draws.reshape(-1)[:sb["draws"].numel()], non_blocking=True)
+        self._own_engine()
+        g["graph"].replay()
+        self.iter += 1
+        self.eng.mark_synced(self.mc, self.mf)
+        self.eng.packed_owner = self
+        return self.loss[:2]

@@ -86,6 +86,36 @@ class RaySampler:
         return out
 
 
+class TrainImages:
+    """The training set as nfb_sample_rays_images reads it (NfbTrainImages), built once: the importance map of every image
+    (importance_map above), poses [N,12], expressions [N,76] on the device, and the images [N,H,W,3] FP32 — kept where they are
+    when on the device, otherwise pinned in host memory, from which the sampler reads only the selected pixels.  background:
+    optional [H,W,3], one for the whole set."""
+
+    def __init__(self, images, poses, expressions, bboxs, intrinsics, background=None, p=0.9, device=None):
+        self.dev = device if device is not None else torch.device("cuda", torch.cuda.current_device())
+        n, H, W = images.shape[0], images.shape[1], images.shape[2]
+        if images.shape[3] != 3 or len(bboxs) != n or poses.shape[0] != n or expressions.shape[0] != n:
+            raise ValueError("images [N,H,W,3], poses [N,...], expressions [N,76] and N boxes")
+        self.n_images, self.H, self.W = int(n), int(H), int(W)
+        maps = (capi.NfbRayMap * n)(*[importance_map(H, W, [int(v) for v in bb], p)[0] for bb in bboxs])
+        self.maps = torch.frombuffer(bytearray(bytes(maps)), dtype=torch.uint8).to(self.dev)
+        self.poses = poses.detach().to(device=self.dev, dtype=torch.float32).reshape(n, -1)[:, :12].contiguous()
+        self.expressions = _engine._f32c(expressions, self.dev).reshape(n, 76)
+        self.images = self._keep_in_place(images)
+        self.background = self._keep_in_place(background.reshape(H, W, 3)) if background is not None else None
+        self.intrinsics = [float(v) for v in intrinsics]
+        self.desc = capi.NfbTrainImages(self.maps.data_ptr(), self.poses.data_ptr(), self.expressions.data_ptr(),
+                                        self.images.data_ptr(), self.background.data_ptr() if self.background is not None else None,
+                                        self.n_images, self.H, self.W, 0, (C.c_double * 4)(*self.intrinsics))
+
+    def _keep_in_place(self, t):
+        if t.is_cuda:
+            return t.detach().to(device=self.dev, dtype=torch.float32).contiguous()
+        t = t.detach().to(dtype=torch.float32).contiguous()
+        return t if t.is_pinned() else t.pin_memory()
+
+
 def frame_products(rgb, disparity, w_last, intrinsics, want_disparity=False, like_torch_cpu=False):
     """cast_to_image / torch_normal_map(clean=True) / cast_to_disparity_image of eval_transformed_rays.py (:84-119, :184-198) on
     the device, one launch: [H,W,3] rgb, [H,W] disparity and last-sample weights -> uint8 tensors (rgb, normals [(H-1),(W-1),3],

@@ -33,6 +33,11 @@ extern "C" {
  * call renders and differentiates rays of up to NFB_MAX_FRAMES frames, each ray conditioned on its own frame.  Test this macro. */
 #define NFB_MULTI_FRAME 1
 #define NFB_MAX_FRAMES 1024
+/* Defined when the training-step entries over several images exist (nfb_sample_rays_images, nfb_latent_rows_grad): one step
+ * draws its rays from up to NFB_MAX_STEP_IMAGES training images, reading every per-step input from device memory.  Test this
+ * macro. */
+#define NFB_TRAIN_IMAGES 1
+#define NFB_MAX_STEP_IMAGES 64
 
 typedef struct NfbHandle NfbHandle;
 
@@ -383,6 +388,63 @@ typedef struct {
  * 1 launch (one thread block; the float64 cumulative sum is evaluated exactly without being materialised, csrc/nfb_sampler.h). */
 int nfb_sample_rays(NfbHandle* h, const NfbRayMap* map, const double* draws, int size, int max_rounds, long long* indices,
                     int32_t* state, const NfbRayGather* gather /* nullable */, void* stream);
+/* ---- Training rays from several images per step (NFB_TRAIN_IMAGES) ----
+ * The training set as the sampler reads it, built once: every table holds one row per training image.  `images` and
+ * `background` may be DEVICE memory or pinned HOST memory (read in place through unified addressing: only the selected pixels
+ * are read, so a large FP32 dataset may stay on the host).  The maps must be importance_map's (nerf/ray_sampler.py): height x
+ * width of the batch, the box inside the frame. */
+typedef struct {
+  const NfbRayMap* maps;     /* DEVICE [n_images] */
+  const float* poses;        /* DEVICE [n_images][12] camera-to-world 3x4, row-major */
+  const float* expressions;  /* DEVICE [n_images][76] */
+  const float* images;       /* [n_images][height][width][3] FP32 */
+  const float* background;   /* [height][width][3] FP32 or NULL (one background for the whole set, as the reference loads it) */
+  int32_t n_images, height, width, pad;
+  double intrinsics[4];
+} NfbTrainImages;
+/* What nfb_sample_rays_images writes; every member may be NULL (not written).  Ray k * n + j is ray j of image_index[k]. */
+typedef struct {
+  float* ray_origins;        /* [K * n][3] */
+  float* ray_directions;     /* [K * n][3] */
+  float* target;             /* [K * n][3] */
+  float* background;         /* [K * n][3]; needs data->background */
+  int32_t* pixel_rc;         /* [K * n][2] */
+  long long* indices;        /* [K * n] flat map indices, numpy's order per image */
+  int32_t* frame_index;      /* [K * n] = k: the frame_index of nfb_render_forward_frames[_train] */
+  float* expressions;        /* [K][76] = expressions[image_index[k]]: the expressions of nfb_set_frames */
+  float* latents;            /* [K][32] = latent_table[image_index[k]]: the latents of nfb_set_frames */
+  int32_t* state;            /* [K][3] per image: n_found, rounds run, draws consumed */
+  long long* shortfall;      /* [K] running count: slot k += n - n_found (pixels the selection repeated) */
+} NfbImageBatch;
+/* np.random.choice(H * W, n, replace=False, p=map[image_index[k]]) and the gathers of nfb_sample_rays for K images in ONE launch
+ * (one 1024-thread block per image).  image_index (DEVICE int32 [K], repeats allowed) and draws (DEVICE float64
+ * [K][max_rounds * n]; image k consumes its own slice exactly as nfb_sample_rays consumes `draws`) are read at run time, as is
+ * latent_table ([n_images][32], DEVICE), so a captured launch samples whatever the tables hold at replay.  Per image the indices,
+ * pixel_rc, rays, target and background equal nfb_sample_rays' on that image fed the same draw slice, bit for bit.  The launch
+ * resets its own per-image state (no memset between calls).
+ * Incomplete selection: when max_rounds rounds do not find n distinct pixels of an image (e.g. a tiny box holding most of the
+ * mass), the missing slots j >= n_found repeat the first pixels, slot j taking selected pixel j % n_found, so the batch stays
+ * finite; state[k][0] < n says so, and shortfall[k] adds n - n_found.  A caller that must not train on repeats checks state.
+ * An image index outside [0, n_images), or a map the sampler cannot follow (another shape, a box outside the frame), reads
+ * nothing: that image's rays, target, background and conditioning rows are NaN, its indices and pixel_rc -1 and its frame_index
+ * K, which is out of range for nfb_set_frames of K frames, so those rays render NaN.
+ * Scratch: handle-owned, sized on first use, K * (H * W * 4 B + 708 KiB) (64 MiB of first-occurrence table for 64 images at
+ * 512 x 512).  Errors: NFB_ERR_INVALID for a null handle / data / table / index / draws / out, K, n or max_rounds < 1, n > 2048,
+ * height * width < n, a requested background without one; NFB_ERR_UNSUPPORTED for K > NFB_MAX_STEP_IMAGES.  1 launch (+1 the
+ * first time the scratch grows). */
+int nfb_sample_rays_images(NfbHandle* h, const NfbTrainImages* data, const int32_t* image_index, int K, int n, const double* draws,
+                           int max_rounds, const float* latent_table, const NfbImageBatch* out, void* stream);
+/* The latent-table rows of a flat gradient bucket for a step over K images (what autograd leaves for
+ * mse + mse + reg_weight * sum_k ||latent_table[image_index[k]]||_2 with per-frame conditioning): table_grads ([n_rows][32],
+ * DEVICE) receives, in ascending k, grad_latents[k] (DEVICE [K][32], nfb_render_backward_frames' grad_latents) on row
+ * image_index[k]; then, in ascending k, reg_weight * l / ||l|| with l = latent_table[image_index[k]] (nothing at l == 0, as
+ * torch.norm's subgradient).  Each addition is one FP32 add of one FP32 term: term = (reg_weight * (1 / sqrt(s))) * l, each
+ * operation rounded, s = the sum of the 32 squares in xor-butterfly order (offsets 16, 8, 4, 2, 1).  No atomics: the sums
+ * repeat bit for bit.  Rows not named get nothing; an index outside [0, n_rows) adds nothing.  reg_weight == 0: no
+ * regulariser term.  K in [1, NFB_MAX_STEP_IMAGES].  1 launch. */
+int nfb_latent_rows_grad(NfbHandle* h, const float* grad_latents, const int32_t* image_index, int K, const float* latent_table, int n_rows,
+                         float* table_grads, float reg_weight, void* stream);
+
 /* Host-only test hook of the same arithmetic: out[i] = np.cumsum(p)[ks[i]] (ks[i] == -1: the last entry) for the map with the
  * ascending flat indices zeroed_sorted set to zero.  No CUDA call. */
 int nfb_host_map_cdf(const NfbRayMap* map, const long long* zeroed_sorted, int n_zero, const long long* ks, int n, double* out);
