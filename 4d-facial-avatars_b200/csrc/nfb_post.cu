@@ -182,7 +182,7 @@ __device__ __forceinline__ SelectState select_pixels(const SelectArgs& a, const 
   __shared__ long long cand[kSmpMax];
   __shared__ int warp_sums[kSmpThreads / 32];
   __shared__ double total_s;
-  __shared__ int n_runs_s, n_found_s, consumed_s;
+  __shared__ int n_runs_s, n_segs_s, n_found_s, consumed_s;
   const int tid = threadIdx.x;
   const long long N = (long long)a.map.H * a.map.W;
   if (tid == 0) { n_found_s = resume ? resume[0] : 0; consumed_s = resume ? resume[2] : 0; }
@@ -206,9 +206,13 @@ __device__ __forceinline__ SelectState select_pixels(const SelectArgs& a, const 
       int nr, ns;
       total_s = smp::build_tables(a.map, sorted, n_found, a.runs, nr, a.segs, ns);
       n_runs_s = nr;
+      n_segs_s = ns;
       __threadfence_block();
     }
     __syncthreads();
+    // more segments than the table holds: the selection ends short here, before any search reads an unwritten segment.  No map
+    // of at most kMaxRuns runs gets here (nfb_sampler.h bounds its segments); this keeps the reads inside the tables regardless.
+    if (n_segs_s > smp::kMaxSegs) break;
     const double total = total_s;
     const int n_runs = n_runs_s;
     // ---- searchsorted(cdf / cdf[-1], x, side='right') for this round's draws; first occurrence of every value wins
@@ -362,7 +366,7 @@ __global__ void __launch_bounds__(kSmpThreads, 1) sample_images_kernel(const Ima
   g.indices = a.indices ? a.indices + slot : nullptr;
   g.frame = a.frame ? a.frame + slot : nullptr;
   g.frame_value = k;
-  gather_pixels(g, a.found + slot, r.n_found, n);
+  gather_pixels(g, a.found + slot, r.n_found, r.n_found > 0 ? n : 0);  // nothing selected: nothing to repeat
   // the conditioning rows nfb_set_frames reads: frame k = (expressions[img], latent_table[img])
   if (a.expr_out) for (int i = tid; i < kDimExpr; i += kSmpThreads) a.expr_out[(size_t)k * kDimExpr + i] = a.expr_table[(size_t)img * kDimExpr + i];
   if (a.latent_out)

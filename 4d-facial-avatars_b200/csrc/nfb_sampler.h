@@ -12,6 +12,13 @@
 // s stays inside one binade, every add moves s by the SAME exact multiple d of ulp(s) (the discarded part of c is the same
 // each time) — also when that part is exactly half an ulp, once s sits on an even multiple of ulp (round-half-even keeps it there).  So the partial sums of a run are a short list of exact arithmetic progressions (SEGMENTS), one per
 // binade crossed, and cdf[k] is one multiply-add in exact arithmetic.  Entries zeroed in later rounds only shift the add count.
+// An ABSORBED add (s + c == s: c below half an ulp of s, or exactly half with s on an even multiple) is the case d = 0: s never
+// moves again, so every later add of the run is absorbed too and one segment covers the rest of the run.  (Maps far from the
+// reference's p = 0.9 reach it: p = 1e-12 or 1 - 1e-12 absorbs one of the two constants once the sum nears 1.)
+// Segments per map: a run starts with at most a tie step (odd s -> even) and one progression, and each binade it enters adds at
+// most three (the crossing add, a tie step, a progression), so R runs whose running sum crosses B binades need at most
+// 2 R + 3 B + 1 segments (+1: the first add from s = 0).  A normalised map's sum stays below 2 and no add is below 2^-1074, so
+// B <= 1075 and kMaxRuns runs fit kMaxSegs: 2 * 4096 + 3 * 1075 + 1 = 11,418 <= 16,384.
 #pragma once
 #include <math.h>
 #include <stdint.h>
@@ -73,7 +80,7 @@ NFB_SHD double seq_add(double s, double c, long long t, long long t_base, Seg* s
         d = s1 - s;                           // exact (both multiples of ulp, same binade)
         const double top = ldexp(1.0, e + 1);
         const long long room = (long long)((top - s1) / ulp), step = (long long)(d / ulp);  // exact integers < 2^53
-        k = step > 0 ? room / step : 0;       // further adds that stay <= top
+        k = step > 0 ? room / step : t - done - 1;  // further adds that stay <= top; absorbed (d = 0): all the rest
         if (k > t - done - 1) k = t - done - 1;
         bulk = true;
       }

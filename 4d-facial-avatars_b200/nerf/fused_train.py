@@ -363,10 +363,10 @@ class FusedTrainer:
         sb["img"].copy_(torch.arange(k, dtype=torch.int32) % data.n_images)
         if not device_draws:
             sb["draws"].uniform_()
+        before = self.shortfall.clone()
         body()                      # eager warm-up: sizes the library's buffers (cudaMalloc is not capturable)
         self.grads.zero_()
         torch.cuda.synchronize()
-        before = self.shortfall.clone()
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
             keep = body()

@@ -64,9 +64,9 @@ def test_ray_sampler_matches_numpy_choice(env, H, W, bbox, size, seed):
     rows, cols = expected % H, expected // H
     assert np.array_equal(out["pixel_rc"].cpu().numpy(), np.stack((rows, cols), axis=1))
     ro, rd = O.ray_bundle(H, W, fr["intrinsics"], fr["pose"])
-    if H == W:  # the reference indexes [k % H, k // H] into [H, W] arrays: in range for every k only when H >= W ... square here
-        assert torch.equal(out["ray_directions"].cpu(), rd[rows, cols]) and torch.equal(out["ray_origins"].cpu(), ro[rows, cols])
-        assert torch.equal(out["target"].cpu(), image[rows, cols]) and torch.equal(out["background"].cpu(), bg[rows, cols])
+    # k % H < H and k // H < W for every k < H * W: in range for any H and W
+    assert torch.equal(out["ray_directions"].cpu(), rd[rows, cols]) and torch.equal(out["ray_origins"].cpu(), ro[rows, cols])
+    assert torch.equal(out["target"].cpu(), image[rows, cols]) and torch.equal(out["background"].cpu(), bg[rows, cols])
 
 
 def test_ray_sampler_numpy_lockstep_and_device_rng(env):
