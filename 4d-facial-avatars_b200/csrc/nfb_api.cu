@@ -709,6 +709,18 @@ int nfb_train_debug(NfbHandle* h, NfbTrainDebug* out) {
   return NFB_OK;
 }
 
+int nfb_debug_weights(NfbHandle* h, int net, NfbWeightDebug* out) {
+  if (!h || !out || (net != NFB_NET_COARSE && net != NFB_NET_FINE)) return NFB_ERR_INVALID;
+  const nfb::NetBuffers& nb = h->net[net];
+  if (!nb.loaded) return NFB_ERR_STATE;
+  out->x1 = nb.stream_x1.get(); out->x3 = nb.stream_x3.get(); out->bwd = nb.stream_bwd.get();
+  out->w6 = nb.w6.get(); out->b6 = nb.b6.get(); out->bias_static = nb.bias_static.get(); out->bias_frame = nb.bias_frame.get();
+  out->w0c = nb.w0c.get(); out->w3c = nb.w3c.get(); out->wd0b_t = nb.wd0b_t.get();
+  out->x1_bytes = nfb::kStreamBytesX1; out->x3_bytes = nfb::kStreamBytesX3; out->bwd_bytes = nfb::kBwdStreamBytes;
+  out->bias_floats = nfb::kBiasFloats;
+  return NFB_OK;
+}
+
 int nfb_render_frame_host(NfbHandle* h, const float pose[12], const double intrinsics[4], int height, int width, int row_begin,
                           int rows, float near_, float far_, const float* expression_host, const float* latent_host,
                           const float* background_host, const NfbSampling* sm, float* out_host, void* stream) {

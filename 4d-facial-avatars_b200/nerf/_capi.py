@@ -15,7 +15,7 @@ EXPORTS = ["nfb_version", "nfb_strerror", "nfb_last_cuda_error", "nfb_create", "
            "nfb_render_forward_train", "nfb_render_backward", "nfb_render_backward_ex", "nfb_train_debug", "nfb_debug_schedule", "nfb_loss_mse_grad",
            "nfb_adam_step", "nfb_adam_step_dev", "nfb_repack", "nfb_frame_products", "nfb_sample_rays", "nfb_host_map_cdf",
            "nfb_set_frames", "nfb_render_forward_frames", "nfb_render_forward_frames_train", "nfb_render_backward_frames",
-           "nfb_sample_rays_images", "nfb_latent_rows_grad"]
+           "nfb_sample_rays_images", "nfb_latent_rows_grad", "nfb_debug_weights"]
 NFB_MAX_FRAMES = 1024
 NFB_MAX_STEP_IMAGES = 64
 
@@ -70,6 +70,13 @@ class NfbTrainDebug(C.Structure):
                 ("n_frames", C.c_int32), ("frame", C.c_void_p), ("frame_table", C.c_void_p * 2), ("frame_cond", C.c_void_p),
                 ("ray_sums", C.c_void_p), ("frame_sums", C.c_void_p), ("dw_partials", C.c_void_p), ("dw_slot_floats", C.c_int32),
                 ("dw_parts", C.c_int32 * 2), ("dw_pe_only", C.c_int32), ("ray_bias_sums", C.c_void_p)]
+
+
+class NfbWeightDebug(C.Structure):
+    _fields_ = [("x1", C.c_void_p), ("x3", C.c_void_p), ("bwd", C.c_void_p), ("w6", C.c_void_p), ("b6", C.c_void_p),
+                ("bias_static", C.c_void_p), ("bias_frame", C.c_void_p), ("w0c", C.c_void_p), ("w3c", C.c_void_p),
+                ("wd0b_t", C.c_void_p), ("x1_bytes", C.c_int64), ("x3_bytes", C.c_int64), ("bwd_bytes", C.c_int64),
+                ("bias_floats", C.c_int32)]
 
 
 class NfbAdam(C.Structure):
@@ -132,6 +139,7 @@ def _load():
                                            C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.c_void_p, C.POINTER(NfbInputGrads),
                                            C.c_void_p]
     lib.nfb_train_debug.argtypes = [C.c_void_p, C.POINTER(NfbTrainDebug)]
+    lib.nfb_debug_weights.argtypes = [C.c_void_p, C.c_int, C.POINTER(NfbWeightDebug)]
     lib.nfb_loss_mse_grad.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p]
     lib.nfb_adam_step.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_longlong, C.POINTER(NfbAdam), C.c_void_p]
@@ -160,7 +168,8 @@ def _load():
                "nfb_render_frame_host", "nfb_launch_count", "nfb_host_linspace", "nfb_render_forward_train",
                "nfb_render_backward", "nfb_render_backward_ex", "nfb_train_debug", "nfb_loss_mse_grad", "nfb_adam_step", "nfb_adam_step_dev", "nfb_repack", "nfb_frame_products",
                "nfb_sample_rays", "nfb_host_map_cdf", "nfb_set_frames", "nfb_render_forward_frames",
-               "nfb_render_forward_frames_train", "nfb_render_backward_frames", "nfb_sample_rays_images", "nfb_latent_rows_grad"):
+               "nfb_render_forward_frames_train", "nfb_render_backward_frames", "nfb_sample_rays_images", "nfb_latent_rows_grad",
+               "nfb_debug_weights"):
         getattr(lib, fn).restype = C.c_int
     return lib
 

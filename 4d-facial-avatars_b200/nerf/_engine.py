@@ -371,6 +371,12 @@ class Renderer:
         capi.check(capi.lib.nfb_train_debug(self._h, C.byref(d)), "train_debug")
         return d
 
+    def weights_debug(self, net):
+        """nfb_debug_weights: device pointers and sizes of network `net`'s packed weight buffers (an NfbWeightDebug)."""
+        d = capi.NfbWeightDebug()
+        capi.check(capi.lib.nfb_debug_weights(self._h, int(net), C.byref(d)), "debug_weights")
+        return d
+
     def render_camera(self, pose, intrinsics, height, width, row_begin, rows, near, far, num_coarse, num_fine,
                       background=None, out=None, precision=None, white_bkgd=False, prof=None, debug=False):
         """Deterministic render of image rows [row_begin, row_begin+rows) with in-kernel ray generation

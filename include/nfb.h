@@ -342,7 +342,8 @@ int nfb_adam_step_dev(NfbHandle* h, float* params, float* grads, float* exp_avg,
                       void* stream);
 
 /* nfb_load_weights for both networks at once (params_fine may be NULL), two launches (FP64 fold, pack): the re-pack after an
- * optimizer step. */
+ * optimizer step.  With params_fine NULL only network 0 is re-packed: network 1's buffers keep their bytes (and a network 1
+ * loaded before stays loaded), so a fine network loaded earlier renders with its earlier weights. */
 int nfb_repack(NfbHandle* h, const float* const params_coarse[26], const float* const params_fine[26], void* stream);
 
 /* ---- The steps either side of the path (SURVEY.md 8f ranks 3, 4) ----
@@ -498,6 +499,23 @@ typedef struct {
   const float* ray_bias_sums;
 } NfbTrainDebug;
 int nfb_train_debug(NfbHandle* h, NfbTrainDebug* out);
+
+/* Test hook: device pointers of the packed weights of network `net` (NFB_NET_COARSE / NFB_NET_FINE), the buffers every kernel
+ * reads its weights from, as nfb_load_weights / nfb_repack wrote them (layout: DESIGN.md §3, nfb_layout.h).  x1 [x1_bytes]: the
+ * FP16 forward stream of fast mode; x3 [x3_bytes]: exact mode's stream, per unit the hi unit then the lo unit; bwd [bwd_bytes]:
+ * the transposed FP16 stream of the backward chain; w6 [144][256] and b6 [144]: the folded layers_dir.0[:, :256] . fc_feat
+ * (rows 0..127) and fc_alpha . fc_feat (row 128), rows 129..143 zero; bias_static [bias_floats]: the bias block; bias_frame
+ * [bias_floats]: the bias block with the frame of the last nfb_set_frame folded into the rows of steps 0 and 3 (unwritten before
+ * the first); w0c / w3c [256][108]: the conditioning columns of layers_xyz.0 / .3; wd0b_t [24][128]: the direction columns of
+ * layers_dir.0, transposed.  Valid until the handle is destroyed.  No CUDA call.  NFB_ERR_STATE if that network is not
+ * loaded. */
+typedef struct {
+  const uint8_t *x1, *x3, *bwd;
+  const float *w6, *b6, *bias_static, *bias_frame, *w0c, *w3c, *wd0b_t;
+  int64_t x1_bytes, x3_bytes, bwd_bytes;
+  int32_t bias_floats;
+} NfbWeightDebug;
+int nfb_debug_weights(NfbHandle* h, int net, NfbWeightDebug* out);
 
 /* End-to-end convenience for callers with HOST buffers (bench.py's e2e leg, C/C++ users): copies
  * expression/latent/background to the device, renders image rows [row_begin,row_begin+rows) of a
