@@ -6,6 +6,9 @@
 //     cast_to_disparity_image (:195-198: min/max normalise).  The FP32 operation order of the torch expressions is kept (every
 //     torch op rounds once; torch.cross contracts a1*b2 - a2*b1 into fma(a1, b2, -(a2*b1)) on both of its back ends; torch's CPU
 //     and CUDA back ends differ in two roundings — selectable, see ProductArgs), so the bytes equal the reference function's.
+//     Also at the edges (tests/test_frame_products_gpu.py, every pixel): NaN of either sign, +-inf, +-0, subnormal and constant
+//     disparities, w_last at the FP32 neighbours of 0.22, rgb outside [0, 1], frames from 2x2 to past one grid-stride sweep.
+//     NaN and +-inf become the byte the reference's host-side conversion gives (to_u8).
 //   * ray sampler (before the path): see the second half of this file.
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -32,8 +35,9 @@ struct ProductArgs {
   uint8_t* normals_u8;  // [H - 1, W - 1, 3] or null
   uint32_t* minmax;     // [2] ordered keys of min / max disparity (null: no disparity image requested)
   // Where torch's two back ends round differently (measured on this image, torch 2.11): the CUDA back end divides a tensor by a
-  // host scalar as a multiplication by its FP32 reciprocal (".../ fx") and sums the three squared components as (x2 + z2) + y2;
-  // the CPU back end divides and sums (x2 + y2) + z2.
+  // host scalar as a multiplication by the scalar's reciprocal (".../ fx"), taken in double and rounded to FP32 — not the
+  // reciprocal of the FP32 fx, which differs when fx is not an FP32 — and sums the three squared components as (x2 + z2) + y2;
+  // the CPU back end divides by the FP32 fx and sums (x2 + y2) + z2.
   int like_cpu;
   float inv_fx, inv_fy;
 };
@@ -45,8 +49,12 @@ __device__ __forceinline__ void back_project(const ProductArgs& a, int r, int c,
   y = -(a.like_cpu ? __fdiv_rn(v, a.fy) : __fmul_rn(v, a.inv_fy));
 }
 __device__ __forceinline__ float cross_term(float a1, float b2, float a2, float b1) { return __fmaf_rn(a1, b2, -__fmul_rn(a2, b1)); }
-__device__ __forceinline__ uint8_t to_u8(float v) {  // numpy astype('uint8') / torch .byte() of a value in [0, 255]: truncate
-  return (uint8_t)(int)v;                              // NaN (0/0 normal of a degenerate patch) -> 0
+// numpy astype('uint8') / torch .byte() as an x86-64 host computes them: truncate to int32 (cvttss2si: NaN, +-inf and values
+// outside the int32 range give 0x80000000), keep the low byte.  A value in [0, 256) truncates.  NaN (0/0: the normal of a
+// degenerate patch, any NaN disparity or colour) gives 0, and so does +-inf (a normal whose squared components underflow to a
+// zero length while a component does not) — where the device's saturating conversion would give 255 for +inf.
+__device__ __forceinline__ uint8_t to_u8(float v) {
+  return fabsf(v) < 2147483648.f ? (uint8_t)__float2int_rz(v) : (uint8_t)0;
 }
 
 __global__ void __launch_bounds__(256) frame_products_kernel(const ProductArgs a) {
@@ -121,8 +129,8 @@ cudaError_t launch_frame_products(const float* rgb, const float* disp, const flo
                                   cudaStream_t st, long long* launches) {
   ProductArgs a;
   a.like_cpu = like_torch_cpu;
-  a.inv_fx = 1.0f / (float)intr[0];
-  a.inv_fy = 1.0f / (float)intr[1];
+  a.inv_fx = (float)(1.0 / intr[0]);
+  a.inv_fy = (float)(1.0 / intr[1]);
   a.rgb = rgb; a.disp = disp; a.w_last = w_last; a.H = H; a.W = W;
   a.fx = (float)intr[0]; a.fy = (float)intr[1];
   a.cx = (float)(intr[2] * (double)H);  // the reference multiplies by depthmap.shape[0] for x and shape[1] for y (square frames)

@@ -353,8 +353,8 @@ int nfb_repack(NfbHandle* h, const float* const params_coarse[26], const float* 
  * clean=True) (:84-119, called at :469 with disp_fine and weights_fine[:, -1]), disparity_u8 = cast_to_disparity_image (:195-198).
  * Any output (and w_last) may be NULL.  The bytes equal the reference functions' (same FP32 operation order).  torch's two back
  * ends round torch_normal_map differently in two places: CUDA turns ".../ fx" (division by a host scalar) into a multiplication by
- * the FP32 reciprocal and sums the normal's squared components as (x2 + z2) + y2; the CPU divides and sums (x2 + y2) + z2.  The
- * default follows the CUDA back end — what the eval script computes on a GPU; NFB_PRODUCTS_LIKE_TORCH_CPU follows the CPU back
+ * the reciprocal (1 / fx in double, rounded to FP32) and sums the normal's squared components as (x2 + z2) + y2; the CPU divides
+ * and sums (x2 + y2) + z2.  The default follows the CUDA back end — what the eval script computes on a GPU; NFB_PRODUCTS_LIKE_TORCH_CPU follows the CPU back
  * end (the two differ by one level in ~2e-4 of the bytes).  Square frames only for the normal map (the reference's expression
  * does not broadcast otherwise).  1 launch (+1 for disparity_u8). */
 enum { NFB_PRODUCTS_LIKE_TORCH_CPU = 1 };

@@ -27,9 +27,9 @@ def reference_root(staged_only=False):
     return None
 
 
-def script_path(name):
+def script_path(name, staged_only=False):
     """Absolute path of train_transformed_rays.py / eval_transformed_rays.py / a config YAML in the reference tree."""
-    r = reference_root()
+    r = reference_root(staged_only)
     return os.path.join(r, NP, name) if r else None
 
 
@@ -103,15 +103,16 @@ def reference_renderer(ref, frame, params_c, params_f, H, W, rows, cols, nc, nf,
     return run, h * w
 
 
-def load_eval_script(name="eval_transformed_rays.py"):
+def load_eval_script(name="eval_transformed_rays.py", staged_only=False):
     """The reference's eval script as a module WITHOUT running main(): gives tests the unmodified post-render functions
     (torch_normal_map :84-119, cast_to_image :184-192, cast_to_disparity_image :195-198).  matplotlib / imageio get inert
-    stand-ins when absent; `from nerf import ...` inside the script resolves to the reference package for the import only."""
+    stand-ins when absent; `from nerf import ...` inside the script resolves to the reference package for the import only.
+    `staged_only=True` takes the script and the package from the staged copy alone (None when nothing is staged)."""
     key = "nerf_reference_eval_script"
     if key in sys.modules:
         return sys.modules[key]
-    ref = load_reference()
-    path = script_path(name)
+    ref = load_reference(staged_only=staged_only)
+    path = script_path(name, staged_only)
     if ref is None or not path or not os.path.exists(path):
         return None
 
