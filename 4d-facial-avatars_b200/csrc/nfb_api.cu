@@ -40,6 +40,9 @@ struct NfbHandle {
   nfb::NetBuffers net[2];
   bool frame_set = false;
   long long launches = 0;
+  // nfb_buffer_epoch = frees + tr.frees: the buffers a training step's launches take an address of count their re-allocations
+  // into one of the two (the linspace tables count every refill for another n)
+  long long frees = 0;
   // cached torch.linspace(0,1,n) tables on the device, and the n each was filled for
   DevBuf<float> lin_c, lin_f;
   int lin_c_n = 0, lin_f_n = 0;
@@ -47,23 +50,24 @@ struct NfbHandle {
   DevBuf<float> d_expr, d_latent, d_bg, d_out;
   // training state: what nfb_render_forward_train saved for nfb_render_backward (grow-only buffers)
   struct Train {
-    DevBuf<uint8_t> rec;                                // per-tile activation records (nfb_layout.h kRec*)
-    DevBuf<float> draw;                                 // [tiles][128][4]
-    DevBuf<float> z_c, raw_c, z_f, raw_f, dnorm;
-    DevBuf<float> acc[2];                               // kAccFloats each
+    long long frees = 0;
+    DevBuf<uint8_t> rec{&frees};                        // per-tile activation records (nfb_layout.h kRec*)
+    DevBuf<float> draw{&frees};                         // [tiles][128][4]
+    DevBuf<float> z_c{&frees}, raw_c{&frees}, z_f{&frees}, raw_f{&frees}, dnorm{&frees};
+    DevBuf<float> acc[2]{DevBuf<float>(&frees), DevBuf<float>(&frees)};  // kAccFloats each
     // what the backward sums in a fixed order instead of with atomics: per-ray bias sums of the compositing backward
     // ([pass][ray][4]) and one weight-gradient partial per (network, part) (nfb::dw_workspace_floats)
-    DevBuf<float> bsum, dw_ws;
-    DevBuf<float> scal;                                 // [0] scale, [1] 1/scale, [2] max |d raw| (bits)
-    DevBuf<float> cond;                                 // [108] conditioning vector of the frame the forward rendered
+    DevBuf<float> bsum{&frees}, dw_ws{&frees};
+    DevBuf<float> scal{&frees};                         // [0] scale, [1] 1/scale, [2] max |d raw| (bits)
+    DevBuf<float> cond{&frees};                         // [108] conditioning vector of the frame the forward rendered
     nfb::TileGeom geom = {};                            // of the whole forward call
     int has_bg = 0, white_bkgd = 0;
     bool valid = false;
     // for input gradients (nfb_render_backward_ex): the forward's rays (copied unless chunked), per-row / per-ray scratch
     bool has_rays = false, has_dir_z = false;
-    DevBuf<float> ray;                                  // [n][7] = (o, d, v0), written by the SAVE forward
-    DevBuf<float> rows;                                 // [tiles][128][4]
-    DevBuf<float> ray_dn, ray_bg;
+    DevBuf<float> ray{&frees};                          // [n][7] = (o, d, v0), written by the SAVE forward
+    DevBuf<float> rows{&frees};                         // [tiles][128][4]
+    DevBuf<float> ray_dn{&frees}, ray_bg{&frees};
     // what the last one-launch backward of this forward left in ray_dn / ray_bg, rows and raysum / fsum (nfb_train_debug)
     bool per_ray_formed = false, rows_formed = false, frame_sums_formed = false;
     // ... and in dw_ws / bsum: the split and slot size of its weight-gradient launch (dw_parts 0, 0: none ran)
@@ -75,23 +79,23 @@ struct NfbHandle {
     nfb::RenderParams full;      // the forward call's parameters (pointers into caller memory)
     // handle-owned state `full` points at, copied at the forward: the folded per-frame biases (nfb_set_frame overwrites
     // bias_frame in place) and the linspace tables when they came from the handle's cache (a later sample count replaces it)
-    DevBuf<float> bias[2];
-    DevBuf<float> lin_c, lin_f;
+    DevBuf<float> bias[2]{DevBuf<float>(&frees), DevBuf<float>(&frees)};
+    DevBuf<float> lin_c{&frees}, lin_f{&frees};
     int chunk_rays = 0, precision = 0;
-    DevBuf<float> scratch_out;   // [11 * chunk_rays] outputs of the re-run forwards (discarded)
+    DevBuf<float> scratch_out{&frees};   // [11 * chunk_rays] outputs of the re-run forwards (discarded)
     // multi-frame forward (nfb_render_forward_frames_train): the frame table and conditioning vectors it rendered with (copied,
     // as bias / cond are), the frame slot of every ray (written by the forward), and the backward's per-ray / per-frame sums
     bool multi = false;
     int n_frames = 0;
-    DevBuf<float> ftab[2], fcond;
-    DevBuf<int> frame;
-    DevBuf<float> raysum, fsum;
+    DevBuf<float> ftab[2]{DevBuf<float>(&frees), DevBuf<float>(&frees)}, fcond{&frees};
+    DevBuf<int> frame{&frees};
+    DevBuf<float> raysum{&frees}, fsum{&frees};
   } tr;
   size_t train_budget = 0;       // bytes the per-tile records of one launch may take (0: not decided yet)
   DevBuf<float> cond;            // [108] = [expression / 3 ; latent] of the current frame
   // nfb_set_frames: per network [n_frames + 1][kFrameRows] folded rows (the last NaN), and [n_frames][108] conditioning vectors;
   // independent of the single frame above
-  DevBuf<float> ftab[2], fcond;
+  DevBuf<float> ftab[2]{DevBuf<float>(&frees), DevBuf<float>(&frees)}, fcond{&frees};
   int n_frames = 0;
   // scratch of the steps either side of the path
   DevBuf<uint32_t> minmax;       // disparity-image min / max keys
@@ -99,10 +103,10 @@ struct NfbHandle {
   DevBuf<nfb::smp::Seg> smp_segs;
   DevBuf<int> smp_first;
   // nfb_sample_rays_images: per-image copies of the above, and the selected indices
-  DevBuf<nfb::smp::Run> smpi_runs;
-  DevBuf<nfb::smp::Seg> smpi_segs;
-  DevBuf<int> smpi_first;
-  DevBuf<long long> smpi_found;
+  DevBuf<nfb::smp::Run> smpi_runs{&frees};
+  DevBuf<nfb::smp::Seg> smpi_segs{&frees};
+  DevBuf<int> smpi_first{&frees};
+  DevBuf<long long> smpi_found{&frees};
 };
 
 extern "C" {
@@ -277,10 +281,11 @@ int nfb_set_frames(NfbHandle* h, const float* expressions, const float* latents,
   return NFB_OK;
 }
 
-static int ensure_linspace(DevBuf<float>& buf, int* cached_n, int n, cudaStream_t st) {
+static int ensure_linspace(DevBuf<float>& buf, int* cached_n, int n, long long* frees, cudaStream_t st) {
   if (*cached_n == n && buf.get()) return NFB_OK;
   std::vector<float> host(n);
   nfb_host_linspace(host.data(), n);
+  if (*cached_n) ++*frees;  // a table a graph may have captured now holds other values
   *cached_n = 0;
   NFB_CUDA(buf.reserve((size_t)n));
   // pageable source: the runtime stages it before returning, so `host` may die afterwards
@@ -368,14 +373,14 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
   p.white_bkgd = sm->white_background ? 1 : 0;
   if (sm->t_coarse) p.t_coarse = sm->t_coarse;
   else {
-    int rc = ensure_linspace(h->lin_c, &h->lin_c_n, nc, st);
+    int rc = ensure_linspace(h->lin_c, &h->lin_c_n, nc, &h->frees, st);
     if (rc) return rc;
     p.t_coarse = h->lin_c.get();
   }
   if (nf > 0) {
     if (sm->u_fine) p.u_fine = sm->u_fine;
     else {
-      int rc = ensure_linspace(h->lin_f, &h->lin_f_n, nf, st);
+      int rc = ensure_linspace(h->lin_f, &h->lin_f_n, nf, &h->frees, st);
       if (rc) return rc;
       p.u_fine = h->lin_f.get();
     }
@@ -887,6 +892,12 @@ int nfb_debug_schedule(int which, int index, uint32_t* out, int out_words) {
     case 4: return index < 0 ? 1 : nfb::debug_dw_split(out);  // in/out: {num_sms, tiles 0, tiles 1} -> {parts0, parts1, groups}
     default: return -1;
   }
+}
+
+int nfb_buffer_epoch(NfbHandle* h, long long* out) {
+  if (!h || !out) return NFB_ERR_INVALID;
+  *out = h->frees + h->tr.frees;
+  return NFB_OK;
 }
 
 int nfb_launch_count(NfbHandle* h, long long* out) {

@@ -10,11 +10,13 @@
 
 namespace nfb {
 
-// A device allocation its owner frees.  Grow-only; what it held is gone once it has grown.
+// A device allocation its owner frees.  Grow-only; what it held is gone once it has grown.  Built with a counter, it adds one to
+// it every time it frees a live allocation to grow (nfb_buffer_epoch: addresses taken before are stale).
 template <class T>
 class DevBuf {
  public:
   DevBuf() = default;
+  explicit DevBuf(long long* frees) : frees_(frees) {}
   DevBuf(const DevBuf&) = delete;
   DevBuf& operator=(const DevBuf&) = delete;
   ~DevBuf() { cudaFree(p_); }
@@ -23,6 +25,7 @@ class DevBuf {
   cudaError_t reserve(size_t n, bool* grew = nullptr) {
     if (grew) *grew = false;
     if (p_ && cap_ >= n) return cudaSuccess;
+    if (p_ && frees_) ++*frees_;
     cudaError_t e = p_ ? cudaFree(p_) : cudaSuccess;
     p_ = nullptr; cap_ = 0;
     if (e == cudaSuccess) e = cudaMalloc(reinterpret_cast<void**>(&p_), n * sizeof(T));
@@ -35,6 +38,7 @@ class DevBuf {
  private:
   T* p_ = nullptr;
   size_t cap_ = 0;
+  long long* frees_ = nullptr;
 };
 
 // Device buffers of one loaded network.

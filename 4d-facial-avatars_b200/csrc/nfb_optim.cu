@@ -5,6 +5,9 @@
 // re-pack that follows is fold_feat_kernel + repack_kernel (nfb_pack.cu), two more launches.
 #include <cuda_runtime.h>
 
+#include <cstddef>
+
+#include "../../include/nfb.h"
 #include "nfb_internal.h"
 #include "nfb_layout.h"
 
@@ -53,66 +56,13 @@ __global__ void __launch_bounds__(kLossThreads) loss_grad_kernel(const float* __
 // Latent-code regulariser (train_transformed_rays.py:369-372,386: 10 * 0.0005 * ||latent||_2 on the frame's row of the
 // table): its gradient reg_w * l / ||l|| (0 at l == 0, as torch.norm's backward gives) is added to that row's gradient here,
 // after any all-reduce, so every rank adds it exactly once.
-struct AdamArgs {
-  float* p; float* g; float* m; float* v;
-  long long n;
-  float lr_over_bc1, sqrt_bc2, b1, b2, eps, grad_scale;
-  long long reg_off;   // float offset of the regularised 32-vector inside the bucket; < 0: none
-  float reg_w;
-};
-__global__ void __launch_bounds__(256) adam_kernel(const AdamArgs a) {
+// The element-wise update both Adam kernels run over [0, n), grid-strided, from this step's scalars: one body, so the host-scalar
+// and the device-state entries cannot drift apart.
+__device__ __forceinline__ void adam_update(float* __restrict__ P, float* __restrict__ G, float* __restrict__ M, float* __restrict__ V,
+                                            long long n, float lr_over_bc1, float sqrt_bc2, float b1, float b2, float eps, float gs,
+                                            long long reg_off, float reg_w) {
   __shared__ float reg_inv_norm;
-  if (a.reg_off >= 0) {  // every block that touches the row needs 1 / ||l||: 32 values, recomputed per block (cheap, uniform)
-    if (threadIdx.x < 32) {
-      const float l = a.p[a.reg_off + threadIdx.x];
-      float s = l * l;
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) s += __shfl_xor_sync(0xffffffffu, s, o);
-      if (threadIdx.x == 0) reg_inv_norm = s > 0.f ? rsqrtf(s) : 0.f;
-    }
-    __syncthreads();
-  }
-  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < a.n; i += (long long)gridDim.x * blockDim.x) {
-    float g = a.g[i] * a.grad_scale;
-    const float p = a.p[i];
-    if (a.reg_off >= 0 && i >= a.reg_off && i < a.reg_off + kDimLatent) g = fmaf(a.reg_w * reg_inv_norm, p, g);
-    float m = a.m[i], v = a.v[i];
-    m = fmaf(g - m, 1.f - a.b1, m);
-    v = fmaf(g * g, 1.f - a.b2, v * a.b2);
-    const float denom = sqrtf(v) / a.sqrt_bc2 + a.eps;
-    a.p[i] = p - a.lr_over_bc1 * (m / denom);
-    a.m[i] = m;
-    a.v[i] = v;
-    a.g[i] = 0.f;
-  }
-}
-
-// Graph-capturable variant: the step counter, the learning-rate schedule and the regularised row live in DEVICE memory, so one
-// captured CUDA graph replays every iteration.  adam_prepare_kernel (1 thread) advances the step and derives this step's
-// scalars exactly as launch_adam does on the host (double precision); adam_dev_kernel is adam_kernel reading them.
-struct AdamDevState {  // mirrors NfbAdamDev (include/nfb.h)
-  int step, pad;
-  float lr0, decay_factor, decay_steps, b1, b2, eps, grad_scale, reg_w;
-  long long table_off;       // float offset of the latent table in the bucket (< 0: no regulariser)
-  const long long* row;      // device pointer to the current row index
-  float lr_over_bc1, sqrt_bc2;
-  long long reg_off;
-};
-__global__ void adam_prepare_kernel(AdamDevState* st) {
-  const int step = ++st->step;  // 1-based number of the step being taken
-  const int i = step - 1;       // the reference's loop index (train_transformed_rays.py:393-399: lr set AFTER step i)
-  const double lr = (i <= 0) ? (double)st->lr0 : (double)st->lr0 * pow((double)st->decay_factor, (double)(i - 1) / (double)st->decay_steps);
-  const double bc1 = 1.0 - pow((double)st->b1, (double)step), bc2 = 1.0 - pow((double)st->b2, (double)step);
-  st->lr_over_bc1 = (float)(lr / bc1);
-  st->sqrt_bc2 = (float)sqrt(bc2);
-  st->reg_off = (st->table_off >= 0 && st->row) ? st->table_off + (long long)kDimLatent * st->row[0] : -1;
-}
-__global__ void __launch_bounds__(256) adam_dev_kernel(float* __restrict__ P, float* __restrict__ G, float* __restrict__ M, float* __restrict__ V,
-                                                       long long n, const AdamDevState* __restrict__ st) {
-  __shared__ float reg_inv_norm;
-  const long long reg_off = st->reg_off;
-  const float lr_over_bc1 = st->lr_over_bc1, sqrt_bc2 = st->sqrt_bc2, b1 = st->b1, b2 = st->b2, eps = st->eps, gs = st->grad_scale, reg_w = st->reg_w;
-  if (reg_off >= 0) {
+  if (reg_off >= 0) {  // every block that touches the row needs 1 / ||l||: 32 values, recomputed per block (cheap, uniform)
     if (threadIdx.x < 32) {
       const float l = P[reg_off + threadIdx.x];
       float s = l * l;
@@ -135,6 +85,49 @@ __global__ void __launch_bounds__(256) adam_dev_kernel(float* __restrict__ P, fl
     V[i] = v;
     G[i] = 0.f;
   }
+}
+
+struct AdamArgs {
+  float* p; float* g; float* m; float* v;
+  long long n;
+  float lr_over_bc1, sqrt_bc2, b1, b2, eps, grad_scale;
+  long long reg_off;   // float offset of the regularised 32-vector inside the bucket; < 0: none
+  float reg_w;
+};
+__global__ void __launch_bounds__(256) adam_kernel(const AdamArgs a) {
+  adam_update(a.p, a.g, a.m, a.v, a.n, a.lr_over_bc1, a.sqrt_bc2, a.b1, a.b2, a.eps, a.grad_scale, a.reg_off, a.reg_w);
+}
+
+// Graph-capturable variant: the step counter, the learning-rate schedule and the regularised row live in DEVICE memory, so one
+// captured CUDA graph replays every iteration, and eager steps can share the same state.  adam_prepare_kernel (1 thread) advances
+// the step and derives this step's scalars: the reference's schedule in float64 on the caller's double constants, the bias
+// corrections from the FP32 betas the moments are formed with; adam_dev_kernel runs adam_update on them.
+struct AdamDevState {  // mirrors NfbAdamDev (include/nfb.h)
+  int step, pad;
+  double lr0, decay_factor, decay_steps;
+  float b1, b2, eps, grad_scale, reg_w;
+  long long table_off;       // float offset of the latent table in the bucket (< 0: no regulariser)
+  const long long* row;      // device pointer to the current row index (null or < 0: no regulariser)
+  float lr_over_bc1, sqrt_bc2;
+  long long reg_off;
+};
+static_assert(sizeof(AdamDevState) == sizeof(NfbAdamDev) && offsetof(AdamDevState, lr0) == offsetof(NfbAdamDev, lr0) &&
+                  offsetof(AdamDevState, b1) == offsetof(NfbAdamDev, beta1) && offsetof(AdamDevState, table_off) == offsetof(NfbAdamDev, table_offset) &&
+                  offsetof(AdamDevState, lr_over_bc1) == offsetof(NfbAdamDev, lr_over_bc1) && offsetof(AdamDevState, reg_off) == offsetof(NfbAdamDev, reg_offset),
+              "NfbAdamDev mirror");
+__global__ void adam_prepare_kernel(AdamDevState* st) {
+  const int step = ++st->step;  // 1-based number of the step being taken
+  const int i = step - 1;       // the reference's loop index (train_transformed_rays.py:393-399: lr set AFTER step i)
+  const double lr = (i <= 0) ? st->lr0 : st->lr0 * pow(st->decay_factor, (double)(i - 1) / st->decay_steps);
+  const double bc1 = 1.0 - pow((double)st->b1, (double)step), bc2 = 1.0 - pow((double)st->b2, (double)step);
+  st->lr_over_bc1 = (float)(lr / bc1);
+  st->sqrt_bc2 = (float)sqrt(bc2);
+  const long long row = st->row ? st->row[0] : -1;
+  st->reg_off = (st->table_off >= 0 && row >= 0) ? st->table_off + (long long)kDimLatent * row : -1;
+}
+__global__ void __launch_bounds__(256) adam_dev_kernel(float* __restrict__ P, float* __restrict__ G, float* __restrict__ M, float* __restrict__ V,
+                                                       long long n, const AdamDevState* __restrict__ st) {
+  adam_update(P, G, M, V, n, st->lr_over_bc1, st->sqrt_bc2, st->b1, st->b2, st->eps, st->grad_scale, st->reg_off, st->reg_w);
 }
 cudaError_t launch_adam_dev(float* p, float* g, float* m, float* v, long long n, void* dev_state, cudaStream_t st, long long* launches) {
   AdamDevState* s = static_cast<AdamDevState*>(dev_state);

@@ -15,7 +15,7 @@ EXPORTS = ["nfb_version", "nfb_strerror", "nfb_last_cuda_error", "nfb_create", "
            "nfb_render_forward_train", "nfb_render_backward", "nfb_render_backward_ex", "nfb_train_debug", "nfb_debug_schedule", "nfb_loss_mse_grad",
            "nfb_adam_step", "nfb_adam_step_dev", "nfb_repack", "nfb_frame_products", "nfb_sample_rays", "nfb_host_map_cdf",
            "nfb_set_frames", "nfb_render_forward_frames", "nfb_render_forward_frames_train", "nfb_render_backward_frames",
-           "nfb_sample_rays_images", "nfb_latent_rows_grad", "nfb_debug_weights"]
+           "nfb_sample_rays_images", "nfb_latent_rows_grad", "nfb_debug_weights", "nfb_buffer_epoch"]
 NFB_MAX_FRAMES = 1024
 NFB_MAX_STEP_IMAGES = 64
 
@@ -85,7 +85,7 @@ class NfbAdam(C.Structure):
 
 
 class NfbAdamDev(C.Structure):
-    _fields_ = [("step", C.c_int32), ("pad", C.c_int32), ("lr0", C.c_float), ("decay_factor", C.c_float), ("decay_steps", C.c_float),
+    _fields_ = [("step", C.c_int32), ("pad", C.c_int32), ("lr0", C.c_double), ("decay_factor", C.c_double), ("decay_steps", C.c_double),
                 ("beta1", C.c_float), ("beta2", C.c_float), ("eps", C.c_float), ("grad_scale", C.c_float), ("reg_weight", C.c_float),
                 ("table_offset", C.c_longlong), ("row", C.c_void_p), ("lr_over_bc1", C.c_float), ("sqrt_bc2", C.c_float),
                 ("reg_offset", C.c_longlong)]
@@ -163,13 +163,14 @@ def _load():
     lib.nfb_latent_rows_grad.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p, C.c_float,
                                          C.c_void_p]
     lib.nfb_launch_count.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
+    lib.nfb_buffer_epoch.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
     lib.nfb_host_linspace.argtypes = [C.POINTER(C.c_float), C.c_int]
     for fn in ("nfb_create", "nfb_destroy", "nfb_load_weights", "nfb_set_frame", "nfb_render_forward",
                "nfb_render_frame_host", "nfb_launch_count", "nfb_host_linspace", "nfb_render_forward_train",
                "nfb_render_backward", "nfb_render_backward_ex", "nfb_train_debug", "nfb_loss_mse_grad", "nfb_adam_step", "nfb_adam_step_dev", "nfb_repack", "nfb_frame_products",
                "nfb_sample_rays", "nfb_host_map_cdf", "nfb_set_frames", "nfb_render_forward_frames",
                "nfb_render_forward_frames_train", "nfb_render_backward_frames", "nfb_sample_rays_images", "nfb_latent_rows_grad",
-               "nfb_debug_weights"):
+               "nfb_debug_weights", "nfb_buffer_epoch"):
         getattr(lib, fn).restype = C.c_int
     return lib
 

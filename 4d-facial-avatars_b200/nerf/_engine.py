@@ -139,6 +139,12 @@ class Renderer:
         capi.check(capi.lib.nfb_launch_count(self._h, C.byref(n)))
         return n.value
 
+    def buffer_epoch(self) -> int:
+        """nfb_buffer_epoch: changes whenever the handle frees or refills a buffer a captured training step points at."""
+        n = C.c_longlong()
+        capi.check(capi.lib.nfb_buffer_epoch(self._h, C.byref(n)))
+        return n.value
+
     def render(self, ro, rd, near, far, num_coarse, num_fine, perturb=False, noise_std=0.0, white_bkgd=False,
                background=None, dir_z=None, noise=None, precision=None, debug=False, act_step=None, train=False, frame_index=None):
         """ro, rd: [N,3] CUDA FP32.  noise: dict with t_rand, n_c, u, n_f (any may be None).  Returns a dict

@@ -4,7 +4,8 @@ as kernel launches of libnfb on ONE flat FP32 parameter bucket, with no torch.au
 gradient copies:
 
     set_frame (1 launch) -> training forward (1) -> loss gradient (1) -> backward (writes into the flat gradient bucket)
-    -> [one NCCL all-reduce of that bucket when the batch is sharded over ranks] -> Adam + zero_grad (1) -> re-pack (2: fold, pack)
+    -> [one NCCL all-reduce of that bucket when the batch is sharded over ranks] -> Adam + zero_grad (2: schedule, update)
+    -> re-pack (2: fold, pack)
 
 The models keep their reference `state_dict` (their parameters become views of the bucket), so checkpoints, `.parameters()`
 and the drop-in `run_one_iter_of_nerf` keep working on the same objects.  torch is used for memory, the noise draws (in the
@@ -12,6 +13,7 @@ reference's order) and torch.distributed."""
 import torch
 import torch.distributed as dist
 
+from . import _capi as capi
 from . import _engine
 from ._engine import PARAM_ORDER
 
@@ -28,7 +30,7 @@ class FusedTrainer:
         self.opts = dict(near=float(near), far=float(far), num_coarse=int(num_coarse), num_fine=int(num_fine) if model_fine is not None else 0,
                          perturb=bool(perturb), noise_std=float(noise_std), white_bkgd=bool(white_bkgd), precision=precision)
         self.latent_reg = float(latent_reg)
-        self.iter = 0  # optimizer steps taken so far
+        self._iter = 0
 
         # ---- flat bucket: [coarse 26 tensors | fine 26 tensors | pad to 256 | latent table n_latent x 32]
         models = [model_coarse] + ([model_fine] if model_fine is not None else [])
@@ -62,7 +64,27 @@ class FusedTrainer:
         # pixels the K-image sampler repeated because an image's selection came up short, per batch slot, since construction
         self.shortfall = torch.zeros(64, device=dev, dtype=torch.int64)
         self._g_rgb = {}
+        # ONE optimizer state on the device (NfbAdamDev) for every kind of step — eager, captured, one image or several — so
+        # all of them take one step counter and one learning-rate schedule (nfb_adam_step_dev).  Each step writes the latent
+        # row its regulariser applies to into self._row first (-1: none).
+        self._row = torch.full((1,), -1, device=dev, dtype=torch.int64)
+        st = capi.NfbAdamDev(step=0, pad=0, lr0=self.lr0, decay_factor=self.decay_factor, decay_steps=self.decay_steps,
+                             beta1=self.betas[0], beta2=self.betas[1], eps=self.eps, grad_scale=1.0, reg_weight=self.latent_reg,
+                             table_offset=self.lat_off if self.latent_reg > 0.0 else -1, row=self._row.data_ptr(),
+                             lr_over_bc1=0.0, sqrt_bc2=1.0, reg_offset=-1)
+        self._adam = torch.frombuffer(bytearray(bytes(st)), dtype=torch.uint8).to(dev)
         self._own_engine()
+
+    @property
+    def iter(self):
+        """Optimizer steps taken so far (the host's copy of the device state's step counter)."""
+        return self._iter
+
+    @iter.setter
+    def iter(self, value):
+        """Set the step counter, e.g. on resume: the next step takes the schedule's step value + 1."""
+        self._iter = int(value)
+        self._adam[:4].copy_(torch.tensor([self._iter], dtype=torch.int32).view(torch.uint8))
 
     def _own_engine(self):
         """The device's renderer holds ONE set of packed weights: (re-)pack this trainer's if someone else's are in place (another
@@ -71,13 +93,6 @@ class FusedTrainer:
             self.eng.repack(self._pc, self._pf)
             self.eng.mark_synced(self.mc, self.mf)
             self.eng.packed_owner = self
-
-    def lr(self):
-        """Learning rate of step number self.iter (1-based).  The reference assigns lr0 * factor ** (i / decay) AFTER the
-        optimizer step of loop index i (train_transformed_rays.py:393-399), so loop index i >= 1 runs at exponent (i - 1) / decay
-        and loop index 0 at lr0."""
-        i = self.iter - 1  # the reference's loop index of the step being taken
-        return self.lr0 if i <= 0 else self.lr0 * self.decay_factor ** ((i - 1) / self.decay_steps)
 
     def _draw_noise(self, n):
         """rand[N,Nc], randn[N,Nc], rand[N,Nf], randn[N,Nc+Nf] — the reference's draw order for one chunk (train chunksize =
@@ -132,34 +147,35 @@ class FusedTrainer:
         return self.loss[:2]
 
     def update(self):
-        """Adam over the bucket (+ the latent regulariser's gradient on the last frame's row, + zero_grad), then the re-pack."""
+        """Adam over the bucket (+ the latent regulariser's gradient on the last frame's row, + zero_grad) on the trainer's device
+        state, then the re-pack."""
         eng = self.eng
-        self.iter += 1
-        eng.adam_step(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self.lr(), self.iter, self.betas, self.eps,
-                      reg_offset=self.lat_off + 32 * self._reg_row if self.latent_reg > 0.0 else -1, reg_weight=self.latent_reg)
+        self._row.fill_(self._reg_row)
+        eng.adam_step_dev(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self._adam)
+        self._iter += 1
         eng.repack(self._pc, self._pf)
         eng.mark_synced(self.mc, self.mf)
         eng.packed_owner = self
+
+    def _check_epoch(self, g):
+        """Refuse to replay a graph whose renderer buffers were re-allocated or refilled since capture (nfb_buffer_epoch)."""
+        if self.eng.buffer_epoch() != g["epoch"]:
+            raise RuntimeError("a call on this device since capture re-allocated renderer buffers the graph points at (a larger "
+                               "step, more frames or more images per step, on any trainer): capture again")
 
     # ---- the whole iteration as ONE CUDA graph (launch-bound at small per-rank batches: ~20 kernels of 3-800 us)
     def capture(self, n, has_background=True, world=1, n_total=None, group=None):
         """Capture gradients() + update() for batches of exactly n rays on this rank into a CUDA graph.  Everything that changes
         from step to step lives in device memory: the inputs (static buffers filled by step_graph), the latent row index, and the
-        optimizer's step counter / learning rate (nfb_adam_step_dev).  The noise is drawn inside the graph (torch's graph-safe
-        Philox state), in the reference's order.  With world > 1 the NCCL all-reduce of the flat bucket is part of the graph."""
-        import ctypes as C
-        from . import _capi as capi
+        optimizer's step counter / learning rate (the trainer's one nfb_adam_step_dev state, which its eager steps share).  The
+        noise is drawn inside the graph (torch's graph-safe Philox state), in the reference's order.  With world > 1 the NCCL all-reduce of the flat bucket is part of the graph."""
         dev, eng, o = self.dev, self.eng, self.opts
         n_total = n * world if n_total is None else n_total
         z = lambda *shape, dt=torch.float32: torch.zeros(shape, device=dev, dtype=dt)  # noqa: E731
         sb = dict(ro=z(n, 3), rd=z(n, 3), tgt=z(n, 3), bg=z(n, 3) if has_background else None, expr=z(76), idx=z(1, dt=torch.int64),
                   lat=z(32), glat=z(32), g0=z(n, 3), g1=z(n, 3))
         sb["rd"][:, 2] = -1.0  # a valid ray for the warm-up
-        st = capi.NfbAdamDev(step=self.iter, pad=0, lr0=self.lr0, decay_factor=self.decay_factor, decay_steps=self.decay_steps,
-                             beta1=self.betas[0], beta2=self.betas[1], eps=self.eps, grad_scale=1.0, reg_weight=self.latent_reg,
-                             table_offset=self.lat_off if self.latent_reg > 0.0 else -1, row=sb["idx"].data_ptr(),
-                             lr_over_bc1=0.0, sqrt_bc2=1.0, reg_offset=-1)
-        sb["adam"] = torch.frombuffer(bytearray(bytes(st)), dtype=torch.uint8).to(dev)
+        sb["adam"] = self._adam     # the optimizer state the graph advances: the trainer's one state, not a copy
         has_fine = o["num_fine"] > 0
         table_grads = self.grads[self.lat_off:].view(-1, 32)
 
@@ -179,6 +195,7 @@ class FusedTrainer:
 
         self._own_engine()
         forward_backward()          # eager warm-up: sizes the library's training buffers (cudaMalloc is not capturable)
+        epoch = eng.buffer_epoch()
         self.grads.zero_()
         torch.cuda.synchronize()
         graph = torch.cuda.CUDAGraph()
@@ -186,15 +203,19 @@ class FusedTrainer:
             keep = forward_backward()
             if world > 1:
                 dist.all_reduce(self.grads, group=group)
-            eng.adam_step_dev(self.params, self.grads, self.exp_avg, self.exp_avg_sq, sb["adam"])
+            self._row.copy_(sb["idx"])
+            eng.adam_step_dev(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self._adam)
             eng.repack(self._pc, self._pf)
-        self._graph = dict(graph=graph, sb=sb, n=n, keep=keep)
+        self._graph = dict(graph=graph, sb=sb, n=n, keep=keep, epoch=epoch)
         return self
 
     def step_graph(self, ray_origins, ray_directions, target, expressions, latent_index, background=None):
         """One optimizer step by replaying the captured graph (capture() first): copies the step's inputs into the static buffers —
-        on the current stream, so the caller may keep them on the device or in pinned host memory — and replays."""
+        on the current stream, so the caller may keep them on the device or in pinned host memory — and replays.  Raises
+        RuntimeError, before it copies or launches anything, when a call on this device has re-allocated the renderer buffers the
+        graph points at since capture (nfb_buffer_epoch): capture again."""
         g = self._graph
+        self._check_epoch(g)
         sb = g["sb"]
         if ray_origins.shape[0] != g["n"]:
             raise ValueError(f"the graph was captured for {g['n']} rays per step")
@@ -207,7 +228,7 @@ class FusedTrainer:
         sb["expr"].copy_(expressions.reshape(-1), non_blocking=True)
         sb["idx"].fill_(int(latent_index))
         g["graph"].replay()
-        self.iter += 1
+        self._iter += 1
         self.eng.mark_synced(self.mc, self.mf)
         self.eng.packed_owner = self
         return self.loss[:2]
@@ -267,17 +288,6 @@ class FusedTrainer:
                              0.0 if k == 1 else self.latent_reg / k)
         return out
 
-    def _adam_dev_state(self, k, row_ptr=None):
-        """NfbAdamDev for a K-image step: from this trainer's step counter; the regulariser on the row at row_ptr (K = 1) or off
-        (K >= 2: nfb_latent_rows_grad added it)."""
-        from . import _capi as capi
-        reg = k == 1 and self.latent_reg > 0.0
-        st = capi.NfbAdamDev(step=self.iter, pad=0, lr0=self.lr0, decay_factor=self.decay_factor, decay_steps=self.decay_steps,
-                             beta1=self.betas[0], beta2=self.betas[1], eps=self.eps, grad_scale=1.0, reg_weight=self.latent_reg,
-                             table_offset=self.lat_off if reg else -1, row=row_ptr if reg else None, lr_over_bc1=0.0, sqrt_bc2=1.0,
-                             reg_offset=-1)
-        return torch.frombuffer(bytearray(bytes(st)), dtype=torch.uint8).to(self.dev)
-
     def _check_images(self, data, k, n, world):
         if world != 1:
             raise NotImplementedError("steps over several images are single-rank: world must be 1")
@@ -295,10 +305,10 @@ class FusedTrainer:
         mse(rgb_c, t) + mse(rgb_f, t) + (latent_reg / K) * sum_k ||latent[image_index[k]]|| over all K * n rays.  K = 1 is step()
         on the sampled rays, bit for bit.  Raises RuntimeError, before any gradient is formed, when an image's selection came
         up short of n distinct pixels within max_rounds rounds.
-        Launches (within the memory budget; +1 the first time the sampler's scratch grows): K = 1: 15 = sample 1, set_frame 1,
-        forward 1, loss 1, backward 7, latent rows 1, Adam 1, re-pack 2; K >= 2: 19 = sample 1, set_frames 1, forward 1, loss 1,
-        backward 10, latent rows 1, Adam 2 (device-side schedule, as in the graph), re-pack 2.  Returns the device tensor
-        [mse_coarse, mse_fine]."""
+        Launches (within the memory budget; +1 the first time the sampler's scratch grows): K = 1: 16 = sample 1, set_frame 1,
+        forward 1, loss 1, backward 7, latent rows 1, Adam 2, re-pack 2; K >= 2: 19 = sample 1, set_frames 1, forward 1, loss 1,
+        backward 10, latent rows 1, Adam 2, re-pack 2 (Adam: schedule and update on the trainer's device state, as in every step,
+        eager or captured).  Returns the device tensor [mse_coarse, mse_fine]."""
         k, n = len(image_index), int(n_per_image)
         self._check_images(data, k, n, world)
         if any(not 0 <= int(i) < data.n_images for i in image_index):
@@ -317,17 +327,9 @@ class FusedTrainer:
             raise RuntimeError(f"ray sampler: {max_rounds} rounds of draws found fewer than {n} distinct pixels for (image, found) "
                                f"{short}; raise max_rounds")
         self._images_gradients(sb, k, n)
-        if k == 1:
-            self._reg_row = int(image_index[0])
-            self.update()
-        else:
-            eng = self.eng
-            st = self._adam_dev_state(k)
-            eng.adam_step_dev(self.params, self.grads, self.exp_avg, self.exp_avg_sq, st)
-            self.iter += 1
-            eng.repack(self._pc, self._pf)
-            eng.mark_synced(self.mc, self.mf)
-            eng.packed_owner = self
+        # K = 1: the regulariser in Adam on the image's row, as in step(); K >= 2: none (nfb_latent_rows_grad added it)
+        self._reg_row = int(image_index[0]) if k == 1 else -1
+        self.update()
         return self.loss[:2]
 
     def capture_images(self, data, k, n_per_image, has_background=True, max_rounds=32, device_draws=True, world=1):
@@ -336,9 +338,9 @@ class FusedTrainer:
         with its device-side schedule, re-pack.  Only the K image indices change between replays.  An incomplete selection does
         not stop the graph: the image's missing slots repeat its first pixels and self.shortfall[k] counts them (include/nfb.h,
         nfb_sample_rays_images).  Launches per replay: 16 at K = 1, 19 at K >= 2.
-        The graph holds the renderer's device buffers as sized at capture, and they only grow: a later call on the same device
-        that needs more room (more images or rays per step, a larger render with gradients) re-allocates them and leaves this
-        graph pointing at freed memory.  Run the largest step first, or capture again after it."""
+        The graph holds the renderer's device buffers as sized at capture, and they only grow: a later call on the same device,
+        by any trainer, that needs more room (more images or rays per step, more frames, a larger render with gradients)
+        re-allocates them.  step_images_graph then raises RuntimeError instead of replaying (nfb_buffer_epoch): capture again."""
         n = int(n_per_image)
         self._check_images(data, k, n, world)
         if has_background != (data.background is not None):
@@ -348,13 +350,9 @@ class FusedTrainer:
         for name, t in list(sb.items()):
             if t is not None and name != "shortfall":
                 sb[name] = torch.zeros_like(t)
-        sb["idx64"] = torch.zeros(1, device=dev, dtype=torch.int64)
         sb["draws"] = None if device_draws else torch.zeros(k * max_rounds * n, device=dev, dtype=torch.float64)
-        sb["adam"] = self._adam_dev_state(k, sb["idx64"].data_ptr())
 
         def body():
-            if k == 1:
-                sb["idx64"].copy_(sb["img"])  # the Adam regulariser's row
             draws = torch.rand(k * max_rounds * n, dtype=torch.float64, device=dev) if device_draws else sb["draws"]
             self._images_sample(data, sb, n, draws, max_rounds)
             return self._images_gradients(sb, k, n), draws
@@ -365,21 +363,28 @@ class FusedTrainer:
             sb["draws"].uniform_()
         before = self.shortfall.clone()
         body()                      # eager warm-up: sizes the library's buffers (cudaMalloc is not capturable)
+        epoch = eng.buffer_epoch()
         self.grads.zero_()
         torch.cuda.synchronize()
         graph = torch.cuda.CUDAGraph()
         with torch.cuda.graph(graph):
             keep = body()
-            eng.adam_step_dev(self.params, self.grads, self.exp_avg, self.exp_avg_sq, sb["adam"])
+            if k == 1:
+                self._row.copy_(sb["img"])  # the Adam regulariser's row
+            else:
+                self._row.fill_(-1)
+            eng.adam_step_dev(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self._adam)
             eng.repack(self._pc, self._pf)
         self.shortfall.copy_(before)  # the warm-up's selections are not a step's
-        self._igraph = dict(graph=graph, sb=sb, k=k, n=n, max_rounds=max_rounds, keep=keep)
+        self._igraph = dict(graph=graph, sb=sb, k=k, n=n, max_rounds=max_rounds, keep=keep, epoch=epoch)
         return self
 
     def step_images_graph(self, image_index, draws=None):
         """One optimizer step by replaying the graph of capture_images: copies the K image indices (host ints, or an int32 CUDA /
-        pinned tensor: no host sync) and, when captured with device_draws=False, the draws, then replays."""
+        pinned tensor: no host sync) and, when captured with device_draws=False, the draws, then replays.  Raises RuntimeError, as
+        step_graph does, when the renderer buffers the graph points at were re-allocated since capture."""
         g = self._igraph
+        self._check_epoch(g)
         sb = g["sb"]
         if len(image_index) != g["k"]:
             raise ValueError(f"the graph was captured for {g['k']} images per step")
@@ -391,7 +396,7 @@ class FusedTrainer:
             sb["draws"].copy_(draws.reshape(-1)[:sb["draws"].numel()], non_blocking=True)
         self._own_engine()
         g["graph"].replay()
-        self.iter += 1
+        self._iter += 1
         self.eng.mark_synced(self.mc, self.mf)
         self.eng.packed_owner = self
         return self.loss[:2]

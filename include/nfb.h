@@ -25,7 +25,7 @@
 extern "C" {
 #endif
 
-#define NFB_VERSION 130
+#define NFB_VERSION 131
 /* Defined when the backward and the loss repeat bit for bit (no floating-point atomics; see nfb_render_backward).  The
  * version number stayed 130 for this addition, so test this macro rather than the version. */
 #define NFB_REPRODUCIBLE_BACKWARD 1
@@ -327,12 +327,16 @@ int nfb_adam_step(NfbHandle* h, float* params, float* grads, float* exp_avg, flo
 
 /* nfb_adam_step with its per-step scalars in DEVICE memory, so that a whole training iteration can be captured once in a CUDA graph
  * and replayed: `dev_state` points to an NfbAdamDev on the device.  Each call first advances `step` and evaluates the reference's
- * learning-rate schedule lr0 * decay_factor ^ ((i - 1) / decay_steps) for loop index i = step - 1 >= 1 (train_transformed_rays.py:393-399)
- * and the bias corrections on the device (1 thread, float64), then runs the Adam kernel.  The regularised row is
- * table_offset + 32 * row[0] (row = device pointer to the current latent index; table_offset < 0: no regulariser).  2 launches. */
+ * learning-rate schedule lr0 * decay_factor ^ ((i - 1) / decay_steps) for loop index i = step - 1 >= 1 (lr0 at i = 0;
+ * train_transformed_rays.py:393-399) in float64 on the caller's double constants, and the bias corrections 1 - beta^step from the
+ * FP32 betas the moment update uses (1 thread), then runs the Adam kernel; lr_over_bc1 and sqrt_bc2 are rounded to FP32 once.  The
+ * regularised row is table_offset + 32 * row[0]; there is none when table_offset < 0, row is NULL or row[0] < 0 (row = device pointer
+ * to the current latent index, so eager steps and graph replays of one trainer can share one state and one step counter).
+ * 2 launches.  Version 131 made lr0, decay_factor and decay_steps double (they were float). */
 typedef struct {
   int32_t step, pad;               /* in/out: steps taken so far (start at 0) */
-  float lr0, decay_factor, decay_steps, beta1, beta2, eps, grad_scale, reg_weight;
+  double lr0, decay_factor, decay_steps;
+  float beta1, beta2, eps, grad_scale, reg_weight;
   long long table_offset;
   const long long* row;
   float lr_over_bc1, sqrt_bc2;     /* out: this step's scalars (written by the prepare kernel) */
@@ -537,6 +541,14 @@ int nfb_debug_schedule(int which, int index, uint32_t* out, int out_words);
 
 /* Number of kernel launches issued by this handle so far (all kernels of this library). */
 int nfb_launch_count(NfbHandle* h, long long* out);
+
+/* The handle's buffer epoch: how many times it has freed (to grow) or refilled a device buffer whose address a training step's
+ * launches take — the training state nfb_render_forward_train saves, the frame table of nfb_set_frames, the scratch of
+ * nfb_sample_rays_images and the linspace tables.  A CUDA graph captured over the handle's calls is valid while the epoch is the
+ * one read after capture; once it has changed, the graph points at freed or rewritten memory and must be captured again.  The
+ * staging buffers of nfb_render_frame_host and the scratch of nfb_frame_products / nfb_sample_rays are not counted (no training
+ * step reads them).  Host read, no CUDA call and no synchronisation. */
+int nfb_buffer_epoch(NfbHandle* h, long long* out);
 
 /* Host helper: out[i] = torch.linspace(0, 1, n)[i] bit-for-bit (ATen's CPU kernel: step = 1/(n-1) in
  * FP32; first half start + i*step, second half end - (n-1-i)*step).  Used for t_coarse / u_fine when the

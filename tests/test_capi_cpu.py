@@ -41,6 +41,35 @@ def test_invalid_arguments_return_codes(built_lib):
     assert lib.nfb_launch_count(None, None) == 1
 
 
+def test_adam_dev_struct_matches_the_header(built_lib, tmp_path):
+    """_capi.NfbAdamDev has the size and field offsets a C compiler gives include/nfb.h's NfbAdamDev (the schedule's constants
+    are double since version 131; a float mirror would hand the device shifted fields)."""
+    import shutil
+    import subprocess
+    from nerf import _capi
+    cc = shutil.which("cc") or shutil.which("gcc")
+    assert cc, "a C compiler is needed to read the header's layout"
+    fields = [name for name, _ in _capi.NfbAdamDev._fields_]
+    src = tmp_path / "layout.c"
+    src.write_text('#include <stdio.h>\n#include <stddef.h>\n#include "nfb.h"\nint main(void) {\n'
+                   '  printf("%zu\\n", sizeof(NfbAdamDev));\n'
+                   + "".join(f'  printf("%zu\\n", offsetof(NfbAdamDev, {f}));\n' for f in fields) + "  return 0;\n}\n")
+    exe = tmp_path / "layout"
+    subprocess.run([cc, "-I", os.path.join(ROOT, "include"), "-o", str(exe), str(src)], check=True)
+    got = [int(v) for v in subprocess.run([str(exe)], capture_output=True, text=True, check=True).stdout.split()]
+    want = [ctypes.sizeof(_capi.NfbAdamDev)] + [getattr(_capi.NfbAdamDev, f).offset for f in fields]
+    assert got == want, dict(zip(["sizeof"] + fields, zip(got, want)))
+    assert {f: t for f, t in _capi.NfbAdamDev._fields_ if f in ("lr0", "decay_factor", "decay_steps")} == dict.fromkeys(
+        ("lr0", "decay_factor", "decay_steps"), ctypes.c_double)
+
+
+def test_buffer_epoch_is_exported_and_rejects_null(built_lib):
+    lib = ctypes.CDLL(built_lib)
+    out = ctypes.c_longlong(-5)
+    assert lib.nfb_buffer_epoch(None, ctypes.byref(out)) == 1 and out.value == -5  # NFB_ERR_INVALID, nothing written
+    assert lib.nfb_buffer_epoch(None, None) == 1
+
+
 def test_python_surface_matches_reference_names(built_lib):
     import nerf
     for name in ["load_flame_data", "CfgNode", "get_embedding_function", "get_ray_bundle", "img2mse", "load_llff_data",

@@ -169,6 +169,48 @@ def test_adam_kernel_matches_torch_adam(env):
     assert torch.equal(p[:100], p0[:100])
 
 
+def test_adam_dev_kernel_matches_torch_adam(env):
+    """nfb_adam_step_dev — step counter, the reference's LR schedule and the regularised row in an NfbAdamDev on the device —
+    against torch.optim.Adam over the same 10 steps as test_adam_kernel_matches_torch_adam (gradients from 1e-12 to 1, the latent
+    regulariser on one 32-float row); the state ends at step 10 with that row as its regularised offset."""
+    from nerf import _capi
+    nerf, _engine, fused_train, dev = env
+    eng = _engine.renderer_for(dev)
+    g = torch.Generator().manual_seed(11)
+    n, row = 256 * 40 + 64, 256 * 40 + 32
+    p0 = ((torch.rand(n, generator=g) - 0.5) * 0.2).to(dev)
+    p_ref = p0.clone().requires_grad_(True)
+    opt = torch.optim.Adam([p_ref], lr=5e-4)
+    p, m, v = p0.clone(), torch.zeros(n, device=dev), torch.zeros(n, device=dev)
+    lr0, decay, factor = 5e-4, 250.0, 0.1
+    row_index = torch.full((1,), 1, device=dev, dtype=torch.int64)  # the table starts one row before the regularised one
+    st = _capi.NfbAdamDev(step=0, pad=0, lr0=lr0, decay_factor=factor, decay_steps=decay, beta1=0.9, beta2=0.999, eps=1e-8,
+                          grad_scale=1.0, reg_weight=0.005, table_offset=row - 32, row=row_index.data_ptr(), lr_over_bc1=0.0,
+                          sqrt_bc2=1.0, reg_offset=-1)
+    dev_state = torch.frombuffer(bytearray(bytes(st)), dtype=torch.uint8).to(dev)
+    for i in range(10):
+        mag = 10.0 ** (torch.rand(n, generator=g) * 12.0 - 12.0)
+        grad = ((torch.rand(n, generator=g) - 0.5) * 2.0 * mag).to(dev)
+        grad[:100] = 0.0
+        for gp in opt.param_groups:
+            gp["lr"] = lr0 if i == 0 else lr0 * factor ** ((i - 1) / decay)
+        opt.zero_grad()
+        reg = torch.norm(p_ref[row:row + 32]) * 0.005
+        reg.backward()
+        p_ref.grad += grad
+        opt.step()
+        gbuf = grad.clone()
+        eng.adam_step_dev(p, gbuf, m, v, dev_state)
+        assert float(gbuf.abs().max()) == 0.0
+    torch.cuda.synchronize()
+    got = _capi.NfbAdamDev.from_buffer_copy(bytes(dev_state.cpu().numpy().tobytes()))
+    assert got.step == 10 and got.reg_offset == row
+    d = (p - p_ref.detach()).abs()
+    print(f"device-state adam kernel vs torch.optim.Adam, 10 steps: max|d| = {float(d.max()):.3e}")
+    assert float(d.max()) <= 1e-6
+    assert torch.equal(p[:100], p0[:100])
+
+
 def test_fused_step_launch_budget(env):
     """After the backward: Adam (+ zero_grad) is one launch and the re-pack two (FP64 fold, pack) — 3 in all; the whole step stays
     under 20 launches."""

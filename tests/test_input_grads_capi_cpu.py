@@ -12,13 +12,13 @@ def lib(built_lib):
     return ctypes.CDLL(built_lib)
 
 
-def test_backward_ex_exported_and_version(lib):
+def test_backward_ex_exported_at_version_131(lib):
     lib.nfb_version.restype = ctypes.c_int
-    assert lib.nfb_version() == 130
+    assert lib.nfb_version() == 131
     assert hasattr(lib, "nfb_render_backward_ex")
     with open(os.path.join(ROOT, "include", "nfb.h")) as f:
         h = f.read()
-    assert "#define NFB_VERSION 130" in h and "NfbInputGrads" in h
+    assert "#define NFB_VERSION 131" in h and "NfbInputGrads" in h
 
 
 def test_backward_ex_rejects_null_handle(lib):

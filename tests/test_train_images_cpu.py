@@ -1,5 +1,5 @@
 """The K-image training-step entries (NFB_TRAIN_IMAGES) without a GPU: declared, the ctypes mirrors laid out as the header's
-structs, argument checks before any CUDA call, and the version left where it was."""
+structs, argument checks before any CUDA call, and the library's version."""
 import ctypes as C
 import os
 import re
@@ -30,17 +30,17 @@ def _struct_fields(name):
     return out
 
 
-def test_header_declares_the_feature():
+def test_header_declares_the_feature_at_version_131():
     h = open(HEADER).read()
     assert re.search(r"#define NFB_TRAIN_IMAGES 1\b", h)
     assert re.search(r"#define NFB_MAX_STEP_IMAGES 64\b", h)
-    assert re.search(r"#define NFB_VERSION 130\b", h)
+    assert re.search(r"#define NFB_VERSION 131\b", h)
     for fn in ("nfb_sample_rays_images", "nfb_latent_rows_grad"):
         assert re.search(rf"\bint {fn}\(", h), fn
 
 
-def test_version_is_still_130(capi):
-    assert capi.lib.nfb_version() == 130
+def test_version_is_131(capi):
+    assert capi.lib.nfb_version() == 131
     assert capi.NFB_MAX_STEP_IMAGES == 64
     assert {"nfb_sample_rays_images", "nfb_latent_rows_grad"} <= set(capi.EXPORTS)
 

@@ -350,6 +350,7 @@ def test_launches_per_step_are_the_documented_ones(env):
     eng = _engine.renderer_for(dev)
     doc = fused_train.FusedTrainer.step_images.__doc__
     one, many = int(re.search(r"K = 1: (\d+) =", doc).group(1)), int(re.search(r"K >= 2: (\d+) =", doc).group(1))
+    assert (one, many) == (16, 19)  # Adam is 2 launches (device-side schedule) in every step
     data, frs, images = dataset(ray_sampler, dev, 3, 32, 32, [(8, 24, 6, 26)] * 3)
     tr = _trainer(nerf, fused_train, dev, 3, True)
     for ids, want in (([1], one), ([0, 2], many), ([0, 1, 2, 1], many)):
