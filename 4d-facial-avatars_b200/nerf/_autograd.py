@@ -15,17 +15,25 @@ import torch
 
 from ._engine import PARAM_ORDER
 
-_N_IN = 8  # inputs before the parameters: eng, args, has_fine, rays, expr, latent, background, dir_z
+_N_IN = 9  # inputs before the parameters: eng, args, has_fine, rays, frame_index, expr, latent, background, dir_z
 
 
 class _RenderFn(torch.autograd.Function):
+    """A training render and its backward.  frame_index None: one frame (expr [76], latent [32]; nfb_set_frame,
+    nfb_render_forward_train, nfb_render_backward_ex); otherwise ray i is conditioned on frame frame_index[i] of expr [F,76] and
+    latent [F,32] (nfb_set_frames, nfb_render_forward_frames_train, nfb_render_backward_frames)."""
     @staticmethod
-    def forward(ctx, eng, args, has_fine, rays, expr, latent, background, dir_z, *params):
-        out = eng.render(rays[:, :3], rays[:, 3:6], train=True, background=background, dir_z=dir_z, **args)
+    def forward(ctx, eng, args, has_fine, rays, frame_index, expr, latent, background, dir_z, *params):
+        if frame_index is None:
+            eng.set_frame(expr, latent)
+        else:
+            eng.set_frames(expr, latent)
+        out = eng.render(rays[:, :3], rays[:, 3:6], train=True, background=background, dir_z=dir_z, frame_index=frame_index, **args)
         ctx.eng = eng
         ctx.keep = out.get("_keep")  # the chunked backward (include/nfb.h) re-reads the forward's inputs
         ctx.token = eng.train_token
         ctx.has_fine = has_fine
+        ctx.frames = frame_index is not None
         ctx.shapes = dict(rays=rays.shape, expr=expr.shape, latent=latent.shape,
                           background=background.shape if background is not None else None,
                           dir_z=dir_z.shape if dir_z is not None else None)
@@ -43,72 +51,11 @@ class _RenderFn(torch.autograd.Function):
                                "next training-mode render on the same device")
         params = ctx.saved_tensors
         npar = len(PARAM_ORDER)
-        n_in = _N_IN
         if all(g is None for g in gouts):
-            return (None,) * (n_in + len(params))
+            return (None,) * (_N_IN + len(params))
         gouts = [g if (g is not None and g.numel() > 0) else None for g in gouts]
         need = ctx.needs_input_grad
-        want_params = any(need[n_in:])
-        inputs = []
-        if need[3]:
-            inputs += ["ray_origins", "ray_directions"]
-        if need[4]:
-            inputs.append("expression")
-        if need[6]:
-            inputs.append("background")
-        if need[7]:
-            inputs.append("dir_z")
-        grads_c, grads_f, glat, ing = eng.backward(gouts, params[:npar], params[npar:2 * npar] if ctx.has_fine else None,
-                                                   want_params=want_params, inputs=inputs)
-        if want_params:
-            gpar = tuple(grads_c) + (tuple(grads_f) if ctx.has_fine else ())
-        else:
-            gpar = (None,) * len(params)
-        g_rays = None
-        if need[3]:
-            g_rays = torch.zeros(ctx.shapes["rays"], device=glat.device, dtype=torch.float32)
-            g_rays[:, 0:3] = ing["ray_origins"]
-            g_rays[:, 3:6] = ing["ray_directions"]
-        g_expr = ing["expression"].reshape(ctx.shapes["expr"]) if need[4] else None
-        g_bg = ing["background"].reshape(ctx.shapes["background"]) if need[6] else None
-        g_dz = ing["dir_z"].reshape(ctx.shapes["dir_z"]) if need[7] else None
-        return (None, None, None, g_rays, g_expr, glat.reshape(ctx.shapes["latent"]), g_bg, g_dz) + gpar
-
-
-class _RenderFramesFn(torch.autograd.Function):
-    """A multi-frame training render (nfb_render_forward_frames_train) and its backward (nfb_render_backward_frames): gradients
-    for the parameters, every frame's expression [F,76] and latent [F,32], the rays, the background and dir_z."""
-    @staticmethod
-    def forward(ctx, eng, args, has_fine, rays, frame_index, expr, latent, background, dir_z, *params):
-        eng.set_frames(expr, latent)
-        out = eng.render(rays[:, :3], rays[:, 3:6], train=True, background=background, dir_z=dir_z, frame_index=frame_index, **args)
-        ctx.eng = eng
-        ctx.keep = out.get("_keep")
-        ctx.token = eng.train_token
-        ctx.has_fine = has_fine
-        ctx.shapes = dict(rays=rays.shape, expr=expr.shape, latent=latent.shape,
-                          background=background.shape if background is not None else None,
-                          dir_z=dir_z.shape if dir_z is not None else None)
-        ctx.save_for_backward(*params)
-        ctx.set_materialize_grads(False)
-        res = (out["rgb_coarse"], out["disp_coarse"], out["acc_coarse"],
-               out.get("rgb_fine"), out.get("disp_fine"), out.get("acc_fine"), out["w_last"])
-        return tuple(r if r is not None else rays.new_zeros(0) for r in res)
-
-    @staticmethod
-    def backward(ctx, *gouts):
-        eng = ctx.eng
-        if ctx.token != eng.train_token:
-            raise RuntimeError("the renderer keeps the saved state of ONE training forward; call backward() before the "
-                               "next training-mode render on the same device")
-        params = ctx.saved_tensors
-        npar = len(PARAM_ORDER)
-        n_in = 9
-        if all(g is None for g in gouts):
-            return (None,) * (n_in + len(params))
-        gouts = [g if (g is not None and g.numel() > 0) else None for g in gouts]
-        need = ctx.needs_input_grad
-        want_params = any(need[n_in:])
+        want_params = any(need[_N_IN:])
         inputs = []
         if need[3]:
             inputs += ["ray_origins", "ray_directions"]
@@ -118,12 +65,15 @@ class _RenderFramesFn(torch.autograd.Function):
             inputs.append("background")
         if need[8]:
             inputs.append("dir_z")
+        # the single-frame backward always asks for d latent (an input-only one then keeps its PE-only weight-gradient launch); the
+        # multi-frame one only when the latents require grad
         grads_c, grads_f, glat, ing = eng.backward(gouts, params[:npar], params[npar:2 * npar] if ctx.has_fine else None,
-                                                   want_latent=need[6], want_params=want_params, inputs=inputs, frames=True)
+                                                   want_latent=need[6] or not ctx.frames, want_params=want_params, inputs=inputs,
+                                                   frames=ctx.frames)
         gpar = (tuple(grads_c) + (tuple(grads_f) if ctx.has_fine else ())) if want_params else (None,) * len(params)
         g_rays = None
         if need[3]:
-            g_rays = torch.zeros(ctx.shapes["rays"], device=ing["ray_origins"].device, dtype=torch.float32)
+            g_rays = torch.zeros(ctx.shapes["rays"], device=eng.device, dtype=torch.float32)
             g_rays[:, 0:3] = ing["ray_origins"]
             g_rays[:, 3:6] = ing["ray_directions"]
         g_expr = ing["expression"].reshape(ctx.shapes["expr"]) if need[5] else None
@@ -133,21 +83,9 @@ class _RenderFramesFn(torch.autograd.Function):
         return (None, None, None, g_rays, None, g_expr, g_lat, g_bg, g_dz) + gpar
 
 
-def render_frames_with_grad(eng, rays, frame_index, model_coarse, model_fine, expressions, latent_codes, args):
-    """The multi-frame counterpart of render_with_grad: expressions [F,76], latent_codes [F,32], frame_index [N]."""
-    params = [dict(model_coarse.named_parameters())[k] for k in PARAM_ORDER]
-    has_fine = model_fine is not None
-    if has_fine:
-        sd_f = dict(model_fine.named_parameters())
-        params += [sd_f[k] for k in PARAM_ORDER]
-    args = dict(args)
-    background, dir_z = args.pop("background", None), args.pop("dir_z", None)
-    res = _RenderFramesFn.apply(eng, args, has_fine, rays, frame_index, expressions, latent_codes, background, dir_z, *params)
-    return tuple(r if r.numel() > 0 else None for r in res)
-
-
-def render_with_grad(eng, rays, model_coarse, model_fine, expressions, latent_code, args):
-    """args: the keyword arguments of Renderer.render; its `background` and `dir_z` tensors become inputs of the graph."""
+def render_with_grad(eng, rays, model_coarse, model_fine, expressions, latent_code, args, frame_index=None):
+    """args: the keyword arguments of Renderer.render; its `background` and `dir_z` tensors become inputs of the graph.
+    frame_index [N]: a multi-frame render over expressions [F,76] and latent_code [F,32]."""
     sd_c = dict(model_coarse.named_parameters())
     params = [sd_c[k] for k in PARAM_ORDER]
     has_fine = model_fine is not None
@@ -156,5 +94,5 @@ def render_with_grad(eng, rays, model_coarse, model_fine, expressions, latent_co
         params += [sd_f[k] for k in PARAM_ORDER]
     args = dict(args)
     background, dir_z = args.pop("background", None), args.pop("dir_z", None)
-    res = _RenderFn.apply(eng, args, has_fine, rays, expressions, latent_code, background, dir_z, *params)
+    res = _RenderFn.apply(eng, args, has_fine, rays, frame_index, expressions, latent_code, background, dir_z, *params)
     return tuple(r if r.numel() > 0 else None for r in res)

@@ -44,6 +44,31 @@ def _f32c(t, device):
     return t.detach().to(device=device, dtype=torch.float32).contiguous()
 
 
+OUTPUTS = ("rgb_coarse", "disp_coarse", "acc_coarse", "rgb_fine", "disp_fine", "acc_fine", "w_last")  # members of NfbOutputs
+
+
+def _ptrs(tensors):
+    """The C array of 26 pointers (PARAM_ORDER) the library takes for one network's parameters or gradients; None entries are
+    null, and None gives a null array."""
+    return (C.c_void_p * 26)(*[(t.data_ptr() if t is not None else None) for t in tensors]) if tensors is not None else None
+
+
+def _outputs(out, has_fine):
+    """NfbOutputs pointing at the seven tensors of `out` (the fine ones null without a fine network)."""
+    return capi.NfbOutputs(*[(out[k].data_ptr() if has_fine or not k.endswith("_fine") else None) for k in OUTPUTS])
+
+
+def _out_grads(out_grads, device, keep):
+    """NfbOutGrads from 7 tensors or None in OUTPUTS order; the FP32 copies handed to the library are appended to `keep`."""
+    og = capi.NfbOutGrads()
+    for field, g in zip(OUTPUTS, out_grads):
+        if g is not None:
+            g = _f32c(g, device)
+            keep.append(g)
+            setattr(og, field, g.data_ptr())
+    return og
+
+
 class Renderer:
     """One NfbHandle on one CUDA device plus the bookkeeping that decides when weights must be re-packed."""
 
@@ -98,8 +123,7 @@ class Renderer:
             if fp == self._versions[which]:
                 continue
             tensors = [_f32c(t, self.device) for t in self._params(model)]
-            arr = (C.c_void_p * 26)(*[t.data_ptr() for t in tensors])
-            capi.check(capi.lib.nfb_load_weights(self._h, which, arr, _stream()), "load_weights")
+            capi.check(capi.lib.nfb_load_weights(self._h, which, _ptrs(tensors), _stream()), "load_weights")
             self.packed_owner = None
             self._keep[which] = tensors
             self._versions[which] = fp
@@ -111,6 +135,12 @@ class Renderer:
         if t is None:
             t = self._lin[n] = torch.linspace(0.0, 1.0, n, dtype=torch.float32).to(self.device)
         return t
+
+    def _sampling(self, num_coarse, num_fine, precision, white_bkgd, perturb=False, noise_std=0.0):
+        prec = precision or _precision
+        return capi.NfbSampling(num_coarse, num_fine, int(bool(perturb)), float(noise_std), int(bool(white_bkgd)), 0,
+                                capi.NFB_PREC_EXACT if prec == "exact" else capi.NFB_PREC_FAST, self.linspace(num_coarse).data_ptr(),
+                                self.linspace(num_fine).data_ptr() if num_fine > 0 else None)
 
     def set_frame(self, expressions, latent_code):
         e = _f32c(expressions, self.device).reshape(-1)
@@ -156,10 +186,7 @@ class Renderer:
         n = ro.shape[0]
         has_fine = num_fine > 0
         out = {k: torch.empty((n, 3) if k.startswith("rgb") else (n,), device=dev, dtype=torch.float32)
-               for k in ("rgb_coarse", "disp_coarse", "acc_coarse", "w_last")}
-        if has_fine:
-            out.update({k: torch.empty((n, 3) if k.startswith("rgb") else (n,), device=dev, dtype=torch.float32)
-                        for k in ("rgb_fine", "disp_fine", "acc_fine")})
+               for k in OUTPUTS if has_fine or not k.endswith("_fine")}
         rays = capi.NfbRays()
         rays.o, rays.d, rays.n_rays = ro.data_ptr(), rd.data_ptr(), n
         rays.near_, rays.far_ = float(near), float(far)
@@ -172,11 +199,7 @@ class Renderer:
             dz = _f32c(dir_z, dev).reshape(n)
             rays.dir_z = dz.data_ptr()
             keep.append(dz)
-        prec = precision or _precision
-        sm = capi.NfbSampling(num_coarse, num_fine, int(bool(perturb)), float(noise_std), int(bool(white_bkgd)), 0,
-                              capi.NFB_PREC_EXACT if prec == "exact" else capi.NFB_PREC_FAST,
-                              self.linspace(num_coarse).data_ptr(),
-                              self.linspace(num_fine).data_ptr() if has_fine else None)
+        sm = self._sampling(num_coarse, num_fine, precision, white_bkgd, perturb, noise_std)
         nz = capi.NfbNoise()
         if noise:
             for field, key in (("t_rand", "t_rand"), ("sigma_noise_c", "n_c"), ("u", "u"), ("sigma_noise_f", "n_f")):
@@ -185,10 +208,7 @@ class Renderer:
                     t = _f32c(t, dev)
                     keep.append(t)
                     setattr(nz, field, t.data_ptr())
-        o = capi.NfbOutputs(out["rgb_coarse"].data_ptr(), out["disp_coarse"].data_ptr(), out["acc_coarse"].data_ptr(),
-                            out["rgb_fine"].data_ptr() if has_fine else None,
-                            out["disp_fine"].data_ptr() if has_fine else None,
-                            out["acc_fine"].data_ptr() if has_fine else None, out["w_last"].data_ptr())
+        o = _outputs(out, has_fine)
         dbg = None
         if debug or act_step is not None:
             dbg = self._debug_dumps(out, n, num_coarse, num_fine)
@@ -200,23 +220,20 @@ class Renderer:
                 raise ValueError("a multi-frame render takes no debug dumps")
             fi = frame_index.detach().to(device=dev, dtype=torch.int32).reshape(n).contiguous()
             keep.append(fi)
-            fn = capi.lib.nfb_render_forward_frames_train if train else capi.lib.nfb_render_forward_frames
-            if train:
-                self.train_token += 1
-                self.train_rays = n
-                self.train_frames = self.n_frames
-            capi.check(fn(self._h, C.byref(rays), _ptr(fi), C.byref(sm), C.byref(nz) if noise else None, C.byref(o), _stream()),
-                       "render_forward_frames")
-        elif train:
+        if train:
             self.train_token += 1
             self.train_rays = n
-            self.train_frames = None
-            capi.check(capi.lib.nfb_render_forward_train(self._h, C.byref(rays), C.byref(sm), C.byref(nz) if noise else None,
-                                                         C.byref(o), _stream()), "render_forward_train")
+            self.train_frames = self.n_frames if frame_index is not None else None
+        nzp = C.byref(nz) if noise else None
+        if frame_index is not None:
+            fn = capi.lib.nfb_render_forward_frames_train if train else capi.lib.nfb_render_forward_frames
+            capi.check(fn(self._h, C.byref(rays), _ptr(fi), C.byref(sm), nzp, C.byref(o), _stream()), "render_forward_frames")
+        elif train:
+            capi.check(capi.lib.nfb_render_forward_train(self._h, C.byref(rays), C.byref(sm), nzp, C.byref(o), _stream()),
+                       "render_forward_train")
         else:
-            capi.check(capi.lib.nfb_render_forward(self._h, C.byref(rays), C.byref(sm), C.byref(nz) if noise else None,
-                                                   C.byref(o), C.byref(dbg) if dbg is not None else None, _stream()),
-                       "render_forward")
+            capi.check(capi.lib.nfb_render_forward(self._h, C.byref(rays), C.byref(sm), nzp, C.byref(o),
+                                                   C.byref(dbg) if dbg is not None else None, _stream()), "render_forward")
         out["_keep"] = keep  # inputs must outlive the asynchronous launch
         return out
 
@@ -255,36 +272,19 @@ class Renderer:
 
     def repack(self, params_c, params_f):
         """nfb_repack: both networks' FP32 parameter tensors (lists in PARAM_ORDER) -> kernel-layout streams, one launch."""
-        pc = (C.c_void_p * 26)(*[t.data_ptr() for t in params_c])
-        pf = (C.c_void_p * 26)(*[t.data_ptr() for t in params_f]) if params_f is not None else None
-        capi.check(capi.lib.nfb_repack(self._h, pc, pf, _stream()), "repack")
+        capi.check(capi.lib.nfb_repack(self._h, _ptrs(params_c), _ptrs(params_f), _stream()), "repack")
 
-    def backward_into(self, out_grads, params_c, params_f, grads_c, grads_f, grad_latent):
+    def backward_into(self, out_grads, params_c, params_f, grads_c, grads_f, grad_latent, frames=False):
         """nfb_render_backward writing straight into caller-owned gradient tensors (views of a flat bucket): params_* / grads_*
-        are lists of 26 contiguous FP32 CUDA tensors in PARAM_ORDER (grads of layers_dir.3.* may be None)."""
-        og = capi.NfbOutGrads()
+        are lists of 26 contiguous FP32 CUDA tensors in PARAM_ORDER (grads of layers_dir.3.* may be None).  frames=True:
+        nfb_render_backward_frames after a multi-frame training forward, per-frame d latent into grad_latent [F,32]."""
         keep = []
-        for field, g in zip(("rgb_coarse", "disp_coarse", "acc_coarse", "rgb_fine", "disp_fine", "acc_fine", "w_last"), out_grads):
-            if g is not None:
-                keep.append(g)
-                setattr(og, field, g.data_ptr())
-        arr = lambda ts: (C.c_void_p * 26)(*[(t.data_ptr() if t is not None else None) for t in ts]) if ts is not None else None  # noqa: E731
-        capi.check(capi.lib.nfb_render_backward(self._h, C.byref(og), arr(params_c), arr(params_f), arr(grads_c), arr(grads_f),
-                                                _ptr(grad_latent), _stream()), "render_backward")
-        self._bwd_keep = keep
-
-    def backward_frames_into(self, out_grads, params_c, params_f, grads_c, grads_f, grad_latents):
-        """nfb_render_backward_frames after a multi-frame training forward, writing straight into caller-owned tensors as
-        backward_into does: parameter gradients into the 26 + 26 views, per-frame d latent into grad_latents [F,32]."""
-        og = capi.NfbOutGrads()
-        keep = []
-        for field, g in zip(("rgb_coarse", "disp_coarse", "acc_coarse", "rgb_fine", "disp_fine", "acc_fine", "w_last"), out_grads):
-            if g is not None:
-                keep.append(g)
-                setattr(og, field, g.data_ptr())
-        arr = lambda ts: (C.c_void_p * 26)(*[(t.data_ptr() if t is not None else None) for t in ts]) if ts is not None else None  # noqa: E731
-        capi.check(capi.lib.nfb_render_backward_frames(self._h, C.byref(og), arr(params_c), arr(params_f), arr(grads_c), arr(grads_f),
-                                                       _ptr(grad_latents), None, None, _stream()), "render_backward_frames")
+        args = (self._h, C.byref(_out_grads(out_grads, self.device, keep)), _ptrs(params_c), _ptrs(params_f), _ptrs(grads_c),
+                _ptrs(grads_f), _ptr(grad_latent))
+        if frames:
+            capi.check(capi.lib.nfb_render_backward_frames(*args, None, None, _stream()), "render_backward_frames")
+        else:
+            capi.check(capi.lib.nfb_render_backward(*args, _stream()), "render_backward")
         self._bwd_keep = keep
 
     def sample_images(self, data, image_index, n, draws, max_rounds, latent_table, out):
@@ -315,62 +315,42 @@ class Renderer:
         parameter gradient is formed; grads_c / grads_f are None).  frames=True: nfb_render_backward_frames after a multi-frame
         forward; grad_latent is then [F,32], and "expression" in `inputs` yields [F,76]."""
         dev = self.device
+        if frames and self.train_frames is None:
+            raise RuntimeError("backward(frames=True) needs a multi-frame training forward (render(..., train=True, "
+                               "frame_index=...)); the last training forward was a single-frame one")
         keep = []
-        og = capi.NfbOutGrads()
-        for field, g in zip(("rgb_coarse", "disp_coarse", "acc_coarse", "rgb_fine", "disp_fine", "acc_fine", "w_last"), out_grads):
-            if g is not None:
-                g = _f32c(g, dev)
-                keep.append(g)
-                setattr(og, field, g.data_ptr())
+        og = _out_grads(out_grads, dev, keep)
 
         def pack(params):
             if params is None:
-                return None, None, None
+                return None, None
             ps = [_f32c(t, dev) for t in params]
-            gs = [None if PARAM_ORDER[i].startswith("layers_dir.3") else torch.empty_like(ps[i]) for i in range(26)]
             keep.extend(ps)
-            return ((C.c_void_p * 26)(*[t.data_ptr() for t in ps]),
-                    (C.c_void_p * 26)(*[(g.data_ptr() if g is not None else None) for g in gs]), gs)
+            return ps, [None if k.startswith("layers_dir.3") else torch.empty_like(p) for k, p in zip(PARAM_ORDER, ps)]
 
-        pc, gc, grads_c = pack(params_c)
-        pf, gf, grads_f = pack(params_f)
+        pc, grads_c = pack(params_c)
+        pf, grads_f = pack(params_f)
         if not want_params:
-            gc = gf = grads_c = grads_f = None
+            grads_c = grads_f = None
+        n, nfr = self.train_rays, self.train_frames
+        shapes = dict(ray_origins=(n, 3), ray_directions=(n, 3), dir_z=(n,), background=(n, 3),
+                      expression=(nfr, 76) if frames else (76,))
+        ing = {name: torch.empty(shapes[name], device=dev, dtype=torch.float32) for name in (inputs or ())}
+        # the single-frame backward takes a null NfbInputGrads when no input gradient is asked for; the multi-frame one always
+        # takes the struct, and returns d expression [F,76] through its own argument instead
+        ig = capi.NfbInputGrads() if frames or inputs is not None else None
+        for name, t in ing.items():
+            if not (frames and name == "expression"):
+                setattr(ig, name, t.data_ptr())
+        glat = torch.empty((nfr, 32) if frames else 32, device=dev, dtype=torch.float32) if want_latent else None
+        args = (self._h, C.byref(og), _ptrs(pc), _ptrs(pf), _ptrs(grads_c), _ptrs(grads_f), _ptr(glat))
         if frames:
-            if self.train_frames is None:
-                raise RuntimeError("backward(frames=True) needs a multi-frame training forward (render(..., train=True, "
-                                   "frame_index=...)); the last training forward was a single-frame one")
-            nfr = self.train_frames
-            glat = torch.empty((nfr, 32), device=dev, dtype=torch.float32) if want_latent else None
-            gexp = torch.empty((nfr, 76), device=dev, dtype=torch.float32) if inputs and "expression" in inputs else None
-            ig, ing = capi.NfbInputGrads(), {}
-            n = self.train_rays
-            shapes = dict(ray_origins=(n, 3), ray_directions=(n, 3), dir_z=(n,), background=(n, 3))
-            for name in (inputs or ()):
-                if name != "expression":
-                    ing[name] = torch.empty(shapes[name], device=dev, dtype=torch.float32)
-                    setattr(ig, name, ing[name].data_ptr())
-            if gexp is not None:
-                ing["expression"] = gexp
-            capi.check(capi.lib.nfb_render_backward_frames(self._h, C.byref(og), pc, pf, gc, gf, _ptr(glat), _ptr(gexp), C.byref(ig),
-                                                           _stream()), "render_backward_frames")
-            self._bwd_keep = keep
-            return (grads_c, grads_f, glat, ing) if inputs is not None else (grads_c, grads_f, glat)
-        glat = torch.empty(32, device=dev, dtype=torch.float32) if want_latent else None
-        ig, ing = None, {}
-        if inputs is not None:
-            n = self.train_rays
-            shapes = dict(ray_origins=(n, 3), ray_directions=(n, 3), dir_z=(n,), background=(n, 3), expression=(76,))
-            ig = capi.NfbInputGrads()
-            for name in inputs:
-                ing[name] = torch.empty(shapes[name], device=dev, dtype=torch.float32)
-                setattr(ig, name, ing[name].data_ptr())
-        capi.check(capi.lib.nfb_render_backward_ex(self._h, C.byref(og), pc, pf, gc, gf, _ptr(glat),
-                                                   C.byref(ig) if ig is not None else None, _stream()), "render_backward")
+            capi.check(capi.lib.nfb_render_backward_frames(*args, _ptr(ing.get("expression")), C.byref(ig), _stream()),
+                       "render_backward_frames")
+        else:
+            capi.check(capi.lib.nfb_render_backward_ex(*args, C.byref(ig) if ig is not None else None, _stream()), "render_backward")
         self._bwd_keep = keep
-        if inputs is not None:
-            return grads_c, grads_f, glat, ing
-        return grads_c, grads_f, glat
+        return (grads_c, grads_f, glat, ing) if inputs is not None else (grads_c, grads_f, glat)
 
     def train_debug(self):
         d = capi.NfbTrainDebug()
@@ -409,15 +389,8 @@ class Renderer:
         rays.near_, rays.far_ = float(near), float(far)
         if background is not None:
             rays.background = background.data_ptr()
-        prec = precision or _precision
-        has_fine = num_fine > 0
-        sm = capi.NfbSampling(num_coarse, num_fine, 0, 0.0, int(bool(white_bkgd)), 0,
-                              capi.NFB_PREC_EXACT if prec == "exact" else capi.NFB_PREC_FAST,
-                              self.linspace(num_coarse).data_ptr(), self.linspace(num_fine).data_ptr() if has_fine else None)
-        o = capi.NfbOutputs(views["rgb_coarse"].data_ptr(), views["disp_coarse"].data_ptr(), views["acc_coarse"].data_ptr(),
-                            views["rgb_fine"].data_ptr() if has_fine else None,
-                            views["disp_fine"].data_ptr() if has_fine else None,
-                            views["acc_fine"].data_ptr() if has_fine else None, views["w_last"].data_ptr())
+        sm = self._sampling(num_coarse, num_fine, precision, white_bkgd)
+        o = _outputs(views, num_fine > 0)
         dbg = self._debug_dumps(views, n, num_coarse, num_fine) if debug else None
         if prof is not None:  # int64[64] CUDA tensor of phase-cycle counters
             if dbg is None:
@@ -431,11 +404,7 @@ class Renderer:
     def render_frame_host(self, pose, intrinsics, height, width, row_begin, rows, near, far, expr_host, latent_host,
                           bg_host, num_coarse, num_fine, out_host, precision=None, white_bkgd=False):
         """Host-buffer end-to-end call (bench e2e leg).  All tensors are CPU (ideally pinned) FP32."""
-        prec = precision or _precision
-        sm = capi.NfbSampling(num_coarse, num_fine, 0, 0.0, int(bool(white_bkgd)), 0,
-                              capi.NFB_PREC_EXACT if prec == "exact" else capi.NFB_PREC_FAST,
-                              self.linspace(num_coarse).data_ptr(),
-                              self.linspace(num_fine).data_ptr() if num_fine > 0 else None)
+        sm = self._sampling(num_coarse, num_fine, precision, white_bkgd)
         pose_a = (C.c_float * 12)(*[float(v) for v in pose.reshape(-1)[:12]])
         intr_a = (C.c_double * 4)(*[float(v) for v in intrinsics])
         capi.check(capi.lib.nfb_render_frame_host(self._h, pose_a, intr_a, height, width, row_begin, rows, float(near),

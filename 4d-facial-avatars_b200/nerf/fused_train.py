@@ -15,6 +15,7 @@ import torch.distributed as dist
 
 from . import _capi as capi
 from . import _engine
+from . import train_utils
 from ._engine import PARAM_ORDER
 
 
@@ -64,6 +65,7 @@ class FusedTrainer:
         # pixels the K-image sampler repeated because an image's selection came up short, per batch slot, since construction
         self.shortfall = torch.zeros(64, device=dev, dtype=torch.int64)
         self._g_rgb = {}
+        self._image_bufs = {}
         # ONE optimizer state on the device (NfbAdamDev) for every kind of step — eager, captured, one image or several — so
         # all of them take one step counter and one learning-rate schedule (nfb_adam_step_dev).  Each step writes the latent
         # row its regulariser applies to into self._row first (-1: none).
@@ -95,21 +97,62 @@ class FusedTrainer:
             self.eng.packed_owner = self
 
     def _draw_noise(self, n):
-        """rand[N,Nc], randn[N,Nc], rand[N,Nf], randn[N,Nc+Nf] — the reference's draw order for one chunk (train chunksize =
-        num_random_rays in the shipped YAML, so a batch is one chunk)."""
-        o, kw = self.opts, dict(device=self.dev, dtype=torch.float32)
-        nc, nf = o["num_coarse"], o["num_fine"]
-        out = dict(t_rand=None, n_c=None, u=None, n_f=None)
-        if o["perturb"]:
-            out["t_rand"] = torch.rand((n, nc), **kw)
-        if o["noise_std"] > 0.0:
-            out["n_c"] = torch.randn((n, nc), **kw)
-        if nf > 0:
-            if o["perturb"]:
-                out["u"] = torch.rand((n, nf), **kw)
-            if o["noise_std"] > 0.0:
-                out["n_f"] = torch.randn((n, nc + nf), **kw)
-        return out if (o["perturb"] or o["noise_std"] > 0.0) else None
+        """The reference's draws for one chunk of n rays (train chunksize = num_random_rays in the shipped YAML, so a batch is one
+        chunk); None when neither perturbation nor sigma noise is on."""
+        o = self.opts
+        return train_utils._draw_noise(n, o, self.dev, o["num_fine"] > 0) if (o["perturb"] or o["noise_std"] > 0.0) else None
+
+    def _forward_backward(self, expressions, latents, frame_index, ro, rd, background, target, n_total, noise, g, grad_latent):
+        """Frame fold, training forward, loss gradient and backward of one batch into the flat gradient bucket, d latent into
+        grad_latent.  frame_index None: one frame (expressions [76], latents [32]); otherwise ray i is conditioned on frame
+        frame_index[i] of expressions [F,76] and latents [F,32], and grad_latent is [F,32].  g: the [n,3] loss-gradient buffers."""
+        eng, o = self.eng, self.opts
+        frames = frame_index is not None
+        if frames:
+            eng.set_frames(expressions, latents)
+        else:
+            eng.set_frame(expressions, latents)
+        out = eng.render(ro, rd, o["near"], o["far"], o["num_coarse"], o["num_fine"], perturb=o["perturb"], noise_std=o["noise_std"],
+                         white_bkgd=o["white_bkgd"], background=background, noise=noise, precision=o["precision"], train=True,
+                         frame_index=frame_index)
+        g1 = g[1] if o["num_fine"] > 0 else None
+        self.loss.zero_()
+        eng.loss_mse_grad(out["rgb_coarse"], out.get("rgb_fine"), target, n_total, g[0], g1, self.loss)
+        eng.backward_into((g[0], None, None, g1, None, None, None), self._pc, self._pf, self._gc, self._gf, grad_latent, frames=frames)
+        return out
+
+    def _stepped(self):
+        """Host bookkeeping after an optimizer step: the step counter, and the packed streams now hold this trainer's weights."""
+        self._iter += 1
+        self.eng.mark_synced(self.mc, self.mf)
+        self.eng.packed_owner = self
+
+    def _adam_repack(self, row):
+        """Adam on the trainer's device state with the latent regulariser on `row` (an int, -1 for none, or a device tensor
+        holding it), zero_grad, then the re-pack."""
+        if torch.is_tensor(row):
+            self._row.copy_(row)
+        else:
+            self._row.fill_(row)
+        self.eng.adam_step_dev(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self._adam)
+        self.eng.repack(self._pc, self._pf)
+
+    def _capture(self, body, row, world=1, group=None):
+        """body() once eagerly, then body, the all-reduce (world > 1), Adam with its regulariser on `row` and the re-pack
+        captured into a CUDA graph.  Returns the graph, what the captured body returned (its buffers must outlive the graph) and
+        the renderer's buffer epoch."""
+        self._own_engine()
+        body()                      # eager warm-up: sizes the library's buffers (cudaMalloc is not capturable)
+        epoch = self.eng.buffer_epoch()
+        self.grads.zero_()
+        torch.cuda.synchronize()
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph):
+            keep = body()
+            if world > 1:
+                dist.all_reduce(self.grads, group=group)
+            self._adam_repack(row)
+        return dict(graph=graph, keep=keep, epoch=epoch)
 
     def gradients(self, ray_origins, ray_directions, target, expressions, latent_index, background=None, world=1, n_total=None,
                   noise=None, events=None, group=None):
@@ -117,26 +160,17 @@ class FusedTrainer:
         are one of `world` equal shards of a batch of n_total rays and the bucket is SUM-all-reduced (one collective), after
         which every rank holds the whole batch's gradient.  Returns the device tensor [mse_coarse, mse_fine] of THIS shard's
         share (sum over ranks = batch loss).  `events`: optional (before_collective, after_collective) CUDA events."""
-        eng, o = self.eng, self.opts
         self._own_engine()
         n = ray_origins.shape[0]
         n_total = n * world if n_total is None else n_total
-        row = self.latent_codes[latent_index]
-        eng.set_frame(expressions, row)
         if noise is None:
             noise = self._draw_noise(n)
-        out = eng.render(ray_origins, ray_directions, o["near"], o["far"], o["num_coarse"], o["num_fine"], perturb=o["perturb"],
-                         noise_std=o["noise_std"], white_bkgd=o["white_bkgd"], background=background, noise=noise,
-                         precision=o["precision"], train=True)
         g = self._g_rgb.get(n)
         if g is None:
             g = self._g_rgb[n] = (torch.empty((n, 3), device=self.dev), torch.empty((n, 3), device=self.dev))
-        self.loss.zero_()
-        has_fine = o["num_fine"] > 0
-        eng.loss_mse_grad(out["rgb_coarse"], out["rgb_fine"] if has_fine else None, _engine._f32c(target, self.dev), n_total,
-                          g[0], g[1] if has_fine else None, self.loss)
         glat = self.grads[self.lat_off + 32 * latent_index:self.lat_off + 32 * latent_index + 32]
-        eng.backward_into((g[0], None, None, g[1] if has_fine else None, None, None, None), self._pc, self._pf, self._gc, self._gf, glat)
+        self._forward_backward(expressions, self.latent_codes[latent_index], None, ray_origins, ray_directions, background,
+                               _engine._f32c(target, self.dev), n_total, noise, g, glat)
         if events is not None:
             events[0].record()
         if world > 1:
@@ -149,13 +183,8 @@ class FusedTrainer:
     def update(self):
         """Adam over the bucket (+ the latent regulariser's gradient on the last frame's row, + zero_grad) on the trainer's device
         state, then the re-pack."""
-        eng = self.eng
-        self._row.fill_(self._reg_row)
-        eng.adam_step_dev(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self._adam)
-        self._iter += 1
-        eng.repack(self._pc, self._pf)
-        eng.mark_synced(self.mc, self.mf)
-        eng.packed_owner = self
+        self._adam_repack(self._reg_row)
+        self._stepped()
 
     def _check_epoch(self, g):
         """Refuse to replay a graph whose renderer buffers were re-allocated or refilled since capture (nfb_buffer_epoch)."""
@@ -169,44 +198,23 @@ class FusedTrainer:
         from step to step lives in device memory: the inputs (static buffers filled by step_graph), the latent row index, and the
         optimizer's step counter / learning rate (the trainer's one nfb_adam_step_dev state, which its eager steps share).  The
         noise is drawn inside the graph (torch's graph-safe Philox state), in the reference's order.  With world > 1 the NCCL all-reduce of the flat bucket is part of the graph."""
-        dev, eng, o = self.dev, self.eng, self.opts
+        dev = self.dev
         n_total = n * world if n_total is None else n_total
         z = lambda *shape, dt=torch.float32: torch.zeros(shape, device=dev, dtype=dt)  # noqa: E731
         sb = dict(ro=z(n, 3), rd=z(n, 3), tgt=z(n, 3), bg=z(n, 3) if has_background else None, expr=z(76), idx=z(1, dt=torch.int64),
                   lat=z(32), glat=z(32), g0=z(n, 3), g1=z(n, 3))
         sb["rd"][:, 2] = -1.0  # a valid ray for the warm-up
         sb["adam"] = self._adam     # the optimizer state the graph advances: the trainer's one state, not a copy
-        has_fine = o["num_fine"] > 0
         table_grads = self.grads[self.lat_off:].view(-1, 32)
 
         def forward_backward():
             sb["lat"].copy_(self.latent_codes.index_select(0, sb["idx"])[0])
-            eng.set_frame(sb["expr"], sb["lat"])
-            out = eng.render(sb["ro"], sb["rd"], o["near"], o["far"], o["num_coarse"], o["num_fine"], perturb=o["perturb"],
-                             noise_std=o["noise_std"], white_bkgd=o["white_bkgd"], background=sb["bg"], noise=self._draw_noise(n),
-                             precision=o["precision"], train=True)
-            self.loss.zero_()
-            eng.loss_mse_grad(out["rgb_coarse"], out["rgb_fine"] if has_fine else None, sb["tgt"], n_total, sb["g0"],
-                              sb["g1"] if has_fine else None, self.loss)
-            eng.backward_into((sb["g0"], None, None, sb["g1"] if has_fine else None, None, None, None), self._pc, self._pf, self._gc,
-                              self._gf, sb["glat"])
+            out = self._forward_backward(sb["expr"], sb["lat"], None, sb["ro"], sb["rd"], sb["bg"], sb["tgt"], n_total,
+                                         self._draw_noise(n), (sb["g0"], sb["g1"]), sb["glat"])
             table_grads.index_add_(0, sb["idx"], sb["glat"][None])
             return out
 
-        self._own_engine()
-        forward_backward()          # eager warm-up: sizes the library's training buffers (cudaMalloc is not capturable)
-        epoch = eng.buffer_epoch()
-        self.grads.zero_()
-        torch.cuda.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            keep = forward_backward()
-            if world > 1:
-                dist.all_reduce(self.grads, group=group)
-            self._row.copy_(sb["idx"])
-            eng.adam_step_dev(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self._adam)
-            eng.repack(self._pc, self._pf)
-        self._graph = dict(graph=graph, sb=sb, n=n, keep=keep, epoch=epoch)
+        self._graph = dict(self._capture(forward_backward, sb["idx"], world, group), sb=sb, n=n)
         return self
 
     def step_graph(self, ray_origins, ray_directions, target, expressions, latent_index, background=None):
@@ -228,9 +236,7 @@ class FusedTrainer:
         sb["expr"].copy_(expressions.reshape(-1), non_blocking=True)
         sb["idx"].fill_(int(latent_index))
         g["graph"].replay()
-        self._iter += 1
-        self.eng.mark_synced(self.mc, self.mf)
-        self.eng.packed_owner = self
+        self._stepped()
         return self.loss[:2]
 
     def step(self, *args, **kwargs):
@@ -244,10 +250,8 @@ class FusedTrainer:
     def _images_buffers(self, data, k, n):
         """Per-step buffers of a K-image step (cached per shape: the chunked backward re-reads rays and frame indices)."""
         key = (k, n, data.background is not None)
-        sb = self._image_bufs.get(key) if hasattr(self, "_image_bufs") else None
+        sb = self._image_bufs.get(key)
         if sb is None:
-            if not hasattr(self, "_image_bufs"):
-                self._image_bufs = {}
             N, dev = k * n, self.dev
             z = lambda *shape, dt=torch.float32: torch.zeros(shape, device=dev, dtype=dt)  # noqa: E731
             sb = self._image_bufs[key] = dict(
@@ -263,29 +267,16 @@ class FusedTrainer:
     def _images_gradients(self, sb, k, n):
         """Forward, loss and backward of the sampled batch into the flat bucket, then the latent-table rows.  K = 1 takes the
         single-frame kernels (its regulariser stays in Adam, as in step()); K >= 2 one multi-frame forward and backward."""
-        eng, o = self.eng, self.opts
         N = k * n
         noise = self._draw_noise(N)
-        kw = dict(perturb=o["perturb"], noise_std=o["noise_std"], white_bkgd=o["white_bkgd"], background=sb["background"], noise=noise,
-                  precision=o["precision"], train=True)
         if k == 1:
-            eng.set_frame(sb["expressions"][0], sb["latents"][0])
-            out = eng.render(sb["ray_origins"], sb["ray_directions"], o["near"], o["far"], o["num_coarse"], o["num_fine"], **kw)
+            expr, lat, fi, glat = sb["expressions"][0], sb["latents"][0], None, sb["glat"][0]
         else:
-            eng.set_frames(sb["expressions"], sb["latents"])
-            out = eng.render(sb["ray_origins"], sb["ray_directions"], o["near"], o["far"], o["num_coarse"], o["num_fine"],
-                             frame_index=sb["frame_index"], **kw)
-        has_fine = o["num_fine"] > 0
-        self.loss.zero_()
-        eng.loss_mse_grad(out["rgb_coarse"], out["rgb_fine"] if has_fine else None, sb["target"], N, sb["g0"],
-                          sb["g1"] if has_fine else None, self.loss)
-        og = (sb["g0"], None, None, sb["g1"] if has_fine else None, None, None, None)
-        if k == 1:
-            eng.backward_into(og, self._pc, self._pf, self._gc, self._gf, sb["glat"][0])
-        else:
-            eng.backward_frames_into(og, self._pc, self._pf, self._gc, self._gf, sb["glat"])
-        eng.latent_rows_grad(sb["glat"], sb["img"], self.latent_codes, self.grads[self.lat_off:].view(-1, 32),
-                             0.0 if k == 1 else self.latent_reg / k)
+            expr, lat, fi, glat = sb["expressions"], sb["latents"], sb["frame_index"], sb["glat"]
+        out = self._forward_backward(expr, lat, fi, sb["ray_origins"], sb["ray_directions"], sb["background"], sb["target"], N, noise,
+                                     (sb["g0"], sb["g1"]), glat)
+        self.eng.latent_rows_grad(sb["glat"], sb["img"], self.latent_codes, self.grads[self.lat_off:].view(-1, 32),
+                                  0.0 if k == 1 else self.latent_reg / k)
         return out
 
     def _check_images(self, data, k, n, world):
@@ -345,7 +336,7 @@ class FusedTrainer:
         self._check_images(data, k, n, world)
         if has_background != (data.background is not None):
             raise ValueError("has_background must say whether the training set has a background")
-        dev, eng = self.dev, self.eng
+        dev = self.dev
         sb = dict(self._images_buffers(data, k, n))  # own copies of the per-step buffers: eager steps must not write into them
         for name, t in list(sb.items()):
             if t is not None and name != "shortfall":
@@ -357,26 +348,14 @@ class FusedTrainer:
             self._images_sample(data, sb, n, draws, max_rounds)
             return self._images_gradients(sb, k, n), draws
 
-        self._own_engine()
         sb["img"].copy_(torch.arange(k, dtype=torch.int32) % data.n_images)
         if not device_draws:
             sb["draws"].uniform_()
         before = self.shortfall.clone()
-        body()                      # eager warm-up: sizes the library's buffers (cudaMalloc is not capturable)
-        epoch = eng.buffer_epoch()
-        self.grads.zero_()
-        torch.cuda.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            keep = body()
-            if k == 1:
-                self._row.copy_(sb["img"])  # the Adam regulariser's row
-            else:
-                self._row.fill_(-1)
-            eng.adam_step_dev(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self._adam)
-            eng.repack(self._pc, self._pf)
+        # K = 1: the regulariser in Adam on the image's row; K >= 2: none (nfb_latent_rows_grad adds it)
+        g = self._capture(body, sb["img"] if k == 1 else -1)
         self.shortfall.copy_(before)  # the warm-up's selections are not a step's
-        self._igraph = dict(graph=graph, sb=sb, k=k, n=n, max_rounds=max_rounds, keep=keep, epoch=epoch)
+        self._igraph = dict(g, sb=sb, k=k, n=n, max_rounds=max_rounds)
         return self
 
     def step_images_graph(self, image_index, draws=None):
@@ -396,7 +375,5 @@ class FusedTrainer:
             sb["draws"].copy_(draws.reshape(-1)[:sb["draws"].numel()], non_blocking=True)
         self._own_engine()
         g["graph"].replay()
-        self._iter += 1
-        self.eng.mark_synced(self.mc, self.mf)
-        self.eng.packed_owner = self
+        self._stepped()
         return self.loss[:2]

@@ -12,6 +12,11 @@ def _mode_opts(options, mode):
                 white_bkgd=bool(getattr(o, "white_background", False)), chunksize=int(o.chunksize))
 
 
+def _check_ndc(options):
+    if options.dataset.no_ndc is False:
+        raise NotImplementedError("NDC rays are not implemented (every shipped config sets no_ndc: True)")
+
+
 def _check_models(model_coarse, model_fine):
     for m in (model_coarse, model_fine):
         if m is not None and not (hasattr(m, "fused_supported") and m.fused_supported()):
@@ -48,8 +53,25 @@ def _cat_noise(chunks):
     return {k: (torch.cat([c[k] for c in chunks], dim=0) if chunks[0][k] is not None else None) for k in chunks[0]}
 
 
-def _render(rays, near, far, model_coarse, model_fine, opts, expressions, background_prior, latent_code, dir_z, noise):
-    """rays [N,8] = (o, d, near, far) on a CUDA device -> the 7-tuple of predict_and_render_radiance."""
+def _chunk_noise(n, opts, device, has_fine, shard=None):
+    """The noise of a call of n rays, drawn chunk by chunk in the reference's order; None when the reference draws none.
+    shard = (begin, count, n_full) (see _shard_ctx): the draws are made for all n_full rays and rays [begin, begin + count)
+    kept."""
+    if not (opts["perturb"] or opts["noise_std"] > 0.0):
+        return None
+    begin, count, n_full = shard if shard is not None else (0, n, n)
+    assert count == n
+    chunk = opts["chunksize"]
+    full = _cat_noise([_draw_noise(min(chunk, n_full - st), opts, device, has_fine) for st in range(0, n_full, chunk)])
+    if shard is None:
+        return full
+    return {k: (v[begin:begin + count].contiguous() if v is not None else None) for k, v in full.items()}
+
+
+def _render(rays, near, far, model_coarse, model_fine, opts, expressions, background_prior, latent_code, dir_z, noise,
+            frame_index=None):
+    """rays [N,8] = (o, d, near, far) on a CUDA device -> the 7-tuple of predict_and_render_radiance.  frame_index [N]: ray i is
+    conditioned on expressions[frame_index[i]] ([F,76]) and latent_code[frame_index[i]] ([F,32])."""
     _check_models(model_coarse, model_fine)
     if opts["lindisp"]:
         raise NotImplementedError("lindisp sampling is not implemented (every shipped config sets it to False)")
@@ -58,7 +80,6 @@ def _render(rays, near, far, model_coarse, model_fine, opts, expressions, backgr
     has_fine = model_fine is not None and opts["num_fine"] > 0
     eng = _engine.renderer_for(rays.device)
     eng.sync_weights(model_coarse, model_fine if has_fine else None)
-    eng.set_frame(expressions, latent_code)
     needs_grad = torch.is_grad_enabled() and (
         any(p.requires_grad for p in model_coarse.parameters())
         or (has_fine and any(p.requires_grad for p in model_fine.parameters()))
@@ -68,8 +89,13 @@ def _render(rays, near, far, model_coarse, model_fine, opts, expressions, backgr
                 background=background_prior, dir_z=dir_z, noise=noise)
     if needs_grad:
         from ._autograd import render_with_grad
-        return render_with_grad(eng, rays, model_coarse, model_fine if has_fine else None, expressions, latent_code, args)
-    out = eng.render(rays[:, :3], rays[:, 3:6], **args)
+        return render_with_grad(eng, rays, model_coarse, model_fine if has_fine else None, expressions, latent_code, args,
+                                frame_index)
+    if frame_index is None:
+        eng.set_frame(expressions, latent_code)
+    else:
+        eng.set_frames(expressions, latent_code)
+    out = eng.render(rays[:, :3], rays[:, 3:6], frame_index=frame_index, **args)
     return (out["rgb_coarse"], out["disp_coarse"], out["acc_coarse"], out.get("rgb_fine"), out.get("disp_fine"),
             out.get("acc_fine"), out["w_last"])
 
@@ -99,8 +125,7 @@ def run_one_iter_of_nerf(height, width, focal_length, model_coarse, model_fine, 
     """Drop-in for train_utils.py:165-290.  Returns the same tuple (7 outputs; 6 in validation mode without a
     fine network), shaped like the reference's.  All rays of the call go through ONE kernel launch; the
     reference's `chunksize` only controls the order of the noise draws (and the ablation quirk)."""
-    if options.dataset.no_ndc is False:
-        raise NotImplementedError("NDC rays are not implemented (every shipped config sets no_ndc: True)")
+    _check_ndc(options)
     opts = _mode_opts(options, mode)
     has_fine = bool(model_fine) and opts["num_fine"] > 0
     shape3, shape1 = ray_directions.shape, ray_directions.shape[:-1]
@@ -111,7 +136,6 @@ def run_one_iter_of_nerf(height, width, focal_length, model_coarse, model_fine, 
     far = options.dataset.far * torch.ones_like(rd[..., :1])
     rays = torch.cat((ro, rd, near, far), dim=-1)
     chunk = opts["chunksize"]
-    bounds = list(range(0, n, chunk))
     dir_z = None
     if torch.is_tensor(ray_directions_ablation):
         # every chunk sees chunk 0 of the ablation bundle (train_utils.py:81-82).  Under data_parallel the bundle is the WHOLE
@@ -127,15 +151,7 @@ def run_one_iter_of_nerf(height, width, focal_length, model_coarse, model_fine, 
         dir_z = torch.cat(parts, dim=0)
         if _shard_ctx is not None:
             dir_z = dir_z[_shard_ctx[0]:_shard_ctx[0] + _shard_ctx[1]].contiguous()
-    noise = None
-    if opts["perturb"] or opts["noise_std"] > 0.0:
-        if _shard_ctx is not None:
-            begin, count, n_full = _shard_ctx
-            assert count == n
-            full = _cat_noise([_draw_noise(min(chunk, n_full - st), opts, rays.device, has_fine) for st in range(0, n_full, chunk)])
-            noise = {k: (v[begin:begin + count].contiguous() if v is not None else None) for k, v in full.items()}
-        else:
-            noise = _cat_noise([_draw_noise(min(chunk, n - st), opts, rays.device, has_fine) for st in bounds])
+    noise = _chunk_noise(n, opts, rays.device, has_fine, _shard_ctx)
     bg = background_prior.reshape(-1, 3) if background_prior is not None else None
     outs = list(_render(rays, options.dataset.near, options.dataset.far, model_coarse, model_fine if has_fine else None, opts, expressions, bg, latent_code, dir_z, noise))
     if mode == "validation":
@@ -156,12 +172,8 @@ def render_frames(ray_origins, ray_directions, frame_index, expressions, latent_
     expression and latent (pass `latent_table[ids]` to route the gradients back into a table), the rays and the background: a
     loss over several frames is one forward and one backward (the renderer keeps one saved training state).  frame_index outside
     [0, F) gives NaN outputs for those rays only.  Up to 1024 frames per call."""
-    if options.dataset.no_ndc is False:
-        raise NotImplementedError("NDC rays are not implemented (every shipped config sets no_ndc: True)")
+    _check_ndc(options)
     opts = _mode_opts(options, mode)
-    _check_models(model_coarse, model_fine)
-    if opts["lindisp"]:
-        raise NotImplementedError("lindisp sampling is not implemented (every shipped config sets it to False)")
     has_fine = bool(model_fine) and opts["num_fine"] > 0
     ro = ray_origins.reshape(-1, 3)
     rd = ray_directions.reshape(-1, 3)
@@ -173,26 +185,9 @@ def render_frames(ray_origins, ray_directions, frame_index, expressions, latent_
         raise ValueError("expressions [F,76] and latent_codes [F,32] must share F")
     near, far = options.dataset.near, options.dataset.far
     rays = torch.cat((ro, rd, near * torch.ones_like(rd[..., :1]), far * torch.ones_like(rd[..., :1])), dim=-1)
-    noise = None
-    if opts["perturb"] or opts["noise_std"] > 0.0:
-        chunk = opts["chunksize"]
-        noise = _cat_noise([_draw_noise(min(chunk, n - st), opts, rays.device, has_fine) for st in range(0, n, chunk)])
+    noise = _chunk_noise(n, opts, rays.device, has_fine)
     bg = background_prior.reshape(-1, 3) if background_prior is not None else None
-    eng = _engine.renderer_for(rays.device)
-    eng.sync_weights(model_coarse, model_fine if has_fine else None)
-    needs_grad = torch.is_grad_enabled() and (
-        any(p.requires_grad for p in model_coarse.parameters())
-        or (has_fine and any(p.requires_grad for p in model_fine.parameters()))
-        or any(t is not None and t.requires_grad for t in (latent_codes, rays, expressions, bg)))
-    args = dict(near=float(near), far=float(far), num_coarse=opts["num_coarse"], num_fine=opts["num_fine"] if has_fine else 0,
-                perturb=opts["perturb"], noise_std=opts["noise_std"], white_bkgd=opts["white_bkgd"], background=bg, noise=noise)
-    if needs_grad:
-        from ._autograd import render_frames_with_grad
-        return render_frames_with_grad(eng, rays, fi, model_coarse, model_fine if has_fine else None, expressions, latent_codes, args)
-    eng.set_frames(expressions, latent_codes)
-    out = eng.render(rays[:, :3], rays[:, 3:6], frame_index=fi, **args)
-    return (out["rgb_coarse"], out["disp_coarse"], out["acc_coarse"], out.get("rgb_fine"), out.get("disp_fine"),
-            out.get("acc_fine"), out["w_last"])
+    return _render(rays, near, far, model_coarse, model_fine, opts, expressions, bg, latent_codes, None, noise, frame_index=fi)
 
 
 render_frames.multi_frame = True  # nerf.parallel.data_parallel refuses it

@@ -7,7 +7,16 @@ refactor of the kernels or of the host layer must leave every digest and the lau
            forward, all 48 parameter gradients, the latent gradient and the five input gradients
   chunked  the same for 200 rays with NFB_TRAIN_MEM_MB=48 (32 rays per chunk, the last chunk ragged)
 
-each in both precision modes, plus the launches each case took.  Usage:
+each in both precision modes, plus the launches each case took; then, through the host paths above the renderer:
+
+  frames   2048 rays of three frames, one multi-frame training forward and backward(frames=True): the seven outputs, the
+           parameter gradients, every frame's latent and expression gradient and the other input gradients (both precisions)
+  dropin/* run_one_iter_of_nerf and render_frames in training mode, then loss.backward(): the outputs and the gradients of
+           the parameters, latents, expressions and background
+  trainer/*  three steps each of FusedTrainer.step, step_graph, step_images at K = 1 and K = 3, and step_images_graph (K = 3):
+           the parameter bucket and the loss after every step
+
+Usage:
 
   python tools/output_digests.py OUT.json          # NFB_LIB selects the library, as everywhere
   NFB_LIB=/path/to/other/libnfb.so python tools/output_digests.py OTHER.json && cmp OUT.json OTHER.json
@@ -91,6 +100,85 @@ def main():
             train_case(f"chunked/{prec}", 200, prec, 1032)
         finally:
             del os.environ["NFB_TRAIN_MEM_MB"]
+
+    n, nfr = 2048, 3
+    g = torch.Generator().manual_seed(1033)
+    fexpr, flat = (torch.randn(nfr, 76, generator=g) * 0.5).to(dev), (torch.randn(nfr, 32, generator=g) * 0.1).to(dev)
+    fidx = torch.randint(0, nfr, (n,), generator=g).to(dev)
+    nz = O.draw_noise(n, O.Sampling(64, 64, True, 0.1, False, 2048), g)
+    fnoise = {k: getattr(nz, k).to(dev) for k in ("t_rand", "n_c", "u", "n_f")}
+    fdz = (torch.rand(n, generator=g) * 2.0 - 1.0).to(dev)
+    fgouts = [((torch.rand(sh, generator=g) - 0.3) / n).to(dev) for sh in [(n, 3), (n,), (n,), (n, 3), (n,), (n,), (n,)]]
+    for prec in ("fast", "exact"):
+        l0 = eng.launch_count()
+        eng.set_frames(fexpr, flat)
+        out = eng.render(ro[:n].contiguous(), rd[:n].contiguous(), NEAR, FAR, 64, 64, perturb=True, noise_std=0.1,
+                         background=bg[:n].contiguous(), dir_z=fdz, noise=fnoise, precision=prec, train=True, frame_index=fidx)
+        gc, gf, gl, ing = eng.backward(fgouts, pc, pf, want_latent=True, want_params=True, inputs=INPUTS, frames=True)
+        named = [(k, out[k]) for k in OUTPUTS]
+        named += [(f"grad_coarse/{PARAM_ORDER[i]}", t) for i, t in enumerate(gc) if t is not None]
+        named += [(f"grad_fine/{PARAM_ORDER[i]}", t) for i, t in enumerate(gf) if t is not None]
+        named += [("grad_latent", gl)] + [("grad_" + k, t) for k, t in sorted(ing.items())]
+        record(f"frames/{prec}", named, l0)
+
+    # the drop-in API in training mode: noise drawn by the driver from torch's seeded generator, gradients by loss.backward()
+    blk = dict(num_coarse=64, num_fine=64, perturb=True, lindisp=False, radiance_field_noise_std=0.1, white_background=False,
+               chunksize=1024)
+    cfg = nerf.CfgNode(dict(nerf=dict(use_viewdirs=True, train=blk), dataset=dict(no_ndc=True, near=NEAR, far=FAR)))
+    target = torch.rand(n, 3, generator=g).to(dev)
+    for case in ("run_one_iter", "render_frames"):
+        dc, df = model(100), model(101)
+        frames = case == "render_frames"
+        e = (fexpr if frames else expr).clone().requires_grad_(True)
+        lt = (flat if frames else latent).clone().requires_grad_(True)
+        b = bg[:n].clone().requires_grad_(True)
+        torch.manual_seed(1034)
+        l0 = eng.launch_count()
+        if frames:
+            outs = nerf.render_frames(ro[:n], rd[:n], fidx, e, lt, dc, df, cfg, background_prior=b)
+        else:
+            outs = nerf.run_one_iter_of_nerf(48, 48, fr["intrinsics"], dc, df, ro[:n], rd[:n], cfg, mode="train", expressions=e,
+                                             background_prior=b, latent_code=lt)
+        loss = ((outs[0] - target) ** 2).mean() + ((outs[3] - target) ** 2).mean() + 0.005 * lt.norm()
+        loss.backward()
+        named = [(k, t) for k, t in zip(OUTPUTS, outs)] + [("loss", loss)]
+        named += [(f"grad_coarse/{k}", p.grad) for k, p in dc.named_parameters() if p.grad is not None]
+        named += [(f"grad_fine/{k}", p.grad) for k, p in df.named_parameters() if p.grad is not None]
+        named += [("grad_latent", lt.grad), ("grad_expression", e.grad), ("grad_background", b.grad)]
+        record(f"dropin/{case}", named, l0)
+
+    # FusedTrainer: three steps of each kind from the same initial state, the bucket and the loss after every step
+    from nerf import fused_train, ray_sampler
+    n_img, H, W, npi = 3, 32, 32, 256
+    ifr = [O.synthetic_frame(30 + i, H, W) for i in range(n_img)]
+    data = ray_sampler.TrainImages(torch.rand(n_img, H, W, 3, generator=g).to(dev),
+                                   torch.stack([f["pose"][:3, :4].reshape(-1) for f in ifr]), torch.stack([f["expr"] for f in ifr]),
+                                   [(8, 24, 6, 26), (4, 20, 10, 30), (10, 30, 0, 20)], ifr[0]["intrinsics"],
+                                   background=ifr[0]["bg"], device=dev)
+    sro, srd, stgt, sbg = ro[:npi].contiguous(), rd[:npi].contiguous(), target[:npi].contiguous(), bg[:npi].contiguous()
+    for case in ("step", "step_graph", "step_images_k1", "step_images_k3", "step_images_graph"):
+        torch.manual_seed(1035)
+        tr = fused_train.FusedTrainer(model(100), model(101), n_latent=n_img, num_coarse=64, num_fine=64, perturb=True,
+                                      noise_std=0.1, near=NEAR, far=FAR, latent_codes=torch.randn(n_img, 32, generator=g) * 0.1)
+        if case == "step_graph":
+            tr.capture(npi)
+        elif case == "step_images_graph":
+            tr.capture_images(data, 3, npi // 3, max_rounds=8)
+        l0 = eng.launch_count()
+        named = []
+        for i in range(3):
+            if case == "step":
+                loss = tr.step(sro, srd, stgt, expr, i % n_img, background=sbg)
+            elif case == "step_graph":
+                loss = tr.step_graph(sro, srd, stgt, expr, i % n_img, background=sbg)
+            elif case == "step_images_k1":
+                loss = tr.step_images(data, [i % n_img], npi, max_rounds=8)
+            elif case == "step_images_k3":
+                loss = tr.step_images(data, [i % n_img, (i + 2) % n_img, i % n_img], npi // 3, max_rounds=8)
+            else:
+                loss = tr.step_images_graph([i % n_img, (i + 2) % n_img, i % n_img])
+            named += [(f"params/{i}", tr.params.clone()), (f"loss/{i}", loss.clone())]
+        record(f"trainer/{case}", named, l0)
 
     res["device"] = torch.cuda.get_device_name(0)
     with open(sys.argv[1], "w") as f:
