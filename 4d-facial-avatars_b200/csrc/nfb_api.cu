@@ -39,6 +39,9 @@ struct NfbHandle {
   int num_sms = 0;
   nfb::NetBuffers net[2];
   bool frame_set = false;
+  // exact-grad mode: set by the first exact-grad training forward, which allocates and writes the backward stream's lo halves; from
+  // then on every weight load and re-pack rewrites them (NetBuffers::stream_bwd_lo).  Fast and exact handles never pay for them.
+  bool bwd_lo = false;
   long long launches = 0;
   // nfb_buffer_epoch = frees + tr.frees: the buffers a training step's launches take an address of count their re-allocations
   // into one of the two (the linspace tables count every refill for another n)
@@ -82,6 +85,7 @@ struct NfbHandle {
     DevBuf<float> bias[2]{DevBuf<float>(&frees), DevBuf<float>(&frees)};
     DevBuf<float> lin_c{&frees}, lin_f{&frees};
     int chunk_rays = 0, precision = 0;
+    bool hilo = false;                   // an exact-grad forward: 2 MiB records with lo halves, the *_x3 backward kernels
     DevBuf<float> scratch_out{&frees};   // [11 * chunk_rays] outputs of the re-run forwards (discarded)
     // multi-frame forward (nfb_render_forward_frames_train): the frame table and conditioning vectors it rendered with (copied,
     // as bias / cond are), the frame slot of every ray (written by the forward), and the backward's per-ray / per-frame sums
@@ -203,6 +207,7 @@ int nfb_load_weights(NfbHandle* h, int which, const float* const params[26], voi
   nfb::NetBuffers* const nbs[2] = {&nb, nullptr};
   const float* const* const ps[2] = {params, nullptr};
   NFB_CUDA(nfb::launch_repack(nbs, ps, 1, st, &h->launches));  // forward streams, transposed backward stream, bias / column blocks
+  if (h->bwd_lo) NFB_CUDA(nfb::launch_bwd_lo(nbs, 1, st, &h->launches));
   nb.loaded = true;
   h->frame_set = false;  // folded biases are stale
   h->n_frames = 0;
@@ -217,6 +222,7 @@ int nfb_repack(NfbHandle* h, const float* const params_coarse[26], const float* 
   nfb::NetBuffers* const nbs[2] = {&h->net[0], &h->net[1]};
   const float* const* const ps[2] = {params_coarse, params_fine};
   NFB_CUDA(nfb::launch_repack(nbs, ps, params_fine ? 2 : 1, static_cast<cudaStream_t>(stream), &h->launches));
+  if (h->bwd_lo) NFB_CUDA(nfb::launch_bwd_lo(nbs, params_fine ? 2 : 1, static_cast<cudaStream_t>(stream), &h->launches));
   h->net[0].loaded = true;
   if (params_fine) h->net[1].loaded = true;
   h->frame_set = false;  // folded biases are stale
@@ -314,7 +320,7 @@ static size_t train_budget(NfbHandle* h) {
 // (Re)size the buffers a training launch of geometry g and its backward write.
 static int ensure_train_buffers(NfbHandle::Train& tr, const nfb::TileGeom& g, int num_sms) {
   const size_t n = (size_t)g.n_rays, tiles = g.tiles();
-  NFB_CUDA(tr.rec.reserve(tiles * nfb::kRecBytes));
+  NFB_CUDA(tr.rec.reserve(tiles * nfb::rec_stride(tr.hilo)));
   NFB_CUDA(tr.draw.reserve(tiles * 512));
   NFB_CUDA(tr.bsum.reserve(8 * n));
   NFB_CUDA(tr.dw_ws.reserve(nfb::dw_workspace_floats(num_sms)));
@@ -344,7 +350,7 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
   const int nc = sm->num_coarse, nf = sm->num_fine;
   if (nc < 3 || nf < 0 || nc + nf > 512) return NFB_ERR_UNSUPPORTED;
   if (sm->lindisp) return NFB_ERR_UNSUPPORTED;
-  if (sm->precision != NFB_PREC_FAST && sm->precision != NFB_PREC_EXACT) return NFB_ERR_INVALID;
+  if (sm->precision != NFB_PREC_FAST && sm->precision != NFB_PREC_EXACT && sm->precision != NFB_PREC_EXACT_GRAD) return NFB_ERR_INVALID;
   if (multi && !rays->o) return NFB_ERR_UNSUPPORTED;  // in-kernel ray generation is one pose per call
   if (!h->net[0].loaded || (nf > 0 && !h->net[1].loaded) || (multi ? h->n_frames < 1 : !h->frame_set)) return NFB_ERR_STATE;
   if (!out->rgb_coarse || !out->disp_coarse || !out->acc_coarse) return NFB_ERR_INVALID;
@@ -386,7 +392,7 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
     }
   }
   if (noise) { p.t_rand = noise->t_rand; p.noise_c = noise->sigma_noise_c; p.u_rand = noise->u; p.noise_f = noise->sigma_noise_f; }
-  const bool exact = sm->precision == NFB_PREC_EXACT;
+  const bool exact = sm->precision != NFB_PREC_FAST;  // exact-grad renders with exact mode's streams and kernels
   for (int n = 0; n < 2; ++n) {
     p.wstream[n] = exact ? h->net[n].stream_x3.get() : h->net[n].stream_x1.get();
     // a multi-frame call takes the folded rows of steps 0 and 3 from the frame table; its other bias entries are the static ones
@@ -408,9 +414,17 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
     tr.valid = false;
     tr.per_ray_formed = tr.rows_formed = tr.frame_sums_formed = tr.bwd_formed = false;
     int rc;
+    tr.hilo = sm->precision == NFB_PREC_EXACT_GRAD;
+    if (tr.hilo && !h->bwd_lo) {  // the first exact-grad training forward: the lo halves of the loaded backward streams
+      for (int n = 0; n < 2; ++n) NFB_CUDA(h->net[n].stream_bwd_lo.reserve(nfb::kBwdStreamBytes));
+      nfb::NetBuffers* const nbs[2] = {&h->net[0], &h->net[1]};
+      NFB_CUDA(nfb::launch_bwd_lo(nbs, h->net[1].loaded ? 2 : 1, st, &h->launches));
+      h->bwd_lo = true;
+    }
+    const size_t rec_bytes = nfb::rec_stride(tr.hilo);
     // a multi-frame backward also keeps per-ray dY0 / dY3 sums: 2 passes x kFrameRows floats = 4 KiB per ray, in the budget too
     const size_t ray_bytes = multi ? 2 * nfb::kFrameRows * sizeof(float) : 0;
-    tr.chunked = p.geom.tiles() * nfb::kRecBytes + (size_t)p.geom.n_rays * ray_bytes > train_budget(h);
+    tr.chunked = p.geom.tiles() * rec_bytes + (size_t)p.geom.n_rays * ray_bytes > train_budget(h);
     tr.multi = multi;
     if (multi) {
       // the frame table and conditioning vectors this forward rendered with: a later nfb_set_frames must not change them
@@ -431,11 +445,11 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
       // e.g. a whole frame rendered with gradients enabled: 1.5-2 MiB of records per ray.  Keep the launch parameters, produce
       // the outputs with the evaluation kernel now, and let the backward re-run the training forward in chunks that fit.
       if (!rays->o) { g_last_cuda_error = "training forward over budget needs explicit rays (o, d)"; return NFB_ERR_UNSUPPORTED; }
-      size_t units = train_budget(h) / ((size_t)p.geom.tiles_per_unit() * nfb::kRecBytes + (size_t)p.geom.rays_per_unit * ray_bytes);
+      size_t units = train_budget(h) / ((size_t)p.geom.tiles_per_unit() * rec_bytes + (size_t)p.geom.rays_per_unit * ray_bytes);
       if (units < 1) units = 1;
       tr.chunk_rays = (int)(units * p.geom.rays_per_unit);
       tr.full = p;
-      tr.precision = exact ? 1 : 0;
+      tr.precision = sm->precision;
       // the re-run forwards must read THIS call's frame and depth tables, whatever is rendered before the backward
       for (int n = 0; n < (nf > 0 ? 2 : 1); ++n) {
         NFB_CUDA(tr.bias[n].reserve(nfb::kBiasFloats));
@@ -466,8 +480,10 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
     tr.has_rays = rays->o != nullptr; tr.has_dir_z = rays->dir_z != nullptr;
     tr.geom = p.geom; tr.has_bg = rays->background != nullptr; tr.white_bkgd = p.white_bkgd;
   }
-  if (multi) NFB_CUDA(nfb::launch_render_frames(p, exact ? 1 : 0, h->num_sms, st, &h->launches));
-  else NFB_CUDA(nfb::launch_render(p, exact ? 1 : 0, h->num_sms, st, &h->launches));
+  // exact-grad mode runs its own kernel only where records are saved (p.save_rec); evaluation renders and the over-budget
+  // training forward, which saves nothing until the backward re-runs it chunk by chunk, run exact mode's
+  if (multi) NFB_CUDA(nfb::launch_render_frames(p, sm->precision, h->num_sms, st, &h->launches));
+  else NFB_CUDA(nfb::launch_render(p, sm->precision, h->num_sms, st, &h->launches));
   if (train) h->tr.valid = true;
   return NFB_OK;
 }
@@ -576,12 +592,14 @@ static int backward_impl(NfbHandle* h, const NfbOutGrads* og, const float* const
     c.rec = tr.rec.get(); c.draw = tr.draw.get(); c.scal = scal;
     c.wstream[0] = h->net[0].stream_bwd.get();
     c.wstream[1] = h->net[fine ? 1 : 0].stream_bwd.get();
-    NFB_CUDA(nfb::launch_chain(c, h->num_sms, st, &h->launches));
+    c.wstream_lo[0] = h->net[0].stream_bwd_lo.get();
+    c.wstream_lo[1] = h->net[fine ? 1 : 0].stream_bwd_lo.get();
+    NFB_CUDA(nfb::launch_chain(c, h->num_sms, st, &h->launches, tr.hilo));
     // input-only: the PE jobs only serve d latent / d expression (a multi-frame backward forms those from the per-frame sums)
     const bool dw = !input_only || (!tr.multi && (grad_latent || ig.expression));
     if (dw) {
       d.rec = tr.rec.get(); d.ws = tr.dw_ws.get(); d.scal = scal;
-      NFB_CUDA(nfb::launch_dw(d, h->num_sms, st, &h->launches, input_only));  // both networks in one launch
+      NFB_CUDA(nfb::launch_dw(d, h->num_sms, st, &h->launches, input_only, tr.hilo));  // both networks in one launch
       tr.dw_parts[0] = d.parts[0]; tr.dw_parts[1] = d.parts[1]; tr.dw_stride = d.ws_stride;
       tr.dw_pe_only = input_only;
     }
@@ -589,7 +607,7 @@ static int backward_impl(NfbHandle* h, const NfbOutGrads* og, const float* const
       nfb::FrameSumParams fs = {};
       fs.rec = tr.rec.get(); fs.geom = g; fs.scal = scal; fs.frame = tr.frame.get(); fs.n_frames = tr.n_frames;
       fs.raysum = tr.raysum.get(); fs.fsum = tr.fsum.get();
-      NFB_CUDA(nfb::launch_frame_sums(fs, st, &h->launches));
+      NFB_CUDA(nfb::launch_frame_sums(fs, st, &h->launches, tr.hilo));
     }
     NFB_CUDA(nfb::launch_grad_reduce(dw ? &d : nullptr, input_only, tr.bsum.get(), g.n_rays, g.passes(), acc, h->num_sms, st,
                                      &h->launches));
@@ -605,7 +623,7 @@ static int backward_impl(NfbHandle* h, const NfbOutGrads* og, const float* const
       a.ray_dn = tr.ray_dn.get(); a.ray_bg = tr.ray_bg.get();
       auto at = [&](float* p, int w) { return p ? p + (size_t)w * begin : nullptr; };
       a.g_o = at(ig.ray_origins, 3); a.g_d = at(ig.ray_directions, 3); a.g_dir_z = at(ig.dir_z, 1); a.g_bg = at(ig.background, 3);
-      NFB_CUDA(nfb::launch_input_grads(r, a, h->num_sms, st, &h->launches));
+      NFB_CUDA(nfb::launch_input_grads(r, a, h->num_sms, st, &h->launches, tr.hilo));
     }
     return NFB_OK;
   };
@@ -687,7 +705,7 @@ int nfb_train_debug(NfbHandle* h, NfbTrainDebug* out) {
   if (!h || !out) return NFB_ERR_INVALID;
   if (!h->tr.valid || h->tr.chunked) return NFB_ERR_STATE;  // chunked: the buffers only ever hold one chunk
   const NfbHandle::Train& tr = h->tr;
-  out->records = tr.rec.get(); out->n_tiles = (long long)tr.geom.tiles(); out->record_bytes = nfb::kRecBytes;
+  out->records = tr.rec.get(); out->n_tiles = (long long)tr.geom.tiles(); out->record_bytes = (int32_t)nfb::rec_stride(tr.hilo);
   out->d_raw = tr.draw.get(); out->acc_coarse = tr.acc[0].get(); out->acc_fine = tr.acc[1].get(); out->acc_floats = nfb::kAccFloats;
   out->scale = tr.scal.get(); out->z_coarse = tr.z_c.get(); out->raw_coarse = tr.raw_c.get(); out->z_fine = tr.z_f.get();
   out->raw_fine = tr.raw_f.get();
@@ -723,6 +741,8 @@ int nfb_debug_weights(NfbHandle* h, int net, NfbWeightDebug* out) {
   out->w0c = nb.w0c.get(); out->w3c = nb.w3c.get(); out->wd0b_t = nb.wd0b_t.get();
   out->x1_bytes = nfb::kStreamBytesX1; out->x3_bytes = nfb::kStreamBytesX3; out->bwd_bytes = nfb::kBwdStreamBytes;
   out->bias_floats = nfb::kBiasFloats;
+  out->bwd_lo = h->bwd_lo ? nb.stream_bwd_lo.get() : nullptr;
+  out->bwd_lo_bytes = h->bwd_lo ? nfb::kBwdStreamBytes : 0;
   return NFB_OK;
 }
 

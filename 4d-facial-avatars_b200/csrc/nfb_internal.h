@@ -53,6 +53,7 @@ struct NetBuffers {
   DevBuf<float> w3c;          // [256,108] conditioning columns of layers_xyz.3
   DevBuf<float> wd0b_t;       // [24,128] direction columns of layers_dir.0, transposed
   DevBuf<uint8_t> stream_bwd; // kBwdStreamBytes: transposed FP16 weights for the backward chain (nfb_train.cu)
+  DevBuf<uint8_t> stream_bwd_lo;  // kBwdStreamBytes: its lo half (exact-grad mode; allocated and written from the first such forward)
   bool loaded = false;
 };
 
@@ -132,6 +133,7 @@ struct ChainParams {
   const float* draw;
   const float* scal;            // [0] = loss scale, [1] = 1 / scale
   const uint8_t* wstream[2];    // backward weight streams (coarse, fine)
+  const uint8_t* wstream_lo[2]; // their lo halves (the exact-grad chain only)
 };
 struct DwParams {  // ONE launch covers both networks: the first parts[0] * groups CTAs work on network 0, the rest on network 1
   const uint8_t* rec;
@@ -156,9 +158,11 @@ int debug_jobs_dw(int index, uint32_t* out);
 int debug_dw_split(uint32_t* io);  // io: {num_sms, tiles net 0, tiles net 1} -> {parts0, parts1, groups}
 cudaError_t train_kernels_setup();
 cudaError_t launch_composite_bwd(const CompBwdParams& q, float* scal, cudaStream_t st, long long* launches);
-cudaError_t launch_chain(const ChainParams& p, int num_sms, cudaStream_t st, long long* launches);
+// hilo (exact-grad mode, here and below): the records are 2 MiB apart and hold lo halves (nfb_layout.h rec_stride); the kernels
+// multiply and sum hi + lo.
+cudaError_t launch_chain(const ChainParams& p, int num_sms, cudaStream_t st, long long* launches, bool hilo = false);
 // Writes one partial per (network, part) into p.ws and fills in p.parts / p.ws_stride for launch_grad_reduce.
-cudaError_t launch_dw(DwParams& p, int num_sms, cudaStream_t st, long long* launches, bool pe_only = false);
+cudaError_t launch_dw(DwParams& p, int num_sms, cudaStream_t st, long long* launches, bool pe_only = false, bool hilo = false);
 size_t dw_workspace_floats(int num_sms);  // floats of DwParams::ws that either weight-gradient launch may write
 // One launch: acc[net] += the partials of the weight-gradient launch `d` in ascending part order (d == nullptr: there was none),
 // and acc[pass][kAccBRaw..+4] += the compositing backward's per-ray sums bsum[pass][0..n_rays) in a fixed order.
@@ -169,17 +173,20 @@ cudaError_t launch_grad_reduce(const DwParams* d, bool pe_only, const float* bsu
 cudaError_t launch_finalize_all(const float* const params_c[26], float* const grads_c[26], const float* acc_c,
                                 const float* const params_f[26], float* const grads_f[26], const float* acc_f, const float* cond,
                                 float* latent_out, cudaStream_t st, long long* launches, float* expr_out = nullptr);
-cudaError_t launch_frame_sums(const FrameSumParams& p, cudaStream_t st, long long* launches);
+cudaError_t launch_frame_sums(const FrameSumParams& p, cudaStream_t st, long long* launches, bool hilo = false);
 // d latent_f, d expression_f [n_frames][32 / 76] from the per-frame sums, and (grads_* non-null) the conditioning columns of dW0 / dW3
 // as sum_f db_f (x) c_f.  One launch.
 cudaError_t launch_frames_grad(const float* const params_c[26], float* const grads_c[26], const float* const params_f[26],
                                float* const grads_f[26], const float* fsum, const float* fcond, int n_frames, float* latent_out,
                                float* expr_out, cudaStream_t st, long long* launches);
-cudaError_t launch_input_grads(const InGradRowParams& r, const InGradRayParams& q, int num_sms, cudaStream_t st, long long* launches);
+cudaError_t launch_input_grads(const InGradRowParams& r, const InGradRayParams& q, int num_sms, cudaStream_t st, long long* launches,
+                               bool hilo = false);
 
 // Two launches (fold, pack): FP32 parameters of n_nets (1 or 2) networks -> forward / backward weight streams, bias block, conditioning and
 // direction columns (nfb_pack.cu: repack_kernel).
 cudaError_t launch_repack(NetBuffers* const nb[2], const float* const* const params[2], int n_nets, cudaStream_t st, long long* launches);
+// One launch: the lo half of the backward stream of n_nets networks (stream_bwd_lo, reserved by the caller) from their x3 streams.
+cudaError_t launch_bwd_lo(NetBuffers* const nb[2], int n_nets, cudaStream_t st, long long* launches);
 // One launch: per-frame bias fold of the loaded networks + cond[108] = [expr / 3 ; latent].
 cudaError_t launch_frame_fold(NetBuffers* const nb[2], int n_nets, const float* expr, const float* latent, float* cond,
                               cudaStream_t st, long long* launches);
@@ -192,7 +199,8 @@ cudaError_t launch_loss_grad(const float* rgb_c, const float* rgb_f, const float
 cudaError_t launch_adam_dev(float* p, float* g, float* m, float* v, long long n, void* dev_state, cudaStream_t st, long long* launches);
 cudaError_t launch_adam(float* p, float* g, float* m, float* v, long long n, float lr, float b1, float b2, float eps, int step,
                         float grad_scale, long long reg_off, float reg_w, cudaStream_t st, long long* launches);
-// precision: 0 = fast (x1), 1 = exact (x3).  num_sms = CTAs to launch at most.
+// precision: 0 = fast (x1), 1 = exact (x3), 2 = exact-grad (exact mode's kernels; a training forward writes the lo records too).
+// num_sms = CTAs to launch at most.
 cudaError_t launch_render(const RenderParams& p, int precision, int num_sms, cudaStream_t st, long long* launches);
 // The multi-frame instantiations (render_frames_kernel): p.frame and p.fbias select each ray's rows of steps 0 and 3.
 cudaError_t launch_render_frames(const RenderParams& p, int precision, int num_sms, cudaStream_t st, long long* launches);

@@ -215,6 +215,10 @@ constexpr int kRecDY6 = kRecDY0 + 6 * 65536;      // dY6..dY8, 128 features
 constexpr int kRecDRaw = kRecDY6 + 3 * 32768;     // scaled (d rgb_raw[3], d sigma_raw) image, 16 rows (4 used)
 constexpr int kRecBytes = kRecDRaw + 4096;
 static_assert(kRecBytes == (1 << 20), "tile record is 1 MiB");
+// Exact-grad mode (NFB_PREC_EXACT_GRAD) keeps a second MiB behind every record: at kRecBytes + the offset of each image above,
+// its lo half, lo = FP16(x - hi), so that hi + lo carries the value to ~2^-22 relative.  The training forward writes the lo images
+// of PE, h0..h5, g0..g2 and PEd; the dX chain those of dY0..dY8 and d raw.  The mask block has no lo half (its bytes are unused).
+NFB_HD constexpr size_t rec_stride(bool hilo) { return hilo ? 2 * (size_t)kRecBytes : (size_t)kRecBytes; }
 NFB_HD constexpr int rec_x_off(int layer) { return layer < 6 ? kRecH0 + layer * 65536 : kRecG0 + (layer - 6) * 32768; }
 NFB_HD constexpr int rec_dy_off(int layer) { return layer < 6 ? kRecDY0 + layer * 65536 : kRecDY6 + (layer - 6) * 32768; }
 NFB_HD constexpr int rec_width(int layer) { return layer < 6 ? 256 : 128; }
@@ -242,7 +246,8 @@ NFB_HD constexpr StepInfo bwd_step_info(int s) {
 // laid out by one rule: a unit = all N rows of a step x one 64-wide K atom, units in consumption order (step by step, K atom
 // by K atom), so unit u of step s starts at (offset of step s) + u * rows * 128.  The x1 stream holds FP16 weights; the x3
 // stream of exact mode holds the hi unit then the lo unit at twice the x1 offset.  Written by repack_kernel (nfb_pack.cu),
-// read by the kernels through the unit program below.
+// read by the kernels through the unit program below.  The backward stream has a lo half of its own for exact-grad mode, a
+// separate buffer with the backward stream's layout (bwd_lo_kernel, nfb_pack.cu).
 enum : int { kFwdStream = 0, kBwdStream = 1 };
 NFB_HD constexpr int stream_steps(int stream) { return stream == kFwdStream ? kNumSteps : kBwdSteps; }
 NFB_HD constexpr StepInfo stream_step(int stream, int s) { return stream == kFwdStream ? step_info(s) : bwd_step_info(s); }

@@ -184,6 +184,42 @@ __global__ void __launch_bounds__(256) repack_kernel(const RepackArgs a) {
   gather_elem(np, b * 256 + threadIdx.x, a.bias_static[net], a.w0c[net], a.w3c[net], a.wd0b_t[net]);
 }
 
+// The lo half of the backward stream (exact-grad mode): element (n, k) of unit (s, u) is the lo entry of the forward weight that
+// pack_bwd_chunk transposes, read from exact mode's x3 stream, so it has the forward's rounding (lo = FP16(w - hi), no saturation)
+// and needs no FP32 parameters.  Same block decomposition as the backward part of repack_kernel.
+__device__ __forceinline__ uint16_t bwd_lo_elem(const uint8_t* __restrict__ x3, int s, int u, int n, int kl) {
+  const StepInfo si = bwd_step_info(s);
+  const int kk = (u - si.pe_first) * 64 + kl;  // output feature of the forward layer (activation atoms)
+  int fs, row = kk, k = n;                     // forward step, its weight row and K index
+  switch (s) {
+    case 0: if (kl >= 3) return 0; fs = 9; row = kl; break;                          // fc_rgb.weight[kl][n]
+    case 1: fs = 8; break;
+    case 2: fs = 7; break;
+    case 3: if (si.pe_first && u == 0) { if (kl != 3) return 0; row = 128; } fs = 6; break;  // m2 row, then M1
+    case 4: fs = 5; break;
+    case 5: fs = 4; break;
+    case 6: fs = 3; k = 64 + n; break;                                               // layers_xyz.3[:, 171:]
+    case 7: fs = 2; break;
+    default: fs = 1; break;
+  }
+  const size_t lo_unit = 2 * (size_t)unit_offset(kFwdStream, fs, k >> 6) + (size_t)unit_rows(kFwdStream, fs) * 128;
+  return *reinterpret_cast<const uint16_t*>(x3 + lo_unit + sw128_offset(row, k & 63));
+}
+struct BwdLoArgs { const uint8_t* x3[2]; uint8_t* lo[2]; };
+__global__ void __launch_bounds__(256) bwd_lo_kernel(const BwdLoArgs a) {
+  const int net = blockIdx.y, b = blockIdx.x;
+  const int s = b / (8 * kMaxBwdUnits), r = b % (8 * kMaxBwdUnits), u = r / 8, idx = (r % 8) * 256 + threadIdx.x;
+  if (u >= bwd_step_info(s).k_atoms) return;
+  const int rows = unit_rows(kBwdStream, s);
+  if (idx >= rows * 8) return;
+  const int c16 = idx & 7, n = idx >> 3;
+  __align__(16) uint16_t h[8];
+#pragma unroll
+  for (int e = 0; e < 8; ++e) h[e] = bwd_lo_elem(a.x3[net], s, u, n, c16 * 8 + e);
+  const int off = unit_offset(kBwdStream, s, u);
+  *reinterpret_cast<uint4*>(a.lo[net] + off + n * 128 + ((c16 ^ (n & 7)) << 4)) = *reinterpret_cast<const uint4*>(h);
+}
+
 // Per-frame conditioning in ONE launch.  Per network kFoldSlabs blocks: bias_frame = bias_static, then rows of step 0 and step 3
 // += W[:, 63:171] . [expr/3 ; latent] (coalesced row loads, the accumulation order of a scalar loop).  One more block:
 // cond[108] = [expr/3 ; latent] (the backward's chain rule through this fold needs it).
@@ -289,6 +325,14 @@ cudaError_t launch_repack(NetBuffers* const nb[2], const float* const* const par
   fold_feat_kernel<<<dim3(144, 4, n_nets), 256, 0, st>>>(f);
   ++*launches;
   repack_kernel<<<dim3(kRepackBlocks, n_nets), 256, 0, st>>>(a);
+  ++*launches;
+  return cudaGetLastError();
+}
+
+cudaError_t launch_bwd_lo(NetBuffers* const nb[2], int n_nets, cudaStream_t st, long long* launches) {
+  BwdLoArgs a = {};
+  for (int n = 0; n < n_nets; ++n) { a.x3[n] = nb[n]->stream_x3.get(); a.lo[n] = nb[n]->stream_bwd_lo.get(); }
+  bwd_lo_kernel<<<dim3(kBwdBlocks, n_nets), 256, 0, st>>>(a);
   ++*launches;
   return cudaGetLastError();
 }

@@ -1,5 +1,5 @@
 // nfb_render.cu — the per-ray hot path as ONE persistent sm_90a kernel: both precision modes, the training forward (SAVE:
-// also writes the activation records the backward reads) and the debug probes.
+// also writes the activation records the backward reads; exact-grad mode's also their lo halves) and the debug probes.
 //
 // Reference path replaced (nerface_code/nerf-pytorch/nerf/):
 //   train_utils.py:36-162  predict_and_render_radiance   (sampling, coarse->fine control flow)
@@ -42,7 +42,7 @@ namespace nfb {
 
 constexpr int kRowsMax = 512;  // sample rows of one pass of one unit of work
 
-// shared memory map (bytes from the 1024-aligned base).  Activation buffers (exact mode only; fast mode keeps the hidden
+// shared memory map (bytes from the 1024-aligned base).  The exact-grad training forward uses exact mode's map.  Activation buffers (exact mode only; fast mode keeps the hidden
 // activations in registers): 4 K atoms x [128 rows x 128 B], swizzled.
 template <bool EXACT>
 struct SmemMap {
@@ -202,7 +202,9 @@ __device__ __forceinline__ void mlp_step_mma(Step step, WeightRing& ring, uint32
 // R*S, the rows of an invalid ray) still go through the MLP, at points no reference evaluates; their records and masks are
 // stored as zero, so that an out-of-range activation there cannot reach a weight gradient as 0 * inf.
 // ROWB (multi-frame kernels): row r0 + 8 adds bias1 instead of bias, as rows of two rays add their own direction terms.
-template <bool EXACT, bool SAVE, bool PROBE, bool ROWB = false>
+// HILO (exact-grad training forward, EXACT and SAVE): also the lo half of the record image, FP16(x - hi) of the value the record
+// holds, at rec + kRecBytes (nfb_layout.h rec_stride).
+template <bool EXACT, bool SAVE, bool PROBE, bool ROWB = false, bool HILO = false>
 __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_base, const float* __restrict__ bias,
                                          const float* dirb0, const float* dirb1, uint8_t* act_hi, uint8_t* act_lo,
                                          uint32_t (&act)[64], int r0, uint8_t* rec, uint32_t live, float* dump,
@@ -241,6 +243,7 @@ __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_ba
       if (db) { x0 = __fadd_rn(x0, db[col]); x1 = __fadd_rn(x1, db[col + 1]); }
       if (PROBE && dump) { dump[R * 256 + col] = relu_nan(x0); dump[R * 256 + col + 1] = relu_nan(x1); }
       uint32_t hi, lo = 0u, saved;
+      uint32_t saved_lo = 0u;
       if constexpr (EXACT) {
         // NaN stays NaN; hi saturates at 65504 and lo carries the rest, so hi + lo reaches ~131008 and beyond that lo is
         // inf: out of range gives a non-finite render, never a clamped one.
@@ -251,6 +254,10 @@ __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_ba
         // the record is one FP16 value: converted without saturation, so an activation beyond its range is inf there (a
         // non-finite weight gradient), not 65504 (a finite, wrong one); equal to hi for every activation up to 65504
         saved = SAVE ? pack_f16x2_inf(a, bb) : hi;
+        if constexpr (HILO) {  // an inf record keeps a non-finite remainder: the weight gradient stays non-finite
+          const float2 s2 = unpack_f16x2(saved);
+          saved_lo = pack_f16x2_inf(a - s2.x, bb - s2.y);
+        }
       } else {
         hi = pack_relu_f16x2(x0, x1);
         saved = hi;
@@ -269,6 +276,11 @@ __device__ __forceinline__ void epi_half(const float (&acc)[64], int s, int c_ba
           const uint32_t v = ((live >> hh) & 1u) ? saved : 0u;
           *reinterpret_cast<uint16_t*>(img_j + img_base[hh][0]) = (uint16_t)(v & 0xFFFFu);
           *reinterpret_cast<uint16_t*>(img_j + img_base[hh][1]) = (uint16_t)(v >> 16);
+          if constexpr (HILO) {
+            const uint32_t vl = ((live >> hh) & 1u) ? saved_lo : 0u;
+            *reinterpret_cast<uint16_t*>(img_j + kRecBytes + img_base[hh][0]) = (uint16_t)(vl & 0xFFFFu);
+            *reinterpret_cast<uint16_t*>(img_j + kRecBytes + img_base[hh][1]) = (uint16_t)(vl >> 16);
+          }
           const uint32_t bits = ((v & 0xFFFFu) ? 1u : 0u) | ((v >> 16) ? 2u : 0u);
           mask[hh][j >> 2] |= bits << ((col & 31));
         }
@@ -348,9 +360,15 @@ struct Hand {
 // MULTI: the multi-frame kernel (render_frames_kernel).  Each ray carries a frame index (RenderParams::frame); the epilogues of
 // steps 0 and 3 add the folded bias row of the ray's own frame (RenderParams::fbias) instead of the call's one frame bias, per
 // accumulator row as the direction term of step 6 is.  Everything else is the same code.
-template <bool EXACT, bool SAVE, bool PROBE, bool MULTI>
+//
+// HILO: the exact-grad training forward (render_hilo_kernel; EXACT and SAVE): exact mode's training forward, whose records are
+// 2 MiB apart and also hold the lo half of every activation image (nfb_layout.h rec_stride).  The first MiB of each is exact
+// mode's record, byte for byte.
+template <bool EXACT, bool SAVE, bool PROBE, bool MULTI, bool HILO = false>
 __device__ __forceinline__ void render_body(const RenderParams& p) {
+  static_assert(!HILO || (EXACT && SAVE), "the lo record belongs to the exact training forward");
   using M = SmemMap<EXACT>;
+  constexpr size_t kRecStride = rec_stride(HILO);
   // Use the dynamic shared array directly (no integer round trip) so the compiler keeps the shared address
   // space and emits LDS/STS instead of generic loads; the swizzled operands need 1024-byte alignment.
   extern __shared__ __align__(1024) uint8_t smem[];
@@ -788,11 +806,19 @@ __device__ __forceinline__ void render_body(const RenderParams& p) {
         }
         if constexpr (SAVE) {  // FP16 encoding of this tile as a transposed image (input of layers_xyz.0 / .3 in dW)
           if (unit < geom.n_units) {
-            uint8_t* rec = p.save_rec + geom.global_tile(unit, pass, t) * kRecBytes;
+            uint8_t* rec = p.save_rec + geom.global_tile(unit, pass, t) * kRecStride;
             uint32_t hh[16];
 #pragma unroll
             for (int e = 0; e < 16; ++e) hh[e] = pack_f16x2(f[2 * e], f[2 * e + 1]);
             store_t32(rec + kRecPE + img_row_base(64, row), row, 32 * half, hh);
+            if constexpr (HILO) {  // the lo half the PE buffer's lo atom holds
+#pragma unroll
+              for (int e = 0; e < 16; ++e) {
+                const float2 hf = unpack_f16x2(hh[e]);
+                hh[e] = pack_f16x2(f[2 * e] - hf.x, f[2 * e + 1] - hf.y);
+              }
+              store_t32(rec + kRecBytes + kRecPE + img_row_base(64, row), row, 32 * half, hh);
+            }
           }
         }
         fence_proxy_async_smem();  // make the generic-proxy PE stores visible to the tensor core
@@ -807,7 +833,7 @@ __device__ __forceinline__ void render_body(const RenderParams& p) {
             const TileGeom::Row rw = geom.row(pass, t, row);
             const bool live = rw.used;
             const RayP& rp = rayp[rw.ray];
-            rec = p.save_rec + geom.global_tile(unit, pass, t) * kRecBytes;
+            rec = p.save_rec + geom.global_tile(unit, pass, t) * kRecStride;
             uint32_t hh[8];  // direction encoding of this row's ray: features [16*half, 16*half+16)
 #pragma unroll
             for (int e = 0; e < 8; ++e) {
@@ -823,6 +849,18 @@ __device__ __forceinline__ void render_body(const RenderParams& p) {
               const int ka = 16 * half + 2 * e, kb = ka + 1;
               *reinterpret_cast<uint16_t*>(img + ka * 128 + ((cr ^ (uint32_t)(ka & 7)) << 4)) = (uint16_t)(hh[e] & 0xFFFFu);
               *reinterpret_cast<uint16_t*>(img + kb * 128 + ((cr ^ (uint32_t)(kb & 7)) << 4)) = (uint16_t)(hh[e] >> 16);
+            }
+            if constexpr (HILO) {
+#pragma unroll
+              for (int e = 0; e < 8; ++e) {
+                const int ka = 16 * half + 2 * e, kb = ka + 1;
+                const float a = (live && rp.valid && ka < kDimDir) ? rp.ped[ka] : 0.f;
+                const float b = (live && rp.valid && kb < kDimDir) ? rp.ped[kb] : 0.f;
+                const float2 hf = unpack_f16x2(hh[e]);
+                const uint32_t l = pack_f16x2(a - hf.x, b - hf.y);
+                *reinterpret_cast<uint16_t*>(img + kRecBytes + ka * 128 + ((cr ^ (uint32_t)(ka & 7)) << 4)) = (uint16_t)(l & 0xFFFFu);
+                *reinterpret_cast<uint16_t*>(img + kRecBytes + kb * 128 + ((cr ^ (uint32_t)(kb & 7)) << 4)) = (uint16_t)(l >> 16);
+              }
             }
           }
         }
@@ -871,18 +909,18 @@ __device__ __forceinline__ void render_body(const RenderParams& p) {
                   const float* fb = p.fbias[pass] + (s == 3 ? 256 : 0);
                   const float* b0 = cond ? fb + (size_t)rayp[ray0].frame * kFrameRows : bias;
                   const float* b1 = cond ? fb + (size_t)rayp[ray1].frame * kFrameRows : bias;
-                  epi_half<EXACT, SAVE, PROBE, true>(acc0, s, 0, b0, db0, db1, act_hi, act_lo, act, r0, rec, live, dump, b1);
+                  epi_half<EXACT, SAVE, PROBE, true, HILO>(acc0, s, 0, b0, db0, db1, act_hi, act_lo, act, r0, rec, live, dump, b1);
                   if (si.nh1 == 128)
-                    epi_half<EXACT, SAVE, PROBE, true>(acc1, s, 128, b0, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump, b1);
+                    epi_half<EXACT, SAVE, PROBE, true, HILO>(acc1, s, 128, b0, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump, b1);
                 } else {
-                  epi_half<EXACT, SAVE, PROBE>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, act, r0, rec, live, dump);
+                  epi_half<EXACT, SAVE, PROBE, false, HILO>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, act, r0, rec, live, dump);
                   if (si.nh1 == 128)
-                    epi_half<EXACT, SAVE, PROBE>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump);
+                    epi_half<EXACT, SAVE, PROBE, false, HILO>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump);
                 }
               } else {
-                epi_half<EXACT, SAVE, PROBE>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, act, r0, rec, live, dump);
+                epi_half<EXACT, SAVE, PROBE, false, HILO>(acc0, s, 0, bias, db0, db1, act_hi, act_lo, act, r0, rec, live, dump);
                 if (si.nh1 == 128)
-                  epi_half<EXACT, SAVE, PROBE>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump);
+                  epi_half<EXACT, SAVE, PROBE, false, HILO>(acc1, s, 128, bias, nullptr, nullptr, act_hi, act_lo, act, r0, rec, live, dump);
               }
               if (s == 6 && (lane & 3) == 0) {  // sigma = first column of the 16-column half
                 const float b = bias[128];
@@ -972,6 +1010,16 @@ template <bool EXACT, bool SAVE, bool PROBE>
 static cudaError_t render_setup_one() {
   return cudaFuncSetAttribute(render_kernel<EXACT, SAVE, PROBE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemMap<EXACT>::kBytes);
 }
+// The exact-grad training forwards (NFB_PREC_EXACT_GRAD): kernels of their own, so the other instantiations keep their names
+// and code.  MULTI: the multi-frame one.
+template <bool MULTI>
+__global__ void __launch_bounds__(kThreads, 1) render_hilo_kernel(const __grid_constant__ RenderParams p) {
+  render_body<true, true, false, MULTI, true>(p);
+}
+template <bool MULTI>
+static cudaError_t render_hilo_setup_one() {
+  return cudaFuncSetAttribute(render_hilo_kernel<MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemMap<true>::kBytes);
+}
 template <bool EXACT, bool SAVE>
 static cudaError_t render_frames_setup_one() {
   return cudaFuncSetAttribute(render_frames_kernel<EXACT, SAVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemMap<EXACT>::kBytes);
@@ -990,11 +1038,12 @@ static void render_launch(const RenderParams& p, bool probe, int grid, cudaStrea
 }
 
 cudaError_t render_kernel_setup() {
-  const cudaError_t e[10] = {render_setup_one<false, false, false>(), render_setup_one<true, false, false>(),
+  const cudaError_t e[12] = {render_setup_one<false, false, false>(), render_setup_one<true, false, false>(),
                              render_setup_one<false, true, false>(),  render_setup_one<true, true, false>(),
                              render_setup_one<false, false, true>(),  render_setup_one<true, false, true>(),
                              render_frames_setup_one<false, false>(), render_frames_setup_one<true, false>(),
-                             render_frames_setup_one<false, true>(),  render_frames_setup_one<true, true>()};
+                             render_frames_setup_one<false, true>(),  render_frames_setup_one<true, true>(),
+                             render_hilo_setup_one<false>(),          render_hilo_setup_one<true>()};
   for (const cudaError_t x : e)
     if (x != cudaSuccess) return x;
   return cudaSuccess;
@@ -1005,7 +1054,9 @@ cudaError_t launch_render(const RenderParams& p, int precision, int num_sms, cud
   if (grid <= 0) return cudaSuccess;
   const bool save = p.save_rec != nullptr;  // training forward: also writes the per-tile activation records
   const bool probe = p.dbg_act != nullptr;  // the activation probe (evaluation only): its own instantiation
-  if (precision == 1) {
+  if (precision == 2 && save) {
+    render_hilo_kernel<false><<<grid, kThreads, SmemMap<true>::kBytes, st>>>(p);
+  } else if (precision != 0) {  // exact, and the evaluation renders of exact-grad mode
     if (save) render_launch<true, true>(p, probe, grid, st);
     else render_launch<true, false>(p, probe, grid, st);
   } else {
@@ -1021,7 +1072,9 @@ cudaError_t launch_render_frames(const RenderParams& p, int precision, int num_s
   if (grid <= 0) return cudaSuccess;
   const bool save = p.save_rec != nullptr;
   constexpr int B = SmemMap<true>::kBytes, F = SmemMap<false>::kBytes;
-  if (precision == 1) {
+  if (precision == 2 && save) {
+    render_hilo_kernel<true><<<grid, kThreads, B, st>>>(p);
+  } else if (precision != 0) {
     if (save) render_frames_kernel<true, true><<<grid, kThreads, B, st>>>(p);
     else render_frames_kernel<true, false><<<grid, kThreads, B, st>>>(p);
   } else {

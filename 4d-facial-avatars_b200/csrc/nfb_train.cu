@@ -25,6 +25,8 @@
 //                             gradients of each network in the reference's state_dict layout, plus d latent_code.
 //
 // Gradients are carried in FP16 with one power-of-two loss scale per backward call (max |d raw| -> 2^10), FP32 accumulate.
+// Exact-grad mode (NFB_PREC_EXACT_GRAD) runs the *_x3 instantiations of stages 2, 3, 5 and the per-frame sums: every FP16
+// operand is hi + lo (records 2 MiB apart, nfb_layout.h rec_stride), multiplied as hi.hi + hi.lo + lo.hi.
 #include <cuda_fp16.h>
 #include <cuda_runtime.h>
 
@@ -231,22 +233,33 @@ namespace chain {
 // repack_kernel in nfb_pack.cu), warpgroups 1 and 2 compute rows [64w, 64w+64) of the tile on wgmma with register
 // accumulators; their epilogue applies the saved ReLU mask, writes the FP16 result in place into the shared-memory activation
 // buffer (A operand of the next step) and as the transposed dY image into the tile record.
-constexpr int kNumSlots = 4;
-using WeightRing = Ring<kNumSlots, kMaxUnitBytes>;
-constexpr int kOffRing = 0;
-constexpr int kOffAct = kOffRing + kNumSlots * kMaxUnitBytes;  // 4 K atoms x [128 rows x 128 B]
-constexpr int kOffOp = kOffAct + 4 * kTileM * 128;             // d raw operand: [128 rows x 64 k] FP16, swizzled (k < 4 used)
-constexpr int kOffBars = kOffOp + kTileM * 128;
-constexpr int kSmemBytes = kOffBars + 2 * kNumSlots * 8;
-static_assert(kSmemBytes <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
+// X3 (exact-grad mode, chain_x3_kernel): every operand is hi + lo.  The activation buffer and the d raw operand get a lo copy,
+// the producer streams each unit's hi weights then its lo weights (wstream_lo) into two ring slots, and each unit is
+// hi.hi + lo.hi (first slot) + hi.lo (second slot); the epilogue writes dY as hi and lo, in shared memory and in the record.
+// 64 KB ring + 128 KB activations + 32 KB operand = 224 KB: the trade exact mode's forward makes (one slot per hi/lo unit).
+template <bool X3>
+struct Smem {
+  static constexpr int kNumSlots = X3 ? 2 : 4;
+  using WeightRing = Ring<kNumSlots, kMaxUnitBytes>;
+  static constexpr int kOffRing = 0;
+  static constexpr int kOffAct = kOffRing + kNumSlots * kMaxUnitBytes;  // 4 K atoms x [128 rows x 128 B]
+  static constexpr int kOffActLo = kOffAct + 4 * kTileM * 128;          // X3: the lo halves
+  static constexpr int kOffOp = kOffActLo + (X3 ? 4 * kTileM * 128 : 0);  // d raw operand: [128 rows x 64 k] FP16, swizzled (k < 4 used)
+  static constexpr int kOffOpLo = kOffOp + kTileM * 128;                // X3: its lo half
+  static constexpr int kOffBars = kOffOpLo + (X3 ? kTileM * 128 : 0);
+  static constexpr int kSmemBytes = kOffBars + 2 * kNumSlots * 8;
+  static_assert(kSmemBytes <= 232448, "exceeds the 227 KB per-CTA shared memory limit");
+};
+static_assert(Smem<false>::kOffOp == 4 * kMaxUnitBytes + 4 * kTileM * 128, "the FP16 chain's map");
 
 constexpr int kTileUnits = prog_units(kBwdStream);  // 28
 __constant__ ProgTable c_prog = make_prog(kBwdStream);
 
 // Epilogue of one 128-column accumulator half: masked gradient -> FP16, in place into the activation buffer and into the
-// record image of dY(L).
+// record image of dY(L).  X3: also its lo half, into act_lo and the lo record.
+template <bool X3>
 __device__ __forceinline__ void bwd_epi_half(const float (&acc)[64], int L, int c_base, const uint32_t* masks, uint8_t* act,
-                                             uint8_t* rec, int r0) {
+                                             uint8_t* act_lo, uint8_t* rec, int r0) {
   const int lane = threadIdx.x & 31, c = lane & 3;
   const int W = rec_width(L);
 #pragma unroll
@@ -269,18 +282,33 @@ __device__ __forceinline__ void bwd_epi_half(const float (&acc)[64], int L, int 
         *reinterpret_cast<uint16_t*>(img + img_offset(W, col, R)) = (uint16_t)(h & 0xFFFFu);
         *reinterpret_cast<uint16_t*>(img + img_offset(W, col + 1, R)) = (uint16_t)(h >> 16);
       }
+      if constexpr (X3) {  // an inf hi leaves a non-finite lo: the overflow stays visible in hi + lo
+        const float2 hf = unpack_f16x2(h);
+        const uint32_t l = pack_f16x2_inf(a0 - hf.x, a1 - hf.y);
+        *reinterpret_cast<uint32_t*>(act_lo + (col >> 6) * (kTileM * 128) + sw128_offset(R, col & 63)) = l;
+        if (rec) {
+          uint8_t* img = rec + kRecBytes + rec_dy_off(L);
+          *reinterpret_cast<uint16_t*>(img + img_offset(W, col, R)) = (uint16_t)(l & 0xFFFFu);
+          *reinterpret_cast<uint16_t*>(img + img_offset(W, col + 1, R)) = (uint16_t)(l >> 16);
+        }
+      }
     }
   }
 }
 
-__global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constant__ ChainParams p) {
+template <bool X3>
+__device__ __forceinline__ void chain_body(const ChainParams& p) {
+  using M = Smem<X3>;
+  constexpr int kOffRing = M::kOffRing, kOffAct = M::kOffAct, kOffOp = M::kOffOp, kOffBars = M::kOffBars;
+  constexpr int NPART = X3 ? 2 : 1;
+  constexpr size_t kRecStride = rec_stride(X3);
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t smem_base = smem_base_aligned(smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  WeightRing ring(smem_base + kOffRing, smem_base + kOffBars);
+  typename M::WeightRing ring(smem_base + kOffRing, smem_base + kOffBars);
   if (threadIdx.x == 0) ring.init();
-  for (int i = threadIdx.x; i < kTileM * 128 / 16; i += kThreads)  // operand chunks 1..7 of every row stay zero
+  for (int i = threadIdx.x; i < NPART * kTileM * 128 / 16; i += kThreads)  // operand chunks 1..7 of every row stay zero (X3: both halves)
     reinterpret_cast<uint4*>(smem + kOffOp)[i] = make_uint4(0u, 0u, 0u, 0u);
   __syncthreads();
 
@@ -294,9 +322,11 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
     if (warp == 0) {
       for (int j = 0; j < n_tiles_cta; ++j) {
         const uint8_t* base = p.wstream[p.geom.net_of(j % tpu)];
+        const uint8_t* base_lo = X3 ? p.wstream_lo[p.geom.net_of(j % tpu)] : nullptr;
         for (int i = 0; i < kTileUnits; ++i) {
           const uint32_t w = c_prog.e[i].w;
           ring.produce(base + ((w & 0xFFFFFu) << 4), (w >> 20) * 128u);
+          if constexpr (X3) ring.produce(base_lo + ((w & 0xFFFFFu) << 4), (w >> 20) * 128u);  // the unit's lo weights
         }
       }
     }
@@ -315,7 +345,7 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
       const int unit = blockIdx.x + (j / tpu) * gridDim.x;
       const bool real = unit < p.geom.n_units;
       const size_t gt = p.geom.global_tile(unit, j % tpu);
-      uint8_t* rec = real ? p.rec + gt * kRecBytes : nullptr;
+      uint8_t* rec = real ? p.rec + gt * kRecStride : nullptr;
       // d raw of tile j -> FP16 operand row in shared memory (+ its transposed image for the weight-gradient kernel)
       if (ch == 0) {
         float4 d = make_float4(0.f, 0.f, 0.f, 0.f);
@@ -330,11 +360,29 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
           *reinterpret_cast<uint16_t*>(img + 2 * 128 + ((cr ^ 2u) << 4)) = (uint16_t)(h23 & 0xFFFFu);
           *reinterpret_cast<uint16_t*>(img + 3 * 128 + ((cr ^ 3u) << 4)) = (uint16_t)(h23 >> 16);
         }
+        if constexpr (X3) {  // the lo half of the scaled d raw: operand row and record image
+          const float2 f01 = unpack_f16x2(h01), f23 = unpack_f16x2(h23);
+          const uint32_t l01 = pack_f16x2_inf(d.x * scale - f01.x, d.y * scale - f01.y);
+          const uint32_t l23 = pack_f16x2_inf(d.z * scale - f23.x, d.w * scale - f23.y);
+          *reinterpret_cast<uint4*>(smem + M::kOffOpLo + row * 128 + ((0 ^ (row & 7)) << 4)) = make_uint4(l01, l23, 0u, 0u);
+          if (real) {
+            uint8_t* img = rec + kRecBytes + kRecDRaw + img_row_base(16, row);
+            const uint32_t cr = (uint32_t)((row & 63) >> 3);
+            *reinterpret_cast<uint16_t*>(img + 0 * 128 + ((cr ^ 0u) << 4)) = (uint16_t)(l01 & 0xFFFFu);
+            *reinterpret_cast<uint16_t*>(img + 1 * 128 + ((cr ^ 1u) << 4)) = (uint16_t)(l01 >> 16);
+            *reinterpret_cast<uint16_t*>(img + 2 * 128 + ((cr ^ 2u) << 4)) = (uint16_t)(l23 & 0xFFFFu);
+            *reinterpret_cast<uint16_t*>(img + 3 * 128 + ((cr ^ 3u) << 4)) = (uint16_t)(l23 >> 16);
+          }
+        }
       } else if (real) {  // rows 4..15 of the image are zero
         uint8_t* img = rec + kRecDRaw + img_row_base(16, row);
         const uint32_t cr = (uint32_t)((row & 63) >> 3);
 #pragma unroll
         for (int k = 4; k < 16; ++k) *reinterpret_cast<uint16_t*>(img + k * 128 + ((cr ^ (uint32_t)(k & 7)) << 4)) = 0;
+        if constexpr (X3) {
+#pragma unroll
+          for (int k = 4; k < 16; ++k) *reinterpret_cast<uint16_t*>(img + kRecBytes + k * 128 + ((cr ^ (uint32_t)(k & 7)) << 4)) = 0;
+        }
       }
       fence_proxy_async_smem();
       named_bar_sync(kRowBarrier, kRowThreads);  // operand of tile j in place
@@ -349,24 +397,33 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
           const ProgEntry e = c_prog.e[prog];
           const uint32_t a = ((e.z & kUnitFromOperand) ? smem_base + kOffOp : smem_base + kOffAct + e.y * (kTileM * 128)) + 64 * wg * 128;
           const uint64_t ad = wgmma_desc_sw128(a);
-          const uint32_t b = ring.wait_full();
-          const uint64_t b0 = wgmma_desc_sw128(b), b1 = wgmma_desc_sw128(b + 128 * 128);
-          wgmma_fence();
+          // X3: the lo half of the A operand, at the same place in the lo buffers
+          const uint64_t al = X3 ? wgmma_desc_sw128(a + ((e.z & kUnitFromOperand) ? M::kOffOpLo - kOffOp : M::kOffActLo - kOffAct)) : 0;
 #pragma unroll
-          for (int ks = 0; ks < 4; ++ks) {
-            const uint32_t accf = (u | ks) ? 1u : 0u;
-            wgmma_n128(acc0, ad + (uint64_t)(ks * 2), b0 + (uint64_t)(ks * 2), accf);
-            if (two) wgmma_n128(acc1, ad + (uint64_t)(ks * 2), b1 + (uint64_t)(ks * 2), accf);
+          for (int part = 0; part < NPART; ++part) {  // X3: the unit's hi weights (hi.hi + lo.hi), then its lo weights (hi.lo)
+            const uint32_t b = ring.wait_full();
+            const uint64_t b0 = wgmma_desc_sw128(b), b1 = wgmma_desc_sw128(b + 128 * 128);
+            wgmma_fence();
+#pragma unroll
+            for (int ks = 0; ks < 4; ++ks) {
+              const uint32_t accf = (u | part | ks) ? 1u : 0u;
+              wgmma_n128(acc0, ad + (uint64_t)(ks * 2), b0 + (uint64_t)(ks * 2), accf);
+              if (two) wgmma_n128(acc1, ad + (uint64_t)(ks * 2), b1 + (uint64_t)(ks * 2), accf);
+              if (X3 && part == 0) {
+                wgmma_n128(acc0, al + (uint64_t)(ks * 2), b0 + (uint64_t)(ks * 2), 1u);
+                if (two) wgmma_n128(acc1, al + (uint64_t)(ks * 2), b1 + (uint64_t)(ks * 2), 1u);
+              }
+            }
+            wgmma_commit();
+            wgmma_wait<0>();
+            reg_fence(acc0);
+            reg_fence(acc1);
+            ring.release();
           }
-          wgmma_commit();
-          wgmma_wait<0>();
-          reg_fence(acc0);
-          reg_fence(acc1);
-          ring.release();
         }
         const int L = 8 - s;  // forward layer whose pre-activation gradient this step produces
-        bwd_epi_half(acc0, L, 0, masks, act, rec, r0);
-        if (two) bwd_epi_half(acc1, L, 128, masks, act, rec, r0);
+        bwd_epi_half<X3>(acc0, L, 0, masks, act, smem + M::kOffActLo, rec, r0);
+        if (two) bwd_epi_half<X3>(acc1, L, 128, masks, act, smem + M::kOffActLo, rec, r0);
         fence_proxy_async_smem();
         named_bar_sync(2 + wg, 128);
       }
@@ -374,6 +431,10 @@ __global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constan
     }
   }
 }
+
+__global__ void __launch_bounds__(kThreads, 1) chain_kernel(const __grid_constant__ ChainParams p) { chain_body<false>(p); }
+// exact-grad mode: hi + lo operands end to end (a kernel of its own, so chain_kernel keeps its name and code)
+__global__ void __launch_bounds__(kThreads, 1) chain_x3_kernel(const __grid_constant__ ChainParams p) { chain_body<true>(p); }
 
 }  // namespace chain
 
@@ -593,6 +654,135 @@ __global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__
         case 64: run_job<kPeOnly, 64>(p, J, j0, j1, smem_base, ring, wg, lane); break;
         case 128: run_job<kPeOnly, 128>(p, J, j0, j1, smem_base, ring, wg, lane); break;
         default: run_job<kPeOnly, 256>(p, J, j0, j1, smem_base, ring, wg, lane); break;
+      }
+    }
+  }
+}
+
+// Exact-grad mode (dw_x3_kernel): the same jobs over the 2 MiB hi/lo records.  Three stages per r-atom, (A hi, B hi),
+// (A hi, B lo), (A lo, B hi), the same MMAs on each; the bias column sums take A hi (first stage) and A lo (third) against the
+// ones row.  Written out beside run_job / dw_kernel so that the FP16 kernels keep their source, and with it their code.
+template <bool kPeOnly, int NB>
+__device__ __forceinline__ void run_job_x3(const DwParams& p, const Job& J, int j0, int j1, uint32_t smem_base, StageRing& ring,
+                                        int wg, int lane) {
+  constexpr int NA = NB > 128 ? 128 : NB;
+  constexpr int NH = NB > 128 ? 2 : 1;
+  float acc[NH][NA / 2];
+  float accb[8];
+  const bool bias = J.bias_layer >= 0;
+  const uint64_t ones = wgmma_desc_sw128(smem_base + kOffOnes);
+  for (int j = j0; j < j1; ++j) {
+    for (int a = 0; a < 2; ++a) {
+#pragma unroll
+      for (int part = 0; part < 3; ++part) {  // (A hi, B hi), (A hi, B lo), (A lo, B hi)
+        const uint32_t sa = ring.wait_full(), sb = sa + 16384;
+        const uint64_t ad = wgmma_desc_sw128(sa + 64 * wg * 128);
+        wgmma_fence();
+#pragma unroll
+        for (int ks = 0; ks < 4; ++ks) {
+          const uint32_t accf = ((j - j0) | a | part | ks) ? 1u : 0u;
+#pragma unroll
+          for (int h = 0; h < NH; ++h) mma_n<NA>(acc[h], ad + (uint64_t)(ks * 2), wgmma_desc_sw128(sb + h * 16384) + (uint64_t)(ks * 2), accf);
+          if (bias && part != 1) wgmma_n16(accb, ad + (uint64_t)(ks * 2), ones + (uint64_t)(ks * 2), accf);  // A hi, A lo
+        }
+        wgmma_commit();
+        wgmma_wait<0>();
+#pragma unroll
+        for (int h = 0; h < NH; ++h) reg_fence(acc[h]);
+        reg_fence(accb);
+        ring.release();
+      }
+    }
+  }
+  constexpr int kG = kPeOnly ? kPeGroups : kGroups;
+  float* slot = p.ws + (size_t)(blockIdx.x / kG) * p.ws_stride;  // this (network, part)'s partial
+  const int bias_acc = bias ? acc_bias_off(J.bias_layer) : 0;
+  const int out_off = kPeOnly ? pe_slot_off(J.out_off) : J.out_off, bias_off = kPeOnly ? pe_slot_off(bias_acc) : bias_acc;
+  const float inv = p.scal[1];
+  const int c = lane & 3, r0 = 64 * wg + 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2);
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int R = r0 + 8 * hh;
+    float* out = slot + out_off + (size_t)(J.out_row0 + R) * J.out_ld;
+#pragma unroll
+    for (int h = 0; h < NH; ++h)
+#pragma unroll
+      for (int jj = 0; jj < NA / 8; ++jj) {
+        const int col = h * 128 + 8 * jj + 2 * c;
+        *reinterpret_cast<float2*>(out + col) = make_float2(acc[h][4 * jj + 2 * hh] * inv, acc[h][4 * jj + 2 * hh + 1] * inv);
+      }
+    if (bias && c == 0) slot[bias_off + J.out_row0 + R] = accb[2 * hh] * inv;
+  }
+}
+
+template <bool kPeOnly>
+__global__ void __launch_bounds__(kThreads, 1) dw_x3_kernel(const __grid_constant__ DwParams p) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  const uint32_t smem_base = smem_base_aligned(smem);
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+  // this CTA: network x job group (blockIdx.x % kGroups) x a contiguous share of the network's tiles
+  constexpr int kG = kPeOnly ? kPeGroups : kGroups;
+  const int group = (kPeOnly ? kPeGroup : 0) + (int)blockIdx.x % kG;
+  int part = (int)blockIdx.x / kG;
+  const int net = (part >= p.parts[0]) ? 1 : 0;
+  if (net) part -= p.parts[0];
+  const int parts = p.parts[net];
+  const int t_cnt = p.geom.tile_count(net);
+  const int total = p.geom.n_units * t_cnt;
+  const int per = (total + parts - 1) / parts;
+  const int j0 = part * per;
+  const int j1 = min(total, j0 + per);
+  if (part >= parts || j0 >= j1) return;  // uniform for the whole CTA
+  const int job0 = c_jobs.group_begin[group] + (kPeOnly ? 1 : 0), job1 = c_jobs.group_begin[group + 1];
+
+  StageRing ring(smem_base, smem_base + kOffBars);
+  if (threadIdx.x == 0) ring.init();
+  for (int i = threadIdx.x; i < 2048 / 4; i += kThreads)  // row 0 (first 128 bytes) = FP16 ones, rows 1..15 = 0
+    reinterpret_cast<uint32_t*>(smem + kOffOnes)[i] = (i < 32) ? 0x3C003C00u : 0u;
+  fence_proxy_async_smem();
+  __syncthreads();
+
+  auto tile_rec = [&](int j) -> const uint8_t* {
+    const int u = j / t_cnt, t = j - u * t_cnt;
+    return p.rec + p.geom.global_tile(u, net, t) * rec_stride(true);
+  };
+
+  if (warp < 4) {
+    // ============================== producer ==============================
+    reg_dec<kRegsLight>();
+    if (warp == 0) {
+      for (int job = job0; job < job1; ++job) {
+        const Job J = c_jobs.j[job];
+        const uint32_t b_bytes = (uint32_t)J.b_rows * 128u;
+        for (int j = j0; j < j1; ++j) {
+          const uint8_t* rec = tile_rec(j);
+          for (int a = 0; a < 2; ++a) {  // per r-atom three stages: (A hi, B hi), (A hi, B lo), (A lo, B hi); lo at +kRecBytes
+            const uint8_t* A = rec + J.a_off + a * J.a_rows * 128 + J.a_half * 16384;
+            const uint8_t* B = rec + J.b_off + a * J.b_rows * 128;
+            ring.produce(A, 16384, 16384, B, b_bytes);
+            ring.produce(A, 16384, 16384, B + kRecBytes, b_bytes);
+            ring.produce(A + kRecBytes, 16384, 16384, B, b_bytes);
+          }
+        }
+      }
+    }
+  } else {
+    // ============================== MMA + epilogue warpgroups ==============================
+    reg_inc<kRegsRow>();
+    const int wg = (warp - 4) >> 2;
+    for (int job = job0; job < job1; ++job) {
+      const Job J = c_jobs.j[job];
+      if constexpr (kPeOnly) {  // both PE jobs multiply by the 64-row PE image: only that shape is compiled in
+        run_job_x3<kPeOnly, 64>(p, J, j0, j1, smem_base, ring, wg, lane);
+        continue;
+      }
+      switch (J.b_rows) {
+        case 16: run_job_x3<kPeOnly, 16>(p, J, j0, j1, smem_base, ring, wg, lane); break;
+        case 32: run_job_x3<kPeOnly, 32>(p, J, j0, j1, smem_base, ring, wg, lane); break;
+        case 64: run_job_x3<kPeOnly, 64>(p, J, j0, j1, smem_base, ring, wg, lane); break;
+        case 128: run_job_x3<kPeOnly, 128>(p, J, j0, j1, smem_base, ring, wg, lane); break;
+        default: run_job_x3<kPeOnly, 256>(p, J, j0, j1, smem_base, ring, wg, lane); break;
       }
     }
   }
@@ -849,18 +1039,28 @@ __global__ void __launch_bounds__(256) cond_grad_kernel(const FinAll f) {
 // atomics: per ray (samples ascending) from the dY images the dX chain left in the tile records, then per frame over the rays in
 // ascending order, added to the running sums of earlier chunks.
 // raysum_kernel: block = (ray, pass), thread = column (0..255: dY0, 256..511: dY3).
-__global__ void __launch_bounds__(kFrameRows) raysum_kernel(const FrameSumParams p) {
+// X3 (raysum_x3_kernel, exact-grad mode): each dY is hi + lo of the 2 MiB record.
+template <bool X3>
+__device__ __forceinline__ float rec_dy(const uint8_t* img, int off) {
+  float v = __half2float(*reinterpret_cast<const __half*>(img + off));
+  if constexpr (X3) v += __half2float(*reinterpret_cast<const __half*>(img + kRecBytes + off));  // exact in FP32
+  return v;
+}
+template <bool X3>
+__device__ __forceinline__ void raysum_body(const FrameSumParams& p) {
   const int g = blockIdx.x, pass = blockIdx.y, t = threadIdx.x;
   const int L = t < 256 ? 0 : 3, n = t & 255;
   const TileGeom::RayRows rows = p.geom.ray_rows(pass, g);
   float s = 0.f;
   for (int i = 0; i < rows.S; ++i) {
     const size_t slot = rows.slot(i);
-    const uint8_t* img = p.rec + (slot >> 7) * kRecBytes + rec_dy_off(L);
-    s += __half2float(*reinterpret_cast<const __half*>(img + img_offset(256, n, (int)(slot & 127))));
+    const uint8_t* img = p.rec + (slot >> 7) * rec_stride(X3) + rec_dy_off(L);
+    s += rec_dy<X3>(img, img_offset(256, n, (int)(slot & 127)));
   }
   p.raysum[((size_t)pass * p.geom.n_rays + g) * kFrameRows + t] = s * p.scal[1];
 }
+__global__ void __launch_bounds__(kFrameRows) raysum_kernel(const FrameSumParams p) { raysum_body<false>(p); }
+__global__ void __launch_bounds__(kFrameRows) raysum_x3_kernel(const FrameSumParams p) { raysum_body<true>(p); }
 // framesum_kernel: block = (frame, pass), thread = column.  Per batch of 512 rays the block first compacts the frame's rays into a
 // list (ballot + warp prefix: ascending ray order, no atomics), then every thread adds its column over that list.  A block reads
 // each frame slot once (n / 512 steps) and sums only its own frame's rays, so the launch costs O(F n / 512 + 512 n), not O(F n 512).
@@ -958,7 +1158,9 @@ constexpr int kOffWd = 2 * kOffW3;              // [128][8]: the v0 columns sin/
 constexpr int kOffRed = kOffWd + 128 * 8 * 4;   // [4][128] float4
 constexpr int kSmemBytes = kOffRed + 4 * 128 * 16;
 
-__global__ void __launch_bounds__(kThreadsRow, 1) row_kernel(const InGradRowParams p) {
+// X3 (row_x3_kernel, exact-grad mode): dY0, dY3 and dY6 are hi + lo of the 2 MiB record.
+template <bool X3>
+__device__ __forceinline__ void row_body(const InGradRowParams& p) {
   extern __shared__ __align__(16) uint8_t smem[];
   float* w0s = reinterpret_cast<float*>(smem);
   float* w3s = reinterpret_cast<float*>(smem + kOffW3);
@@ -986,7 +1188,7 @@ __global__ void __launch_bounds__(kThreadsRow, 1) row_kernel(const InGradRowPara
   for (int j = part; j < total; j += parts) {
     const int unit = j / t_cnt, tl = j - unit * t_cnt;
     const size_t gt = p.geom.global_tile(unit, net, tl);
-    const uint8_t* rec = p.rec + gt * kRecBytes;
+    const uint8_t* rec = p.rec + gt * rec_stride(X3);
     float acc[16];
 #pragma unroll
     for (int k = 0; k < 16; ++k) acc[k] = 0.f;
@@ -996,7 +1198,7 @@ __global__ void __launch_bounds__(kThreadsRow, 1) row_kernel(const InGradRowPara
       const float* ws = (L ? w3s : w0s) + 16 * kq;
 #pragma unroll 4
       for (int n = 0; n < 256; ++n) {
-        const float dy = __half2float(*reinterpret_cast<const __half*>(img + img_offset(256, n, row)));
+        const float dy = rec_dy<X3>(img, img_offset(256, n, row));
         const float4* w4 = reinterpret_cast<const float4*>(ws + n * 64);
 #pragma unroll
         for (int q = 0; q < 4; ++q) {
@@ -1011,7 +1213,7 @@ __global__ void __launch_bounds__(kThreadsRow, 1) row_kernel(const InGradRowPara
       const uint8_t* img = rec + rec_dy_off(6);
 #pragma unroll 4
       for (int n = 0; n < 128; ++n) {
-        const float dy = __half2float(*reinterpret_cast<const __half*>(img + img_offset(128, n, row)));
+        const float dy = rec_dy<X3>(img, img_offset(128, n, row));
         ds = fmaf(wds[n * 8 + 2 * kq], dy, ds);
         dc = fmaf(wds[n * 8 + 2 * kq + 1], dy, dc);
       }
@@ -1059,6 +1261,8 @@ __global__ void __launch_bounds__(kThreadsRow, 1) row_kernel(const InGradRowPara
     __syncthreads();
   }
 }
+__global__ void __launch_bounds__(kThreadsRow, 1) row_kernel(const InGradRowParams p) { row_body<false>(p); }
+__global__ void __launch_bounds__(kThreadsRow, 1) row_x3_kernel(const InGradRowParams p) { row_body<true>(p); }
 
 // One warp per ray: sums the row float4s of both passes (lane-strided over the samples, then a butterfly: deterministic, no
 // atomics), d o += dp, d d += z dp, and adds the |d| term of the compositing and the background term.
@@ -1130,13 +1334,18 @@ int debug_jobs_dw(int index, uint32_t* out) {
 }
 
 cudaError_t train_kernels_setup() {
-  cudaError_t e = cudaFuncSetAttribute(chain::chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, chain::kSmemBytes);
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(dw::dw_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dw::kSmemBytes);
-  if (e != cudaSuccess) return e;
-  e = cudaFuncSetAttribute(dw::dw_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, dw::kSmemBytes);
-  if (e != cudaSuccess) return e;
-  return cudaFuncSetAttribute(ing::row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ing::kSmemBytes);
+  const cudaError_t e[8] = {
+      cudaFuncSetAttribute(chain::chain_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, chain::Smem<false>::kSmemBytes),
+      cudaFuncSetAttribute(chain::chain_x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, chain::Smem<true>::kSmemBytes),
+      cudaFuncSetAttribute(dw::dw_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dw::kSmemBytes),
+      cudaFuncSetAttribute(dw::dw_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, dw::kSmemBytes),
+      cudaFuncSetAttribute(dw::dw_x3_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, dw::kSmemBytes),
+      cudaFuncSetAttribute(dw::dw_x3_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, dw::kSmemBytes),
+      cudaFuncSetAttribute(ing::row_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ing::kSmemBytes),
+      cudaFuncSetAttribute(ing::row_x3_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, ing::kSmemBytes)};
+  for (const cudaError_t x : e)
+    if (x != cudaSuccess) return x;
+  return cudaSuccess;
 }
 
 cudaError_t launch_composite_bwd(const CompBwdParams& q, float* scal, cudaStream_t st, long long* launches) {
@@ -1149,10 +1358,11 @@ cudaError_t launch_composite_bwd(const CompBwdParams& q, float* scal, cudaStream
   return cudaGetLastError();
 }
 
-cudaError_t launch_chain(const ChainParams& p, int num_sms, cudaStream_t st, long long* launches) {
+cudaError_t launch_chain(const ChainParams& p, int num_sms, cudaStream_t st, long long* launches, bool hilo) {
   const int grid = p.geom.n_units < num_sms ? p.geom.n_units : num_sms;
   if (grid <= 0) return cudaSuccess;
-  chain::chain_kernel<<<grid, kThreads, chain::kSmemBytes, st>>>(p);
+  if (hilo) chain::chain_x3_kernel<<<grid, kThreads, chain::Smem<true>::kSmemBytes, st>>>(p);
+  else chain::chain_kernel<<<grid, kThreads, chain::Smem<false>::kSmemBytes, st>>>(p);
   ++*launches;
   return cudaGetLastError();
 }
@@ -1189,15 +1399,21 @@ size_t dw_workspace_floats(int num_sms) {  // the most parts dw_split deals out 
   return full > pe ? full : pe;
 }
 
-cudaError_t launch_dw(DwParams& p, int num_sms, cudaStream_t st, long long* launches, bool pe_only) {
+cudaError_t launch_dw(DwParams& p, int num_sms, cudaStream_t st, long long* launches, bool pe_only, bool hilo) {
   p.parts[0] = p.parts[1] = 0;
   p.ws_stride = pe_only ? dw::kPeSlotFloats : kAccBRaw;
   const long long tot0 = (long long)p.geom.n_units * p.geom.tiles_c, tot1 = (long long)p.geom.n_units * p.geom.tiles_f;
   if (tot0 + tot1 <= 0) return cudaSuccess;
   dw_split(dw_split_sms(num_sms, pe_only), tot0, tot1, &p.parts[0], &p.parts[1]);
   if (p.parts[0] + p.parts[1] < 1) return cudaSuccess;
-  if (pe_only) dw::dw_kernel<true><<<(p.parts[0] + p.parts[1]) * dw::kPeGroups, kThreads, dw::kSmemBytes, st>>>(p);
-  else dw::dw_kernel<false><<<(p.parts[0] + p.parts[1]) * dw::kGroups, kThreads, dw::kSmemBytes, st>>>(p);
+  const int blocks = (p.parts[0] + p.parts[1]) * (pe_only ? dw::kPeGroups : dw::kGroups);
+  if (hilo) {
+    if (pe_only) dw::dw_x3_kernel<true><<<blocks, kThreads, dw::kSmemBytes, st>>>(p);
+    else dw::dw_x3_kernel<false><<<blocks, kThreads, dw::kSmemBytes, st>>>(p);
+  } else {
+    if (pe_only) dw::dw_kernel<true><<<blocks, kThreads, dw::kSmemBytes, st>>>(p);
+    else dw::dw_kernel<false><<<blocks, kThreads, dw::kSmemBytes, st>>>(p);
+  }
   ++*launches;
   return cudaGetLastError();
 }
@@ -1264,9 +1480,10 @@ cudaError_t launch_finalize_all(const float* const params_c[26], float* const gr
   return cudaGetLastError();
 }
 
-cudaError_t launch_frame_sums(const FrameSumParams& p, cudaStream_t st, long long* launches) {
+cudaError_t launch_frame_sums(const FrameSumParams& p, cudaStream_t st, long long* launches, bool hilo) {
   if (p.geom.n_rays <= 0) return cudaSuccess;
-  raysum_kernel<<<dim3(p.geom.n_rays, p.geom.passes()), kFrameRows, 0, st>>>(p);
+  if (hilo) raysum_x3_kernel<<<dim3(p.geom.n_rays, p.geom.passes()), kFrameRows, 0, st>>>(p);
+  else raysum_kernel<<<dim3(p.geom.n_rays, p.geom.passes()), kFrameRows, 0, st>>>(p);
   ++*launches;
   framesum_kernel<<<dim3(p.n_frames, p.geom.passes()), kFrameRows, 0, st>>>(p);
   ++*launches;
@@ -1293,13 +1510,15 @@ cudaError_t launch_frames_grad(const float* const params_c[26], float* const gra
   return cudaGetLastError();
 }
 
-cudaError_t launch_input_grads(const InGradRowParams& r_in, const InGradRayParams& q_in, int num_sms, cudaStream_t st, long long* launches) {
+cudaError_t launch_input_grads(const InGradRowParams& r_in, const InGradRayParams& q_in, int num_sms, cudaStream_t st, long long* launches,
+                               bool hilo) {
   InGradRayParams q = q_in;
   if (q.g_o || q.g_d || q.g_dir_z) {
     InGradRowParams r = r_in;
     const long long tot0 = (long long)r.geom.n_units * r.geom.tiles_c, tot1 = (long long)r.geom.n_units * r.geom.tiles_f;
     dw_split(num_sms * dw::kGroups, tot0, tot1, &r.parts[0], &r.parts[1]);  // num_sms CTAs, split by tile counts
-    ing::row_kernel<<<r.parts[0] + r.parts[1], ing::kThreadsRow, ing::kSmemBytes, st>>>(r);
+    if (hilo) ing::row_x3_kernel<<<r.parts[0] + r.parts[1], ing::kThreadsRow, ing::kSmemBytes, st>>>(r);
+    else ing::row_kernel<<<r.parts[0] + r.parts[1], ing::kThreadsRow, ing::kSmemBytes, st>>>(r);
     ++*launches;
     q.rows = r.out;
   } else {

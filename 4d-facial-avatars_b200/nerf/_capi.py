@@ -8,7 +8,7 @@ LIB_PATH = os.environ.get("NFB_LIB") or os.path.join(os.path.dirname(_HERE), "li
 
 NFB_OK = 0
 NFB_NET_COARSE, NFB_NET_FINE = 0, 1
-NFB_PREC_FAST, NFB_PREC_EXACT = 0, 1
+NFB_PREC_FAST, NFB_PREC_EXACT, NFB_PREC_EXACT_GRAD = 0, 1, 2
 
 EXPORTS = ["nfb_version", "nfb_strerror", "nfb_last_cuda_error", "nfb_create", "nfb_destroy", "nfb_load_weights",
            "nfb_set_frame", "nfb_render_forward", "nfb_render_frame_host", "nfb_launch_count", "nfb_host_linspace",
@@ -76,7 +76,7 @@ class NfbWeightDebug(C.Structure):
     _fields_ = [("x1", C.c_void_p), ("x3", C.c_void_p), ("bwd", C.c_void_p), ("w6", C.c_void_p), ("b6", C.c_void_p),
                 ("bias_static", C.c_void_p), ("bias_frame", C.c_void_p), ("w0c", C.c_void_p), ("w3c", C.c_void_p),
                 ("wd0b_t", C.c_void_p), ("x1_bytes", C.c_int64), ("x3_bytes", C.c_int64), ("bwd_bytes", C.c_int64),
-                ("bias_floats", C.c_int32)]
+                ("bias_floats", C.c_int32), ("bwd_lo", C.c_void_p), ("bwd_lo_bytes", C.c_int64)]
 
 
 class NfbAdam(C.Structure):

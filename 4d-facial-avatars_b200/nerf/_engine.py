@@ -20,11 +20,16 @@ INPUT_GRADS = ("ray_origins", "ray_directions", "dir_z", "background", "expressi
 _precision = os.environ.get("NFB_PRECISION", "fast")
 
 
+# precision name -> NfbSampling.precision (include/nfb.h NFB_PREC_*)
+PRECISIONS = {"fast": capi.NFB_PREC_FAST, "exact": capi.NFB_PREC_EXACT, "exact_grad": capi.NFB_PREC_EXACT_GRAD}
+
+
 def set_precision(mode: str):
-    """'fast' = FP16 operands / FP32 accumulate; 'exact' = 3-pass FP16 hi/lo split (see include/nfb.h)."""
+    """'fast' = FP16 operands / FP32 accumulate; 'exact' = 3-pass FP16 hi/lo split of the forward; 'exact_grad' = exact's forward
+    and a hi/lo backward (see include/nfb.h)."""
     global _precision
-    if mode not in ("fast", "exact"):
-        raise ValueError("precision must be 'fast' or 'exact'")
+    if mode not in PRECISIONS:
+        raise ValueError("precision must be 'fast', 'exact' or 'exact_grad'")
     _precision = mode
 
 
@@ -138,8 +143,10 @@ class Renderer:
 
     def _sampling(self, num_coarse, num_fine, precision, white_bkgd, perturb=False, noise_std=0.0):
         prec = precision or _precision
+        if prec not in PRECISIONS:  # a misspelt mode must not quietly train in another one
+            raise ValueError(f"precision must be 'fast', 'exact' or 'exact_grad', not {prec!r}")
         return capi.NfbSampling(num_coarse, num_fine, int(bool(perturb)), float(noise_std), int(bool(white_bkgd)), 0,
-                                capi.NFB_PREC_EXACT if prec == "exact" else capi.NFB_PREC_FAST, self.linspace(num_coarse).data_ptr(),
+                                PRECISIONS[prec], self.linspace(num_coarse).data_ptr(),
                                 self.linspace(num_fine).data_ptr() if num_fine > 0 else None)
 
     def set_frame(self, expressions, latent_code):

@@ -38,6 +38,9 @@ extern "C" {
  * macro. */
 #define NFB_TRAIN_IMAGES 1
 #define NFB_MAX_STEP_IMAGES 64
+/* Defined when precision NFB_PREC_EXACT_GRAD exists (hi + lo gradients, see below), with NfbTrainDebug.record_bytes reporting the
+ * record stride and NfbWeightDebug's bwd_lo members.  The version number stayed 131 for this addition: test this macro. */
+#define NFB_EXACT_GRAD 1
 
 typedef struct NfbHandle NfbHandle;
 
@@ -56,8 +59,21 @@ enum { NFB_NET_COARSE = 0, NFB_NET_FINE = 1 };
 /* Arithmetic used by the tensor-core MLP.
  *   NFB_PREC_FAST  : FP16 operands (round-to-nearest), FP32 accumulate, one wgmma pass.
  *   NFB_PREC_EXACT : every operand split x = hi + lo in FP16; hi*hi + hi*lo + lo*hi, FP32
- *                    accumulate (3 wgmma passes, ~2^-21 relative operand error). */
-enum { NFB_PREC_FAST = 0, NFB_PREC_EXACT = 1 };
+ *                    accumulate (3 wgmma passes, ~2^-21 relative operand error).  The backward carries FP16 operands (one
+ *                    value per activation and gradient): exact-mode gradients are FP16-grade.
+ *   NFB_PREC_EXACT_GRAD : exact mode's forward, bit for bit (outputs, and the first MiB of every training record), and a backward
+ *                    on hi + lo operands end to end: the training records hold a lo half of every activation image, the dX chain
+ *                    multiplies hi + lo gradients by the hi + lo transposed weights and the weight-gradient GEMMs hi + lo images,
+ *                    each as hi*hi + hi*lo + lo*hi (operand error ~2^-22 relative, below FP32 accumulation; gradients still carry
+ *                    one power-of-two loss scale).  Non-finite values as in the other modes: an activation recorded as inf or NaN
+ *                    (hi) gives non-finite gradients, as does a scaled gradient beyond the FP16 range (hi inf, lo non-finite).
+ *                    Cost: 2 MiB of records per 128-row tile instead of 1 (the memory budget of nfb_render_forward_train counts
+ *                    it); measured on an H100 80GB HBM3 (700 W) at 2048 rays, 64c+64f: 2.2x exact mode's dX-chain and
+ *                    weight-gradient time, 1.87x its training step (DESIGN.md §6c); one extra launch per weight load / re-pack
+ *                    once the handle has run an exact-grad training forward (it writes the lo half of the backward weight stream).
+ *                    Evaluation renders run exact mode's kernel.  The backward entries follow the mode of the training forward.
+ * Any other value is NFB_ERR_INVALID. */
+enum { NFB_PREC_FAST = 0, NFB_PREC_EXACT = 1, NFB_PREC_EXACT_GRAD = 2 };
 
 /* Encoder / conditioning dimensions; mirrors the constructor arguments of
  * ConditionalBlendshapePaperNeRFModel (models.py:193-206).  Only the shipped paper configuration
@@ -457,7 +473,8 @@ int nfb_host_map_cdf(const NfbRayMap* map, const long long* zeroed_sorted, int n
 /* Test hook: device pointers of the training state (valid until the next forward_train on the handle).  NFB_ERR_STATE after a
  * chunked (over-budget) forward: its buffers only ever hold one chunk. */
 typedef struct {
-  const uint8_t* records;      /* n_tiles records of record_bytes (layout: nfb_layout.h kRec*) */
+  const uint8_t* records;      /* n_tiles records of record_bytes (layout: nfb_layout.h kRec*); 1 MiB, 2 MiB after an exact-grad
+                                  forward: the lo images at +1 MiB, at the offsets of their hi images */
   long long n_tiles;
   int32_t record_bytes;
   const float* d_raw;          /* [n_tiles][128][4] dL/d(rgb_raw, sigma_raw), unscaled */
@@ -518,6 +535,10 @@ typedef struct {
   const float *w6, *b6, *bias_static, *bias_frame, *w0c, *w3c, *wd0b_t;
   int64_t x1_bytes, x3_bytes, bwd_bytes;
   int32_t bias_floats;
+  /* The lo half of the backward stream (exact-grad mode; bwd's layout): the transposition of the lo units of x3 as bwd is of its hi
+   * units.  NULL and 0 until the handle's first exact-grad training forward. */
+  const uint8_t* bwd_lo;
+  int64_t bwd_lo_bytes;
 } NfbWeightDebug;
 int nfb_debug_weights(NfbHandle* h, int net, NfbWeightDebug* out);
 
