@@ -137,10 +137,10 @@ class FusedTrainer:
         self.eng.adam_step_dev(self.params, self.grads, self.exp_avg, self.exp_avg_sq, self._adam)
         self.eng.repack(self._pc, self._pf)
 
-    def _capture(self, body, row, world=1, group=None):
-        """body() once eagerly, then body, the all-reduce (world > 1), Adam with its regulariser on `row` and the re-pack
-        captured into a CUDA graph.  Returns the graph, what the captured body returned (its buffers must outlive the graph) and
-        the renderer's buffer epoch."""
+    def _capture(self, body, row, world=1, group=None, after_collective=None):
+        """body() once eagerly, then body, the all-reduce (world > 1) followed by after_collective(), Adam with its regulariser
+        on `row` and the re-pack captured into a CUDA graph.  Returns the graph, what the captured body returned (its buffers
+        must outlive the graph) and the renderer's buffer epoch."""
         self._own_engine()
         body()                      # eager warm-up: sizes the library's buffers (cudaMalloc is not capturable)
         epoch = self.eng.buffer_epoch()
@@ -151,6 +151,8 @@ class FusedTrainer:
             keep = body()
             if world > 1:
                 dist.all_reduce(self.grads, group=group)
+                if after_collective is not None:
+                    after_collective()
             self._adam_repack(row)
         return dict(graph=graph, keep=keep, epoch=epoch)
 
@@ -246,7 +248,8 @@ class FusedTrainer:
         return loss
 
     # ---- steps over rays of several training images (DESIGN.md 8c): sample, gather, fold, forward, loss, backward, latent rows,
-    # Adam and re-pack from K image indices alone
+    # Adam and re-pack from K image indices alone.  world > 1: every rank samples the whole batch of N = K * n rays on the same
+    # draws and renders its slice [rank * N / world, (rank + 1) * N / world); one SUM all-reduce of the bucket joins the slices.
     def _images_buffers(self, data, k, n):
         """Per-step buffers of a K-image step (cached per shape: the chunked backward re-reads rays and frame indices)."""
         key = (k, n, data.background is not None)
@@ -258,58 +261,96 @@ class FusedTrainer:
                 img=z(k, dt=torch.int32), ray_origins=z(N, 3), ray_directions=z(N, 3), target=z(N, 3),
                 background=z(N, 3) if data.background is not None else None, frame_index=z(N, dt=torch.int32),
                 expressions=z(k, 76), latents=z(k, 32), state=z(k, 3, dt=torch.int32), shortfall=self.shortfall[:k],
-                glat=z(k, 32), g0=z(N, 3), g1=z(N, 3))
+                glat=z(k, 32), g0=z(N, 3), g1=z(N, 3), zero_lat=z(k, 32))
         return sb
 
     def _images_sample(self, data, sb, n, draws, max_rounds):
         self.eng.sample_images(data, sb["img"], n, draws, max_rounds, self.latent_codes, sb)
 
-    def _images_gradients(self, sb, k, n):
-        """Forward, loss and backward of the sampled batch into the flat bucket, then the latent-table rows.  K = 1 takes the
-        single-frame kernels (its regulariser stays in Adam, as in step()); K >= 2 one multi-frame forward and backward."""
+    def _images_gradients(self, sb, k, n, world=1, rank=0):
+        """Forward, loss and backward of this rank's slice of the sampled batch into the flat bucket, then the latent-table rows.
+        K = 1 takes the single-frame kernels (its regulariser stays in Adam, as in step()); K >= 2 one multi-frame forward and
+        backward over all K frames (a frame without rays in the slice gets exactly zero d latent).  The noise is drawn for the
+        whole batch and sliced, and the loss is divided by the whole batch's N = K * n rays, so the slices' buckets sum to the
+        single-process gradient.  The K >= 2 regulariser is added here only when world == 1 (else _images_regulariser, after
+        the collective, adds it once)."""
         N = k * n
+        per = N // world
+        sl = slice(rank * per, (rank + 1) * per)
         noise = self._draw_noise(N)
+        if world > 1 and noise is not None:
+            noise = {key: (v[sl] if v is not None else None) for key, v in noise.items()}
         if k == 1:
             expr, lat, fi, glat = sb["expressions"][0], sb["latents"][0], None, sb["glat"][0]
         else:
-            expr, lat, fi, glat = sb["expressions"], sb["latents"], sb["frame_index"], sb["glat"]
-        out = self._forward_backward(expr, lat, fi, sb["ray_origins"], sb["ray_directions"], sb["background"], sb["target"], N, noise,
-                                     (sb["g0"], sb["g1"]), glat)
+            expr, lat, fi, glat = sb["expressions"], sb["latents"], sb["frame_index"][sl], sb["glat"]
+        bg = sb["background"][sl] if sb["background"] is not None else None
+        out = self._forward_backward(expr, lat, fi, sb["ray_origins"][sl], sb["ray_directions"][sl], bg, sb["target"][sl], N, noise,
+                                     (sb["g0"][sl], sb["g1"][sl]), glat)
         self.eng.latent_rows_grad(sb["glat"], sb["img"], self.latent_codes, self.grads[self.lat_off:].view(-1, 32),
-                                  0.0 if k == 1 else self.latent_reg / k)
+                                  self.latent_reg / k if k >= 2 and world == 1 else 0.0)
         return out
 
-    def _check_images(self, data, k, n, world):
-        if world != 1:
-            raise NotImplementedError("steps over several images are single-rank: world must be 1")
+    def _images_regulariser(self, sb, k):
+        """K >= 2 after the collective: the regulariser terms (latent_reg / K) * l / ||l|| added once, in ascending k, onto the
+        summed latent rows (nfb_latent_rows_grad with zero frame gradients: adding +0.0 leaves a row as it is)."""
+        if k >= 2:
+            self.eng.latent_rows_grad(sb["zero_lat"], sb["img"], self.latent_codes, self.grads[self.lat_off:].view(-1, 32),
+                                      self.latent_reg / k)
+
+    def _check_images(self, data, k, n, world, group=None, rank=None):
+        """Argument checks of a K-image step, all before any launch or collective; returns this rank's index.  world > 1 needs
+        the collective: without an initialised torch.distributed process group and without an explicit rank the step cannot
+        run data-parallel (NotImplementedError, as for any world > 1 step before data-parallel steps existed)."""
+        if world < 1:
+            raise ValueError(f"world = {world}: a step runs on at least one rank")
+        if world > 1:
+            if rank is None:
+                if not (dist.is_available() and dist.is_initialized()):
+                    raise NotImplementedError("steps over several images with world > 1 run over a torch.distributed process "
+                                              "group: initialise one (or pass rank=) first")
+                rank = dist.get_rank(group)
+            rank = int(rank)
+            if not 0 <= rank < world:
+                raise ValueError(f"rank {rank} is outside [0, {world})")
         if not 1 <= k <= 64:
             raise ValueError("1 <= K <= 64 images per step")
         if not 1 <= n <= 2048 or n > data.H * data.W:
             raise ValueError("1 <= n_per_image <= 2048 rays per image (and no more than the frame's pixels)")
         if data.n_images > self.latent_codes.shape[0]:
             raise ValueError("the latent table has fewer rows than the training set has images")
+        if (k * n) % world:
+            raise ValueError(f"a batch of K * n_per_image = {k * n} rays does not split evenly over world = {world} ranks")
+        return 0 if world == 1 else rank
 
-    def step_images(self, data, image_index, n_per_image, draws=None, max_rounds=32, world=1):
+    def step_images(self, data, image_index, n_per_image, draws=None, max_rounds=32, world=1, group=None, rank=None):
         """One optimizer step on n_per_image rays of each of the K images image_index (host ints, repeats allowed; image i
         conditions on expressions[i] and latent row i).  data: ray_sampler.TrainImages.  draws: float64 CUDA [K * max_rounds * n]
         (image k consumes slice k as RandomState.rand inside np.random.choice); None: torch.rand on the device.  The loss is
         mse(rgb_c, t) + mse(rgb_f, t) + (latent_reg / K) * sum_k ||latent[image_index[k]]|| over all K * n rays.  K = 1 is step()
         on the sampled rays, bit for bit.  Raises RuntimeError, before any gradient is formed, when an image's selection came
         up short of n distinct pixels within max_rounds rounds.
+        world > 1 (rank: dist.get_rank(group), or the explicit `rank`): data-parallel over `world` ranks, K * n must divide by
+        world (ValueError otherwise); without an initialised process group and without `rank` it raises NotImplementedError, as
+        every world > 1 step did before data-parallel steps existed.  Every rank samples the whole batch and renders its slice
+        of K * n / world rays; one SUM all-reduce of the bucket over `group` follows, then (K >= 2) the regulariser, once.  Every rank must pass the same
+        image_index and draws (with draws=None, seed torch alike on every rank): the argument checks and the short-selection
+        error then raise on all ranks together, before the collective.
         Launches (within the memory budget; +1 the first time the sampler's scratch grows): K = 1: 16 = sample 1, set_frame 1,
         forward 1, loss 1, backward 7, latent rows 1, Adam 2, re-pack 2; K >= 2: 19 = sample 1, set_frames 1, forward 1, loss 1,
         backward 10, latent rows 1, Adam 2, re-pack 2 (Adam: schedule and update on the trainer's device state, as in every step,
-        eager or captured).  Returns the device tensor [mse_coarse, mse_fine]."""
+        eager or captured).  world > 1 adds the all-reduce, and at K >= 2 one latent-rows launch after it (20).  Returns the
+        device tensor [mse_coarse, mse_fine] (world > 1: this rank's share; the shares sum to the batch loss)."""
         k, n = len(image_index), int(n_per_image)
-        self._check_images(data, k, n, world)
+        rank = self._check_images(data, k, n, world, group, rank)
         if any(not 0 <= int(i) < data.n_images for i in image_index):
             raise ValueError("image index out of range")
+        if draws is not None and draws.numel() < k * max_rounds * n:
+            raise ValueError("draws must hold K * max_rounds * n_per_image values")
         sb = self._images_buffers(data, k, n)
         sb["img"].copy_(torch.tensor([int(i) for i in image_index], dtype=torch.int32))
         if draws is None:
             draws = torch.rand(k * max_rounds * n, dtype=torch.float64, device=self.dev)
-        elif draws.numel() < k * max_rounds * n:
-            raise ValueError("draws must hold K * max_rounds * n_per_image values")
         self._own_engine()
         self._images_sample(data, sb, n, draws, max_rounds)
         found = sb["state"][:, 0].cpu()
@@ -317,23 +358,29 @@ class FusedTrainer:
             short = [(int(image_index[j]), int(found[j])) for j in range(k) if int(found[j]) < n]
             raise RuntimeError(f"ray sampler: {max_rounds} rounds of draws found fewer than {n} distinct pixels for (image, found) "
                                f"{short}; raise max_rounds")
-        self._images_gradients(sb, k, n)
+        self._images_gradients(sb, k, n, world, rank)
+        if world > 1:
+            dist.all_reduce(self.grads, group=group)  # ONE collective over the flat bucket
+            self._images_regulariser(sb, k)
         # K = 1: the regulariser in Adam on the image's row, as in step(); K >= 2: none (nfb_latent_rows_grad added it)
         self._reg_row = int(image_index[0]) if k == 1 else -1
         self.update()
         return self.loss[:2]
 
-    def capture_images(self, data, k, n_per_image, has_background=True, max_rounds=32, device_draws=True, world=1):
+    def capture_images(self, data, k, n_per_image, has_background=True, max_rounds=32, device_draws=True, world=1, group=None,
+                       rank=None):
         """Capture a whole K-image step into a CUDA graph: sampler (draws from torch.rand(float64) inside the graph, or with
-        device_draws=False from a static buffer step_images_graph fills), fold, noise, forward, loss, backward, latent rows, Adam
-        with its device-side schedule, re-pack.  Only the K image indices change between replays.  An incomplete selection does
-        not stop the graph: the image's missing slots repeat its first pixels and self.shortfall[k] counts them (include/nfb.h,
-        nfb_sample_rays_images).  Launches per replay: 16 at K = 1, 19 at K >= 2.
+        device_draws=False from a static buffer step_images_graph fills), fold, noise, forward, loss, backward, latent rows,
+        [world > 1: the all-reduce of the bucket, then at K >= 2 the regulariser], Adam with its device-side schedule, re-pack.
+        Only the K image indices change between replays.  world, group and rank as in step_images; with device_draws=True every
+        rank must seed torch alike, so that the ranks sample the same batch.  An incomplete selection does not stop the graph:
+        the image's missing slots repeat its first pixels and self.shortfall[k] counts them (include/nfb.h,
+        nfb_sample_rays_images).  Launches per replay: 16 at K = 1, 19 at K >= 2 (world > 1: + the all-reduce, and 20 at K >= 2).
         The graph holds the renderer's device buffers as sized at capture, and they only grow: a later call on the same device,
         by any trainer, that needs more room (more images or rays per step, more frames, a larger render with gradients)
         re-allocates them.  step_images_graph then raises RuntimeError instead of replaying (nfb_buffer_epoch): capture again."""
         n = int(n_per_image)
-        self._check_images(data, k, n, world)
+        rank = self._check_images(data, k, n, world, group, rank)
         if has_background != (data.background is not None):
             raise ValueError("has_background must say whether the training set has a background")
         dev = self.dev
@@ -346,14 +393,14 @@ class FusedTrainer:
         def body():
             draws = torch.rand(k * max_rounds * n, dtype=torch.float64, device=dev) if device_draws else sb["draws"]
             self._images_sample(data, sb, n, draws, max_rounds)
-            return self._images_gradients(sb, k, n), draws
+            return self._images_gradients(sb, k, n, world, rank), draws
 
         sb["img"].copy_(torch.arange(k, dtype=torch.int32) % data.n_images)
         if not device_draws:
             sb["draws"].uniform_()
         before = self.shortfall.clone()
         # K = 1: the regulariser in Adam on the image's row; K >= 2: none (nfb_latent_rows_grad adds it)
-        g = self._capture(body, sb["img"] if k == 1 else -1)
+        g = self._capture(body, sb["img"] if k == 1 else -1, world, group, after_collective=lambda: self._images_regulariser(sb, k))
         self.shortfall.copy_(before)  # the warm-up's selections are not a step's
         self._igraph = dict(g, sb=sb, k=k, n=n, max_rounds=max_rounds)
         return self

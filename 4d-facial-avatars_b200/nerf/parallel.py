@@ -89,6 +89,20 @@ def _gather_cat(local: torch.Tensor, group=None):
     return out
 
 
+def _gather_train(outs, begin, count, world, group=None):
+    """A training shard's outputs (rows [begin, begin + count) of the call) -> the whole call's: the other shards' rows
+    all-gathered without gradient, the local rows through _ScaleGrad(world)."""
+    full = []
+    for o in outs:
+        if o is None:
+            full.append(None)
+            continue
+        g = _gather_cat(o, group)
+        local = _ScaleGrad.apply(o, float(world)) if o.requires_grad else o
+        full.append(torch.cat((g[:begin], local, g[begin + count:]), dim=0))
+    return tuple(full)
+
+
 def data_parallel(run_fn, group=None):
     """Wrap a function with the signature of run_one_iter_of_nerf (train_utils.py:165-181) so that an UNMODIFIED caller
     (train_transformed_rays.py:336-352, eval_transformed_rays.py:449-467) runs it data-parallel, one process per GPU:
@@ -105,9 +119,9 @@ def data_parallel(run_fn, group=None):
     (train_utils._shard_ctx), so a seeded multi-rank run renders exactly what the seeded single-process run renders and the
     ranks' RNG streams stay in lock-step for the caller's own draws (ray selection).
 
-    Multi-frame calls (nerf.render_frames) are not sharded: NotImplementedError."""
+    Multi-frame calls (a run_fn with the signature of nerf.render_frames, marked `multi_frame`): see _data_parallel_frames."""
     if getattr(run_fn, "multi_frame", False):
-        raise NotImplementedError("data_parallel does not shard multi-frame calls (nerf.render_frames): run them in one process")
+        return _data_parallel_frames(run_fn, group)
     def wrapped(height, width, focal_length, model_coarse, model_fine, ray_origins, ray_directions, options, mode="train",
                 encode_position_fn=None, encode_direction_fn=None, expressions=None, background_prior=None, latent_code=None,
                 ray_directions_ablation=None):
@@ -145,13 +159,42 @@ def data_parallel(run_fn, group=None):
                           encode_position_fn, encode_direction_fn, expressions, bg, latent_code, abl)
         finally:
             train_utils._shard_ctx = None
-        full = []
-        for o in outs:
-            if o is None:
-                full.append(None)
-                continue
-            g = _gather_cat(o, group)
-            local = _ScaleGrad.apply(o, float(world)) if o.requires_grad else o
-            full.append(torch.cat((g[:begin], local, g[begin + per:]), dim=0))
-        return tuple(full)
+        return _gather_train(outs, begin, per, world, group)
+    return wrapped
+
+
+def _data_parallel_frames(run_fn, group=None):
+    """data_parallel for nerf.render_frames: the flattened rays are split into contiguous shards, evenly in training mode
+    (shard_batch) and by shard_rows' rule in validation mode, and frame_index and the background are sliced with them; every
+    rank gets all F frames' expressions and latent codes.  The outputs are all-gathered as in data_parallel, and in training
+    mode the local rows carry the gradient, scaled by the world size, so that per-frame latent gradients reach a latent table
+    (`latent_table[ids]`) through the same averaging all-reduce as the parameters'.  The noise of the whole call is drawn on
+    every rank and sliced (train_utils._shard_ctx)."""
+    def wrapped(ray_origins, ray_directions, frame_index, expressions, latent_codes, model_coarse, model_fine, options, mode="train",
+                background_prior=None):
+        world = dist.get_world_size(group) if dist.is_initialized() else 1
+        if world == 1:
+            return run_fn(ray_origins, ray_directions, frame_index, expressions, latent_codes, model_coarse, model_fine, options, mode,
+                          background_prior)
+        if torch.is_grad_enabled() and any(torch.is_tensor(t) and t.requires_grad for t in (
+                ray_origins, ray_directions, expressions, background_prior)):
+            raise NotImplementedError("data_parallel differentiates the parameters and the latent codes only: gradients with "
+                                      "respect to rays, expressions or background would need all-reduces it does not do "
+                                      "(run the fit in one process)")
+        rank = dist.get_rank(group)
+        ro, rd, fi = ray_origins.reshape(-1, 3), ray_directions.reshape(-1, 3), frame_index.reshape(-1)
+        n = rd.shape[0]
+        if fi.shape[0] != n:
+            raise ValueError(f"frame_index has {fi.shape[0]} entries for {n} rays")
+        begin, count = shard_rows(n, world, rank) if mode == "validation" else shard_batch(n, world, rank)
+        sl = slice(begin, begin + count)
+        bg = background_prior.reshape(-1, 3)[sl] if background_prior is not None else None
+        train_utils._shard_ctx = (begin, count, n)
+        try:
+            outs = run_fn(ro[sl], rd[sl], fi[sl], expressions, latent_codes, model_coarse, model_fine, options, mode, bg)
+        finally:
+            train_utils._shard_ctx = None
+        if mode == "validation":
+            return tuple(gather_rows(o.contiguous(), n, group) if o is not None else None for o in outs)
+        return _gather_train(outs, begin, count, world, group)
     return wrapped

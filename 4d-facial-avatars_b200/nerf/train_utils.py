@@ -185,12 +185,12 @@ def render_frames(ray_origins, ray_directions, frame_index, expressions, latent_
         raise ValueError("expressions [F,76] and latent_codes [F,32] must share F")
     near, far = options.dataset.near, options.dataset.far
     rays = torch.cat((ro, rd, near * torch.ones_like(rd[..., :1]), far * torch.ones_like(rd[..., :1])), dim=-1)
-    noise = _chunk_noise(n, opts, rays.device, has_fine)
+    noise = _chunk_noise(n, opts, rays.device, has_fine, _shard_ctx)
     bg = background_prior.reshape(-1, 3) if background_prior is not None else None
     return _render(rays, near, far, model_coarse, model_fine, opts, expressions, bg, latent_codes, None, noise, frame_index=fi)
 
 
-render_frames.multi_frame = True  # nerf.parallel.data_parallel refuses it
+render_frames.multi_frame = True  # nerf.parallel.data_parallel shards it by rays, with the signature above
 
 
 class GaussianSmoothing(torch.nn.Module):
