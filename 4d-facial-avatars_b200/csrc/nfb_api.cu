@@ -111,6 +111,8 @@ struct NfbHandle {
   DevBuf<nfb::smp::Seg> smpi_segs{&frees};
   DevBuf<int> smpi_first{&frees};
   DevBuf<long long> smpi_found{&frees};
+  // nfb_fit_rows_grad: the per-slot pose sums [NFB_MAX_STEP_IMAGES][12] (allocated once at full size, so it never moves)
+  DevBuf<float> fit_slots{&frees};
 };
 
 extern "C" {
@@ -871,6 +873,26 @@ int nfb_latent_rows_grad(NfbHandle* h, const float* grad_latents, const int32_t*
   NFB_CUDA(cudaSetDevice(h->device));
   NFB_CUDA(nfb::launch_latent_rows(grad_latents, image_index, K, latent_table, n_rows, table_grads, reg_weight,
                                    static_cast<cudaStream_t>(stream), &h->launches));
+  return NFB_OK;
+}
+
+int nfb_fit_rows_grad(NfbHandle* h, const NfbTrainImages* d, const int32_t* image_index, int K, int n, const int32_t* pixel_rc,
+                      const float* grad_ray_origins, const float* grad_ray_directions, float* pose_grads, const float* grad_expressions,
+                      float* expression_grads, void* stream) {
+  if (!h || !d || !image_index || K < 1 || n < 1 || n > nfb::kSmpMax) return NFB_ERR_INVALID;
+  if (K > NFB_MAX_STEP_IMAGES) return NFB_ERR_UNSUPPORTED;
+  if (d->n_images < 1 || d->height < 1 || d->width < 1) return NFB_ERR_INVALID;
+  if (pose_grads && (!pixel_rc || (!grad_ray_origins && !grad_ray_directions))) return NFB_ERR_INVALID;
+  if (!expression_grads != !grad_expressions) return NFB_ERR_INVALID;
+  if (!pose_grads && !expression_grads) return NFB_OK;  // nothing asked for: nothing written, no launch
+  NFB_CUDA(cudaSetDevice(h->device));
+  NFB_CUDA(h->fit_slots.reserve((size_t)NFB_MAX_STEP_IMAGES * 12));  // once, at its largest: a graph's address stays valid
+  const float fx = static_cast<float>(d->intrinsics[0]), fy = static_cast<float>(d->intrinsics[1]);
+  const float wcx = static_cast<float>(static_cast<double>(d->width) * d->intrinsics[2]);  // as nfb_sample_rays_images rounds them
+  const float hcy = static_cast<float>(static_cast<double>(d->height) * d->intrinsics[3]);
+  NFB_CUDA(nfb::launch_fit_rows(image_index, K, n, d->n_images, pixel_rc, grad_ray_origins, grad_ray_directions, fx, fy, wcx, hcy,
+                                h->fit_slots.get(), pose_grads, grad_expressions, expression_grads, static_cast<cudaStream_t>(stream),
+                                &h->launches));
   return NFB_OK;
 }
 

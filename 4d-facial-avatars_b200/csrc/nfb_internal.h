@@ -268,6 +268,11 @@ cudaError_t launch_sample_images(const ImageSampleArgs& a, cudaStream_t st, long
 // nfb_latent_rows_grad).
 cudaError_t launch_latent_rows(const float* grad_latents, const int* image_index, int K, const float* table, int n_rows, float* table_grads,
                                float reg_w, cudaStream_t st, long long* launches);
+// One or two launches (nfb_optim.cu): the pose rows (slot sums into `slots` [K][12], then the rows) and the expression rows of a
+// fitting step over K images (order: include/nfb.h, nfb_fit_rows_grad).  pose_grads NULL: the expression rows only, one launch.
+cudaError_t launch_fit_rows(const int* image_index, int K, int n, int n_rows, const int* pixel_rc, const float* g_o, const float* g_d,
+                            float fx, float fy, float wcx, float hcy, float* slots, float* pose_grads, const float* g_expr,
+                            float* expr_grads, cudaStream_t st, long long* launches);
 cudaError_t launch_fill_int(int* p, long long n, int v, cudaStream_t st, long long* launches);
 
 }  // namespace nfb

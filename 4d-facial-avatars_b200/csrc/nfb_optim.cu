@@ -177,6 +177,87 @@ cudaError_t launch_latent_rows(const float* grad_latents, const int* image_index
   return cudaGetLastError();
 }
 
+// The pose and expression rows of a fitting step over K images (nfb_fit_rows_grad; order: include/nfb.h).  Ray j of slot k sits
+// at pixel (row, col) = pixel_rc[k * n + j] with camera direction c = (cx, cy, -1) (smp::camera_dir, the sampler's own bits),
+// d = R c and o = t, so the 3x4 pose row gets dR[q] = sum_j dd_j[q] * (cx_j, cy_j, -1) and dt[q] = sum_j do_j[q].
+// fit_pose_slots_kernel: block k sums slot k's rays into slots[k][12] (entry 4q + m of the row-major 3x4).  Thread t adds the
+// terms of rays j = t, t + 256, ... in ascending j, each term one rounded FP32 product (dd * cx, dd * cy), a negation (-dd) or the
+// value itself (do), added with one rounded FP32 add; the 256 partials then meet in a halving tree, partial[t] += partial[t + s]
+// for s = 128, 64, ..., 1.  A NULL dd (do) gives zero for columns 0..2 (3).
+constexpr int kFitThreads = 256;
+__global__ void __launch_bounds__(kFitThreads) fit_pose_slots_kernel(const int* __restrict__ pixel_rc, const float* __restrict__ g_o,
+                                                                     const float* __restrict__ g_d, int n, float fx, float fy, float wcx,
+                                                                     float hcy, float* __restrict__ slots) {
+  __shared__ float part[12][kFitThreads];
+  const int k = blockIdx.x, t = threadIdx.x;
+  float acc[12];
+#pragma unroll
+  for (int c = 0; c < 12; ++c) acc[c] = 0.f;
+  for (int j = t; j < n; j += kFitThreads) {
+    const size_t i = (size_t)k * n + j;
+    if (g_d) {
+      float cx, cy;
+      smp::camera_dir(pixel_rc[2 * i], pixel_rc[2 * i + 1], fx, fy, wcx, hcy, cx, cy);
+#pragma unroll
+      for (int q = 0; q < 3; ++q) {
+        const float dd = g_d[3 * i + q];
+        acc[4 * q] = __fadd_rn(acc[4 * q], __fmul_rn(dd, cx));
+        acc[4 * q + 1] = __fadd_rn(acc[4 * q + 1], __fmul_rn(dd, cy));
+        acc[4 * q + 2] = __fadd_rn(acc[4 * q + 2], -dd);
+      }
+    }
+    if (g_o) {
+#pragma unroll
+      for (int q = 0; q < 3; ++q) acc[4 * q + 3] = __fadd_rn(acc[4 * q + 3], g_o[3 * i + q]);
+    }
+  }
+#pragma unroll
+  for (int c = 0; c < 12; ++c) part[c][t] = acc[c];
+  __syncthreads();
+  for (int s = kFitThreads / 2; s > 0; s >>= 1) {
+    if (t < s) {
+#pragma unroll
+      for (int c = 0; c < 12; ++c) part[c][t] = __fadd_rn(part[c][t], part[c][t + s]);
+    }
+    __syncthreads();
+  }
+  if (t < 12) slots[(size_t)k * 12 + t] = part[t][0];
+}
+
+// fit_rows_kernel: one block, thread c = one column of the 12 pose columns (c < 12: slots) and the 76 expression columns
+// (12 <= c < 88: grad_expressions), in ascending k:  G[img[k]][c] += term[k][c], one FP32 add each; no atomics.  An index outside
+// [0, n_rows) adds nothing.  A NULL source or destination leaves its columns alone.
+__global__ void __launch_bounds__(96) fit_rows_kernel(const int* __restrict__ img, int K, int n_rows, const float* __restrict__ slots,
+                                                      float* __restrict__ pose_grads, const float* __restrict__ g_expr,
+                                                      float* __restrict__ expr_grads) {
+  const int c = threadIdx.x;
+  const bool pose = c < 12 && pose_grads, expr = c >= 12 && c < 12 + kDimExpr && expr_grads;
+  if (!pose && !expr) return;
+  for (int k = 0; k < K; ++k) {
+    const int r = img[k];
+    if (r < 0 || r >= n_rows) continue;
+    if (pose) {
+      float* g = pose_grads + (size_t)r * 12 + c;
+      *g = __fadd_rn(*g, slots[(size_t)k * 12 + c]);
+    } else {
+      float* g = expr_grads + (size_t)r * kDimExpr + (c - 12);
+      *g = __fadd_rn(*g, g_expr[(size_t)k * kDimExpr + (c - 12)]);
+    }
+  }
+}
+
+cudaError_t launch_fit_rows(const int* image_index, int K, int n, int n_rows, const int* pixel_rc, const float* g_o, const float* g_d,
+                            float fx, float fy, float wcx, float hcy, float* slots, float* pose_grads, const float* g_expr,
+                            float* expr_grads, cudaStream_t st, long long* launches) {
+  if (pose_grads) {
+    fit_pose_slots_kernel<<<K, kFitThreads, 0, st>>>(pixel_rc, g_o, g_d, n, fx, fy, wcx, hcy, slots);
+    ++*launches;
+  }
+  fit_rows_kernel<<<1, 96, 0, st>>>(image_index, K, n_rows, slots, pose_grads, g_expr, expr_grads);
+  ++*launches;
+  return cudaGetLastError();
+}
+
 cudaError_t launch_loss_grad(const float* rgb_c, const float* rgb_f, const float* target, int n_rays, long long n_total, float* g_c,
                              float* g_f, float* loss, cudaStream_t st, long long* launches) {
   const int n = 3 * n_rays;

@@ -301,8 +301,8 @@ __device__ __forceinline__ void gather_pixels(const GatherArgs& a, const long lo
     if (a.indices) a.indices[i] = k;
     if (a.frame) a.frame[i] = a.frame_value;
     if (a.ray_d) {  // get_ray_bundle (nerf_helpers.py:111-122) at pixel (row, col), same FP32 operation order as the render kernels
-      const float cx = __fdiv_rn(__fsub_rn((float)col, a.wcx), a.fx);
-      const float cy = -__fdiv_rn(__fsub_rn((float)row, a.hcy), a.fy);
+      float cx, cy;
+      smp::camera_dir(row, col, a.fx, a.fy, a.wcx, a.hcy, cx, cy);
       for (int q = 0; q < 3; ++q)
         a.ray_d[3 * i + q] = __fadd_rn(__fadd_rn(__fmul_rn(cx, a.pose[4 * q]), __fmul_rn(cy, a.pose[4 * q + 1])), __fmul_rn(-1.f, a.pose[4 * q + 2]));
       if (a.ray_o) for (int q = 0; q < 3; ++q) a.ray_o[3 * i + q] = a.pose[4 * q + 3];

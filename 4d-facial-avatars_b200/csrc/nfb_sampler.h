@@ -149,5 +149,16 @@ NFB_SHD long long search_right(double x, double total, long long N, const Run* r
   return lo;
 }
 
+#if defined(__CUDACC__)
+// Camera-space direction (cx, cy, -1) of pixel (row, col), as get_ray_bundle (nerf_helpers.py:111-122) forms it in FP32:
+// cx = (col - W * cx0) / fx, cy = -(row - H * cy0) / fy, with wcx = W * cx0 and hcy = H * cy0 rounded to FP32 once.  The
+// samplers' gathers and the pose-gradient rows of nfb_fit_rows_grad both call it, so the pose gradient multiplies by the very
+// bits the rays were built from.
+__device__ __forceinline__ void camera_dir(int row, int col, float fx, float fy, float wcx, float hcy, float& cx, float& cy) {
+  cx = __fdiv_rn(__fsub_rn((float)col, wcx), fx);
+  cy = -__fdiv_rn(__fsub_rn((float)row, hcy), fy);
+}
+#endif
+
 }  // namespace smp
 }  // namespace nfb

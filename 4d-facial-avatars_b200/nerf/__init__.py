@@ -12,7 +12,9 @@ from .train_utils import GaussianSmoothing, predict_and_render_radiance, render_
 from .load_flame import load_flame_data
 from .load_llff import load_llff_data
 from ._engine import get_precision, set_precision
+from .fused_fit import FusedFitter
 
 __all__ = ["models", "CfgNode", "get_embedding_function", "get_minibatches", "get_ray_bundle", "img2mse", "meshgrid_xy",
            "mse2psnr", "positional_encoding", "dump_rays", "GaussianSmoothing", "predict_and_render_radiance",
-           "run_one_iter_of_nerf", "render_frames", "load_flame_data", "load_llff_data", "get_precision", "set_precision"]
+           "run_one_iter_of_nerf", "render_frames", "load_flame_data", "load_llff_data", "get_precision", "set_precision",
+           "FusedFitter"]

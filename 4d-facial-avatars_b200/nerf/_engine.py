@@ -281,15 +281,22 @@ class Renderer:
         """nfb_repack: both networks' FP32 parameter tensors (lists in PARAM_ORDER) -> kernel-layout streams, one launch."""
         capi.check(capi.lib.nfb_repack(self._h, _ptrs(params_c), _ptrs(params_f), _stream()), "repack")
 
-    def backward_into(self, out_grads, params_c, params_f, grads_c, grads_f, grad_latent, frames=False):
+    def backward_into(self, out_grads, params_c, params_f, grads_c, grads_f, grad_latent, frames=False, grad_expressions=None,
+                      grad_ray_origins=None, grad_ray_directions=None):
         """nfb_render_backward writing straight into caller-owned gradient tensors (views of a flat bucket): params_* / grads_*
-        are lists of 26 contiguous FP32 CUDA tensors in PARAM_ORDER (grads of layers_dir.3.* may be None).  frames=True:
-        nfb_render_backward_frames after a multi-frame training forward, per-frame d latent into grad_latent [F,32]."""
+        are lists of 26 contiguous FP32 CUDA tensors in PARAM_ORDER (grads of layers_dir.3.* may be None; grads_c and grads_f
+        both None: input-only mode).  frames=True: nfb_render_backward_frames after a multi-frame training forward, per-frame
+        d latent into grad_latent [F,32], and into caller-owned buffers too d expression [F,76] (grad_expressions) and the per-ray
+        ray gradients [N,3] (grad_ray_origins, grad_ray_directions), each when given."""
         keep = []
         args = (self._h, C.byref(_out_grads(out_grads, self.device, keep)), _ptrs(params_c), _ptrs(params_f), _ptrs(grads_c),
                 _ptrs(grads_f), _ptr(grad_latent))
         if frames:
-            capi.check(capi.lib.nfb_render_backward_frames(*args, None, None, _stream()), "render_backward_frames")
+            ig = None
+            if grad_ray_origins is not None or grad_ray_directions is not None:
+                ig = capi.NfbInputGrads(ray_origins=_ptr(grad_ray_origins), ray_directions=_ptr(grad_ray_directions))
+            capi.check(capi.lib.nfb_render_backward_frames(*args, _ptr(grad_expressions) if grad_expressions is not None else None,
+                                                           C.byref(ig) if ig is not None else None, _stream()), "render_backward_frames")
         else:
             capi.check(capi.lib.nfb_render_backward(*args, _stream()), "render_backward")
         self._bwd_keep = keep
@@ -312,6 +319,15 @@ class Renderer:
         reg_weight * l / ||l|| in ascending k (all CUDA tensors; image_index int32 [K])."""
         capi.check(capi.lib.nfb_latent_rows_grad(self._h, _ptr(grad_latents), _ptr(image_index), image_index.numel(), _ptr(table),
                                                  table.shape[0], _ptr(table_grads), float(reg_weight), _stream()), "latent_rows_grad")
+
+    def fit_rows_grad(self, data, image_index, n, pixel_rc, grad_ray_origins, grad_ray_directions, pose_grads, grad_expressions,
+                      expression_grads):
+        """nfb_fit_rows_grad: pose_grads[image_index[k]] ([n_images,12]) += slot k's pose gradient from the per-ray ray gradients at
+        pixel_rc, and expression_grads[image_index[k]] ([n_images,76]) += grad_expressions[k], in ascending k (CUDA tensors; any
+        pair may be None; data = ray_sampler.TrainImages)."""
+        capi.check(capi.lib.nfb_fit_rows_grad(self._h, C.byref(data.desc), _ptr(image_index), image_index.numel(), int(n), _ptr(pixel_rc),
+                                              _ptr(grad_ray_origins), _ptr(grad_ray_directions), _ptr(pose_grads), _ptr(grad_expressions),
+                                              _ptr(expression_grads), _stream()), "fit_rows_grad")
 
     def backward(self, out_grads, params_c, params_f, want_latent=True, want_params=True, inputs=None, frames=False):
         """nfb_render_backward_ex for the last training forward.  out_grads: 7 CUDA tensors or None (rgb_c, disp_c, acc_c,

@@ -19,6 +19,54 @@ from . import train_utils
 from ._engine import PARAM_ORDER
 
 
+def _draw_noise(opts, dev, n):
+    """The reference's draws for one chunk of n rays (train chunksize = num_random_rays in the shipped YAML, so a batch is one
+    chunk); None when neither perturbation nor sigma noise is on.  Shared by the fused training and fitting steps."""
+    return train_utils._draw_noise(n, opts, dev, opts["num_fine"] > 0) if (opts["perturb"] or opts["noise_std"] > 0.0) else None
+
+
+def _capture(own_engine, eng, grads, body, tail):
+    """The capture skeleton of the fused steps: own the renderer's packed weights, body() once eagerly (the warm-up sizes the
+    library's buffers: cudaMalloc is not capturable), read the buffer epoch, zero the gradient bucket, then body() and tail()
+    captured into a CUDA graph.  Returns the graph, what the captured body returned (its buffers must outlive the graph) and
+    the epoch."""
+    own_engine()
+    body()
+    epoch = eng.buffer_epoch()
+    grads.zero_()
+    torch.cuda.synchronize()
+    graph = torch.cuda.CUDAGraph()
+    with torch.cuda.graph(graph):
+        keep = body()
+        tail()
+    return dict(graph=graph, keep=keep, epoch=epoch)
+
+
+def _check_epoch(eng, g):
+    """Refuse to replay a graph whose renderer buffers were re-allocated or refilled since capture (nfb_buffer_epoch)."""
+    if eng.buffer_epoch() != g["epoch"]:
+        raise RuntimeError("a call on this device since capture re-allocated renderer buffers the graph points at (a larger "
+                           "step, more frames or more images per step, on any trainer): capture again")
+
+
+def _image_buffers(cache, dev, data, k, n, shortfall, **extra):
+    """Per-step buffers of a K-image step, cached per (K, n, background): the sampler's outputs for N = K * n rays, the
+    loss-gradient buffers g0 / g1 [N,3] and the caller's `extra` buffers, name -> shape (float32) or (shape, dtype).  The chunked backward re-reads
+    rays and frame indices, so they outlive the step."""
+    key = (k, n, data.background is not None)
+    sb = cache.get(key)
+    if sb is None:
+        N = k * n
+        z = lambda *shape, dt=torch.float32: torch.zeros(shape, device=dev, dtype=dt)  # noqa: E731
+        sb = cache[key] = dict(
+            img=z(k, dt=torch.int32), ray_origins=z(N, 3), ray_directions=z(N, 3), target=z(N, 3),
+            background=z(N, 3) if data.background is not None else None, frame_index=z(N, dt=torch.int32),
+            expressions=z(k, 76), latents=z(k, 32), state=z(k, 3, dt=torch.int32), shortfall=shortfall[:k],
+            g0=z(N, 3), g1=z(N, 3),
+            **{name: (z(*s[0], dt=s[1]) if isinstance(s[-1], torch.dtype) else z(*s)) for name, s in extra.items()})
+    return sb
+
+
 class FusedTrainer:
     def __init__(self, model_coarse, model_fine, n_latent, lr=5e-4, lr_decay_steps=250000, lr_decay_factor=0.1,
                  betas=(0.9, 0.999), eps=1e-8, num_coarse=64, num_fine=64, perturb=True, noise_std=0.1, near=0.2, far=0.8,
@@ -97,10 +145,7 @@ class FusedTrainer:
             self.eng.packed_owner = self
 
     def _draw_noise(self, n):
-        """The reference's draws for one chunk of n rays (train chunksize = num_random_rays in the shipped YAML, so a batch is one
-        chunk); None when neither perturbation nor sigma noise is on."""
-        o = self.opts
-        return train_utils._draw_noise(n, o, self.dev, o["num_fine"] > 0) if (o["perturb"] or o["noise_std"] > 0.0) else None
+        return _draw_noise(self.opts, self.dev, n)
 
     def _forward_backward(self, expressions, latents, frame_index, ro, rd, background, target, n_total, noise, g, grad_latent):
         """Frame fold, training forward, loss gradient and backward of one batch into the flat gradient bucket, d latent into
@@ -141,20 +186,13 @@ class FusedTrainer:
         """body() once eagerly, then body, the all-reduce (world > 1) followed by after_collective(), Adam with its regulariser
         on `row` and the re-pack captured into a CUDA graph.  Returns the graph, what the captured body returned (its buffers
         must outlive the graph) and the renderer's buffer epoch."""
-        self._own_engine()
-        body()                      # eager warm-up: sizes the library's buffers (cudaMalloc is not capturable)
-        epoch = self.eng.buffer_epoch()
-        self.grads.zero_()
-        torch.cuda.synchronize()
-        graph = torch.cuda.CUDAGraph()
-        with torch.cuda.graph(graph):
-            keep = body()
+        def tail():
             if world > 1:
                 dist.all_reduce(self.grads, group=group)
                 if after_collective is not None:
                     after_collective()
             self._adam_repack(row)
-        return dict(graph=graph, keep=keep, epoch=epoch)
+        return _capture(self._own_engine, self.eng, self.grads, body, tail)
 
     def gradients(self, ray_origins, ray_directions, target, expressions, latent_index, background=None, world=1, n_total=None,
                   noise=None, events=None, group=None):
@@ -189,10 +227,7 @@ class FusedTrainer:
         self._stepped()
 
     def _check_epoch(self, g):
-        """Refuse to replay a graph whose renderer buffers were re-allocated or refilled since capture (nfb_buffer_epoch)."""
-        if self.eng.buffer_epoch() != g["epoch"]:
-            raise RuntimeError("a call on this device since capture re-allocated renderer buffers the graph points at (a larger "
-                               "step, more frames or more images per step, on any trainer): capture again")
+        _check_epoch(self.eng, g)
 
     # ---- the whole iteration as ONE CUDA graph (launch-bound at small per-rank batches: ~20 kernels of 3-800 us)
     def capture(self, n, has_background=True, world=1, n_total=None, group=None):
@@ -252,17 +287,7 @@ class FusedTrainer:
     # draws and renders its slice [rank * N / world, (rank + 1) * N / world); one SUM all-reduce of the bucket joins the slices.
     def _images_buffers(self, data, k, n):
         """Per-step buffers of a K-image step (cached per shape: the chunked backward re-reads rays and frame indices)."""
-        key = (k, n, data.background is not None)
-        sb = self._image_bufs.get(key)
-        if sb is None:
-            N, dev = k * n, self.dev
-            z = lambda *shape, dt=torch.float32: torch.zeros(shape, device=dev, dtype=dt)  # noqa: E731
-            sb = self._image_bufs[key] = dict(
-                img=z(k, dt=torch.int32), ray_origins=z(N, 3), ray_directions=z(N, 3), target=z(N, 3),
-                background=z(N, 3) if data.background is not None else None, frame_index=z(N, dt=torch.int32),
-                expressions=z(k, 76), latents=z(k, 32), state=z(k, 3, dt=torch.int32), shortfall=self.shortfall[:k],
-                glat=z(k, 32), g0=z(N, 3), g1=z(N, 3), zero_lat=z(k, 32))
-        return sb
+        return _image_buffers(self._image_bufs, self.dev, data, k, n, self.shortfall, glat=(k, 32), zero_lat=(k, 32))
 
     def _images_sample(self, data, sb, n, draws, max_rounds):
         self.eng.sample_images(data, sb["img"], n, draws, max_rounds, self.latent_codes, sb)

@@ -109,6 +109,17 @@ class TrainImages:
                                         self.images.data_ptr(), self.background.data_ptr() if self.background is not None else None,
                                         self.n_images, self.H, self.W, 0, (C.c_double * 4)(*self.intrinsics))
 
+    def alias_tables(self, poses, expressions):
+        """Point the descriptor's pose and expression tables at caller-owned rows instead of this object's copies: poses [N,12] and
+        expressions [N,76], contiguous FP32 tensors on this device, read in place by every later sampler call (and by every
+        replay of a graph captured over one), so that writes into them change the rays and conditioning rows drawn next.  The
+        caller keeps them alive while this object is used.  (The fitter's parameter tables are such rows.)"""
+        for name, t, w in (("poses", poses, 12), ("expressions", expressions, 76)):
+            if (t.dtype != torch.float32 or t.device != self.dev or tuple(t.shape) != (self.n_images, w) or not t.is_contiguous()):
+                raise ValueError(f"{name} must be a contiguous FP32 [{self.n_images},{w}] tensor on {self.dev}")
+        self.poses, self.expressions = poses, expressions
+        self.desc.poses, self.desc.expressions = poses.data_ptr(), expressions.data_ptr()
+
     def _keep_in_place(self, t):
         if t.is_cuda:
             return t.detach().to(device=self.dev, dtype=torch.float32).contiguous()

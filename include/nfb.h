@@ -41,6 +41,10 @@ extern "C" {
 /* Defined when precision NFB_PREC_EXACT_GRAD exists (hi + lo gradients, see below), with NfbTrainDebug.record_bytes reporting the
  * record stride and NfbWeightDebug's bwd_lo members.  The version number stayed 131 for this addition: test this macro. */
 #define NFB_EXACT_GRAD 1
+/* Defined when nfb_fit_rows_grad exists: the pose and expression rows of a fitting step over several images (a frozen avatar's
+ * per-frame camera pose, expression and latent fitted to photos).  The version number stayed 131 for this addition: test this
+ * macro. */
+#define NFB_FIT_STEP 1
 
 typedef struct NfbHandle NfbHandle;
 
@@ -465,6 +469,41 @@ int nfb_sample_rays_images(NfbHandle* h, const NfbTrainImages* data, const int32
  * regulariser term.  K in [1, NFB_MAX_STEP_IMAGES].  1 launch. */
 int nfb_latent_rows_grad(NfbHandle* h, const float* grad_latents, const int32_t* image_index, int K, const float* latent_table, int n_rows,
                          float* table_grads, float reg_weight, void* stream);
+/* ---- Fitting steps over several images (NFB_FIT_STEP) ----
+ * The pose and expression rows of a fitting step's gradient: what autograd leaves in data->poses and data->expressions (as
+ * [n_images][12] and [n_images][76] leaves) for a loss over the K * n rays nfb_sample_rays_images drew from `data` with the same
+ * image_index, given the per-ray ray gradients and per-frame expression gradients of nfb_render_backward_frames.
+ *
+ * Pose rows.  Ray j of slot k sits at pixel (row, col) = pixel_rc[k * n + j] (nfb_sample_rays_images' pixel_rc); the sampler
+ * built it as d = R c, o = t from the 3x4 row-major pose [R | t] and the camera direction c = (cx, cy, -1), cx = (col - W * cx0)
+ * / fx, cy = -(row - H * cy0) / fy in FP32 (the same device helper forms both, so these are the rays' own bits).  So
+ *     dR[q][0] = sum_j dd_j[q] * cx_j,  dR[q][1] = sum_j dd_j[q] * cy_j,  dR[q][2] = sum_j (-dd_j[q]),  dt[q] = sum_j do_j[q].
+ * Order (no atomics: the rows repeat bit for bit).  First, per slot k, 256 partial sums: partial t adds the terms of rays
+ * j = t, t + 256, t + 512, ... in ascending j, each term one rounded FP32 product (dd * cx, dd * cy), a negation (-dd) or the
+ * value (do), each addition one rounded FP32 add starting from +0; then the partials meet in a halving tree, partial[t] +=
+ * partial[t + s] for s = 128, 64, 32, 16, 8, 4, 2, 1, and partial[0] is slot k's sum.  Then, in ascending k, slot k's 12 sums
+ * are added (one FP32 add each) onto pose_grads[image_index[k]]: rows are ADDED to, and an image named twice accumulates both
+ * slots in that order.  A NULL grad_ray_directions (origins) counts as zero for the R (t) columns.
+ * Expression rows.  In ascending k, grad_expressions[k] ([K][76], nfb_render_backward_frames' grad_expressions) is added onto
+ * expression_grads[image_index[k]], one FP32 add per element, in the same launch as the pose rows.
+ * Edges.  An image_index outside [0, n_images) adds nothing (its slot's sums are formed and dropped).  A NaN ray gradient
+ * reaches only its own slot's row.  An incomplete selection (state[k][0] < n: repeated pixels) counts every repeat, each
+ * repeated pixel being a ray of the batch.  Rows not named get nothing.
+ * Errors, before any CUDA call: NFB_ERR_INVALID for a null handle / data / image_index, K or n < 1, n > 2048, a data set with
+ * n_images, height or width < 1, pose_grads without pixel_rc or without any ray gradient, expression_grads without
+ * grad_expressions or the other way round; NFB_ERR_UNSUPPORTED for K > NFB_MAX_STEP_IMAGES.  With pose_grads and
+ * expression_grads both NULL nothing is written and nothing launched.
+ * Launches: 2 with pose rows (slot sums: K blocks of 256 threads; rows: one block), 1 with expression rows only.  Scratch: the
+ * handle's [NFB_MAX_STEP_IMAGES][12] slot sums, allocated once at the first call (it never moves: nfb_buffer_epoch does not
+ * change). */
+int nfb_fit_rows_grad(NfbHandle* h, const NfbTrainImages* data, const int32_t* image_index, int K, int n,
+                      const int32_t* pixel_rc,           /* [K*n][2], nfb_sample_rays_images' */
+                      const float* grad_ray_origins,     /* [K*n][3] or NULL */
+                      const float* grad_ray_directions,  /* [K*n][3] or NULL */
+                      float* pose_grads,                 /* [n_images][12] or NULL: rows ADDED to */
+                      const float* grad_expressions,     /* [K][76] or NULL */
+                      float* expression_grads,           /* [n_images][76] or NULL: rows ADDED to */
+                      void* stream);
 
 /* Host-only test hook of the same arithmetic: out[i] = np.cumsum(p)[ks[i]] (ks[i] == -1: the last entry) for the map with the
  * ascending flat indices zeroed_sorted set to zero.  No CUDA call. */
