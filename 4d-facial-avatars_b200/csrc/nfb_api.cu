@@ -341,6 +341,14 @@ static int ensure_train_buffers(NfbHandle::Train& tr, const nfb::TileGeom& g, in
   return NFB_OK;
 }
 
+// A training forward (a whole one, or one chunk of it re-run by the backward) saves what the backward reads into tr's buffers.
+static void set_save_slots(nfb::RenderParams& p, NfbHandle::Train& tr) {
+  p.save_rec = tr.rec.get(); p.save_dnorm = tr.dnorm.get(); p.save_raw_c = tr.raw_c.get(); p.save_raw_f = tr.raw_f.get();
+  p.dbg_z_c = tr.z_c.get(); p.dbg_z_f = tr.z_f.get();
+  p.save_ray = tr.ray.get();  // the rays, for input gradients (the backward does not read the caller's buffers)
+  if (tr.multi) p.save_frame = tr.frame.get();
+}
+
 // frame_index non-null: a multi-frame call (the frame table of nfb_set_frames instead of the frame of nfb_set_frame).
 static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm, const NfbNoise* noise, const NfbOutputs* out,
                        const NfbDebug* dbg, void* stream, bool train, const int32_t* frame_index = nullptr) {
@@ -473,19 +481,13 @@ static int render_impl(NfbHandle* h, const NfbRays* rays, const NfbSampling* sm,
     // a later nfb_set_frame (e.g. a validation render before the backward) must not change what the backward differentiates
     if (!multi) NFB_CUDA(cudaMemcpyAsync(tr.cond.get(), h->cond.get(), nfb::kDimCond * sizeof(float), cudaMemcpyDeviceToDevice, st));
     else NFB_CUDA(cudaMemsetAsync(tr.cond.get(), 0, nfb::kDimCond * sizeof(float), st));
-    if (!tr.chunked) {
-      p.save_rec = tr.rec.get(); p.save_dnorm = tr.dnorm.get(); p.save_raw_c = tr.raw_c.get(); p.save_raw_f = tr.raw_f.get();
-      p.dbg_z_c = tr.z_c.get(); p.dbg_z_f = tr.z_f.get();
-      p.save_ray = tr.ray.get();  // the rays, for input gradients (the backward does not read the caller's buffers)
-      if (multi) p.save_frame = tr.frame.get();
-    }
+    if (!tr.chunked) set_save_slots(p, tr);
     tr.has_rays = rays->o != nullptr; tr.has_dir_z = rays->dir_z != nullptr;
     tr.geom = p.geom; tr.has_bg = rays->background != nullptr; tr.white_bkgd = p.white_bkgd;
   }
   // exact-grad mode runs its own kernel only where records are saved (p.save_rec); evaluation renders and the over-budget
   // training forward, which saves nothing until the backward re-runs it chunk by chunk, run exact mode's
-  if (multi) NFB_CUDA(nfb::launch_render_frames(p, sm->precision, h->num_sms, st, &h->launches));
-  else NFB_CUDA(nfb::launch_render(p, sm->precision, h->num_sms, st, &h->launches));
+  NFB_CUDA(nfb::launch_render(p, sm->precision, h->num_sms, st, &h->launches));
   if (train) h->tr.valid = true;
   return NFB_OK;
 }
@@ -655,19 +657,12 @@ static int backward_impl(NfbHandle* h, const NfbOutGrads* og, const float* const
       if (p.noise_c) p.noise_c += b * g.nc;
       if (p.u_rand) p.u_rand += b * g.nf;
       if (p.noise_f) p.noise_f += b * g.samples(1);
+      if (p.frame) p.frame += b;
       float* so = tr.scratch_out.get();
       p.rgb_c = so; p.disp_c = so + 3 * cn; p.acc_c = so + 4 * cn; p.rgb_f = so + 5 * cn; p.disp_f = so + 8 * cn; p.acc_f = so + 9 * cn;
       p.w_last = so + 10 * cn;
-      p.save_rec = tr.rec.get(); p.save_dnorm = tr.dnorm.get(); p.save_raw_c = tr.raw_c.get(); p.save_raw_f = tr.raw_f.get();
-      p.save_ray = tr.ray.get();
-      p.dbg_z_c = tr.z_c.get(); p.dbg_z_f = tr.z_f.get();
-      if (tr.multi) {
-        p.frame += b;
-        p.save_frame = tr.frame.get();
-        NFB_CUDA(nfb::launch_render_frames(p, tr.precision, h->num_sms, st, &h->launches));
-      } else {
-        NFB_CUDA(nfb::launch_render(p, tr.precision, h->num_sms, st, &h->launches));
-      }
+      set_save_slots(p, tr);
+      NFB_CUDA(nfb::launch_render(p, tr.precision, h->num_sms, st, &h->launches));
       rc = backward_rays(begin, g);
       if (rc) return rc;
     }

@@ -200,10 +200,9 @@ cudaError_t launch_adam_dev(float* p, float* g, float* m, float* v, long long n,
 cudaError_t launch_adam(float* p, float* g, float* m, float* v, long long n, float lr, float b1, float b2, float eps, int step,
                         float grad_scale, long long reg_off, float reg_w, cudaStream_t st, long long* launches);
 // precision: 0 = fast (x1), 1 = exact (x3), 2 = exact-grad (exact mode's kernels; a training forward writes the lo records too).
-// num_sms = CTAs to launch at most.
+// num_sms = CTAs to launch at most.  p.frame set: a multi-frame call (render_frames_kernel), where p.frame and p.fbias select
+// each ray's rows of steps 0 and 3.
 cudaError_t launch_render(const RenderParams& p, int precision, int num_sms, cudaStream_t st, long long* launches);
-// The multi-frame instantiations (render_frames_kernel): p.frame and p.fbias select each ray's rows of steps 0 and 3.
-cudaError_t launch_render_frames(const RenderParams& p, int precision, int num_sms, cudaStream_t st, long long* launches);
 cudaError_t render_kernel_setup();  // opt-in to the large dynamic shared memory size
 
 // ---- either side of the path (nfb_post.cu)

@@ -1006,44 +1006,34 @@ __global__ void __launch_bounds__(kThreads, 1) render_frames_kernel(const __grid
   render_body<EXACT, SAVE, false, true>(p);
 }
 
-template <bool EXACT, bool SAVE, bool PROBE>
-static cudaError_t render_setup_one() {
-  return cudaFuncSetAttribute(render_kernel<EXACT, SAVE, PROBE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemMap<EXACT>::kBytes);
-}
 // The exact-grad training forwards (NFB_PREC_EXACT_GRAD): kernels of their own, so the other instantiations keep their names
 // and code.  MULTI: the multi-frame one.
 template <bool MULTI>
 __global__ void __launch_bounds__(kThreads, 1) render_hilo_kernel(const __grid_constant__ RenderParams p) {
   render_body<true, true, false, MULTI, true>(p);
 }
-template <bool MULTI>
-static cudaError_t render_hilo_setup_one() {
-  return cudaFuncSetAttribute(render_hilo_kernel<MULTI>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemMap<true>::kBytes);
+template <class Kernel>
+static cudaError_t smem_opt_in(Kernel* kernel, int bytes) {
+  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
 }
+// The training forward takes no debug dumps (nfb_render_forward_train), and a multi-frame call none at all, so only the
+// single-frame evaluation kernels have a probe instantiation.
 template <bool EXACT, bool SAVE>
-static cudaError_t render_frames_setup_one() {
-  return cudaFuncSetAttribute(render_frames_kernel<EXACT, SAVE>, cudaFuncAttributeMaxDynamicSharedMemorySize, SmemMap<EXACT>::kBytes);
-}
-// The training forward takes no debug dumps (nfb_render_forward_train), so only the evaluation kernels have a probe
-// instantiation.
-template <bool EXACT, bool SAVE>
-static void render_launch(const RenderParams& p, bool probe, int grid, cudaStream_t st) {
-  if constexpr (!SAVE) {
-    if (probe) {
-      render_kernel<EXACT, false, true><<<grid, kThreads, SmemMap<EXACT>::kBytes, st>>>(p);
-      return;
-    }
-  }
-  render_kernel<EXACT, SAVE, false><<<grid, kThreads, SmemMap<EXACT>::kBytes, st>>>(p);
+static void render_launch(const RenderParams& p, bool probe, bool multi, int grid, cudaStream_t st) {
+  constexpr int kBytes = SmemMap<EXACT>::kBytes;
+  if (multi) render_frames_kernel<EXACT, SAVE><<<grid, kThreads, kBytes, st>>>(p);
+  else if (!SAVE && probe) render_kernel<EXACT, false, true><<<grid, kThreads, kBytes, st>>>(p);
+  else render_kernel<EXACT, SAVE, false><<<grid, kThreads, kBytes, st>>>(p);
 }
 
 cudaError_t render_kernel_setup() {
-  const cudaError_t e[12] = {render_setup_one<false, false, false>(), render_setup_one<true, false, false>(),
-                             render_setup_one<false, true, false>(),  render_setup_one<true, true, false>(),
-                             render_setup_one<false, false, true>(),  render_setup_one<true, false, true>(),
-                             render_frames_setup_one<false, false>(), render_frames_setup_one<true, false>(),
-                             render_frames_setup_one<false, true>(),  render_frames_setup_one<true, true>(),
-                             render_hilo_setup_one<false>(),          render_hilo_setup_one<true>()};
+  constexpr int B = SmemMap<true>::kBytes, F = SmemMap<false>::kBytes;
+  const cudaError_t e[12] = {smem_opt_in(render_kernel<false, false, false>, F), smem_opt_in(render_kernel<true, false, false>, B),
+                             smem_opt_in(render_kernel<false, true, false>, F),  smem_opt_in(render_kernel<true, true, false>, B),
+                             smem_opt_in(render_kernel<false, false, true>, F),  smem_opt_in(render_kernel<true, false, true>, B),
+                             smem_opt_in(render_frames_kernel<false, false>, F), smem_opt_in(render_frames_kernel<true, false>, B),
+                             smem_opt_in(render_frames_kernel<false, true>, F),  smem_opt_in(render_frames_kernel<true, true>, B),
+                             smem_opt_in(render_hilo_kernel<false>, B),          smem_opt_in(render_hilo_kernel<true>, B)};
   for (const cudaError_t x : e)
     if (x != cudaSuccess) return x;
   return cudaSuccess;
@@ -1054,32 +1044,16 @@ cudaError_t launch_render(const RenderParams& p, int precision, int num_sms, cud
   if (grid <= 0) return cudaSuccess;
   const bool save = p.save_rec != nullptr;  // training forward: also writes the per-tile activation records
   const bool probe = p.dbg_act != nullptr;  // the activation probe (evaluation only): its own instantiation
+  const bool multi = p.frame != nullptr;    // multi-frame call: render_frames_kernel / render_hilo_kernel<true>
   if (precision == 2 && save) {
-    render_hilo_kernel<false><<<grid, kThreads, SmemMap<true>::kBytes, st>>>(p);
+    if (multi) render_hilo_kernel<true><<<grid, kThreads, SmemMap<true>::kBytes, st>>>(p);
+    else render_hilo_kernel<false><<<grid, kThreads, SmemMap<true>::kBytes, st>>>(p);
   } else if (precision != 0) {  // exact, and the evaluation renders of exact-grad mode
-    if (save) render_launch<true, true>(p, probe, grid, st);
-    else render_launch<true, false>(p, probe, grid, st);
+    if (save) render_launch<true, true>(p, probe, multi, grid, st);
+    else render_launch<true, false>(p, probe, multi, grid, st);
   } else {
-    if (save) render_launch<false, true>(p, probe, grid, st);
-    else render_launch<false, false>(p, probe, grid, st);
-  }
-  ++*launches;
-  return cudaGetLastError();
-}
-
-cudaError_t launch_render_frames(const RenderParams& p, int precision, int num_sms, cudaStream_t st, long long* launches) {
-  const int grid = p.geom.n_units < num_sms ? p.geom.n_units : num_sms;
-  if (grid <= 0) return cudaSuccess;
-  const bool save = p.save_rec != nullptr;
-  constexpr int B = SmemMap<true>::kBytes, F = SmemMap<false>::kBytes;
-  if (precision == 2 && save) {
-    render_hilo_kernel<true><<<grid, kThreads, B, st>>>(p);
-  } else if (precision != 0) {
-    if (save) render_frames_kernel<true, true><<<grid, kThreads, B, st>>>(p);
-    else render_frames_kernel<true, false><<<grid, kThreads, B, st>>>(p);
-  } else {
-    if (save) render_frames_kernel<false, true><<<grid, kThreads, F, st>>>(p);
-    else render_frames_kernel<false, false><<<grid, kThreads, F, st>>>(p);
+    if (save) render_launch<false, true>(p, probe, multi, grid, st);
+    else render_launch<false, false>(p, probe, multi, grid, st);
   }
   ++*launches;
   return cudaGetLastError();

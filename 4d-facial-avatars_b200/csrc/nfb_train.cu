@@ -538,135 +538,17 @@ template <int N> __device__ __forceinline__ void mma_n(float (&d)[N / 2], uint64
 constexpr int kPeGroup = 4, kPeGroups = 2;
 
 // One job over the CTA's tiles j0..j1 for this warpgroup's 64 output features: NB = N of the B image (<= 128 per accumulator;
-// 256 runs as two 128-column halves).  The result and the bias column sums go to the CTA's partial slot; where exactly is
-// worked out only after the tile loop, from the parameter block, so no address stays live in registers across it.
-template <bool kPeOnly, int NB>
+// 256 runs as two 128-column halves).  X3 (exact-grad mode, dw_x3_kernel): the records are the 2 MiB hi/lo ones and every
+// r-atom takes three stages, (A hi, B hi), (A hi, B lo), (A lo, B hi), with the same MMAs on each; the bias column sums take
+// A hi (first stage) and A lo (third) against the ones row.  The result and the bias column sums go to the CTA's partial
+// slot; where exactly is worked out only after the tile loop, from the parameter block, so no address stays live in
+// registers across it.
+template <bool kPeOnly, bool X3, int NB>
 __device__ __forceinline__ void run_job(const DwParams& p, const Job& J, int j0, int j1, uint32_t smem_base, StageRing& ring,
                                         int wg, int lane) {
   constexpr int NA = NB > 128 ? 128 : NB;
   constexpr int NH = NB > 128 ? 2 : 1;
-  float acc[NH][NA / 2];
-  float accb[8];
-  const bool bias = J.bias_layer >= 0;
-  const uint64_t ones = wgmma_desc_sw128(smem_base + kOffOnes);
-  for (int j = j0; j < j1; ++j) {
-    for (int a = 0; a < 2; ++a) {
-      const uint32_t sa = ring.wait_full(), sb = sa + 16384;
-      const uint64_t ad = wgmma_desc_sw128(sa + 64 * wg * 128);
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        const uint32_t accf = ((j - j0) | a | ks) ? 1u : 0u;
-#pragma unroll
-        for (int h = 0; h < NH; ++h) mma_n<NA>(acc[h], ad + (uint64_t)(ks * 2), wgmma_desc_sw128(sb + h * 16384) + (uint64_t)(ks * 2), accf);
-        if (bias) wgmma_n16(accb, ad + (uint64_t)(ks * 2), ones + (uint64_t)(ks * 2), accf);
-      }
-      wgmma_commit();
-      wgmma_wait<0>();
-#pragma unroll
-      for (int h = 0; h < NH; ++h) reg_fence(acc[h]);
-      reg_fence(accb);
-      ring.release();
-    }
-  }
-  constexpr int kG = kPeOnly ? kPeGroups : kGroups;
-  float* slot = p.ws + (size_t)(blockIdx.x / kG) * p.ws_stride;  // this (network, part)'s partial
-  const int bias_acc = bias ? acc_bias_off(J.bias_layer) : 0;
-  const int out_off = kPeOnly ? pe_slot_off(J.out_off) : J.out_off, bias_off = kPeOnly ? pe_slot_off(bias_acc) : bias_acc;
-  const float inv = p.scal[1];
-  const int c = lane & 3, r0 = 64 * wg + 16 * ((threadIdx.x >> 5) & 3) + (lane >> 2);
-#pragma unroll
-  for (int hh = 0; hh < 2; ++hh) {
-    const int R = r0 + 8 * hh;
-    float* out = slot + out_off + (size_t)(J.out_row0 + R) * J.out_ld;
-#pragma unroll
-    for (int h = 0; h < NH; ++h)
-#pragma unroll
-      for (int jj = 0; jj < NA / 8; ++jj) {
-        const int col = h * 128 + 8 * jj + 2 * c;
-        *reinterpret_cast<float2*>(out + col) = make_float2(acc[h][4 * jj + 2 * hh] * inv, acc[h][4 * jj + 2 * hh + 1] * inv);
-      }
-    if (bias && c == 0) slot[bias_off + J.out_row0 + R] = accb[2 * hh] * inv;
-  }
-}
-
-template <bool kPeOnly>
-__global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__ DwParams p) {
-  extern __shared__ __align__(1024) uint8_t smem[];
-  const uint32_t smem_base = smem_base_aligned(smem);
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-
-  // this CTA: network x job group (blockIdx.x % kGroups) x a contiguous share of the network's tiles
-  constexpr int kG = kPeOnly ? kPeGroups : kGroups;
-  const int group = (kPeOnly ? kPeGroup : 0) + (int)blockIdx.x % kG;
-  int part = (int)blockIdx.x / kG;
-  const int net = (part >= p.parts[0]) ? 1 : 0;
-  if (net) part -= p.parts[0];
-  const int parts = p.parts[net];
-  const int t_cnt = p.geom.tile_count(net);
-  const int total = p.geom.n_units * t_cnt;
-  const int per = (total + parts - 1) / parts;
-  const int j0 = part * per;
-  const int j1 = min(total, j0 + per);
-  if (part >= parts || j0 >= j1) return;  // uniform for the whole CTA
-  const int job0 = c_jobs.group_begin[group] + (kPeOnly ? 1 : 0), job1 = c_jobs.group_begin[group + 1];
-
-  StageRing ring(smem_base, smem_base + kOffBars);
-  if (threadIdx.x == 0) ring.init();
-  for (int i = threadIdx.x; i < 2048 / 4; i += kThreads)  // row 0 (first 128 bytes) = FP16 ones, rows 1..15 = 0
-    reinterpret_cast<uint32_t*>(smem + kOffOnes)[i] = (i < 32) ? 0x3C003C00u : 0u;
-  fence_proxy_async_smem();
-  __syncthreads();
-
-  auto tile_rec = [&](int j) -> const uint8_t* {
-    const int u = j / t_cnt, t = j - u * t_cnt;
-    return p.rec + p.geom.global_tile(u, net, t) * kRecBytes;
-  };
-
-  if (warp < 4) {
-    // ============================== producer ==============================
-    reg_dec<kRegsLight>();
-    if (warp == 0) {
-      for (int job = job0; job < job1; ++job) {
-        const Job J = c_jobs.j[job];
-        const uint32_t b_bytes = (uint32_t)J.b_rows * 128u;
-        for (int j = j0; j < j1; ++j) {
-          const uint8_t* rec = tile_rec(j);
-          for (int a = 0; a < 2; ++a)  // one stage = the A and the B image of one r-atom
-            ring.produce(rec + J.a_off + a * J.a_rows * 128 + J.a_half * 16384, 16384, 16384, rec + J.b_off + a * J.b_rows * 128,
-                         b_bytes);
-        }
-      }
-    }
-  } else {
-    // ============================== MMA + epilogue warpgroups ==============================
-    reg_inc<kRegsRow>();
-    const int wg = (warp - 4) >> 2;
-    for (int job = job0; job < job1; ++job) {
-      const Job J = c_jobs.j[job];
-      if constexpr (kPeOnly) {  // both PE jobs multiply by the 64-row PE image: only that shape is compiled in
-        run_job<kPeOnly, 64>(p, J, j0, j1, smem_base, ring, wg, lane);
-        continue;
-      }
-      switch (J.b_rows) {
-        case 16: run_job<kPeOnly, 16>(p, J, j0, j1, smem_base, ring, wg, lane); break;
-        case 32: run_job<kPeOnly, 32>(p, J, j0, j1, smem_base, ring, wg, lane); break;
-        case 64: run_job<kPeOnly, 64>(p, J, j0, j1, smem_base, ring, wg, lane); break;
-        case 128: run_job<kPeOnly, 128>(p, J, j0, j1, smem_base, ring, wg, lane); break;
-        default: run_job<kPeOnly, 256>(p, J, j0, j1, smem_base, ring, wg, lane); break;
-      }
-    }
-  }
-}
-
-// Exact-grad mode (dw_x3_kernel): the same jobs over the 2 MiB hi/lo records.  Three stages per r-atom, (A hi, B hi),
-// (A hi, B lo), (A lo, B hi), the same MMAs on each; the bias column sums take A hi (first stage) and A lo (third) against the
-// ones row.  Written out beside run_job / dw_kernel so that the FP16 kernels keep their source, and with it their code.
-template <bool kPeOnly, int NB>
-__device__ __forceinline__ void run_job_x3(const DwParams& p, const Job& J, int j0, int j1, uint32_t smem_base, StageRing& ring,
-                                        int wg, int lane) {
-  constexpr int NA = NB > 128 ? 128 : NB;
-  constexpr int NH = NB > 128 ? 2 : 1;
+  constexpr int NPART = X3 ? 3 : 1;
   float acc[NH][NA / 2];
   float accb[8];
   const bool bias = J.bias_layer >= 0;
@@ -674,7 +556,7 @@ __device__ __forceinline__ void run_job_x3(const DwParams& p, const Job& J, int 
   for (int j = j0; j < j1; ++j) {
     for (int a = 0; a < 2; ++a) {
 #pragma unroll
-      for (int part = 0; part < 3; ++part) {  // (A hi, B hi), (A hi, B lo), (A lo, B hi)
+      for (int part = 0; part < NPART; ++part) {
         const uint32_t sa = ring.wait_full(), sb = sa + 16384;
         const uint64_t ad = wgmma_desc_sw128(sa + 64 * wg * 128);
         wgmma_fence();
@@ -715,8 +597,8 @@ __device__ __forceinline__ void run_job_x3(const DwParams& p, const Job& J, int 
   }
 }
 
-template <bool kPeOnly>
-__global__ void __launch_bounds__(kThreads, 1) dw_x3_kernel(const __grid_constant__ DwParams p) {
+template <bool kPeOnly, bool X3>
+__device__ __forceinline__ void dw_body(const DwParams& p) {
   extern __shared__ __align__(1024) uint8_t smem[];
   const uint32_t smem_base = smem_base_aligned(smem);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -745,7 +627,7 @@ __global__ void __launch_bounds__(kThreads, 1) dw_x3_kernel(const __grid_constan
 
   auto tile_rec = [&](int j) -> const uint8_t* {
     const int u = j / t_cnt, t = j - u * t_cnt;
-    return p.rec + p.geom.global_tile(u, net, t) * rec_stride(true);
+    return p.rec + p.geom.global_tile(u, net, t) * rec_stride(X3);
   };
 
   if (warp < 4) {
@@ -757,12 +639,14 @@ __global__ void __launch_bounds__(kThreads, 1) dw_x3_kernel(const __grid_constan
         const uint32_t b_bytes = (uint32_t)J.b_rows * 128u;
         for (int j = j0; j < j1; ++j) {
           const uint8_t* rec = tile_rec(j);
-          for (int a = 0; a < 2; ++a) {  // per r-atom three stages: (A hi, B hi), (A hi, B lo), (A lo, B hi); lo at +kRecBytes
+          for (int a = 0; a < 2; ++a) {  // one stage = the A and the B image of one r-atom (X3: three stages, lo at +kRecBytes)
             const uint8_t* A = rec + J.a_off + a * J.a_rows * 128 + J.a_half * 16384;
             const uint8_t* B = rec + J.b_off + a * J.b_rows * 128;
             ring.produce(A, 16384, 16384, B, b_bytes);
-            ring.produce(A, 16384, 16384, B + kRecBytes, b_bytes);
-            ring.produce(A + kRecBytes, 16384, 16384, B, b_bytes);
+            if constexpr (X3) {
+              ring.produce(A, 16384, 16384, B + kRecBytes, b_bytes);
+              ring.produce(A + kRecBytes, 16384, 16384, B, b_bytes);
+            }
           }
         }
       }
@@ -774,19 +658,25 @@ __global__ void __launch_bounds__(kThreads, 1) dw_x3_kernel(const __grid_constan
     for (int job = job0; job < job1; ++job) {
       const Job J = c_jobs.j[job];
       if constexpr (kPeOnly) {  // both PE jobs multiply by the 64-row PE image: only that shape is compiled in
-        run_job_x3<kPeOnly, 64>(p, J, j0, j1, smem_base, ring, wg, lane);
+        run_job<kPeOnly, X3, 64>(p, J, j0, j1, smem_base, ring, wg, lane);
         continue;
       }
       switch (J.b_rows) {
-        case 16: run_job_x3<kPeOnly, 16>(p, J, j0, j1, smem_base, ring, wg, lane); break;
-        case 32: run_job_x3<kPeOnly, 32>(p, J, j0, j1, smem_base, ring, wg, lane); break;
-        case 64: run_job_x3<kPeOnly, 64>(p, J, j0, j1, smem_base, ring, wg, lane); break;
-        case 128: run_job_x3<kPeOnly, 128>(p, J, j0, j1, smem_base, ring, wg, lane); break;
-        default: run_job_x3<kPeOnly, 256>(p, J, j0, j1, smem_base, ring, wg, lane); break;
+        case 16: run_job<kPeOnly, X3, 16>(p, J, j0, j1, smem_base, ring, wg, lane); break;
+        case 32: run_job<kPeOnly, X3, 32>(p, J, j0, j1, smem_base, ring, wg, lane); break;
+        case 64: run_job<kPeOnly, X3, 64>(p, J, j0, j1, smem_base, ring, wg, lane); break;
+        case 128: run_job<kPeOnly, X3, 128>(p, J, j0, j1, smem_base, ring, wg, lane); break;
+        default: run_job<kPeOnly, X3, 256>(p, J, j0, j1, smem_base, ring, wg, lane); break;
       }
     }
   }
 }
+
+template <bool kPeOnly>
+__global__ void __launch_bounds__(kThreads, 1) dw_kernel(const __grid_constant__ DwParams p) { dw_body<kPeOnly, false>(p); }
+// exact-grad mode: hi + lo records (a kernel of its own, so dw_kernel keeps its name)
+template <bool kPeOnly>
+__global__ void __launch_bounds__(kThreads, 1) dw_x3_kernel(const __grid_constant__ DwParams p) { dw_body<kPeOnly, true>(p); }
 
 }  // namespace dw
 

@@ -6,11 +6,14 @@ refactor of the kernels or of the host layer must leave every digest and the lau
   train    2048 rays at 64c+64f, stratified sampling, sigma noise 0.1, background, dir_z: the seven outputs of the training
            forward, all 48 parameter gradients, the latent gradient and the five input gradients
   chunked  the same for 200 rays with NFB_TRAIN_MEM_MB=48 (32 rays per chunk, the last chunk ragged)
-
-each in both precision modes, plus the launches each case took; then, through the host paths above the renderer:
-
+  input_only  the train case on other noise with an input-only backward (want_params=False): the seven outputs, the latent
+           gradient and the five input gradients, which the PE-only weight-gradient launch serves
   frames   2048 rays of three frames, one multi-frame training forward and backward(frames=True): the seven outputs, the
-           parameter gradients, every frame's latent and expression gradient and the other input gradients (both precisions)
+           parameter gradients, every frame's latent and expression gradient and the other input gradients
+
+each in all three precisions (fast, exact, exact_grad), plus the launches each case took; then, through the host paths above
+the renderer:
+
   dropin/* run_one_iter_of_nerf and render_frames in training mode, then loss.backward(): the outputs and the gradients of
            the parameters, latents, expressions and background
   trainer/*  three steps each of FusedTrainer.step, step_graph, step_images at K = 1 and K = 3, and step_images_graph (K = 3):
@@ -35,6 +38,7 @@ sys.path.insert(0, os.path.join(ROOT, "4d-facial-avatars_b200"))
 NEAR, FAR = 0.2, 0.8
 OUTPUTS = ("rgb_coarse", "disp_coarse", "acc_coarse", "rgb_fine", "disp_fine", "acc_fine", "w_last")
 INPUTS = ["ray_origins", "ray_directions", "expression", "background", "dir_z"]
+PRECISIONS = ("fast", "exact", "exact_grad")
 
 
 def digest(t):
@@ -73,7 +77,7 @@ def main():
         res[case] = {k: digest(t) for k, t in named}
         res[case]["launches"] = eng.launch_count() - l0
 
-    def train_case(case, n, prec, seed):
+    def train_case(case, n, prec, seed, want_params=True):
         g = torch.Generator().manual_seed(seed)
         nz = O.draw_noise(n, O.Sampling(64, 64, True, 0.1, False, 2048), g)
         noise = {k: getattr(nz, k).to(dev) for k in ("t_rand", "n_c", "u", "n_f")}
@@ -83,18 +87,19 @@ def main():
         l0 = eng.launch_count()
         out = eng.render(ro[:n].contiguous(), rd[:n].contiguous(), NEAR, FAR, 64, 64, perturb=True, noise_std=0.1,
                          background=bg[:n].contiguous(), dir_z=dz, noise=noise, precision=prec, train=True)
-        gc, gf, gl, ing = eng.backward(gouts, pc, pf, want_latent=True, want_params=True, inputs=INPUTS)
+        gc, gf, gl, ing = eng.backward(gouts, pc, pf, want_latent=True, want_params=want_params, inputs=INPUTS)
         named = [(k, out[k]) for k in OUTPUTS]
-        named += [(f"grad_coarse/{PARAM_ORDER[i]}", t) for i, t in enumerate(gc) if t is not None]
-        named += [(f"grad_fine/{PARAM_ORDER[i]}", t) for i, t in enumerate(gf) if t is not None]
+        named += [(f"grad_coarse/{PARAM_ORDER[i]}", t) for i, t in enumerate(gc or []) if t is not None]
+        named += [(f"grad_fine/{PARAM_ORDER[i]}", t) for i, t in enumerate(gf or []) if t is not None]
         named += [("grad_latent", gl)] + [("grad_" + k, t) for k, t in sorted(ing.items())]
         record(case, named, l0)
 
-    for prec in ("fast", "exact"):
+    for prec in PRECISIONS:
         l0 = eng.launch_count()
         out = eng.render(ro, rd, NEAR, FAR, 64, 128, background=bg, precision=prec)
         record(f"eval/{prec}", [(k, out[k]) for k in OUTPUTS], l0)
         train_case(f"train/{prec}", 2048, prec, 1031)
+        train_case(f"input_only/{prec}", 2048, prec, 1036, want_params=False)
         os.environ["NFB_TRAIN_MEM_MB"] = "48"  # read by the library on every call
         try:
             train_case(f"chunked/{prec}", 200, prec, 1032)
@@ -109,7 +114,7 @@ def main():
     fnoise = {k: getattr(nz, k).to(dev) for k in ("t_rand", "n_c", "u", "n_f")}
     fdz = (torch.rand(n, generator=g) * 2.0 - 1.0).to(dev)
     fgouts = [((torch.rand(sh, generator=g) - 0.3) / n).to(dev) for sh in [(n, 3), (n,), (n,), (n, 3), (n,), (n,), (n,)]]
-    for prec in ("fast", "exact"):
+    for prec in PRECISIONS:
         l0 = eng.launch_count()
         eng.set_frames(fexpr, flat)
         out = eng.render(ro[:n].contiguous(), rd[:n].contiguous(), NEAR, FAR, 64, 64, perturb=True, noise_std=0.1,
