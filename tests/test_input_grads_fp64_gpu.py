@@ -218,9 +218,11 @@ def row_formula64(c, s, m, inv, dy0, dy3, dy6, ray, z, fused=False):
     return torch.cat((dp, dv[:, None]), 1), torch.cat((ap, av[:, None]), 1)
 
 
-def check_rows(E, c, s, t, tag, chunk=1 << 16):
-    recs = dev_tensor(t.dbg.records, (s.n_tiles, t.dbg.record_bytes // 2), "<i2")
-    dy = [decode_image(recs, dy_off(L), 256 if L < 6 else 128) for L in (0, 3, 6)]
+def check_rows(E, c, s, t, tag, chunk=1 << 16, dy=None):
+    """dy: the decoded dY0, dY3, dY6 images the row kernel read (by default the FP16 records; exact-grad passes hi + lo)."""
+    if dy is None:
+        recs = dev_tensor(t.dbg.records, (s.n_tiles, t.dbg.record_bytes // 2), "<i2")
+        dy = [decode_image(recs, dy_off(L), 256 if L < 6 else 128) for L in (0, 3, 6)]
     used = torch.zeros(s.n_tiles, 128, dtype=torch.bool, device=E.dev)
     parts = row_parts(E, c, s)
     tpu = s.tc + s.tf

@@ -174,9 +174,10 @@ def dy_rows(E, c, s, t):
     return out
 
 
-def check_raysums(E, c, s, t, tag, valid, db64=None):
+def check_raysums(E, c, s, t, tag, valid, db64=None, dy=None):
+    """dy: per pass the dY0 | dY3 rows raysum read, [n, S, 512] (by default the FP16 records; exact-grad passes hi + lo)."""
     worst, l2 = 0.0, 0.0
-    for pas, x in enumerate(dy_rows(E, c, s, t)):
+    for pas, x in enumerate(dy_rows(E, c, s, t) if dy is None else dy):
         got = t.raysum[pas]
         acc = torch.zeros(c.n, ROWS, device=x.device)
         for i in range(x.shape[1]):  # raysum_kernel's order: samples ascending, FP32, then the inverse scale (a power of two)
