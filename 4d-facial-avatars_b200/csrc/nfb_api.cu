@@ -891,6 +891,28 @@ int nfb_fit_rows_grad(NfbHandle* h, const NfbTrainImages* d, const int32_t* imag
   return NFB_OK;
 }
 
+int nfb_background_rows_grad(NfbHandle* h, const int32_t* pixel_rc, int n_rays, int height, int width, const float* grad_bg_render,
+                             const float* grad_bg_loss, float* table_grads, void* stream) {
+  if (!h || !pixel_rc || !grad_bg_render || !table_grads || n_rays < 0 || height < 1 || width < 1) return NFB_ERR_INVALID;
+  if ((long long)height * width > 0x7FFFFFFFLL) return NFB_ERR_INVALID;  // the kernel keys pixels by an int index
+  if (n_rays == 0) return NFB_OK;  // nothing to add: no launch
+  NFB_CUDA(cudaSetDevice(h->device));
+  NFB_CUDA(nfb::launch_background_rows(pixel_rc, n_rays, height, width, grad_bg_render, grad_bg_loss, table_grads,
+                                       static_cast<cudaStream_t>(stream), &h->launches));
+  return NFB_OK;
+}
+
+int nfb_loss_background_grad(NfbHandle* h, const float* bg_rays, const float* target, const float* w_last, int n_rays, long long n_total,
+                             float weight, float* grad_bg_rays, float* grad_w_last, float* loss, void* stream) {
+  if (!h || !bg_rays || !target || !w_last || !grad_bg_rays || !grad_w_last || !loss || n_rays < 0 || n_total < n_rays || n_total <= 0)
+    return NFB_ERR_INVALID;
+  if (n_rays == 0) return NFB_OK;  // an empty shard adds nothing: no launch
+  NFB_CUDA(cudaSetDevice(h->device));
+  NFB_CUDA(nfb::launch_loss_background(bg_rays, target, w_last, n_rays, n_total, weight, grad_bg_rays, grad_w_last, loss,
+                                       static_cast<cudaStream_t>(stream), &h->launches));
+  return NFB_OK;
+}
+
 int nfb_host_map_cdf(const NfbRayMap* map, const long long* zeroed_sorted, int n_zero, const long long* ks, int n, double* out) {
   if (!map || !ks || !out || n < 0 || n_zero < 0 || (n_zero && !zeroed_sorted)) return NFB_ERR_INVALID;
   nfb::smp::Map m;

@@ -272,6 +272,12 @@ cudaError_t launch_latent_rows(const float* grad_latents, const int* image_index
 cudaError_t launch_fit_rows(const int* image_index, int K, int n, int n_rows, const int* pixel_rc, const float* g_o, const float* g_d,
                             float fx, float fy, float wcx, float hcy, float* slots, float* pose_grads, const float* g_expr,
                             float* expr_grads, cudaStream_t st, long long* launches);
+// One launch each (nfb_optim.cu; none for n_rays == 0): a learned background's rows of the bucket gradient, and the supervised
+// background loss with its two gradients (orders: include/nfb.h, nfb_background_rows_grad / nfb_loss_background_grad).
+cudaError_t launch_background_rows(const int* pixel_rc, int n_rays, int H, int W, const float* g_render, const float* g_loss,
+                                   float* table_grads, cudaStream_t st, long long* launches);
+cudaError_t launch_loss_background(const float* bg, const float* target, const float* w_last, int n_rays, long long n_total, float weight,
+                                   float* g_bg, float* g_w, float* loss, cudaStream_t st, long long* launches);
 cudaError_t launch_fill_int(int* p, long long n, int v, cudaStream_t st, long long* launches);
 
 }  // namespace nfb

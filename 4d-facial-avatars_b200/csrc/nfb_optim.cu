@@ -258,6 +258,98 @@ cudaError_t launch_fit_rows(const int* image_index, int K, int n, int n_rows, co
   return cudaGetLastError();
 }
 
+// The learned background's rows of the bucket gradient (nfb_background_rows_grad; order: include/nfb.h).  The pixels are split
+// between warps instead of the rays: warp w of the grid owns the table rows whose index is w modulo the number of warps, and walks
+// ALL rays in ascending order, 32 at a time.  In each group of 32, __match_any_sync gathers the lanes whose ray falls on the same
+// owned pixel, and the lowest of them adds the group's rays in ascending lane order; __syncwarp orders one group's row writes
+// before the next group's reads.  So every pixel receives its rays in ascending order from one warp, whatever the batch holds
+// (repeats inside a slot, pixels shared across slots, a rank's slice cutting either), with no atomics and no sort; how many warps
+// run changes which warp owns a pixel, never the order of its adds.  Every warp reads every ray's pixel (8 B a ray, from L1/L2).
+constexpr int kBgWarps = 8, kBgBlocks = 128;
+__global__ void __launch_bounds__(kBgWarps * 32) background_rows_kernel(const int* __restrict__ pixel_rc, int n_rays, int H, int W,
+                                                                         const float* __restrict__ g_render, const float* __restrict__ g_loss,
+                                                                         float* __restrict__ table) {
+  const int lane = threadIdx.x & 31;
+  const int part = blockIdx.x * kBgWarps + (threadIdx.x >> 5), parts = gridDim.x * kBgWarps;
+  for (int base = 0; base < n_rays; base += 32) {
+    const int r = base + lane;
+    int key = -1;
+    if (r < n_rays) {
+      const int row = pixel_rc[2 * (size_t)r], col = pixel_rc[2 * (size_t)r + 1];
+      if (row >= 0 && row < H && col >= 0 && col < W) key = (int)smp::pixel_index(row, col, W);
+    }
+    const bool mine = key >= 0 && key % parts == part;
+    const unsigned group = __match_any_sync(0xffffffffu, mine ? key : -2 - lane);  // lanes not owning their pixel match no one
+    if (mine && lane == __ffs(group) - 1) {
+      float* g = table + 3 * (size_t)key;
+      float a0 = g[0], a1 = g[1], a2 = g[2];
+      for (unsigned m = group; m; m &= m - 1) {
+        const size_t i = 3 * (size_t)(base + __ffs(m) - 1);
+        if (g_loss) {
+          a0 = __fadd_rn(a0, __fadd_rn(g_render[i], g_loss[i]));
+          a1 = __fadd_rn(a1, __fadd_rn(g_render[i + 1], g_loss[i + 1]));
+          a2 = __fadd_rn(a2, __fadd_rn(g_render[i + 2], g_loss[i + 2]));
+        } else {
+          a0 = __fadd_rn(a0, g_render[i]);
+          a1 = __fadd_rn(a1, g_render[i + 1]);
+          a2 = __fadd_rn(a2, g_render[i + 2]);
+        }
+      }
+      g[0] = a0; g[1] = a1; g[2] = a2;
+    }
+    __syncwarp();  // this group's rows are written (and visible to the warp) before the next group reads them
+  }
+}
+
+cudaError_t launch_background_rows(const int* pixel_rc, int n_rays, int H, int W, const float* g_render, const float* g_loss,
+                                   float* table_grads, cudaStream_t st, long long* launches) {
+  if (n_rays <= 0) return cudaSuccess;
+  background_rows_kernel<<<kBgBlocks, kBgWarps * 32, 0, st>>>(pixel_rc, n_rays, H, W, g_render, g_loss, table_grads);
+  ++*launches;
+  return cudaGetLastError();
+}
+
+// The supervised background term (nfb_loss_background_grad; order: include/nfb.h), 0.001 * mean(w_last * ||bg - target||^2) in
+// the reference: per ray d = bg - t, e = (d0 d0 + d1 d1) + d2 d2, then g_bg = (2 d) (s w), g_w = s e and the loss term w e, with
+// s = weight * (1 / n_total).  ONE block, the loss terms meeting in loss_grad_kernel's fixed order.
+__global__ void __launch_bounds__(kLossThreads) loss_background_kernel(const float* __restrict__ bg, const float* __restrict__ target,
+                                                                       const float* __restrict__ w_last, int n_rays, float s,
+                                                                       float* __restrict__ g_bg, float* __restrict__ g_w,
+                                                                       float* __restrict__ loss) {
+  __shared__ float part[kLossThreads / 32];
+  float acc = 0.f;
+  for (int r = threadIdx.x; r < n_rays; r += kLossThreads) {
+    const size_t i = 3 * (size_t)r;
+    const float d0 = __fsub_rn(bg[i], target[i]), d1 = __fsub_rn(bg[i + 1], target[i + 1]), d2 = __fsub_rn(bg[i + 2], target[i + 2]);
+    const float e = __fadd_rn(__fadd_rn(__fmul_rn(d0, d0), __fmul_rn(d1, d1)), __fmul_rn(d2, d2));
+    const float w = w_last[r], sw = __fmul_rn(s, w);
+    g_bg[i] = __fmul_rn(2.f * d0, sw);
+    g_bg[i + 1] = __fmul_rn(2.f * d1, sw);
+    g_bg[i + 2] = __fmul_rn(2.f * d2, sw);
+    g_w[r] = __fmul_rn(s, e);
+    acc = __fadd_rn(acc, __fmul_rn(w, e));
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc = __fadd_rn(acc, __shfl_xor_sync(0xffffffffu, acc, o));
+  const int wp = threadIdx.x >> 5, l = threadIdx.x & 31;
+  if (l == 0) part[wp] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    float sum = 0.f;
+    for (int k = 0; k < kLossThreads / 32; ++k) sum = __fadd_rn(sum, part[k]);
+    loss[0] = __fadd_rn(loss[0], __fmul_rn(sum, s));
+  }
+}
+
+cudaError_t launch_loss_background(const float* bg, const float* target, const float* w_last, int n_rays, long long n_total, float weight,
+                                   float* g_bg, float* g_w, float* loss, cudaStream_t st, long long* launches) {
+  if (n_rays <= 0) return cudaSuccess;
+  const float s = weight * (1.f / (float)n_total);  // two FP32 roundings, as autograd's mean backward forms it on CUDA
+  loss_background_kernel<<<1, kLossThreads, 0, st>>>(bg, target, w_last, n_rays, s, g_bg, g_w, loss);
+  ++*launches;
+  return cudaGetLastError();
+}
+
 cudaError_t launch_loss_grad(const float* rgb_c, const float* rgb_f, const float* target, int n_rays, long long n_total, float* g_c,
                              float* g_f, float* loss, cudaStream_t st, long long* launches) {
   const int n = 3 * n_rays;

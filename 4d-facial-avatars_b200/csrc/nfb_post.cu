@@ -307,7 +307,7 @@ __device__ __forceinline__ void gather_pixels(const GatherArgs& a, const long lo
         a.ray_d[3 * i + q] = __fadd_rn(__fadd_rn(__fmul_rn(cx, a.pose[4 * q]), __fmul_rn(cy, a.pose[4 * q + 1])), __fmul_rn(-1.f, a.pose[4 * q + 2]));
       if (a.ray_o) for (int q = 0; q < 3; ++q) a.ray_o[3 * i + q] = a.pose[4 * q + 3];
     }
-    const size_t px = ((size_t)row * W + col) * 3;
+    const size_t px = smp::pixel_index(row, col, W) * 3;
     if (a.target) for (int q = 0; q < 3; ++q) a.target[3 * i + q] = a.image[px + q];
     if (a.bg_out) for (int q = 0; q < 3; ++q) a.bg_out[3 * i + q] = a.background[px + q];
   }

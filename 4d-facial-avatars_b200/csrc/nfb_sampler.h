@@ -21,6 +21,7 @@
 // B <= 1075 and kMaxRuns runs fit kMaxSegs: 2 * 4096 + 3 * 1075 + 1 = 11,418 <= 16,384.
 #pragma once
 #include <math.h>
+#include <stddef.h>
 #include <stdint.h>
 
 #if defined(__CUDACC__)
@@ -159,6 +160,11 @@ __device__ __forceinline__ void camera_dir(int row, int col, float fx, float fy,
   cy = -__fdiv_rn(__fsub_rn((float)row, hcy), fy);
 }
 #endif
+
+// Row of pixel (row, col) in an [H][W] table (image, background), row-major.  The samplers' gathers read the target and
+// background colours there and nfb_background_rows_grad adds the background's gradient there: one helper, so the scatter
+// writes exactly the pixel the gather read (the flat draw index k maps to (row, col) = (k % H, k / H) before this, in the gather).
+NFB_SHD size_t pixel_index(int row, int col, int W) { return (size_t)row * W + col; }
 
 }  // namespace smp
 }  // namespace nfb

@@ -15,7 +15,8 @@ EXPORTS = ["nfb_version", "nfb_strerror", "nfb_last_cuda_error", "nfb_create", "
            "nfb_render_forward_train", "nfb_render_backward", "nfb_render_backward_ex", "nfb_train_debug", "nfb_debug_schedule", "nfb_loss_mse_grad",
            "nfb_adam_step", "nfb_adam_step_dev", "nfb_repack", "nfb_frame_products", "nfb_sample_rays", "nfb_host_map_cdf",
            "nfb_set_frames", "nfb_render_forward_frames", "nfb_render_forward_frames_train", "nfb_render_backward_frames",
-           "nfb_sample_rays_images", "nfb_latent_rows_grad", "nfb_debug_weights", "nfb_buffer_epoch", "nfb_fit_rows_grad"]
+           "nfb_sample_rays_images", "nfb_latent_rows_grad", "nfb_debug_weights", "nfb_buffer_epoch", "nfb_fit_rows_grad",
+           "nfb_background_rows_grad", "nfb_loss_background_grad"]
 NFB_MAX_FRAMES = 1024
 NFB_MAX_STEP_IMAGES = 64
 
@@ -164,6 +165,10 @@ def _load():
                                          C.c_void_p]
     lib.nfb_fit_rows_grad.argtypes = [C.c_void_p, C.POINTER(NfbTrainImages), C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.nfb_background_rows_grad.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_void_p]
+    lib.nfb_loss_background_grad.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_longlong, C.c_float,
+                                             C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.nfb_launch_count.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
     lib.nfb_buffer_epoch.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
     lib.nfb_host_linspace.argtypes = [C.POINTER(C.c_float), C.c_int]
@@ -172,7 +177,7 @@ def _load():
                "nfb_render_backward", "nfb_render_backward_ex", "nfb_train_debug", "nfb_loss_mse_grad", "nfb_adam_step", "nfb_adam_step_dev", "nfb_repack", "nfb_frame_products",
                "nfb_sample_rays", "nfb_host_map_cdf", "nfb_set_frames", "nfb_render_forward_frames",
                "nfb_render_forward_frames_train", "nfb_render_backward_frames", "nfb_sample_rays_images", "nfb_latent_rows_grad",
-               "nfb_debug_weights", "nfb_buffer_epoch", "nfb_fit_rows_grad"):
+               "nfb_debug_weights", "nfb_buffer_epoch", "nfb_fit_rows_grad", "nfb_background_rows_grad", "nfb_loss_background_grad"):
         getattr(lib, fn).restype = C.c_int
     return lib
 

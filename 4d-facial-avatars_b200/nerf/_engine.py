@@ -282,21 +282,25 @@ class Renderer:
         capi.check(capi.lib.nfb_repack(self._h, _ptrs(params_c), _ptrs(params_f), _stream()), "repack")
 
     def backward_into(self, out_grads, params_c, params_f, grads_c, grads_f, grad_latent, frames=False, grad_expressions=None,
-                      grad_ray_origins=None, grad_ray_directions=None):
+                      grad_ray_origins=None, grad_ray_directions=None, grad_background=None):
         """nfb_render_backward writing straight into caller-owned gradient tensors (views of a flat bucket): params_* / grads_*
         are lists of 26 contiguous FP32 CUDA tensors in PARAM_ORDER (grads of layers_dir.3.* may be None; grads_c and grads_f
         both None: input-only mode).  frames=True: nfb_render_backward_frames after a multi-frame training forward, per-frame
         d latent into grad_latent [F,32], and into caller-owned buffers too d expression [F,76] (grad_expressions) and the per-ray
-        ray gradients [N,3] (grad_ray_origins, grad_ray_directions), each when given."""
+        ray gradients [N,3] (grad_ray_origins, grad_ray_directions), each when given.  grad_background: the per-ray background
+        gradient [N,3] (NfbInputGrads.background; the single-frame call is then nfb_render_backward_ex)."""
         keep = []
         args = (self._h, C.byref(_out_grads(out_grads, self.device, keep)), _ptrs(params_c), _ptrs(params_f), _ptrs(grads_c),
                 _ptrs(grads_f), _ptr(grad_latent))
+        ig = None
+        if grad_ray_origins is not None or grad_ray_directions is not None or grad_background is not None:
+            ig = capi.NfbInputGrads(ray_origins=_ptr(grad_ray_origins), ray_directions=_ptr(grad_ray_directions),
+                                    background=_ptr(grad_background))
         if frames:
-            ig = None
-            if grad_ray_origins is not None or grad_ray_directions is not None:
-                ig = capi.NfbInputGrads(ray_origins=_ptr(grad_ray_origins), ray_directions=_ptr(grad_ray_directions))
             capi.check(capi.lib.nfb_render_backward_frames(*args, _ptr(grad_expressions) if grad_expressions is not None else None,
                                                            C.byref(ig) if ig is not None else None, _stream()), "render_backward_frames")
+        elif ig is not None:
+            capi.check(capi.lib.nfb_render_backward_ex(*args, C.byref(ig), _stream()), "render_backward")
         else:
             capi.check(capi.lib.nfb_render_backward(*args, _stream()), "render_backward")
         self._bwd_keep = keep
@@ -328,6 +332,20 @@ class Renderer:
         capi.check(capi.lib.nfb_fit_rows_grad(self._h, C.byref(data.desc), _ptr(image_index), image_index.numel(), int(n), _ptr(pixel_rc),
                                               _ptr(grad_ray_origins), _ptr(grad_ray_directions), _ptr(pose_grads), _ptr(grad_expressions),
                                               _ptr(expression_grads), _stream()), "fit_rows_grad")
+
+    def background_rows_grad(self, pixel_rc, height, width, grad_bg_render, grad_bg_loss, table_grads):
+        """nfb_background_rows_grad: table_grads ([H,W,3] or its flat view) += each ray's background gradient (grad_bg_render
+        [+ grad_bg_loss], [n,3]) at its pixel_rc ([n,2] int32), in ascending ray order (CUDA tensors; grad_bg_loss may be None)."""
+        capi.check(capi.lib.nfb_background_rows_grad(self._h, _ptr(pixel_rc), pixel_rc.shape[0], int(height), int(width),
+                                                     _ptr(grad_bg_render), _ptr(grad_bg_loss), _ptr(table_grads), _stream()),
+                   "background_rows_grad")
+
+    def loss_background_grad(self, bg_rays, target, w_last, n_total, weight, grad_bg_rays, grad_w_last, loss):
+        """nfb_loss_background_grad: weight * mean(w_last * ||bg - target||^2) over n_total rays; writes grad_bg_rays [n,3] and
+        grad_w_last [n], loss[0] += this shard's share (CUDA tensors)."""
+        capi.check(capi.lib.nfb_loss_background_grad(self._h, _ptr(bg_rays), _ptr(target), _ptr(w_last), bg_rays.shape[0],
+                                                     int(n_total), float(weight), _ptr(grad_bg_rays), _ptr(grad_w_last), _ptr(loss),
+                                                     _stream()), "loss_background_grad")
 
     def backward(self, out_grads, params_c, params_f, want_latent=True, want_params=True, inputs=None, frames=False):
         """nfb_render_backward_ex for the last training forward.  out_grads: 7 CUDA tensors or None (rgb_c, disp_c, acc_c,

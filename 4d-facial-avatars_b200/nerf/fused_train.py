@@ -68,9 +68,28 @@ def _image_buffers(cache, dev, data, k, n, shortfall, **extra):
 
 
 class FusedTrainer:
+    background = None      # the learned background's [H,W,3] rows (None: the training set's background, if any, is fixed)
+    background_loss = 0.0  # the supervised background term's weight
+
     def __init__(self, model_coarse, model_fine, n_latent, lr=5e-4, lr_decay_steps=250000, lr_decay_factor=0.1,
                  betas=(0.9, 0.999), eps=1e-8, num_coarse=64, num_fine=64, perturb=True, noise_std=0.1, near=0.2, far=0.8,
-                 latent_reg=0.005, white_bkgd=False, latent_codes=None, precision=None):
+                 latent_reg=0.005, white_bkgd=False, latent_codes=None, precision=None, background=None, background_loss=0.0):
+        """background: the initial [H,W,3] image of a background this trainer LEARNS (train_transformed_rays.py:128-157,
+        train_background): it joins the bucket as its own rows, steps over several images gather it at their pixels and Adam
+        updates it with everything else (the reference's second parameter group has the same learning rate and decay).  None: the
+        background, if any, is the training set's fixed one.  background_loss: the weight of the supervised term
+        weight * mean(w_last * ||bg - target||^2) (supervised_train_background; 0.001 in the reference, 0: off).  Initialise it
+        as the reference does from the training images [N,H,W,3]:  bg = images.mean(0)  (optionally blurred first:
+        nerf.GaussianSmoothing(3, 11, 11)(bg.permute(2, 0, 1)[None])[0].permute(1, 2, 0))."""
+        self.background_loss = float(background_loss)  # checked before the renderer is touched
+        if background is not None:
+            background = torch.as_tensor(background)
+            if background.dim() != 3 or background.shape[2] != 3:
+                raise ValueError("background must be an [H,W,3] image")
+        elif self.background_loss != 0.0:
+            raise ValueError("background_loss supervises a learned background: pass background=")
+        if self.background_loss < 0.0:
+            raise ValueError("background_loss must be >= 0")
         dev = next(model_coarse.parameters()).device
         self.eng = _engine.renderer_for(dev)
         self.dev, self.mc, self.mf = dev, model_coarse, model_fine
@@ -81,12 +100,17 @@ class FusedTrainer:
         self.latent_reg = float(latent_reg)
         self._iter = 0
 
-        # ---- flat bucket: [coarse 26 tensors | fine 26 tensors | pad to 256 | latent table n_latent x 32]
+        # ---- flat bucket: [coarse 26 tensors | fine 26 tensors | pad to 256 | latent table n_latent x 32
+        #                    (| pad to 256 | learned background H x W x 3)]
         models = [model_coarse] + ([model_fine] if model_fine is not None else [])
         tensors = [dict(m.named_parameters())[k] for m in models for k in PARAM_ORDER]
         n_mlp = sum(t.numel() for t in tensors)
         self.lat_off = (n_mlp + 255) // 256 * 256
-        n_total = self.lat_off + n_latent * 32
+        self._lat_end = n_total = self.lat_off + n_latent * 32
+        self.bg_off = None
+        if background is not None:
+            self.bg_off = (n_total + 255) // 256 * 256
+            n_total = self.bg_off + background.numel()
         self.params = torch.zeros(n_total, device=dev, dtype=torch.float32)
         self.grads = torch.zeros_like(self.params)
         self.exp_avg = torch.zeros_like(self.params)
@@ -101,9 +125,15 @@ class FusedTrainer:
             self._views.append(view)
             self._gviews.append(self.grads[off:off + n].view(t.shape))
             off += n
-        self.latent_codes = self.params[self.lat_off:].view(n_latent, 32)
+        self.latent_codes = self.params[self.lat_off:self._lat_end].view(n_latent, 32)
         if latent_codes is not None:
             self.latent_codes.copy_(latent_codes.detach().to(dev))
+        # the learned background: an [H,W,3] view of its rows (what a reference-format checkpoint stores under "background")
+        self.background = self._bg_grads = None
+        if background is not None:
+            self.background = self.params[self.bg_off:].view(background.shape)
+            self.background.copy_(background.detach().to(device=dev, dtype=torch.float32))
+            self._bg_grads = self.grads[self.bg_off:].view(background.shape)
         npar = len(PARAM_ORDER)
         skip = [k.startswith("layers_dir.3") for k in PARAM_ORDER]  # unused by the forward (models.py:257): no gradient
         self._pc, self._pf = self._views[:npar], (self._views[npar:] if model_fine is not None else None)
@@ -147,10 +177,22 @@ class FusedTrainer:
     def _draw_noise(self, n):
         return _draw_noise(self.opts, self.dev, n)
 
-    def _forward_backward(self, expressions, latents, frame_index, ro, rd, background, target, n_total, noise, g, grad_latent):
+    def _latent_grads(self):
+        """The latent table's rows of the gradient bucket, [n_latent,32]."""
+        return self.grads[self.lat_off:self._lat_end].view(-1, 32)
+
+    def _single_image(self, name):
+        if self.background is not None:
+            raise ValueError(f"{name}() takes background rays gathered by the caller and no pixel indices, so it cannot learn a "
+                             "background: a trainer built with background= steps with step_images / capture_images")
+
+    def _forward_backward(self, expressions, latents, frame_index, ro, rd, background, target, n_total, noise, g, grad_latent,
+                          grad_background=None):
         """Frame fold, training forward, loss gradient and backward of one batch into the flat gradient bucket, d latent into
         grad_latent.  frame_index None: one frame (expressions [76], latents [32]); otherwise ray i is conditioned on frame
-        frame_index[i] of expressions [F,76] and latents [F,32], and grad_latent is [F,32].  g: the [n,3] loss-gradient buffers."""
+        frame_index[i] of expressions [F,76] and latents [F,32], and grad_latent is [F,32].  g: the [n,3] loss-gradient buffers
+        (g0, g1), and with the supervised background term also its [n,3] background and [n] w_last gradient buffers.
+        grad_background: [n,3] receives the per-ray background gradient of the render (a learned background)."""
         eng, o = self.eng, self.opts
         frames = frame_index is not None
         if frames:
@@ -163,7 +205,12 @@ class FusedTrainer:
         g1 = g[1] if o["num_fine"] > 0 else None
         self.loss.zero_()
         eng.loss_mse_grad(out["rgb_coarse"], out.get("rgb_fine"), target, n_total, g[0], g1, self.loss)
-        eng.backward_into((g[0], None, None, g1, None, None, None), self._pc, self._pf, self._gc, self._gf, grad_latent, frames=frames)
+        g_wlast = None
+        if len(g) > 2:  # the supervised background term on the last pass's w_last; its share goes to loss[2]
+            eng.loss_background_grad(background, target, out["w_last"], n_total, self.background_loss, g[2], g[3], self.loss[2:3])
+            g_wlast = g[3]
+        eng.backward_into((g[0], None, None, g1, None, None, g_wlast), self._pc, self._pf, self._gc, self._gf, grad_latent,
+                          frames=frames, grad_background=grad_background)
         return out
 
     def _stepped(self):
@@ -199,7 +246,9 @@ class FusedTrainer:
         """Forward, loss and backward of this rank's rays ([n,3] CUDA tensors) into the flat gradient bucket; world > 1: the rays
         are one of `world` equal shards of a batch of n_total rays and the bucket is SUM-all-reduced (one collective), after
         which every rank holds the whole batch's gradient.  Returns the device tensor [mse_coarse, mse_fine] of THIS shard's
-        share (sum over ranks = batch loss).  `events`: optional (before_collective, after_collective) CUDA events."""
+        share (sum over ranks = batch loss).  `events`: optional (before_collective, after_collective) CUDA events.  A trainer
+        that learns its background raises ValueError (so do step, capture and step_graph)."""
+        self._single_image("gradients")
         self._own_engine()
         n = ray_origins.shape[0]
         n_total = n * world if n_total is None else n_total
@@ -235,6 +284,7 @@ class FusedTrainer:
         from step to step lives in device memory: the inputs (static buffers filled by step_graph), the latent row index, and the
         optimizer's step counter / learning rate (the trainer's one nfb_adam_step_dev state, which its eager steps share).  The
         noise is drawn inside the graph (torch's graph-safe Philox state), in the reference's order.  With world > 1 the NCCL all-reduce of the flat bucket is part of the graph."""
+        self._single_image("capture")
         dev = self.dev
         n_total = n * world if n_total is None else n_total
         z = lambda *shape, dt=torch.float32: torch.zeros(shape, device=dev, dtype=dt)  # noqa: E731
@@ -242,7 +292,7 @@ class FusedTrainer:
                   lat=z(32), glat=z(32), g0=z(n, 3), g1=z(n, 3))
         sb["rd"][:, 2] = -1.0  # a valid ray for the warm-up
         sb["adam"] = self._adam     # the optimizer state the graph advances: the trainer's one state, not a copy
-        table_grads = self.grads[self.lat_off:].view(-1, 32)
+        table_grads = self._latent_grads()
 
         def forward_backward():
             sb["lat"].copy_(self.latent_codes.index_select(0, sb["idx"])[0])
@@ -259,6 +309,7 @@ class FusedTrainer:
         on the current stream, so the caller may keep them on the device or in pinned host memory — and replays.  Raises
         RuntimeError, before it copies or launches anything, when a call on this device has re-allocated the renderer buffers the
         graph points at since capture (nfb_buffer_epoch): capture again."""
+        self._single_image("step_graph")
         g = self._graph
         self._check_epoch(g)
         sb = g["sb"]
@@ -278,6 +329,7 @@ class FusedTrainer:
 
     def step(self, *args, **kwargs):
         """One optimizer step: gradients(...) then update().  Returns gradients()'s loss tensor."""
+        self._single_image("step")
         loss = self.gradients(*args, **kwargs)
         self.update()
         return loss
@@ -286,8 +338,19 @@ class FusedTrainer:
     # Adam and re-pack from K image indices alone.  world > 1: every rank samples the whole batch of N = K * n rays on the same
     # draws and renders its slice [rank * N / world, (rank + 1) * N / world); one SUM all-reduce of the bucket joins the slices.
     def _images_buffers(self, data, k, n):
-        """Per-step buffers of a K-image step (cached per shape: the chunked backward re-reads rays and frame indices)."""
-        return _image_buffers(self._image_bufs, self.dev, data, k, n, self.shortfall, glat=(k, 32), zero_lat=(k, 32))
+        """Per-step buffers of a K-image step (cached per shape: the chunked backward re-reads rays and frame indices); with a
+        learned background also the pixels, the per-ray background gradient and (supervised) the background term's gradients."""
+        extra = dict(glat=(k, 32), zero_lat=(k, 32))
+        if self.background is not None:
+            extra.update(pixel_rc=((k * n, 2), torch.int32), g_bg=(k * n, 3))
+            if self.background_loss > 0.0:
+                extra.update(g_bgl=(k * n, 3), g_wl=(k * n,))
+        return _image_buffers(self._image_bufs, self.dev, data, k, n, self.shortfall, **extra)
+
+    def _images_data(self, data):
+        """What the sampler reads: with a learned background, a copy of the caller's set whose background is the bucket's rows
+        (read in place, so every step and every replay gathers the current estimate); otherwise the caller's set."""
+        return data.with_background(self.background) if self.background is not None else data
 
     def _images_sample(self, data, sb, n, draws, max_rounds):
         self.eng.sample_images(data, sb["img"], n, draws, max_rounds, self.latent_codes, sb)
@@ -298,7 +361,8 @@ class FusedTrainer:
         backward over all K frames (a frame without rays in the slice gets exactly zero d latent).  The noise is drawn for the
         whole batch and sliced, and the loss is divided by the whole batch's N = K * n rays, so the slices' buckets sum to the
         single-process gradient.  The K >= 2 regulariser is added here only when world == 1 (else _images_regulariser, after
-        the collective, adds it once)."""
+        the collective, adds it once).  A learned background: the supervised term (background_loss > 0) after the MSE, the
+        per-ray background gradient from the backward, and the slice's background rows before the latent rows."""
         N = k * n
         per = N // world
         sl = slice(rank * per, (rank + 1) * per)
@@ -310,9 +374,14 @@ class FusedTrainer:
         else:
             expr, lat, fi, glat = sb["expressions"], sb["latents"], sb["frame_index"][sl], sb["glat"]
         bg = sb["background"][sl] if sb["background"] is not None else None
+        learn, supervised = self.background is not None, self.background_loss > 0.0
+        g = (sb["g0"][sl], sb["g1"][sl]) + ((sb["g_bgl"][sl], sb["g_wl"][sl]) if supervised else ())
         out = self._forward_backward(expr, lat, fi, sb["ray_origins"][sl], sb["ray_directions"][sl], bg, sb["target"][sl], N, noise,
-                                     (sb["g0"][sl], sb["g1"][sl]), glat)
-        self.eng.latent_rows_grad(sb["glat"], sb["img"], self.latent_codes, self.grads[self.lat_off:].view(-1, 32),
+                                     g, glat, grad_background=sb["g_bg"][sl] if learn else None)
+        if learn:
+            self.eng.background_rows_grad(sb["pixel_rc"][sl], self.background.shape[0], self.background.shape[1], sb["g_bg"][sl],
+                                          sb["g_bgl"][sl] if supervised else None, self._bg_grads)
+        self.eng.latent_rows_grad(sb["glat"], sb["img"], self.latent_codes, self._latent_grads(),
                                   self.latent_reg / k if k >= 2 and world == 1 else 0.0)
         return out
 
@@ -320,8 +389,7 @@ class FusedTrainer:
         """K >= 2 after the collective: the regulariser terms (latent_reg / K) * l / ||l|| added once, in ascending k, onto the
         summed latent rows (nfb_latent_rows_grad with zero frame gradients: adding +0.0 leaves a row as it is)."""
         if k >= 2:
-            self.eng.latent_rows_grad(sb["zero_lat"], sb["img"], self.latent_codes, self.grads[self.lat_off:].view(-1, 32),
-                                      self.latent_reg / k)
+            self.eng.latent_rows_grad(sb["zero_lat"], sb["img"], self.latent_codes, self._latent_grads(), self.latent_reg / k)
 
     def _check_images(self, data, k, n, world, group=None, rank=None):
         """Argument checks of a K-image step, all before any launch or collective; returns this rank's index.  world > 1 needs
@@ -346,6 +414,12 @@ class FusedTrainer:
             raise ValueError("the latent table has fewer rows than the training set has images")
         if (k * n) % world:
             raise ValueError(f"a batch of K * n_per_image = {k * n} rays does not split evenly over world = {world} ranks")
+        if self.background is not None:
+            if data.background is not None:
+                raise ValueError("this trainer learns the background: the training set must not carry one of its own")
+            if tuple(self.background.shape[:2]) != (data.H, data.W):
+                raise ValueError(f"the learned background is {tuple(self.background.shape[:2])} but the training set's frames are "
+                                 f"{(data.H, data.W)}")
         return 0 if world == 1 else rank
 
     def step_images(self, data, image_index, n_per_image, draws=None, max_rounds=32, world=1, group=None, rank=None):
@@ -365,13 +439,20 @@ class FusedTrainer:
         forward 1, loss 1, backward 7, latent rows 1, Adam 2, re-pack 2; K >= 2: 19 = sample 1, set_frames 1, forward 1, loss 1,
         backward 10, latent rows 1, Adam 2, re-pack 2 (Adam: schedule and update on the trainer's device state, as in every step,
         eager or captured).  world > 1 adds the all-reduce, and at K >= 2 one latent-rows launch after it (20).  Returns the
-        device tensor [mse_coarse, mse_fine] (world > 1: this rank's share; the shares sum to the batch loss)."""
+        device tensor [mse_coarse, mse_fine] (world > 1: this rank's share; the shares sum to the batch loss).
+        A learned background (background= at construction; DESIGN.md 8e): the sampler gathers the background rays from the
+        bucket's rows, the backward also forms the per-ray background gradient (+1 launch) and nfb_background_rows_grad adds this
+        rank's rays onto the rows before the latent rows (+1): 18 launches at K = 1 and 21 at K >= 2.  background_loss > 0 adds
+        the supervised term weight * mean(w_last * ||bg - target||^2) after the MSE (+1: 19 and 22), its w_last gradient
+        feeding the backward; its share of the loss is in self.loss[2].  The argument checks also raise ValueError when `data`
+        carries a background of its own or its frames are not the learned background's H x W."""
         k, n = len(image_index), int(n_per_image)
         rank = self._check_images(data, k, n, world, group, rank)
         if any(not 0 <= int(i) < data.n_images for i in image_index):
             raise ValueError("image index out of range")
         if draws is not None and draws.numel() < k * max_rounds * n:
             raise ValueError("draws must hold K * max_rounds * n_per_image values")
+        data = self._images_data(data)
         sb = self._images_buffers(data, k, n)
         sb["img"].copy_(torch.tensor([int(i) for i in image_index], dtype=torch.int32))
         if draws is None:
@@ -400,15 +481,17 @@ class FusedTrainer:
         Only the K image indices change between replays.  world, group and rank as in step_images; with device_draws=True every
         rank must seed torch alike, so that the ranks sample the same batch.  An incomplete selection does not stop the graph:
         the image's missing slots repeat its first pixels and self.shortfall[k] counts them (include/nfb.h,
-        nfb_sample_rays_images).  Launches per replay: 16 at K = 1, 19 at K >= 2 (world > 1: + the all-reduce, and 20 at K >= 2).
+        nfb_sample_rays_images).  Launches per replay: 16 at K = 1, 19 at K >= 2 (world > 1: + the all-reduce, and 20 at K >= 2);
+        a learned background adds step_images' 2, and its supervised term 1 more.  has_background is ignored then.
         The graph holds the renderer's device buffers as sized at capture, and they only grow: a later call on the same device,
         by any trainer, that needs more room (more images or rays per step, more frames, a larger render with gradients)
         re-allocates them.  step_images_graph then raises RuntimeError instead of replaying (nfb_buffer_epoch): capture again."""
         n = int(n_per_image)
         rank = self._check_images(data, k, n, world, group, rank)
-        if has_background != (data.background is not None):
+        if self.background is None and has_background != (data.background is not None):
             raise ValueError("has_background must say whether the training set has a background")
         dev = self.dev
+        data = self._images_data(data)
         sb = dict(self._images_buffers(data, k, n))  # own copies of the per-step buffers: eager steps must not write into them
         for name, t in list(sb.items()):
             if t is not None and name != "shortfall":

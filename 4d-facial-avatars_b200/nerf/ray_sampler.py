@@ -1,6 +1,7 @@
 """The per-iteration ray selection of train_transformed_rays.py:230-239 (importance maps) and :303-331 (np.random.choice +
 gathers) on the device (SURVEY.md §8f rank 3): nfb_sample_rays returns the indices numpy would return for the same uniform
 draws, bit for bit, and gathers ray origins / directions, target and background colours of the selected pixels in the same launch."""
+import copy
 import ctypes as C
 
 import numpy as np
@@ -119,6 +120,20 @@ class TrainImages:
                 raise ValueError(f"{name} must be a contiguous FP32 [{self.n_images},{w}] tensor on {self.dev}")
         self.poses, self.expressions = poses, expressions
         self.desc.poses, self.desc.expressions = poses.data_ptr(), expressions.data_ptr()
+
+    def with_background(self, background):
+        """A copy of this set whose sampler reads `background` ([H,W,3] contiguous FP32 on this device) in place: every later
+        sampler call, and every replay of a graph captured over one, gathers what the table holds then (a trainer's learned
+        background is such a table).  The copy shares every other table with this object, which is left unchanged.  The caller
+        keeps `background` alive while the copy is used."""
+        if (background.dtype != torch.float32 or background.device != self.dev or tuple(background.shape) != (self.H, self.W, 3)
+                or not background.is_contiguous()):
+            raise ValueError(f"the background must be a contiguous FP32 [{self.H},{self.W},3] tensor on {self.dev}")
+        view = copy.copy(self)
+        view.background = background
+        view.desc = capi.NfbTrainImages.from_buffer_copy(self.desc)
+        view.desc.background = background.data_ptr()
+        return view
 
     def _keep_in_place(self, t):
         if t.is_cuda:

@@ -45,6 +45,10 @@ extern "C" {
  * per-frame camera pose, expression and latent fitted to photos).  The version number stayed 131 for this addition: test this
  * macro. */
 #define NFB_FIT_STEP 1
+/* Defined when nfb_background_rows_grad and nfb_loss_background_grad exist: a training step over several images that learns the
+ * background image (the reference's train_background / supervised_train_background).  The version number stayed 131 for this
+ * addition: test this macro. */
+#define NFB_TRAIN_BACKGROUND 1
 
 typedef struct NfbHandle NfbHandle;
 
@@ -504,6 +508,41 @@ int nfb_fit_rows_grad(NfbHandle* h, const NfbTrainImages* data, const int32_t* i
                       const float* grad_expressions,     /* [K][76] or NULL */
                       float* expression_grads,           /* [n_images][76] or NULL: rows ADDED to */
                       void* stream);
+
+/* ---- A learned background (NFB_TRAIN_BACKGROUND) ----
+ * The rows of a learned [height][width][3] background table's gradient: what autograd leaves in the table for a loss over rays
+ * whose background colours were gathered from it at pixel_rc (nfb_sample_rays_images' pixel_rc, or any slice [r0, r1) of it, as a
+ * data-parallel rank passes its own rays), given the per-ray render term grad_bg_render (NfbInputGrads.background of the
+ * backward) and the per-ray loss term grad_bg_loss (nfb_loss_background_grad's grad_bg_rays; NULL: none), each [n_rays][3].
+ * Ray r sits at table row row * width + col, the index the sampler's gathers read (one shared device helper forms both).
+ * Order: table_grads[row r][c] += g_r[c] for r = 0 .. n_rays - 1 in ascending r, where g_r = grad_bg_render[r] +
+ * grad_bg_loss[r] is rounded once (g_r = grad_bg_render[r] without a loss term) and each add into a row is one rounded FP32 add.
+ * Rows are ADDED to; rows no ray names get nothing.  No atomics: the rows repeat bit for bit.  (The pixels are split between the
+ * 1024 warps of the launch by table index; each warp walks all rays in ascending order, 32 at a time, and one lane adds each of
+ * its pixels' rays of those 32 in ascending order.  So the order holds for any batch, with no sort.)
+ * Edges: a pixel_rc entry outside the table (-1, as the sampler writes for an out-of-range image slot) adds nothing.  A NaN in
+ * g_r reaches only its own pixel's row.  A pixel named several times (an incomplete selection's repeats, two slots drawing the
+ * same pixel) accumulates every ray in ascending r.
+ * Errors, before any CUDA call: NFB_ERR_INVALID for a null handle / pixel_rc / grad_bg_render / table_grads, n_rays < 0,
+ * height or width < 1, height * width > 2^31 - 1.  n_rays == 0 adds nothing and launches nothing.  Launches: 1. */
+int nfb_background_rows_grad(NfbHandle* h, const int32_t* pixel_rc /* [n_rays][2] */, int n_rays, int height, int width,
+                             const float* grad_bg_render /* [n_rays][3] */, const float* grad_bg_loss /* [n_rays][3] or NULL */,
+                             float* table_grads /* [height][width][3]: rows ADDED to */, void* stream);
+/* The supervised background term of train_transformed_rays.py:375-387, weight * mean_r(w_last[r] * ||bg[r] - target[r]||^2) with
+ * the mean over n_total rays (the GLOBAL batch when these n_rays are one shard of it, as in nfb_loss_mse_grad); the reference's
+ * weight is 0.001 and its w_last the last pass's (NfbOutputs.w_last).
+ * Order, every operation one FP32 rounding: s = weight * (1 / n_total) (as autograd's mean backward forms it on CUDA); per ray
+ * d[c] = bg[c] - target[c], e = (d[0] * d[0] + d[1] * d[1]) + d[2] * d[2];  grad_bg_rays[r][c] = (2 * d[c]) * (s * w_last[r]),
+ * grad_w_last[r] = s * e (OVERWRITTEN);  loss[0] += S * s, S the sum of the terms w_last[r] * e over the rays in loss_mse_grad's
+ * fixed order: thread t of one 1024-thread block adds rays t, t + 1024, ... in ascending order from +0, the lanes of each warp
+ * meet by xor butterfly (offsets 16, 8, 4, 2, 1: lane value += the partner's), and warp 0 .. 31's lane-0 sums are added in
+ * ascending order from +0.  So the loss repeats bit for bit, and the shards' shares sum to the batch's loss to rounding.
+ * Errors, before any CUDA call: NFB_ERR_INVALID for any null pointer, n_rays < 0, n_total < n_rays or n_total <= 0.  n_rays == 0
+ * writes and launches nothing.  Launches: 1 (one thread block). */
+int nfb_loss_background_grad(NfbHandle* h, const float* bg_rays /* [n_rays][3] */, const float* target /* [n_rays][3] */,
+                             const float* w_last /* [n_rays] */, int n_rays, long long n_total, float weight,
+                             float* grad_bg_rays /* [n_rays][3] */, float* grad_w_last /* [n_rays] */, float* loss /* ADDED to */,
+                             void* stream);
 
 /* Host-only test hook of the same arithmetic: out[i] = np.cumsum(p)[ks[i]] (ks[i] == -1: the last entry) for the map with the
  * ascending flat indices zeroed_sorted set to zero.  No CUDA call. */
